@@ -1,4 +1,4 @@
-/* b2_ddp_bert.h — C ABI of libb2ddpbert.so: the sm_100a kernels behind the DDP BERT fine-tuning step.
+/* b2_ddp_bert.h — C ABI of libb2ddpbert.so: the sm_90a (H100) kernels behind the DDP BERT fine-tuning step.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  The reference (taishan1994/pytorch-distributed-NLP) has no
  * native code; the work these entry points replace is issued by third-party Python modules that
@@ -32,7 +32,7 @@ int32_t b2_abi_version(void);             /* bumped when a struct below changes 
 int64_t b2_launch_count(void);            /* kernels launched by this library so far (process-wide) */
 
 /* ------------------------------------------------------------------------------------------------------ */
-/* GEMM (tcgen05 + TMA)                                                                                   */
+/* GEMM (wgmma + TMA)                                                                                     */
 /*   replaces: cuBLAS addmm issued by SP/transformers/models/bert/modeling_bert.py:179-181 (Q,K,V),       */
 /*   :295 (attention output dense), :340 (intermediate dense), :353 (output dense) and the dgrad/wgrad    */
 /*   GEMMs autograd runs for them inside `loss.backward()` (multi-gpu-distributed-cls.py:173).            */
@@ -72,10 +72,10 @@ typedef struct b2_gemm_args {
   uint32_t rng_site;      /* distinct per dropout site                                                       */
   void* workspace;        /* fp32 scratch for split-K (may be NULL -> never split)                           */
   int64_t workspace_bytes;
-  int32_t force_bn;       /* 0 = auto, else 128 / 192 / 256 (tests, tuning)                                  */
+  int32_t force_bn;       /* 0 = auto, else 128 / 256 (tests, tuning)                                        */
   int32_t force_splits;   /* 0 = auto, else >= 1                                                             */
-  int32_t force_kernel;   /* 0 = auto, 1 = single-CTA 128xBN kernel, 2 = CTA-pair (cta_group::2) 256xBN kernel        */
-  void* debug_timing;     /* NULL, or device int64[grid][8]: clock64 phase stamps (CTA-pair GEMM, b2_gemm_ln_fwd)    */
+  int32_t force_kernel;   /* kernel choice (tests, tuning); the H100 build has one GEMM kernel and ignores it       */
+  void* debug_timing;     /* unused (NULL)                                                                        */
   float* colsum_out;      /* NULL, or fp32 [N]: += column sums of the (bf16-rounded) output D, by atomic add        */
 } b2_gemm_args_t;
 
@@ -93,7 +93,7 @@ int32_t b2_gemm_bf16_grouped(const b2_gemm_args_t* args, int32_t count, void* st
  * FP32 [M, N] (ld_aux_in in elements): the residual stream stays in fp32 end to end.  D receives the pre-LayerNorm sum
  * rounded to bf16 (kept for the backward), y the normalised output as bf16 (the next GEMM's operand), y_f32 (optional)
  * the same as fp32 (the next block's residual), mean / rstd (fp32 [M]) the row statistics -- computed from the
- * UNROUNDED fp32 sum.  A row's N columns are spread over a cluster of N / 256 CTA pairs; the row statistics travel
+ * UNROUNDED fp32 sum.  A row's N columns are spread over a cluster of N / 256 CTAs; the row statistics travel
  * through distributed shared memory.
  * b2_gemm_ln_max_clusters(hidden): how many such clusters the device can hold at once (0 = shape / device not
  * supported: issue b2_gemm_bf16 + b2_layernorm_fwd instead).                                                    */

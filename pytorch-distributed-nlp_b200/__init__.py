@@ -1,6 +1,6 @@
-"""B200-native DDP BERT fine-tuning step behind the surface of taishan1994/pytorch-distributed-NLP's
+"""H100-native DDP BERT fine-tuning step behind the surface of taishan1994/pytorch-distributed-NLP's
 ``multi-gpu-distributed-cls.py``: same ``BertForSequenceClassification`` / ``DistributedDataParallel`` /
-``build_optimizer`` / ``Trainer`` names, hand-written sm_100a kernels underneath (libb2ddpbert.so, C ABI in
+``build_optimizer`` / ``Trainer`` names, hand-written sm_90a kernels underneath (libb2ddpbert.so, C ABI in
 include/b2_ddp_bert.h).  Importing never touches the GPU; the library is loaded (and required) on first use."""
 from . import _lib
 from .modeling import (BertConfig, BertForSequenceClassification, SequenceClassifierOutput, bert_base_config,

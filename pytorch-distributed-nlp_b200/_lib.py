@@ -107,7 +107,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            "libb2ddpbert.so is not built (%s). Run `python __graft_entry__.py` (nvcc, sm_100a). "
+            "libb2ddpbert.so is not built (%s). Run `python __graft_entry__.py` (nvcc, sm_90a). "
             "There is no CPU or PyTorch fallback for this path." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     lib.b2_last_error.restype = C.c_char_p

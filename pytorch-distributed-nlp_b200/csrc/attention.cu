@@ -1,19 +1,20 @@
-// Fused multi-head self-attention, forward and backward, on tcgen05 tensor cores (head_dim 64, seq % 128 == 0).
+// Fused multi-head self-attention, forward and backward, on Hopper tensor cores (wgmma; head_dim 64, seq % 128 == 0).
 //
 // Replaces the eager attention of BertSelfAttention (SP/transformers/models/bert/modeling_bert.py:115-140:
 // matmul -> *scale -> +mask -> softmax -> dropout -> matmul, and the transpose/contiguous head merge at :138,:206)
 // plus its autograd backward (SURVEY.md K3-K6).  The [B,12,S,S] probability tensor never exists in HBM: the
 // backward recomputes it from Q, K and the saved log-sum-exp.
 //
-// One CTA = 256 threads = 128 query (fwd) or key (bwd) rows = the 128 TMEM lanes, TWO threads per row: warps 0-3
-// take key columns 0-63 of a 128-wide score block, warps 4-7 columns 64-127 (a warp may touch TMEM lanes
-// 32*(warp%4)..+31, any columns), which halves the per-row softmax / dS work that bounded the 128-thread version.
-// Tiles move HBM->smem by TMA straight out of the packed [tokens, 3*hidden] QKV activation (128B swizzle);
-// the same smem tile serves as a K-major operand for one product and as an MN-major operand for another
-// (e.g. dO is A of dP = dO V^T and B of dV = P^T dO), so nothing is ever transposed in memory.  Results leave the
-// same way: the context tile, dQ, dK and dV are written into operand tiles the last MMAs have released and stored
-// with TMA; the key-padding mask is a 64-bit register pair per thread.  Kernels: attention_fwd128_kernel (seq 128,
-// 4 CTAs/SM), attention_fwd_kernel (any seq <= 512, online softmax), attention_bwd_kernel<kOneQ>.
+// One CTA = 256 threads = two warpgroups = 128 query (fwd) or key (bwd) rows: warpgroup g computes rows
+// [64 g, 64 g + 64) of every product with wgmma m64nNk16, accumulators in registers.  In the accumulator layout a
+// row's columns are spread over the four lanes of a quad (lane / 4 picks the row, lane % 4 the column pair in each
+// 8-column group), so row maxima and sums take two quad shuffles, and each lane draws the dropout decisions of a
+// quarter of the row's 8-key groups and shares them within the quad.  Tiles move HBM->smem by TMA straight out of
+// the packed [tokens, 3*hidden] QKV activation (128B swizzle); the same smem tile serves as a K-major operand for
+// one product and as an MN-major operand for another (e.g. dO is A of dP = dO V^T and B of dV = P^T dO), so nothing
+// is ever transposed in memory.  Results leave the same way: the context tile, dQ, dK and dV are written into
+// operand tiles the last products have released and stored with TMA.  Kernels: attention_fwd128_kernel (seq 128),
+// attention_fwd_kernel (any seq <= 512, online softmax), attention_bwd_kernel<kOneQ>.
 #include "common.cuh"
 #include "../../include/b2_ddp_bert.h"
 
@@ -25,11 +26,13 @@ constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 constexpr float kMaskBias = -3.4028234663852886e38f;  // torch.finfo(float32).min, what HF adds for masked keys
 
-// [128 rows x 128 cols] bf16 tile as two 64-column sub-tiles of 128-byte swizzled rows.  Read as a K-major operand
-// (rows = M, cols = K) or as an MN-major operand (rows = K, cols = M) depending on the descriptor.
-__device__ __forceinline__ void st_tile_chunk(uint8_t* tile, int row, int chunk /*0..15, 8 elements each*/, uint4 v) {
-  const int sub = chunk >> 3, ch = chunk & 7;
-  *reinterpret_cast<uint4*>(tile + sub * TILE_BYTES + row * 128 + ((ch ^ (row & 7)) << 4)) = v;
+// Byte offset of element (row, col) in a [128 rows x 64 cols] bf16 tile of 128-byte swizzled rows (the TMA layout).
+__device__ __forceinline__ uint32_t sw_off(int row, int col) {
+  return row * 128 + ((((col >> 3) ^ (row & 7))) << 4) + (col & 7) * 2;
+}
+// two adjacent bf16 (col even) of a [128 x 128] tile kept as two 64-column sub-tiles `lo`, `hi`
+__device__ __forceinline__ void st_pair(uint8_t* lo, uint8_t* hi, int row, int col, float a, float b) {
+  *reinterpret_cast<uint32_t*>((col < 64 ? lo : hi) + sw_off(row, col & 63)) = pack_bf16(a, b);
 }
 
 struct AttnParams {
@@ -44,67 +47,97 @@ struct AttnParams {
   __nv_bfloat16* d_qkv; float* dq_accum;
   float* dbias;                   // optional fp32 [3*hidden]: += column sums of d_qkv (QKV bias gradient)
   // optional (seq == 128, dropout on): the forward's dropout decisions, one 64-bit word per (b, h, query row, key
-  // half) -- written by the forward, read by the backward instead of regenerating Philox (38 % of its instructions)
+  // half) -- written by the forward, read by the backward instead of regenerating Philox
   unsigned long long* keep_bits;
   // optional (seq == 128): packed bins -- row r of bin b may attend to keys [lo, hi) of the same bin only,
   // seg[b * 128 + r] = lo | hi << 16 (pytorch-distributed-nlp_b200/packing.py); replaces the key-padding mask
   const int* seg;
 };
 
-// masked-key bits (1 = masked) of the 64 key columns [half * 64, half * 64 + 64) for a row whose keys are [lo, hi)
-__device__ __forceinline__ void seg_key_bits(int seg_word, int half, uint32_t& mb0, uint32_t& mb1) {
-  int lo = (seg_word & 0xffff) - half * 64, hi = (seg_word >> 16) - half * 64;
-  lo = lo < 0 ? 0 : (lo > 64 ? 64 : lo);
-  hi = hi < 0 ? 0 : (hi > 64 ? 64 : hi);
-  unsigned long long allowed = 0ull;
-  if (hi > lo) {
-    const unsigned long long upto_hi = hi == 64 ? ~0ull : ((1ull << hi) - 1ull);
-    const unsigned long long upto_lo = lo == 64 ? ~0ull : ((1ull << lo) - 1ull);
-    allowed = upto_hi & ~upto_lo;
-  }
-  const unsigned long long masked = ~allowed;
-  mb0 = (uint32_t)masked;
-  mb1 = (uint32_t)(masked >> 32);
-}
+// Fragment coordinates of this thread in a warpgroup-wide m64 accumulator (see wgmma.cuh): rows r and r + 8 of the
+// CTA's 128, column pair 2 t (+1) of every 8-column group.
+struct Frag {
+  int r, t;
+  __device__ __forceinline__ Frag(int warp, int lane)
+      : r((warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2)), t(lane & 3) {}
+  // accumulator index i of an n-wide product -> row (0: r, 1: r + 8) and column
+  __device__ __forceinline__ static int hi(int i) { return (i >> 1) & 1; }
+  __device__ __forceinline__ int col(int i) const { return 8 * (i >> 2) + 2 * t + (i & 1); }
+};
 
-// Sum v[j] over the 32 lanes for every j: 31 shuffles (butterfly with halving); lane l returns the total of column l.
-__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
+// Dropout decisions of the 16 eight-key groups of one 128-key row whose key 0 has Philox element index `base`:
+// lane t of the quad draws groups t, t + 4, t + 8, t + 12; after the exchange keep[j] holds group j's 8 bits.
+__device__ __forceinline__ void quad_keep16(const DropCtx& d, unsigned long long base, int lane, uint32_t (&keep)[16]) {
+  uint32_t own[4];
 #pragma unroll
-  for (int off = 16; off >= 1; off >>= 1) {
-    const bool upper = (lane & off) != 0;
+  for (int jj = 0; jj < 4; ++jj) own[jj] = dropout_keep8(d, base + 8ull * (4 * jj + (lane & 3)));
 #pragma unroll
-    for (int j = 0; j < off; ++j) {
-      const float send = upper ? v[j] : v[j + off];
-      const float keep = upper ? v[j + off] : v[j];
-      v[j] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+  for (int j = 0; j < 16; ++j) keep[j] = __shfl_sync(0xffffffffu, own[j >> 2], (lane & ~3) | (j & 3));
+}
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+// is key `col` (0..127 within the block) masked for a row: packed bins compare against the row's own [lo, hi); the
+// key-padding mask is one bit per key (mw: the block's four 32-key words)
+template <bool kSeg>
+__device__ __forceinline__ bool key_masked(const uint32_t (&mw)[4], int seg_word, int col) {
+  if (kSeg) return col < (seg_word & 0xffff) || col >= (seg_word >> 16);
+  return (mw[col >> 5] >> (col & 31)) & 1u;
+}
+// Column sums over the 128 rows of an m64n64 accumulator pair (one warpgroup per 64 rows), added into out[0, 64)
+__device__ __forceinline__ void frag_colsum64(const float (&f)[32], int lane, float* out) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float v = f[4 * j + e] + f[4 * j + 2 + e];
+      v += __shfl_xor_sync(0xffffffffu, v, 4);
+      v += __shfl_xor_sync(0xffffffffu, v, 8);
+      v += __shfl_xor_sync(0xffffffffu, v, 16);
+      if (lane < 4) atomicAdd(out + 8 * j + 2 * lane + e, v);
     }
   }
-  return v[0];
+}
+// S[128 x 128] (+)= A[128 x 64] B[128 x 64]^T, both K-major tiles (Q K^T, dO V^T): warpgroup wg's 64 rows
+__device__ __forceinline__ void mma_nt_128(float (&s)[64], const uint8_t* a, const uint8_t* b, int wg) {
+  const uint32_t aa = smem_u32(a) + wg * 8192, ab = smem_u32(b);
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    wgmma_bf16<128, 0, 0>(s, make_smem_desc(aa + k * 32, 16, 1024), make_smem_desc(ab + k * 32, 16, 1024),
+                          k > 0 ? 1u : 0u);
+}
+// O[128 x 64] = P[128 x 128] V[128 x 64]: P K-major in two 64-key sub-tiles, V MN-major (rows = keys)
+__device__ __forceinline__ void mma_pv(float (&o)[32], const uint8_t* p_lo, const uint8_t* p_hi, const uint8_t* v,
+                                       int wg) {
+  const uint32_t a0 = smem_u32(p_lo) + wg * 8192, a1 = smem_u32(p_hi) + wg * 8192, av = smem_u32(v);
+#pragma unroll
+  for (int k = 0; k < 8; ++k)
+    wgmma_bf16<64, 0, 1>(o, make_smem_desc((k < 4 ? a0 : a1) + (k & 3) * 32, 16, 1024),
+                         make_smem_desc(av + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
 }
 
 // ------------------------------------------------------------------------------------------------------------
 // forward: grid (seq/128, heads, batch)
 // ------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(ATT_THREADS) attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
-                                                                   const __grid_constant__ CUtensorMap tmap_ctx,
-                                                                   const AttnParams p) {
+__global__ void __launch_bounds__(ATT_THREADS, 1) attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
+                                                                      const __grid_constant__ CUtensorMap tmap_ctx,
+                                                                      const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align_1024(smem_raw);
   uint8_t* sQ = smem;
   uint8_t* sK = smem + TILE_BYTES;
   uint8_t* sV = smem + 2 * TILE_BYTES;
   uint8_t* sP = smem + 3 * TILE_BYTES;  // 2 tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 5 * TILE_BYTES);
-  uint64_t* bar_load = &bars[0];
-  uint64_t* bar_s = &bars[1];
-  uint64_t* bar_o = &bars[2];
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(&bars[4]);
+  uint64_t* bar_load = reinterpret_cast<uint64_t*>(smem + 5 * TILE_BYTES);
   uint32_t* s_mbits = reinterpret_cast<uint32_t*>(smem + 5 * TILE_BYTES + 64);  // [seq / 32 <= 16] masked-key bits
-  float* s_red = reinterpret_cast<float*>(smem + 5 * TILE_BYTES + 128);         // [2][128] row exchange between halves
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int row = (warp & 3) * 32 + lane;   // TMEM lane == query row of this thread
-  const int half = warp >> 2;               // which 64 of the 128 key columns (and which 32 of the 64 output dims)
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const Frag fr(warp, lane);
   const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int nkv = p.seq / 128;
 
@@ -112,11 +145,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_fwd_kernel(const __grid
     tma_prefetch_desc(&tmap_qkv);
     tma_prefetch_desc(&tmap_ctx);
     mbar_init(bar_load, 1);
-    mbar_init(bar_s, 1);
-    mbar_init(bar_o, 1);
     fence_mbar_init();
   }
-  if (warp == 0) tmem_alloc(tmem_holder, 256);
   pdl_wait();               // PDL: setup above overlapped the predecessor's tail; global reads start below
   pdl_launch_dependents();
   for (int c = tid; c < p.seq; c += ATT_THREADS) {   // seq % 128 == 0: whole warps take part in every round
@@ -124,15 +154,9 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_fwd_kernel(const __grid
     const unsigned bits = __ballot_sync(0xffffffffu, masked);
     if (lane == 0) s_mbits[c >> 5] = bits;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_holder;
-  const uint32_t tmem_s = tmem, tmem_o = tmem + 128;
-  const uint32_t lane_base = ((uint32_t)((warp & 3) * 32)) << 16;
 
   const int row0 = b * p.seq;           // first token row of this sequence
-  const int q_row = qb * 128 + row;     // query index inside the sequence
   const int col_q = h * 64, col_k = p.hidden + h * 64, col_v = 2 * p.hidden + h * 64;
   const DropCtx drop = make_drop_ctx(p.rng, p.rng_site, p.dropout_p);
   const float c2 = p.scale * kLog2e;
@@ -140,11 +164,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_fwd_kernel(const __grid
   float o_acc[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) o_acc[i] = 0.f;
-  float m_run = -INFINITY, l_run = 0.f;   // l_run: this thread's half of the row sum
-  uint32_t ph_load = 0, ph_s = 0, ph_o = 0;
-
-  constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, false, false);
-  constexpr uint32_t idesc_o = make_idesc_bf16(128, 64, false, true);
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // l_run: this lane's share of the row sum
+  uint32_t ph_load = 0;
 
   for (int j = 0; j < nkv; ++j) {
     if (tid == 0) {
@@ -152,151 +173,100 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_fwd_kernel(const __grid
       if (j == 0) tma_load_2d(sQ, &tmap_qkv, bar_load, col_q, row0 + qb * 128);
       tma_load_2d(sK, &tmap_qkv, bar_load, col_k, row0 + j * 128);
       tma_load_2d(sV, &tmap_qkv, bar_load, col_v, row0 + j * 128);
-      mbar_wait(bar_load, ph_load);
-      tc_fence_after();
-      const uint32_t aq = smem_u32(sQ), ak = smem_u32(sK);
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        umma_bf16(tmem_s, make_smem_desc(aq + k * 32, 16, 1024), make_smem_desc(ak + k * 32, 16, 1024), idesc_s,
-                  k > 0 ? 1u : 0u);
-      umma_commit(bar_s);
     }
+    mbar_wait(bar_load, ph_load);
     ph_load ^= 1;
-    __syncwarp();
-    mbar_wait(bar_s, ph_s);
-    ph_s ^= 1;
-    tc_fence_after();
+    float s[64];
+    wgmma_fence();
+    mma_nt_128(s, sQ, sK, wg);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
 
-    // this thread's 64 key columns of the block: masked-key bits in two registers; the common unmasked block takes
-    // a warp-uniform fast path (no per-element select)
-    const uint32_t mb0 = s_mbits[j * 4 + half * 2], mb1 = s_mbits[j * 4 + half * 2 + 1];
-    const bool any_masked = (mb0 | mb1) != 0u;
-    // pass 1: maximum of this thread's 64 scaled + masked scores (log2 domain), then across the two halves
-    float m_loc = -INFINITY;
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      const uint32_t mbits = c == 0 ? mb0 : mb1;
-      uint32_t v[32];
-      tmem_ld32(tmem_s + lane_base + half * 64 + c * 32, v);
-      tmem_ld_wait();
-      if (!any_masked) {
+    const uint32_t mw[4] = {s_mbits[j * 4], s_mbits[j * 4 + 1], s_mbits[j * 4 + 2], s_mbits[j * 4 + 3]};
+    // maximum of the row's scaled + masked scores (log2 domain); a masked key counts as score*c2 + (-3.4e38),
+    // which is -3.4e38 in fp32
+    float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-        for (int i = 0; i < 32; ++i) m_loc = fmaxf(m_loc, __uint_as_float(v[i]));
-      } else {
+    for (int i = 0; i < 64; ++i)
+      if (!key_masked<false>(mw, 0, fr.col(i))) mx[Frag::hi(i)] = fmaxf(mx[Frag::hi(i)], s[i]);
+    float m_new[2], alpha[2];
 #pragma unroll
-        for (int i = 0; i < 32; ++i)
-          m_loc = fmaxf(m_loc, ((mbits >> i) & 1u) ? -INFINITY : __uint_as_float(v[i]));
-      }
+    for (int u = 0; u < 2; ++u) {
+      const float mb = fmaxf(quad_max(mx[u]) * c2, kMaskBias);   // scale after the max (c2 > 0)
+      m_new[u] = fmaxf(m_run[u], mb);
+      alpha[u] = exp2f(m_run[u] - m_new[u]);                      // first block: exp2(-inf) = 0
     }
-    // scale after the max (c2 > 0); a masked key counts as score*c2 + (-3.4e38), which is -3.4e38 in fp32
-    m_loc = m_loc * c2;
-    if (any_masked) m_loc = fmaxf(m_loc, kMaskBias);
-    s_red[half * 128 + row] = m_loc;
-    __syncthreads();
-    const float m_new = fmaxf(m_run, fmaxf(s_red[row], s_red[128 + row]));
-    const float alpha = exp2f(m_run - m_new);  // first block: exp2(-inf) = 0
-    float l_blk = 0.f;
-    // pass 2: probabilities -> (dropout) -> bf16 P tile in smem
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      const uint32_t mbits = c == 0 ? mb0 : mb1;
-      uint32_t v[32];
-      tmem_ld32(tmem_s + lane_base + half * 64 + c * 32, v);
-      tmem_ld_wait();
-      float pr[32];
+    // probabilities -> (dropout) -> bf16 P tile in smem
+    uint32_t keep[2][16];
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        float x = fmaf(__uint_as_float(v[i]), c2, -m_new);
-        if (any_masked && ((mbits >> i) & 1u)) x = kMaskBias - m_new;
-        pr[i] = ex2_approx(x);
-        l_blk += pr[i];
-      }
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const unsigned long long idx = (((unsigned long long)(b * p.heads + h) * p.seq + q_row) * p.seq) + j * 128 +
-                                       half * 64 + c * 32 + g * 8;
-        const uint32_t keep = dropout_keep8(drop, idx);
-        float q8[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) q8[i] = ((keep >> i) & 1u) ? pr[g * 8 + i] * drop.scale : 0.f;
-        uint4 o;
-        o.x = pack_bf16(q8[0], q8[1]); o.y = pack_bf16(q8[2], q8[3]);
-        o.z = pack_bf16(q8[4], q8[5]); o.w = pack_bf16(q8[6], q8[7]);
-        st_tile_chunk(sP, row, half * 8 + c * 4 + g, o);
-      }
+    for (int u = 0; u < 2; ++u) {
+      const int q_row = qb * 128 + fr.r + 8 * u;
+      quad_keep16(drop, (((unsigned long long)(b * p.heads + h) * p.seq + q_row) * p.seq) + j * 128, lane, keep[u]);
     }
-    l_run = l_run * alpha + l_blk;
-    m_run = m_new;
-
+    float l_blk[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) {
+      const int u = Frag::hi(i), c = fr.col(i);
+      float q2[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float x = fmaf(s[i + e], c2, -m_new[u]);
+        if (key_masked<false>(mw, 0, c + e)) x = kMaskBias - m_new[u];
+        const float pr = ex2_approx(x);
+        l_blk[u] += pr;
+        q2[e] = ((keep[u][c >> 3] >> ((c + e) & 7)) & 1u) ? pr * drop.scale : 0.f;
+      }
+      st_pair(sP, sP + TILE_BYTES, fr.r + 8 * u, c, q2[0], q2[1]);
+    }
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      l_run[u] = l_run[u] * alpha[u] + l_blk[u];
+      m_run[u] = m_new[u];
+    }
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    if (tid == 0) {
-      tc_fence_after();
-      const uint32_t ap = smem_u32(sP), av = smem_u32(sV);
+    float ob[32];
+    wgmma_fence();
+    mma_pv(ob, sP, sP + TILE_BYTES, sV, wg);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(ob);
 #pragma unroll
-      for (int k = 0; k < 8; ++k)
-        umma_bf16(tmem_o, make_smem_desc(ap + (k >> 2) * TILE_BYTES + (k & 3) * 32, 16, 1024),
-                  make_smem_desc(av + k * 2048, 16, 1024), idesc_o, k > 0 ? 1u : 0u);
-      umma_commit(bar_o);
-    }
-    __syncwarp();
-    mbar_wait(bar_o, ph_o);
-    ph_o ^= 1;
-    tc_fence_after();
-    {
-      uint32_t v[32];
-      tmem_ld32(tmem_o + lane_base + half * 32, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) o_acc[i] = o_acc[i] * alpha + __uint_as_float(v[i]);
-    }
-    // all TMEM reads of this iteration must retire before thread 0 issues the next QK^T / PV
-    tc_fence_before();
-    __syncthreads();
+    for (int i = 0; i < 32; ++i) o_acc[i] = o_acc[i] * alpha[Frag::hi(i)] + ob[i];
+    __syncthreads();   // every product of this block is complete: K, V and P may be overwritten
   }
 
-  // total row sum = the two halves' partial sums
-  s_red[half * 128 + row] = l_run;
-  __syncthreads();
-  const float l_tot = s_red[row] + s_red[128 + row];
-  const float inv_l = 1.0f / l_tot;
-  // the context tile leaves through Q's tile (its last reader, the final QK^T, completed long ago) as one TMA store:
-  // per-thread row stores would touch 32 different lines per instruction
+  // the context tile leaves through Q's tile (its last reader, the final QK^T, completed) as one TMA store
+  float inv_l[2];
 #pragma unroll
-  for (int i = 0; i < 32; i += 8) {
-    uint4 o;
-    o.x = pack_bf16(o_acc[i] * inv_l, o_acc[i + 1] * inv_l);
-    o.y = pack_bf16(o_acc[i + 2] * inv_l, o_acc[i + 3] * inv_l);
-    o.z = pack_bf16(o_acc[i + 4] * inv_l, o_acc[i + 5] * inv_l);
-    o.w = pack_bf16(o_acc[i + 6] * inv_l, o_acc[i + 7] * inv_l);
-    st_tile_chunk(sQ, row, half * 4 + (i >> 3), o);
+  for (int u = 0; u < 2; ++u) {
+    const float l_tot = quad_sum(l_run[u]);
+    inv_l[u] = 1.0f / l_tot;
+    if (p.lse != nullptr && fr.t == 0)
+      p.lse[((size_t)b * p.heads + h) * p.seq + qb * 128 + fr.r + 8 * u] = (m_run[u] + log2f(l_tot)) * kLn2;
   }
-  if (p.lse != nullptr && half == 0)
-    p.lse[((size_t)b * p.heads + h) * p.seq + q_row] = (m_run + log2f(l_tot)) * kLn2;
-
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int u = Frag::hi(i);
+    st_pair(sQ, sQ, fr.r + 8 * u, fr.col(i), o_acc[i] * inv_l[u], o_acc[i + 1] * inv_l[u]);
+  }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
   if (tid == 0) {
     tma_store_2d(&tmap_ctx, sQ, h * 64, row0 + qb * 128);
     tma_store_commit_and_wait();
   }
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 256);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------------------
 // forward, seq == 128 (the benchmark shape): one key block, so no online rescale and no accumulator carried across
-// iterations.  The CTA is trimmed to fit FOUR per SM (ncu on the general kernel: a third of its samples are
-// mbarrier spins -- TMA / MMA latency -- and 384 CTAs need two waves at 2 per SM): 3 smem tiles (P overwrites Q and K
-// once S = QK^T has completed), 128 TMEM columns (O overwrites the drained S columns), 16-column register passes
-// (62 registers).  Same arithmetic, same Philox indexing as attention_fwd_kernel.
+// iterations.  3 smem tiles (P overwrites Q and K once S = QK^T has completed, the context tile overwrites V).
+// Same arithmetic, same Philox indexing as attention_fwd_kernel; also records the dropout decisions (keep_bits) for
+// the backward.
 // ------------------------------------------------------------------------------------------------------------
 template <bool kSeg>   // kSeg: packed bins (per-row segment mask, p.seg) instead of the key-padding mask
-__global__ void __launch_bounds__(ATT_THREADS, 4) attention_fwd128_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
+__global__ void __launch_bounds__(ATT_THREADS, 2) attention_fwd128_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
                                                                          const __grid_constant__ CUtensorMap tmap_ctx,
                                                                          const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -304,28 +274,19 @@ __global__ void __launch_bounds__(ATT_THREADS, 4) attention_fwd128_kernel(const 
   uint8_t* sQ = smem;                      // later: keys 0-63 of P
   uint8_t* sK = smem + TILE_BYTES;         // later: keys 64-127 of P
   uint8_t* sV = smem + 2 * TILE_BYTES;     // later: the context tile on its way out
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 3 * TILE_BYTES);
-  uint64_t* bar_load = &bars[0];
-  uint64_t* bar_s = &bars[1];
-  uint64_t* bar_o = &bars[2];
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(&bars[3]);
+  uint64_t* bar_load = reinterpret_cast<uint64_t*>(smem + 3 * TILE_BYTES);
   uint32_t* s_mbits = reinterpret_cast<uint32_t*>(smem + 3 * TILE_BYTES + 48);   // [4]
-  float* s_red = reinterpret_cast<float*>(smem + 3 * TILE_BYTES + 64);           // [2][128]
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int row = (warp & 3) * 32 + lane;   // TMEM lane == query row of this thread
-  const int half = warp >> 2;               // which 64 of the 128 key columns (and which 32 of the 64 output dims)
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const Frag fr(warp, lane);
   const int h = blockIdx.y, b = blockIdx.z;
 
   if (tid == 0) {
     tma_prefetch_desc(&tmap_qkv);
     tma_prefetch_desc(&tmap_ctx);
     mbar_init(bar_load, 1);
-    mbar_init(bar_s, 1);
-    mbar_init(bar_o, 1);
     fence_mbar_init();
   }
-  if (warp == 0) tmem_alloc(tmem_holder, 128);
   pdl_wait();               // PDL: setup above overlapped the predecessor's tail; global reads start below
   pdl_launch_dependents();
   if (tid < 128) {
@@ -333,147 +294,102 @@ __global__ void __launch_bounds__(ATT_THREADS, 4) attention_fwd128_kernel(const 
     const unsigned bits = __ballot_sync(0xffffffffu, masked);
     if (lane == 0) s_mbits[warp] = bits;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_holder;
-  const uint32_t lane_base = ((uint32_t)((warp & 3) * 32)) << 16;
   const int row0 = b * 128;
   const int col_q = h * 64, col_k = p.hidden + h * 64, col_v = 2 * p.hidden + h * 64;
-  const DropCtx drop = make_drop_ctx(p.rng, p.rng_site, p.dropout_p);
-  const float c2 = p.scale * kLog2e;
-  uint32_t mb0 = s_mbits[half * 2], mb1 = s_mbits[half * 2 + 1];
-  bool any_masked = (mb0 | mb1) != 0u;   // warp-uniform
-  if (kSeg) {                            // packed bins: the keys of this thread's own sequence only
-    seg_key_bits(p.seg[(size_t)b * 128 + row], half, mb0, mb1);
-    any_masked = __any_sync(0xffffffffu, (mb0 | mb1) != 0u);
-  }
-
   if (tid == 0) {
     mbar_expect_tx(bar_load, 3 * TILE_BYTES);
     tma_load_2d(sQ, &tmap_qkv, bar_load, col_q, row0);
     tma_load_2d(sK, &tmap_qkv, bar_load, col_k, row0);
     tma_load_2d(sV, &tmap_qkv, bar_load, col_v, row0);
-    mbar_wait(bar_load, 0);
-    tc_fence_after();
-    constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, false, false);
-    const uint32_t aq = smem_u32(sQ), ak = smem_u32(sK);
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      umma_bf16(tmem, make_smem_desc(aq + k * 32, 16, 1024), make_smem_desc(ak + k * 32, 16, 1024), idesc_s,
-                k > 0 ? 1u : 0u);
-    umma_commit(bar_s);
   }
-  __syncwarp();
-  mbar_wait(bar_s, 0);
-  tc_fence_after();
+  const DropCtx drop = make_drop_ctx(p.rng, p.rng_site, p.dropout_p);
+  const float c2 = p.scale * kLog2e;
+  const uint32_t mw[4] = {s_mbits[0], s_mbits[1], s_mbits[2], s_mbits[3]};
+  int seg[2] = {0, 0};
+  if (kSeg) {                            // packed bins: the keys of this row's own sequence only
+    seg[0] = p.seg[(size_t)b * 128 + fr.r];
+    seg[1] = p.seg[(size_t)b * 128 + fr.r + 8];
+  }
+  // the dropout decisions do not depend on the scores: drawn while the operands are in flight
+  uint32_t keep[2][16];
+#pragma unroll
+  for (int u = 0; u < 2; ++u)
+    quad_keep16(drop, ((unsigned long long)(b * p.heads + h) * 128 + fr.r + 8 * u) * 128, lane, keep[u]);
 
-  // pass 1: maximum of this thread's 64 scores, then across the two halves of the row
-  float m_loc = -INFINITY;
-#pragma unroll 1
-  for (int c = 0; c < 4; ++c) {
-    const uint32_t mbits = (c < 2 ? mb0 : mb1) >> ((c & 1) * 16);
-    uint32_t v[16];
-    tmem_ld16(tmem + lane_base + half * 64 + c * 16, v);
-    tmem_ld_wait();
-    if (!any_masked) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) m_loc = fmaxf(m_loc, __uint_as_float(v[i]));
-    } else {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) m_loc = fmaxf(m_loc, ((mbits >> i) & 1u) ? -INFINITY : __uint_as_float(v[i]));
-    }
-  }
-  m_loc = m_loc * c2;                                  // scale after the max (c2 > 0)
-  if (any_masked) m_loc = fmaxf(m_loc, kMaskBias);     // a masked key counts as score*c2 + (-3.4e38) = -3.4e38
-  s_red[half * 128 + row] = m_loc;
-  __syncthreads();
-  const float m_new = fmaxf(s_red[row], s_red[128 + row]);
-  __syncthreads();                                     // s_red is reused for the row sums below
+  mbar_wait(bar_load, 0);
+  float s[64];
+  wgmma_fence();
+  mma_nt_128(s, sQ, sK, wg);
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_regs(s);
 
-  // pass 2: probabilities -> (dropout) -> bf16 P in the Q / K tiles (both dead: S has completed)
-  float l_loc = 0.f;
-  uint8_t* sP = half ? sK : sQ;
-  const int q_row = row;
-  unsigned long long kept = 0ull;   // keep decisions of this thread's 64 key columns
-#pragma unroll 1
-  for (int c = 0; c < 4; ++c) {
-    const uint32_t mbits = (c < 2 ? mb0 : mb1) >> ((c & 1) * 16);
-    uint32_t v[16];
-    tmem_ld16(tmem + lane_base + half * 64 + c * 16, v);
-    tmem_ld_wait();
-    float pr[16];
+  float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      float x = fmaf(__uint_as_float(v[i]), c2, -m_new);
-      if (any_masked && ((mbits >> i) & 1u)) x = kMaskBias - m_new;
-      pr[i] = ex2_approx(x);
-      l_loc += pr[i];
+  for (int i = 0; i < 64; ++i)
+    if (!key_masked<kSeg>(mw, seg[Frag::hi(i)], fr.col(i))) mx[Frag::hi(i)] = fmaxf(mx[Frag::hi(i)], s[i]);
+  float m_new[2];
+#pragma unroll
+  for (int u = 0; u < 2; ++u) m_new[u] = fmaxf(quad_max(mx[u]) * c2, kMaskBias);   // see attention_fwd_kernel
+  __syncthreads();   // both warpgroups' products have read Q and K: P may overwrite them
+
+  float l_loc[2] = {0.f, 0.f};
+#pragma unroll
+  for (int i = 0; i < 64; i += 2) {
+    const int u = Frag::hi(i), c = fr.col(i);
+    float q2[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float x = fmaf(s[i + e], c2, -m_new[u]);
+      if (key_masked<kSeg>(mw, seg[u], c + e)) x = kMaskBias - m_new[u];
+      const float pr = ex2_approx(x);
+      l_loc[u] += pr;
+      q2[e] = ((keep[u][c >> 3] >> ((c + e) & 7)) & 1u) ? pr * drop.scale : 0.f;
     }
-#pragma unroll
-    for (int g = 0; g < 2; ++g) {
-      const unsigned long long idx =
-          (((unsigned long long)(b * p.heads + h) * 128 + q_row) * 128) + half * 64 + c * 16 + g * 8;
-      const uint32_t keep = dropout_keep8(drop, idx);
-      kept |= (unsigned long long)(keep & 0xffu) << (c * 16 + g * 8);
-      float q8[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) q8[i] = ((keep >> i) & 1u) ? pr[g * 8 + i] * drop.scale : 0.f;
-      uint4 o;
-      o.x = pack_bf16(q8[0], q8[1]); o.y = pack_bf16(q8[2], q8[3]);
-      o.z = pack_bf16(q8[4], q8[5]); o.w = pack_bf16(q8[6], q8[7]);
-      st_tile_chunk(sP, row, c * 2 + g, o);
-    }
+    st_pair(sQ, sK, fr.r + 8 * u, c, q2[0], q2[1]);
   }
-  if (p.keep_bits != nullptr)
-    p.keep_bits[(((size_t)b * p.heads + h) * 128 + q_row) * 2 + half] = kept;
-  s_red[half * 128 + row] = l_loc;
-  fence_proxy_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  if (tid == 0) {
-    tc_fence_after();
-    constexpr uint32_t idesc_o = make_idesc_bf16(128, 64, false, true);
-    const uint32_t ap0 = smem_u32(sQ), ap1 = smem_u32(sK), av = smem_u32(sV);
-    // O[q, d] = sum_key P[q, key] V[key, d]; O reuses S's first 64 TMEM columns (every thread has drained S)
+  if (p.keep_bits != nullptr && fr.t == 0) {
 #pragma unroll
-    for (int k = 0; k < 8; ++k)
-      umma_bf16(tmem, make_smem_desc((k < 4 ? ap0 : ap1) + (k & 3) * 32, 16, 1024),
-                make_smem_desc(av + k * 2048, 16, 1024), idesc_o, k > 0 ? 1u : 0u);
-    umma_commit(bar_o);
-  }
-  __syncwarp();
-  const float l_tot = s_red[row] + s_red[128 + row];
-  const float inv_l = 1.0f / l_tot;
-  if (p.lse != nullptr && half == 0)
-    p.lse[((size_t)b * p.heads + h) * 128 + q_row] = (m_new + log2f(l_tot)) * kLn2;
-  mbar_wait(bar_o, 0);
-  tc_fence_after();
-  {
-    uint32_t v[32];
-    tmem_ld32(tmem + lane_base + half * 32, v);
-    tmem_ld_wait();
-    // the context tile leaves through V's tile (read for the last time by the product above) as one TMA store
+    for (int u = 0; u < 2; ++u) {
+      unsigned long long w0 = 0ull, w1 = 0ull;
 #pragma unroll
-    for (int i = 0; i < 32; i += 8) {
-      uint4 o;
-      o.x = pack_bf16(__uint_as_float(v[i]) * inv_l, __uint_as_float(v[i + 1]) * inv_l);
-      o.y = pack_bf16(__uint_as_float(v[i + 2]) * inv_l, __uint_as_float(v[i + 3]) * inv_l);
-      o.z = pack_bf16(__uint_as_float(v[i + 4]) * inv_l, __uint_as_float(v[i + 5]) * inv_l);
-      o.w = pack_bf16(__uint_as_float(v[i + 6]) * inv_l, __uint_as_float(v[i + 7]) * inv_l);
-      st_tile_chunk(sV, row, half * 4 + (i >> 3), o);
+      for (int j = 0; j < 8; ++j) {
+        w0 |= (unsigned long long)(keep[u][j] & 0xffu) << (8 * j);
+        w1 |= (unsigned long long)(keep[u][j + 8] & 0xffu) << (8 * j);
+      }
+      unsigned long long* kb = p.keep_bits + (((size_t)b * p.heads + h) * 128 + fr.r + 8 * u) * 2;
+      kb[0] = w0;
+      kb[1] = w1;
     }
   }
   fence_proxy_async_smem();
-  tc_fence_before();
+  __syncthreads();
+  float o[32];
+  wgmma_fence();
+  mma_pv(o, sQ, sK, sV, wg);
+  wgmma_commit();
+  float inv_l[2];
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    const float l_tot = quad_sum(l_loc[u]);
+    inv_l[u] = 1.0f / l_tot;
+    if (p.lse != nullptr && fr.t == 0)
+      p.lse[((size_t)b * p.heads + h) * 128 + fr.r + 8 * u] = (m_new[u] + log2f(l_tot)) * kLn2;
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(o);
+  __syncthreads();   // both warpgroups' products have read V: the context tile may overwrite it
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int u = Frag::hi(i);
+    st_pair(sV, sV, fr.r + 8 * u, fr.col(i), o[i] * inv_l[u], o[i + 1] * inv_l[u]);
+  }
+  fence_proxy_async_smem();
   __syncthreads();
   if (tid == 0) {
     tma_store_2d(&tmap_ctx, sV, h * 64, row0);
     tma_store_commit_and_wait();
-  }
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 128);
   }
 }
 
@@ -481,30 +397,18 @@ __global__ void __launch_bounds__(ATT_THREADS, 4) attention_fwd128_kernel(const 
 // backward: grid (seq/128 kv blocks, heads, batch); loops over query blocks
 // ------------------------------------------------------------------------------------------------------------
 //
-// kOneQ (seq == 128, the benchmark shape): the CTA is trimmed so TWO fit on an SM and hide each other's
-// TMA -> MMA -> TMEM-drain latencies (one CTA alone leaves the SM idle most of its ~13 us dependency chain):
-//   * shared memory 7 tiles (112 KB) instead of 8: V is dead once dP = dO V^T has been issued and completed, so the
-//     first 64-key half of P lives in V's tile;
-//   * TMEM 256 columns instead of 512: with a single query block nothing accumulates across iterations, so dQ / dV
-//     / dK overwrite the S / dP columns, which every thread has drained before the second MMA batch is issued.
-// Memory paths (ncu on the first version: IPC 0.26, stalls = long scoreboard + LSU/MIO throttle from per-thread row
-// accesses): every global access of the hot loop is a TMA tile copy.  O comes in with Q and dO (into P's second
-// half, free until the dS pass) so delta = rowsum(dO * O) reads two swizzled smem rows; dQ / dK / dV leave through
-// the operand tiles that the last MMAs have released, as TMA tile stores; the key mask is a 64-bit register pair per
-// thread (bit tests, and a warp-uniform fast path when the block has no masked key) instead of a shared-memory
-// float per element.
+// kOneQ (seq == 128, the benchmark shape): shared memory 7 tiles instead of 8 -- V is dead once dP = dO V^T has
+// completed, so the first 64-key half of P lives in V's tile.  O comes in with Q and dO (into P's second half, free
+// until the dS pass) so delta = rowsum(dO * O) reads two swizzled smem rows while S and dP are being multiplied; dQ /
+// dK / dV leave through the operand tiles that the last products have released, as TMA tile stores.
 template <bool kOneQ, bool kSeg = false>   // kSeg (with kOneQ): packed bins, per-row segment mask (p.seg)
-__global__ void __launch_bounds__(ATT_THREADS, kOneQ ? 2 : 1)
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
                      const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_dqkv,
                      const AttnParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // kOneQ has no room for alignment slack: the dynamic window of a kernel without static shared memory starts
-  // 1024-aligned (checked below, loudly)
-  uint8_t* smem = kOneQ ? smem_raw
-                        : smem_align_1024(smem_raw);
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_align_1024(smem_raw);
   constexpr int kTiles = kOneQ ? 7 : 8;
-  constexpr uint32_t kTmemCols = kOneQ ? 256 : 512;
   uint8_t* sK = smem;
   uint8_t* sV = smem + TILE_BYTES;
   uint8_t* sQ = smem + 2 * TILE_BYTES;
@@ -515,33 +419,23 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kTiles * TILE_BYTES);
   uint64_t* bar_kv = &bars[0];
   uint64_t* bar_q = &bars[1];
-  uint64_t* bar_s = &bars[2];
-  uint64_t* bar_mma = &bars[3];
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(&bars[4]);
   uint32_t* s_mbits = reinterpret_cast<uint32_t*>(smem + kTiles * TILE_BYTES + 48);  // [4]: masked-key bits of this block
+  float* s_delta = reinterpret_cast<float*>(smem + kTiles * TILE_BYTES + 64);         // [128]
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int row = (warp & 3) * 32 + lane;   // TMEM lane: query row inside the S/dP/dQ tiles, key row for dK/dV
-  const int half = warp >> 2;               // key-column half in the dS pass, output-dim half in the drains
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const Frag fr(warp, lane);
   const int jb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int nq = p.seq / 128;
 
   if (tid == 0) {
-    if (kOneQ && (smem_u32(smem_raw) & 1023u) != 0u) {
-      printf("attention_bwd: dynamic shared memory is not 1024-byte aligned\n");
-      __trap();
-    }
     tma_prefetch_desc(&tmap_qkv);
     tma_prefetch_desc(&tmap_do);
     tma_prefetch_desc(&tmap_o);
     tma_prefetch_desc(&tmap_dqkv);
     mbar_init(bar_kv, 1);
     mbar_init(bar_q, 1);
-    mbar_init(bar_s, 1);
-    mbar_init(bar_mma, 1);
     fence_mbar_init();
   }
-  if (warp == 0) tmem_alloc(tmem_holder, kTmemCols);
   pdl_wait();               // PDL: setup above overlapped the predecessor's tail; global reads start below
   pdl_launch_dependents();
   if (tid < 128) {
@@ -549,222 +443,165 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
     const unsigned bits = __ballot_sync(0xffffffffu, masked);
     if (lane == 0) s_mbits[warp] = bits;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_holder;
-  const uint32_t tm_s = tmem, tm_dp = tmem + 128;
-  const uint32_t tm_dq = tmem + (kOneQ ? 0 : 384), tm_dv = tmem + (kOneQ ? 64 : 256), tm_dk = tmem + (kOneQ ? 128 : 320);
-  const uint32_t lane_base = ((uint32_t)((warp & 3) * 32)) << 16;
-  uint32_t mb0 = s_mbits[half * 2], mb1 = s_mbits[half * 2 + 1];   // this thread's 64 key columns
-  bool any_masked = (mb0 | mb1) != 0u;                              // warp-uniform
-  if (kOneQ && kSeg) {               // packed bins (seq == 128): `row` is this thread's query row of the only block
-    seg_key_bits(p.seg[(size_t)b * 128 + row], half, mb0, mb1);
-    any_masked = __any_sync(0xffffffffu, (mb0 | mb1) != 0u);
+  const uint32_t mw[4] = {s_mbits[0], s_mbits[1], s_mbits[2], s_mbits[3]};
+  int seg[2] = {0, 0};
+  if (kOneQ && kSeg) {               // packed bins (seq == 128): fr.r is a query row of the only block
+    seg[0] = p.seg[(size_t)b * 128 + fr.r];
+    seg[1] = p.seg[(size_t)b * 128 + fr.r + 8];
   }
 
   const int row0 = b * p.seq;
   const int col_q = h * 64, col_k = p.hidden + h * 64, col_v = 2 * p.hidden + h * 64;
   const DropCtx drop = make_drop_ctx(p.rng, p.rng_site, p.dropout_p);
   const float c2 = p.scale * kLog2e;
+  const size_t bh = (size_t)b * p.heads + h;
 
   if (tid == 0) {
     mbar_expect_tx(bar_kv, 2 * TILE_BYTES);
     tma_load_2d(sK, &tmap_qkv, bar_kv, col_k, row0 + jb * 128);
     tma_load_2d(sV, &tmap_qkv, bar_kv, col_v, row0 + jb * 128);
   }
-
-  constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, false, false);   // S, dP
-  constexpr uint32_t idesc_t = make_idesc_bf16(128, 64, true, true);      // dV, dK (A = P^T / dS^T)
-  constexpr uint32_t idesc_q = make_idesc_bf16(128, 64, false, true);     // dQ
-  uint32_t ph_q = 0, ph_s = 0, ph_mma = 0;
+  float dv[32], dk[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+  uint32_t ph_q = 0;
 
   for (int i = 0; i < nq; ++i) {
-    const int q_row = i * 128 + row;  // this thread's query row in the sequence
     if (tid == 0) {
       mbar_expect_tx(bar_q, 3 * TILE_BYTES);
       tma_load_2d(sQ, &tmap_qkv, bar_q, col_q, row0 + i * 128);
       tma_load_2d(sdO, &tmap_do, bar_q, h * 64, row0 + i * 128);
       tma_load_2d(sP1, &tmap_o, bar_q, h * 64, row0 + i * 128);   // O, consumed by the delta pass below
-      if (i == 0) mbar_wait(bar_kv, 0);
-      mbar_wait(bar_q, ph_q);
-      tc_fence_after();
-      const uint32_t aq = smem_u32(sQ), ak = smem_u32(sK), ado = smem_u32(sdO), av = smem_u32(sV);
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        umma_bf16(tm_s, make_smem_desc(aq + k * 32, 16, 1024), make_smem_desc(ak + k * 32, 16, 1024), idesc_s,
-                  k > 0 ? 1u : 0u);
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        umma_bf16(tm_dp, make_smem_desc(ado + k * 32, 16, 1024), make_smem_desc(av + k * 32, 16, 1024), idesc_s,
-                  k > 0 ? 1u : 0u);
-      umma_commit(bar_s);
     }
-    __syncwarp();
-    // delta = rowsum(dO * O) from the two smem tiles while the MMAs run (both threads of a row compute the same value)
+    if (i == 0) mbar_wait(bar_kv, 0);
     mbar_wait(bar_q, ph_q);
     ph_q ^= 1;
-    float delta = 0.f;
+    float s[64], dp[64];
+    wgmma_fence();
+    mma_nt_128(s, sQ, sK, wg);
+    mma_nt_128(dp, sdO, sV, wg);
+    wgmma_commit();
+    // delta = rowsum(dO * O) from the two smem tiles while the products run
+    if (tid < 128) {
+      float delta = 0.f;
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      const int off = row * 128 + ((c ^ (row & 7)) << 4);
-      const uint4 a = *reinterpret_cast<const uint4*>(sP1 + off);
-      const uint4 g = *reinterpret_cast<const uint4*>(sdO + off);
-      delta += bf16_lo(a.x) * bf16_lo(g.x) + bf16_hi(a.x) * bf16_hi(g.x) + bf16_lo(a.y) * bf16_lo(g.y) +
-               bf16_hi(a.y) * bf16_hi(g.y) + bf16_lo(a.z) * bf16_lo(g.z) + bf16_hi(a.z) * bf16_hi(g.z) +
-               bf16_lo(a.w) * bf16_lo(g.w) + bf16_hi(a.w) * bf16_hi(g.w);
+      for (int c = 0; c < 8; ++c) {
+        const int off = tid * 128 + ((c ^ (tid & 7)) << 4);
+        const uint4 a = *reinterpret_cast<const uint4*>(sP1 + off);
+        const uint4 g = *reinterpret_cast<const uint4*>(sdO + off);
+        delta += bf16_lo(a.x) * bf16_lo(g.x) + bf16_hi(a.x) * bf16_hi(g.x) + bf16_lo(a.y) * bf16_lo(g.y) +
+                 bf16_hi(a.y) * bf16_hi(g.y) + bf16_lo(a.z) * bf16_lo(g.z) + bf16_hi(a.z) * bf16_hi(g.z) +
+                 bf16_lo(a.w) * bf16_lo(g.w) + bf16_hi(a.w) * bf16_hi(g.w);
+      }
+      s_delta[tid] = delta;
     }
-    const float lse2 = p.lse[((size_t)b * p.heads + h) * p.seq + q_row] * kLog2e;
+    float lse2[2], delta[2];
+    unsigned long long kept[2][2];
     const bool have_bits = kOneQ && p.keep_bits != nullptr;
-    unsigned long long kept = ~0ull;
-    if (have_bits) kept = p.keep_bits[(((size_t)b * p.heads + h) * 128 + q_row) * 2 + half];
-    __syncthreads();   // every thread has read its O row: P may overwrite the tile in the pass below
-
-    mbar_wait(bar_s, ph_s);
-    ph_s ^= 1;
-    tc_fence_after();
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      const int cb = half * 64 + c * 32;   // first key column of this chunk inside the 128-key block
-      const uint32_t mbits = c == 0 ? mb0 : mb1;
-      uint32_t vs[32], vd[32];
-      tmem_ld32(tm_s + lane_base + cb, vs);
-      tmem_ld32(tm_dp + lane_base + cb, vd);
-      tmem_ld_wait();
+    uint32_t keep[2][16];
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const unsigned long long idx =
-            (((unsigned long long)(b * p.heads + h) * p.seq + q_row) * p.seq) + jb * 128 + cb + g * 8;
-        const uint32_t keep = have_bits ? (uint32_t)(kept >> (c * 32 + g * 8)) & 0xffu : dropout_keep8(drop, idx);
-        float pd[8], ds[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int cc = g * 8 + e;
-          float x = fmaf(__uint_as_float(vs[cc]), c2, -lse2);
-          if (any_masked && ((mbits >> cc) & 1u)) x = kMaskBias - lse2;   // what score*c2 + (-3.4e38) rounds to
-          const float pr = ex2_approx(x);
-          const bool kp = (keep >> e) & 1u;
-          pd[e] = kp ? pr * drop.scale : 0.f;
-          const float dp = kp ? __uint_as_float(vd[cc]) * drop.scale : 0.f;
-          ds[e] = pr * (dp - delta) * p.scale;
-        }
-        uint4 o;
-        o.x = pack_bf16(pd[0], pd[1]); o.y = pack_bf16(pd[2], pd[3]);
-        o.z = pack_bf16(pd[4], pd[5]); o.w = pack_bf16(pd[6], pd[7]);
-        st_tile_chunk(half ? sP1 : sP0, row, c * 4 + g, o);
-        o.x = pack_bf16(ds[0], ds[1]); o.y = pack_bf16(ds[2], ds[3]);
-        o.z = pack_bf16(ds[4], ds[5]); o.w = pack_bf16(ds[6], ds[7]);
-        st_tile_chunk(sdS, row, half * 8 + c * 4 + g, o);
+    for (int u = 0; u < 2; ++u) {
+      const int q_row = i * 128 + fr.r + 8 * u;   // this thread's query rows in the sequence
+      lse2[u] = p.lse[bh * p.seq + q_row] * kLog2e;
+      if (have_bits) {
+        kept[u][0] = p.keep_bits[(bh * 128 + q_row) * 2];
+        kept[u][1] = p.keep_bits[(bh * 128 + q_row) * 2 + 1];
+      } else {
+        quad_keep16(drop, ((bh * p.seq + q_row) * p.seq) + jb * 128, lane, keep[u]);
       }
     }
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    wgmma_fence_regs(dp);
+    __syncthreads();   // delta is in; O has been read and every product has read V: P may overwrite both
+#pragma unroll
+    for (int u = 0; u < 2; ++u) delta[u] = s_delta[fr.r + 8 * u];
+#pragma unroll
+    for (int ii = 0; ii < 64; ii += 2) {
+      const int u = Frag::hi(ii), c = fr.col(ii);
+      float pd[2], ds[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int cc = c + e;
+        float x = fmaf(s[ii + e], c2, -lse2[u]);
+        if (key_masked<kOneQ && kSeg>(mw, seg[u], cc)) x = kMaskBias - lse2[u];   // what score*c2 + (-3.4e38) rounds to
+        const float pr = ex2_approx(x);
+        const bool kp = have_bits ? ((kept[u][cc >> 6] >> (cc & 63)) & 1ull) : ((keep[u][cc >> 3] >> (cc & 7)) & 1u);
+        pd[e] = kp ? pr * drop.scale : 0.f;
+        const float dpv = kp ? dp[ii + e] * drop.scale : 0.f;
+        ds[e] = pr * (dpv - delta[u]) * p.scale;
+      }
+      st_pair(sP0, sP1, fr.r + 8 * u, c, pd[0], pd[1]);
+      st_pair(sdS, sdS + TILE_BYTES, fr.r + 8 * u, c, ds[0], ds[1]);
+    }
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    if (tid == 0) {
-      tc_fence_after();
-      const uint32_t ap = smem_u32(sP0), ads = smem_u32(sdS), ado = smem_u32(sdO), aq = smem_u32(sQ),
-                     ak = smem_u32(sK);
-      const uint32_t p_pitch = smem_u32(sP1) - ap;   // byte distance between the two 64-key slabs of P
-      // dV[key, d] += sum_q P[q, key] dO[q, d]      (A = P as MN-major: rows = q = K index)
+    float dq[32];
+    wgmma_fence();
+    {
+      // dV[key, d] += sum_q P[q, key] dO[q, d]      (A = P as MN-major: rows = q = K index; this warpgroup's 64 keys
+      // are one sub-tile)
+      const uint32_t ap = smem_u32(wg ? sP1 : sP0), ado = smem_u32(sdO);
 #pragma unroll
       for (int k = 0; k < 8; ++k)
-        umma_bf16(tm_dv, make_smem_desc(ap + k * 2048, p_pitch, 1024), make_smem_desc(ado + k * 2048, 16, 1024),
-                  idesc_t, (i > 0 || k > 0) ? 1u : 0u);
+        wgmma_bf16<64, 1, 1>(dv, make_smem_desc(ap + k * 2048, 8192, 1024), make_smem_desc(ado + k * 2048, 8192, 1024),
+                             (i > 0 || k > 0) ? 1u : 0u);
       // dK[key, d] += sum_q dS[q, key] Q[q, d]
+      const uint32_t ads = smem_u32(sdS), aq = smem_u32(sQ), ak = smem_u32(sK);
 #pragma unroll
       for (int k = 0; k < 8; ++k)
-        umma_bf16(tm_dk, make_smem_desc(ads + k * 2048, TILE_BYTES, 1024), make_smem_desc(aq + k * 2048, 16, 1024),
-                  idesc_t, (i > 0 || k > 0) ? 1u : 0u);
+        wgmma_bf16<64, 1, 1>(dk, make_smem_desc(ads + wg * TILE_BYTES + k * 2048, 8192, 1024),
+                             make_smem_desc(aq + k * 2048, 8192, 1024), (i > 0 || k > 0) ? 1u : 0u);
       // dQ[q, d] = sum_key dS[q, key] K[key, d]     (A = dS as K-major)
 #pragma unroll
       for (int k = 0; k < 8; ++k)
-        umma_bf16(tm_dq, make_smem_desc(ads + (k >> 2) * TILE_BYTES + (k & 3) * 32, 16, 1024),
-                  make_smem_desc(ak + k * 2048, 16, 1024), idesc_q, k > 0 ? 1u : 0u);
-      umma_commit(bar_mma);
+        wgmma_bf16<64, 0, 1>(dq, make_smem_desc(ads + (k >> 2) * TILE_BYTES + wg * 8192 + (k & 3) * 32, 16, 1024),
+                             make_smem_desc(ak + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
     }
-    __syncwarp();
-    mbar_wait(bar_mma, ph_mma);
-    ph_mma ^= 1;
-    tc_fence_after();
-    {
-      uint32_t v[32];
-      tmem_ld32(tm_dq + lane_base + half * 32, v);
-      tmem_ld_wait();
-      if (p.dq_accum == nullptr) {
-        // seq == 128: dQ leaves through Q's tile (its last reader, the dK product, has completed) as a TMA store
-        float f[32];   // bf16-rounded values (what the dgrad/wgrad GEMMs will read), for the bias-gradient sums
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(dv);
+    wgmma_fence_regs(dk);
+    wgmma_fence_regs(dq);
+    if (p.dq_accum == nullptr) {
+      // seq == 128: dQ leaves through Q's tile (once both warpgroups' dK products have read it) as a TMA store
+      __syncthreads();
 #pragma unroll
-        for (int e = 0; e < 32; ++e) f[e] = __uint_as_float(v[e]);
-#pragma unroll
-        for (int e = 0; e < 32; e += 8) {
-          uint4 o;
-          o.x = pack_bf16_round(f[e], f[e + 1]);
-          o.y = pack_bf16_round(f[e + 2], f[e + 3]);
-          o.z = pack_bf16_round(f[e + 4], f[e + 5]);
-          o.w = pack_bf16_round(f[e + 6], f[e + 7]);
-          st_tile_chunk(sQ, row, half * 4 + (e >> 3), o);
-        }
-        if (p.dbias != nullptr) {
-          const float t = warp_colsum32(f, lane);
-          atomicAdd(p.dbias + col_q + half * 32 + lane, t);
-        }
-      } else {
-        float* dst = p.dq_accum + (size_t)(row0 + q_row) * p.hidden + h * 64 + half * 32;
-#pragma unroll
-        for (int e = 0; e < 32; ++e) atomicAdd(dst + e, __uint_as_float(v[e]));
+      for (int e = 0; e < 32; e += 2) {
+        (void)pack_bf16_round(dq[e], dq[e + 1]);   // bf16-rounded values (what the GEMMs will read) for the sums
+        st_pair(sQ, sQ, fr.r + 8 * Frag::hi(e), fr.col(e), dq[e], dq[e + 1]);
       }
+      if (p.dbias != nullptr) frag_colsum64(dq, lane, p.dbias + col_q);
+    } else {
+#pragma unroll
+      for (int e = 0; e < 32; ++e)
+        atomicAdd(p.dq_accum + (size_t)(row0 + i * 128 + fr.r + 8 * Frag::hi(e)) * p.hidden + h * 64 + fr.col(e), dq[e]);
     }
-    if (p.dq_accum != nullptr) {
-      tc_fence_before();
-      __syncthreads();   // TMEM / smem reuse by the next query block
-    }
+    if (!kOneQ) __syncthreads();   // the next query block reuses the tiles
   }
 
-  // dK, dV for this thread's key row (32 of the 64 head dims each) -> K's and V's tiles -> TMA stores
-  {
-    tc_fence_after();
-    uint32_t v[32], w[32];
-    tmem_ld32(tm_dk + lane_base + half * 32, v);
-    tmem_ld32(tm_dv + lane_base + half * 32, w);
-    tmem_ld_wait();
-    float f[32], g[32];   // bf16-rounded dK / dV values for the bias-gradient sums
+  // dK, dV of this block's keys -> K's and V's tiles -> TMA stores
+  __syncthreads();   // every product has read K and V (kOneQ: P in V's tile)
 #pragma unroll
-    for (int e = 0; e < 32; ++e) {
-      f[e] = __uint_as_float(v[e]);
-      g[e] = __uint_as_float(w[e]);
-    }
-#pragma unroll
-    for (int e = 0; e < 32; e += 8) {
-      uint4 o;
-      o.x = pack_bf16_round(f[e], f[e + 1]);
-      o.y = pack_bf16_round(f[e + 2], f[e + 3]);
-      o.z = pack_bf16_round(f[e + 4], f[e + 5]);
-      o.w = pack_bf16_round(f[e + 6], f[e + 7]);
-      st_tile_chunk(sK, row, half * 4 + (e >> 3), o);
-      o.x = pack_bf16_round(g[e], g[e + 1]);
-      o.y = pack_bf16_round(g[e + 2], g[e + 3]);
-      o.z = pack_bf16_round(g[e + 4], g[e + 5]);
-      o.w = pack_bf16_round(g[e + 6], g[e + 7]);
-      st_tile_chunk(sV, row, half * 4 + (e >> 3), o);
-    }
-    if (p.dbias != nullptr) {
-      const float tk = warp_colsum32(f, lane), tv = warp_colsum32(g, lane);
-      atomicAdd(p.dbias + col_k + half * 32 + lane, tk);
-      atomicAdd(p.dbias + col_v + half * 32 + lane, tv);
-    }
+  for (int e = 0; e < 32; e += 2) {
+    const int r = fr.r + 8 * Frag::hi(e), c = fr.col(e);
+    (void)pack_bf16_round(dk[e], dk[e + 1]);
+    (void)pack_bf16_round(dv[e], dv[e + 1]);
+    st_pair(sK, sK, r, c, dk[e], dk[e + 1]);
+    st_pair(sV, sV, r, c, dv[e], dv[e + 1]);
+  }
+  if (p.dbias != nullptr) {
+    frag_colsum64(dk, lane, p.dbias + col_k);
+    frag_colsum64(dv, lane, p.dbias + col_v);
   }
   fence_proxy_async_smem();   // generic-proxy tile writes above -> visible to the TMA engine
-  tc_fence_before();
   __syncthreads();
   if (tid == 0) {
     if (p.dq_accum == nullptr) tma_store_2d(&tmap_dqkv, sQ, col_q, row0 + (nq - 1) * 128);
     tma_store_2d(&tmap_dqkv, sK, col_k, row0 + jb * 128);
     tma_store_2d(&tmap_dqkv, sV, col_v, row0 + jb * 128);
     tma_store_commit_and_wait();
-  }
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, kTmemCols);
   }
 }
 
@@ -784,9 +621,9 @@ __global__ void dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* 
   *reinterpret_cast<uint2*>(d_qkv + t * 3 * hidden + c) = o;
 }
 
-constexpr int kFwdSmem = 5 * TILE_BYTES + 128 + 256 * 4 + 1024;
-constexpr int kFwd128Smem = 3 * TILE_BYTES + 64 + 256 * 4 + 1024;
-constexpr int kBwdSmem = 8 * TILE_BYTES + 64 + 1024;
+constexpr int kFwdSmem = 5 * TILE_BYTES + 128 + 1024;
+constexpr int kFwd128Smem = 3 * TILE_BYTES + 64 + 1024;
+constexpr int kBwdSmem = 8 * TILE_BYTES + 64 + 512 + 1024;
 
 // B2_ATTN_FWD128=0 keeps seq == 128 on the general forward kernel (A/B measurements)
 static bool fwd128_enabled() {
@@ -797,7 +634,7 @@ static bool fwd128_enabled() {
   }
   return v == 1;
 }
-constexpr int kBwdSmemOneQ = 7 * TILE_BYTES + 64;   // 114752 B: two CTAs per SM (2 x (this + 1 KB) <= 228 KB)
+constexpr int kBwdSmemOneQ = 7 * TILE_BYTES + 64 + 512 + 1024;
 
 static int32_t check_attn_shapes(const char* who, int64_t batch, int64_t seq, int64_t heads, int64_t head_dim) {
   B2_REQUIRE(batch > 0 && seq > 0 && heads > 0, "%s: empty problem (batch=%lld seq=%lld heads=%lld)", who,

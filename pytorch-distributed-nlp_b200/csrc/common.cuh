@@ -1,16 +1,16 @@
-// Shared device/host helpers for the sm_100a kernels of the DDP BERT fine-tuning step.
-// Everything here is written for one target only: B200, compute_100a.
-//   - raw PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld)
-//   - UMMA shared-memory + instruction descriptors (bit layout documented inline)
+// Shared device/host helpers for the sm_90a kernels of the DDP BERT fine-tuning step.
+// Everything here is written for one target only: H100, compute_90a.
+//   - raw PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), clusters / distributed shared memory
+//   - wgmma shared-memory descriptors (bit layout documented inline; the MMA wrappers are in wgmma.cuh)
 //   - Philox4x32-10 counter RNG for the 38 dropout sites (regenerated, never stored)
 //   - bf16 pack/unpack and warp reductions
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
-#include <cuda/ptx>
 #include <stdint.h>
 #include <cstdio>
+#include "wgmma.cuh"
 
 namespace b2 {
 
@@ -68,7 +68,7 @@ inline void launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-// First 1024-byte boundary inside a dynamic shared-memory window (TMA / UMMA 128-byte-swizzle tiles).  Written as
+// First 1024-byte boundary inside a dynamic shared-memory window (TMA / wgmma 128-byte-swizzle tiles).  Written as
 // `base + offset` -- NOT as a round trip through uintptr_t -- so that every pointer derived from the result is still
 // known to the compiler to be SHARED: the cast form degraded each staging-tile access of the epilogues to a generic
 // LD.E / ST.E (address-space check, L1 tag stage, and a memory barrier that must wait for them) instead of LDS / STS.
@@ -226,18 +226,16 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Bounded wait: a protocol bug must surface as a trapped kernel (-> CUDA error -> RuntimeError on the
-// host), never as a hung GPU.  2^26 polls of a suspending try_wait is seconds, far beyond any tile.
+// host), never as a hung GPU.  2^24 polls of a suspending try_wait is seconds, far beyond any tile.  (No printf here:
+// a function call inside a wgmma mainloop makes ptxas serialise the asynchronous MMAs.)
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 24)) {
-      printf("b2: mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
+    if (++spins > (1u << 24)) __trap();
   }
 }
 
-// generic-proxy writes to smem -> visible to the async proxy (UMMA / TMA reads)
+// generic-proxy writes to smem -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -273,54 +271,36 @@ __device__ __forceinline__ void tma_store_commit_and_wait() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// clusters and distributed shared memory
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_holder, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+__device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+  return r;
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// 8-byte store into the shared memory of a CTA of the cluster (address from mapa_u32)
+__device__ __forceinline__ void st_cluster_f32x2(uint32_t cluster_addr, float a, float b) {
+  asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(cluster_addr), "f"(a), "f"(b) : "memory");
 }
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]; bf16 inputs, fp32 accumulate; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// barrier over `count` threads (whole warps) of the CTA, ids 1..15 (0 is __syncthreads)
+__device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
-// All previously issued MMAs of this thread arrive on `bar` when complete (implies fence::before).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread i of the warp gets lane (base_lane + i), v[j] = column j.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  cuda::ptx::tcgen05_ld_32x32b(v, taddr);
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  cuda::ptx::tcgen05_ld_32x32b(v, taddr);
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// ---- descriptors --------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64 bit), SWIZZLE_128B flavour, version 1 (Blackwell):
+// ---- wgmma shared-memory matrix descriptor (64 bit), SWIZZLE_128B ---------------------------------
 //   [ 0,14) start address >> 4          [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4 [46,48) version = 1      [61,64) layout type (2 = SWIZZLE_128B)
+//   [32,46) stride-dim byte offset >> 4 [49,52) base offset (0: swizzle atoms 1024-byte aligned)
+//   [62,64) layout type (1 = SWIZZLE_128B)
 // K-major operand tile  (rows = M/N index, 64 bf16 = 128 B per row, rows 128 B apart, TMA-swizzled):
-//   SBO = 1024 B (8 rows), LBO unused (1).  Advancing K by 16 elements = +32 B on the start address.
+//   SBO = 1024 B (8 rows), LBO unused.  Advancing K by 16 elements = +32 B on the start address.
 // MN-major operand tile (rows = K index, 64 bf16 of the M/N index per 128 B row; further 64-wide
 //   M/N chunks are separate [BK x 128 B] slabs): SBO = 1024 B (8 k-rows), LBO = slab pitch.
 //   Advancing K by 16 = +16 rows = +2048 B.
@@ -329,16 +309,8 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
   d |= (uint64_t)((saddr >> 4) & 0x3fffu);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// Instruction descriptor (32 bit) for kind::f16, bf16 x bf16 -> fp32:
-//   [4,6) D format (1 = f32)  [7,10) A format (1 = bf16)  [10,13) B format (1 = bf16)
-//   [15] A major (1 = MN)     [16] B major (1 = MN)       [17,23) N >> 3         [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 // Programmatic dependent launch (PDL).  Every kernel of the library starts with pdl_wait(): it returns once all

@@ -152,7 +152,7 @@ __global__ void embed_pos_kernel(const __nv_bfloat16* __restrict__ dx, int batch
 // ---- fast word-row path: fp32 accumulation keyed by the OWNER TOKEN of each vocabulary row ---------------------
 // acc[owner[id]][:] += dx[t][:] for every token (vector reductions at L2; a row met once is a single add into
 // zero, i.e. exact), then the owner converts its row to bf16.  Two fully parallel passes instead of one CTA per
-// token scanning all later tokens for duplicates (32 us at 4096 tokens); the summation order of duplicated rows is
+// token scanning all later tokens for duplicates; the summation order of duplicated rows is
 // no longer fixed (fp32 accumulation, rounded once).
 __global__ void embed_word_accum_kernel(const __nv_bfloat16* __restrict__ dx, const int* __restrict__ ids32, int H,
                                         int pad_id, const int* __restrict__ owner, float* __restrict__ acc) {

@@ -1,371 +1,174 @@
-// bf16 GEMM on the 5th-gen tensor cores: D[M,N] = op(A) * op(B) (+ fused epilogue), fp32 accumulate in TMEM.
+// bf16 GEMM on the Hopper tensor cores (wgmma): D[M,N] = op(A) * op(B) (+ fused epilogue), fp32 accumulate.
 //
 // Replaces the cuBLAS `addmm` calls issued by HF BertSelfAttention / BertSelfOutput / BertIntermediate /
 // BertOutput (transformers modeling_bert.py:179-181, :295, :340, :353) and their autograd dgrad / wgrad
 // twins (SURVEY.md §2.2 K2, K7, K8, K9).
 //
-// Three kernels share one epilogue:
-//   gemm2_bf16_kernel  CTA PAIR (cluster of 2, tcgen05 cta_group::2): the pair owns a 256 x BN output tile, each
-//                      CTA stages its own 128 A rows and HALF of the B tile, the leader's single thread issues
-//                      256 x BN x 16 MMAs that read both halves.  Per flop this moves 1/3 fewer bytes out of L2 and
-//                      through shared memory than a 128 x 256 single-CTA tile -- the first profile showed the
-//                      single-CTA kernel pinned at ~10 TB/s of L2->SM traffic (650 TF/s), not at the tensor pipe.
-//   gemm2_grouped_tn_kernel  the same CTA-pair machinery over a table of up to four TN problems: the weight gradients
-//                      of one encoder layer as ONE persistent launch (b2_gemm_bf16_grouped)
-//   gemm_bf16_kernel   single CTA, 128 x BN (BN 128/256): small or oddly shaped problems.
-// Common structure (persistent, warp specialised, one CTA per SM):
-//   warp 0      TMA producer      global -> 128B-swizzled smem ring (full/empty mbarriers)
-//   warp 1      MMA issuer        one lane issues tcgen05.mma, commits to mbarriers
-//   warp 2      TMEM allocator    2 accumulator stages so tile i+1's MMAs overlap tile i's epilogue
-//   warps 4-19  epilogue          tcgen05.ld -> bias / GELU / dropout / residual -> smem staging -> coalesced stores
-//                                 (gemm_epilogue.cuh); 16 warps by default, 8 (warps 4-11) with B2_GEMM_EPI_WARPS=8
-// Operand layouts are expressed only through the TMA box + UMMA descriptor (no transposes in HBM):
+// Two kernels share one mainloop and one epilogue:
+//   gemm_bf16_kernel         one 128 x BN output tile (BN 128 / 256) per CTA, optional split-K over the contraction
+//   gemm_grouped_tn_kernel   a table of up to four TN problems behind one launch: the weight gradients of one encoder
+//                            layer (b2_gemm_bf16_grouped), optionally with the AdamW update fused into the epilogue
+// CTA structure (384 threads, warp specialised):
+//   warpgroup 0 (warps 0-3)    warp 0 lane 0: TMA producer, global -> 128B-swizzled smem ring (full/empty mbarriers)
+//   warpgroups 1, 2 (4-11)     wgmma consumers, rows 0-63 / 64-127 of the tile, fp32 accumulators in registers; once
+//                              the contraction is done the ring is dead, the accumulators go to shared memory (row
+//                              major, over the ring) and the same 8 warps run the epilogue (gemm_epilogue.cuh)
+// Operand layouts are expressed only through the TMA box + wgmma descriptor (no transposes in HBM):
 //   NT  A[M,K] K-major,  B[N,K] K-major   (forward:  y = x W^T)
 //   NN  A[M,K] K-major,  B[K,N] MN-major  (dgrad:    dx = dy W)
 //   TN  A[K,M] MN-major, B[K,N] MN-major  (wgrad:    dW = dy^T x), optional split-K over the token axis
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
-#include "pair.cuh"
 #include "../../include/b2_ddp_bert.h"
 
 namespace b2 {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int UMMA_K = 16;
-// warps 0-3: TMA producer, MMA issuer, TMEM allocator, spare; warps 4.. : EW epilogue warps (8 or 16, see
-// gemm_epilogue.cuh).  16 is the default; B2_GEMM_EPI_WARPS=8 selects the 12-warp variant (A/B measurements).
-constexpr int gemm_threads(int EW) { return (4 + EW) * 32; }
+constexpr int WGMMA_K = 16;
+constexpr int kGemmThreads = (4 + kEpiWarps) * 32;   // producer warpgroup + two consumer warpgroups
 
-// ------------------------------------------------------------------------------------------------------------
-// single-CTA kernel
-// ------------------------------------------------------------------------------------------------------------
-template <int BN, int EW>
+template <int BN>
 struct GemmCfg {
-  static constexpr int kStages = (BN == 256) ? (EW == 16 ? 3 : 4) : 5;
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kAccStride = (BN <= 128) ? 128 : 256;  // TMEM columns between the 2 accumulators
-  static constexpr int kTmemCols = 2 * kAccStride;            // 256 or 512 (power of two)
-  static constexpr int kPipeBytes = kStages * kStageBytes;
-  static constexpr int kSmemBytes = kPipeBytes + EW * kEpiStageBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int kStages = (BN == 256) ? 4 : 6;
+  static constexpr int kPipeBytes = kStages * kStageBytes;             // 192 KB
+  static constexpr int kAccLd = BN + 4;                                 // fp32 row pitch of the accumulator tile
+  static constexpr int kSmemBytes = kPipeBytes + kEpiWarps * kEpiStageBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(BM * kAccLd * 4 <= kPipeBytes, "the accumulator tile lives in the drained operand ring");
 };
 
-template <int BN, bool A_MN, bool B_MN, int EW>
-__global__ void __launch_bounds__(gemm_threads(EW)) __maxnreg__(EW == 8 ? 128 : 96)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const GemmKernelParams p) {
-  using Cfg = GemmCfg<BN, EW>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_align_1024(smem_raw);
-  uint8_t* epi_stage = smem + Cfg::kPipeBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + EW * kEpiStageBytes);
-  uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tmem_full = empty_bar + Cfg::kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full[s], 1);
-      mbar_init(&tmem_empty[s], EW);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 2) tmem_alloc(tmem_holder, Cfg::kTmemCols);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-  // PDL: everything above (barrier init, TMEM allocation, descriptor prefetch) touches no global data and may overlap
-  // the predecessor's tail; from here on operands / auxiliary tensors written by earlier kernels are read
-  pdl_wait();
-  pdl_launch_dependents();
-
-  const int num_work = p.tiles_m * p.tiles_n * p.splits;
-
+// Contraction over k-blocks [kb0, kb1) of the tile at (m0, n0).  Warp 0 loads, warps 4-11 multiply; on return the
+// consumer warps hold the fp32 tile in shared memory at `smem` (row pitch GemmCfg<BN>::kAccLd) and have synchronised.
+template <int BN, bool A_MN, bool B_MN>
+__device__ __forceinline__ void gemm_mainloop(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                              const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, int m0, int n0,
+                                              int kb0, int kb1, int warp, int lane) {
+  using Cfg = GemmCfg<BN>;
   if (warp == 0) {
     // ------------------------------ TMA producer ------------------------------
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
-      for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-        const int tile = w / p.splits, split = w % p.splits;
-        const int m0 = (tile / p.tiles_n) * BM, n0 = (tile % p.tiles_n) * BN;
-        const int kb0 = split * p.kblocks_per_split;
-        const int kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          uint8_t* sa = smem + stage * Cfg::kStageBytes;
-          uint8_t* sb = sa + Cfg::kABytes;
-          const int k0 = kb * BK;
-          if (!A_MN) {
-            tma_load_2d(sa, &tmap_a, &full_bar[stage], k0, m0);            // box {64 k, 128 rows}
-          } else {
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+        uint8_t* sa = smem + stage * Cfg::kStageBytes;
+        uint8_t* sb = sa + Cfg::kABytes;
+        const int k0 = kb * BK;
+        if (!A_MN) {
+          tma_load_2d(sa, tmap_a, &full_bar[stage], k0, m0);              // box {64 k, 128 rows}
+        } else {
 #pragma unroll
-            for (int j = 0; j < BM / 64; ++j)                                // box {64 m, 64 k-rows}
-              tma_load_2d(sa + j * (BK * 128), &tmap_a, &full_bar[stage], m0 + 64 * j, k0);
-          }
-          if (!B_MN) {
-            tma_load_2d(sb, &tmap_b, &full_bar[stage], k0, n0);            // box {64 k, BN rows}
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN / 64; ++j)
-              tma_load_2d(sb + j * (BK * 128), &tmap_b, &full_bar[stage], n0 + 64 * j, k0);
-          }
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+          for (int j = 0; j < BM / 64; ++j)                                // box {64 m, 64 k-rows}
+            tma_load_2d(sa + j * (BK * 128), tmap_a, &full_bar[stage], m0 + 64 * j, k0);
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(BM, BN, A_MN, B_MN);
-      constexpr uint32_t a_lbo = A_MN ? BK * 128 : 16, b_lbo = B_MN ? BK * 128 : 16;
-      constexpr uint32_t a_kstep = A_MN ? UMMA_K * 128 : UMMA_K * 2;
-      constexpr uint32_t b_kstep = B_MN ? UMMA_K * 128 : UMMA_K * 2;
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-        const int split = w % p.splits;
-        const int kb0 = split * p.kblocks_per_split;
-        const int kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * Cfg::kAccStride;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint32_t sb = sa + Cfg::kABytes;
+        if (!B_MN) {
+          tma_load_2d(sb, tmap_b, &full_bar[stage], k0, n0);              // box {64 k, BN rows}
+        } else {
 #pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            const uint64_t da = make_smem_desc(sa + k * a_kstep, a_lbo, 1024);
-            const uint64_t db = make_smem_desc(sb + k * b_kstep, b_lbo, 1024);
-            umma_bf16(d_tmem, da, db, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // smem slot reusable once these MMAs have read it
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+          for (int j = 0; j < BN / 64; ++j)
+            tma_load_2d(sb + j * (BK * 128), tmap_b, &full_bar[stage], n0 + 64 * j, k0);
         }
-        umma_commit(&tmem_full[acc]);      // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
       }
     }
   } else if (warp >= 4) {
-    // ------------------------------ epilogue ------------------------------
-    const DropCtx drop = make_drop_ctx(p.rng, p.rng_site, p.dropout_p);
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-      const int tile = w / p.splits, split = w % p.splits;
-      const int m0 = (tile / p.tiles_n) * BM, n0 = (tile % p.tiles_n) * BN;
-      epilogue_tile<BN, EW>(p, drop, tmem_base + acc * Cfg::kAccStride, warp, lane, m0, n0, split,
-                        epi_stage + (warp - 4) * kEpiStageBytes, &tmem_full[acc], acc_phase);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+    // ------------------------------ wgmma consumers ------------------------------
+    const int wg = (warp - 4) >> 2;             // rows [64 wg, 64 wg + 64) of the tile
+    constexpr uint32_t a_lbo = A_MN ? BK * 128 : 16, b_lbo = B_MN ? BK * 128 : 16;
+    constexpr uint32_t a_kstep = A_MN ? WGMMA_K * 128 : WGMMA_K * 2;
+    constexpr uint32_t b_kstep = B_MN ? WGMMA_K * 128 : WGMMA_K * 2;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0, prev = -1; uint32_t phase = 0;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      // K-major A: the warpgroup's 64 rows start 64 x 128 B in; MN-major A: its 64 columns are the second slab
+      const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes) + wg * 8192;
+      const uint32_t sb = smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / WGMMA_K; ++k)
+        wgmma_bf16<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, make_smem_desc(sa + k * a_kstep, a_lbo, 1024),
+                                                     make_smem_desc(sb + k * b_kstep, b_lbo, 1024),
+                                                     (kb > kb0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();                            // the previous k-block's products are done: release its stage
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    // every consumer warp is past its last product and every TMA write has been consumed: the ring is dead
+    named_barrier_sync(1, kEpiWarps * 32);
+    float* accs = reinterpret_cast<float*>(smem);
+    const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int c = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      *reinterpret_cast<float2*>(accs + (size_t)r * Cfg::kAccLd + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(accs + (size_t)(r + 8) * Cfg::kAccLd + 8 * j + c) =
+          make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+    named_barrier_sync(1, kEpiWarps * 32);
   }
 }
 
-// ------------------------------------------------------------------------------------------------------------
-// CTA-pair kernel (cta_group::2).  Pair tile 256 x BN; CTA rank r stages A rows [m0 + 128 r, +128) and B rows
-// [n0 + r BN/2, +BN/2).  All mbarriers exist in both CTAs at identical offsets:
-//   full[s]        lives in the LEADER (rank 0): armed by the leader's producer with the bytes of BOTH CTAs; both
-//                  CTAs' TMA loads complete_tx on it; the leader's MMA thread waits on it
-//   empty[s]       one per CTA, released by a multicast tcgen05.commit (both producers wait their own copy)
-//   tmem_full[a]   one per CTA, multicast commit (each CTA's epilogue warps wait their own copy)
-//   tmem_empty[a]  lives in the leader, count 2 x 8: the peer's epilogue warps arrive remotely
-// ------------------------------------------------------------------------------------------------------------
-template <int BN, int EW>
-struct Gemm2Cfg {
-  static constexpr int kABytes = BM * BK * 2;            // this CTA's 128 A rows
-  static constexpr int kBBytes = (BN / 2) * BK * 2;      // this CTA's half of the B tile
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (BN == 256) ? 5 : (EW == 16 ? 6 : 7);
-  static constexpr int kAccStride = (BN <= 128) ? 128 : 256;
-  static constexpr int kTmemCols = 2 * kAccStride;
-  static constexpr int kPipeBytes = kStages * kStageBytes;
-  static constexpr int kSmemBytes = kPipeBytes + EW * kEpiStageBytes + 1024 + 256;
-};
-
-template <int BN, bool A_MN, bool B_MN, int EW>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(gemm_threads(EW)) __maxnreg__(EW == 8 ? 128 : 96)
-gemm2_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                  const GemmKernelParams p) {
-  using Cfg = Gemm2Cfg<BN, EW>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_align_1024(smem_raw);
-  uint8_t* epi_stage = smem + Cfg::kPipeBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + EW * kEpiStageBytes);
-  uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tmem_full = empty_bar + Cfg::kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  if (threadIdx.x == 0) stamp(p, 0);                                  // kernel entry
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < Cfg::kStages; ++s) {
+template <int BN>
+__device__ __forceinline__ void gemm_setup(uint64_t* full_bar, uint64_t* empty_bar) {
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < GemmCfg<BN>::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full[s], 1);
-      mbar_init(&tmem_empty[s], 2 * EW);
+      mbar_init(&empty_bar[s], kEpiWarps);
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc_2sm(tmem_holder, Cfg::kTmemCols);
-  tc_fence_before();
-  cluster_sync_all();   // barrier inits + TMEM allocation visible pair-wide before any remote arrive / TMA credit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-  if (threadIdx.x == 0) stamp(p, 1);                                  // setup done
-  // PDL: everything above (barrier init, TMEM allocation, descriptor prefetch) touches no global data and may overlap
-  // the predecessor's tail; from here on operands / auxiliary tensors written by earlier kernels are read
+  __syncthreads();
+}
+
+template <int BN, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const GemmKernelParams p) {
+  using Cfg = GemmCfg<BN>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_align_1024(smem_raw);
+  uint8_t* epi_stage = smem + Cfg::kPipeBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + kEpiWarps * kEpiStageBytes);
+  uint64_t* empty_bar = full_bar + Cfg::kStages;
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+  }
+  gemm_setup<BN>(full_bar, empty_bar);
+  // PDL: everything above touches no global data and may overlap the predecessor's tail
   pdl_wait();
   pdl_launch_dependents();
 
-  const int num_work = p.tiles_m * p.tiles_n * p.splits;   // tiles_m counts 256-row tiles here
-
-  if (warp == 0) {
-    // ------------------------------ TMA producer (both CTAs) ------------------------------
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int w = pair; w < num_work; w += npairs) {
-        const int tile = w / p.splits, split = w % p.splits;
-        const int m0 = (tile / p.tiles_n) * (2 * BM) + (int)rank * BM;
-        const int n0 = (tile % p.tiles_n) * BN + (int)rank * (BN / 2);
-        const int kb0 = split * p.kblocks_per_split;
-        const int kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (leader) mbar_expect_tx(&full_bar[stage], 2 * Cfg::kStageBytes);
-          const uint32_t bar = mapa_u32(smem_u32(&full_bar[stage]), 0);   // the leader's full barrier
-          uint8_t* sa = smem + stage * Cfg::kStageBytes;
-          uint8_t* sb = sa + Cfg::kABytes;
-          const int k0 = kb * BK;
-          if (!A_MN) {
-            tma_load_2d_2sm(sa, &tmap_a, bar, k0, m0);                     // box {64 k, 128 rows}
-          } else {
-#pragma unroll
-            for (int j = 0; j < BM / 64; ++j)                                // box {64 m, 64 k-rows}
-              tma_load_2d_2sm(sa + j * (BK * 128), &tmap_a, bar, m0 + 64 * j, k0);
-          }
-          if (!B_MN) {
-            tma_load_2d_2sm(sb, &tmap_b, bar, k0, n0);                     // box {64 k, BN/2 rows}
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN / 128; ++j)
-              tma_load_2d_2sm(sb + j * (BK * 128), &tmap_b, bar, n0 + 64 * j, k0);
-          }
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer (leader CTA only) ------------------------------
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(2 * BM, BN, A_MN, B_MN);
-      constexpr uint32_t a_lbo = A_MN ? BK * 128 : 16, b_lbo = B_MN ? BK * 128 : 16;
-      constexpr uint32_t a_kstep = A_MN ? UMMA_K * 128 : UMMA_K * 2;
-      constexpr uint32_t b_kstep = B_MN ? UMMA_K * 128 : UMMA_K * 2;
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int w = pair; w < num_work; w += npairs) {
-        const int split = w % p.splits;
-        const int kb0 = split * p.kblocks_per_split;
-        const int kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * Cfg::kAccStride;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          if (w == pair && kb == kb0) stamp(p, 2);                    // first operands landed
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint32_t sb = sa + Cfg::kABytes;
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            const uint64_t da = make_smem_desc(sa + k * a_kstep, a_lbo, 1024);
-            const uint64_t db = make_smem_desc(sb + k * b_kstep, b_lbo, 1024);
-            umma_bf16_2sm(d_tmem, da, db, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit_2sm(&empty_bar[stage]);
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_2sm(&tmem_full[acc]);
-        if (w + npairs >= num_work) stamp(p, 3);                      // last MMA of the last tile issued
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------ epilogue (both CTAs, own 128 rows) ------------------------------
+  const int tile = blockIdx.x / p.splits, split = blockIdx.x % p.splits;
+  const int m0 = (tile / p.tiles_n) * BM, n0 = (tile % p.tiles_n) * BN;
+  const int kb0 = split * p.kblocks_per_split;
+  const int kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
+  gemm_mainloop<BN, A_MN, B_MN>(smem, full_bar, empty_bar, &tmap_a, &tmap_b, m0, n0, kb0, kb1, warp, lane);
+  if (warp >= 4) {
     const DropCtx drop = make_drop_ctx(p.rng, p.rng_site, p.dropout_p);
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int w = pair; w < num_work; w += npairs) {
-      const int tile = w / p.splits, split = w % p.splits;
-      const int m0 = (tile / p.tiles_n) * (2 * BM) + (int)rank * BM;
-      const int n0 = (tile % p.tiles_n) * BN;
-      epilogue_tile<BN, EW>(p, drop, tmem_base + acc * Cfg::kAccStride, warp, lane, m0, n0, split,
-                        epi_stage + (warp - 4) * kEpiStageBytes, &tmem_full[acc], acc_phase);
-      tc_fence_before();
-      __syncwarp();
-      if (warp == 4 && lane == 0 && w + npairs >= num_work) stamp(p, 5);   // last epilogue done (warp 4)
-      if (lane == 0) {
-        if (leader) mbar_arrive(&tmem_empty[acc]);
-        else mbar_arrive_remote(mapa_u32(smem_u32(&tmem_empty[acc]), 0));
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-
-  // no CTA may exit (or free TMEM) while its partner can still multicast-commit into it or read its smem
-  tc_fence_before();
-  cluster_sync_all();
-  if (threadIdx.x == 0) stamp(p, 6);                                  // pair done
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, Cfg::kTmemCols);
+    epilogue_tile<BN>(p, drop, reinterpret_cast<const float*>(smem), Cfg::kAccLd, warp, lane, m0, n0, split,
+                      epi_stage + (warp - 4) * kEpiStageBytes);
   }
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Grouped CTA-pair kernel: up to kMaxGroup independent TN problems (D_i[M_i,N_i] = A_i^T B_i, both operands MN-major,
-// same contraction length) behind ONE launch.  This is the weight-gradient step of an encoder layer: its four
-// GEMMs are small (4.8-19 GFLOP), so launched one by one each pays the ~7 us fixed cost of a launch (setup, first
-// operands, drain, pair exit, gap) and -- with 9-54 tiles on 74 CTA pairs -- needs split-K partials plus a reduce
-// kernel to fill the machine.  Together they are 108 full-K 256x256 tiles: two waves of one persistent kernel, no
-// partials.  Roles and barriers are those of gemm2_bf16_kernel; only the work decode differs.
+// Grouped kernel: up to kMaxGroup independent TN problems (D_i[M_i,N_i] = A_i^T B_i, both operands MN-major, same
+// contraction length) behind ONE launch.  This is the weight-gradient step of an encoder layer: its four GEMMs are
+// small, so launched one by one each pays a launch's fixed cost and needs split-K partials plus a reduce kernel to
+// fill the machine.  Mainloop and epilogue are those of gemm_bf16_kernel; only the work decode differs.
 // ------------------------------------------------------------------------------------------------------------
 constexpr int kMaxGroup = 4;
 struct GroupedProblem {
@@ -389,18 +192,17 @@ struct GroupedParams {
 // exp_avg_sq and the fp32 master weight of the same elements make one round trip each through the warp's staging
 // tile (coalesced 128-byte rows in, update, coalesced rows out), and the bf16 shadow weight and the bf16 gradient
 // are written.  Same arithmetic, statement for statement, as reduce_adamw_kernel (csrc/optim.cu).  The extra
-// ~26 bytes per parameter move under the next tile's mainloop instead of in a separate HBM-bound kernel.
-template <int EW>
+// ~26 bytes per parameter move in the GEMM's epilogue instead of in a separate HBM-bound kernel.
 __device__ __forceinline__ void epilogue_tile_adamw(const GroupedProblem& pr, const GroupedParams& gp, float step_size,
-                                                    uint32_t tmem_acc, int warp, int lane, int m_base, int n0,
-                                                    uint8_t* stage, uint64_t* acc_bar, uint32_t acc_phase) {
+                                                    const float* acc, int acc_ld, int warp, int lane, int m_base,
+                                                    int n0, uint8_t* stage) {
   constexpr int BN = 256;
-  constexpr int kColsPerWarp = BN / (EW / 4);
+  constexpr int kColsPerWarp = BN / 2;
   const int quarter = warp & 3, cgrp = (warp - 4) >> 2;
   const int row0 = m_base + quarter * 32;
   const int rows_valid = pr.M - row0;
   const int nw = n0 + cgrp * kColsPerWarp;
-  const uint32_t taddr = tmem_acc + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(cgrp * kColsPerWarp);
+  const float* arow = acc + (size_t)(quarter * 32 + lane) * acc_ld + cgrp * kColsPerWarp;
   const bool any = rows_valid > 0;
   auto fetch = [&](const float* base, int n) {
     tile_g2s_async<8>(stage, reinterpret_cast<const uint8_t*>(base + (size_t)row0 * pr.ldd + n), pr.ldd * 4, lane,
@@ -409,17 +211,14 @@ __device__ __forceinline__ void epilogue_tile_adamw(const GroupedProblem& pr, co
   auto put = [&](float* base, int n) {
     tile_s2g<8>(stage, reinterpret_cast<uint8_t*>(base + (size_t)row0 * pr.ldd + n), pr.ldd * 4, lane, rows_valid);
   };
-  if (any && nw < pr.N) fetch(pr.m, nw);   // first exp_avg tile: independent of the accumulator
-  mbar_wait(acc_bar, acc_phase);
-  tc_fence_after();
+  if (any && nw < pr.N) fetch(pr.m, nw);   // first exp_avg tile
 #pragma unroll 1
   for (int c = 0; c < kColsPerWarp / 32; ++c) {
     const int n = nw + c * 32;
     float g[32];
     {
       uint32_t v[32];
-      tmem_ld32(taddr + c * 32, v);
-      tmem_ld_wait();
+      acc_ld32(arow + c * 32, v);
 #pragma unroll
       for (int j = 0; j < 32; ++j) g[j] = __uint_as_float(v[j]);
     }
@@ -505,149 +304,55 @@ __device__ __forceinline__ int grouped_find(const GroupedParams& gp, int w) {
   return pi;
 }
 
-template <int EW>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(gemm_threads(EW)) __maxnreg__(EW == 8 ? 128 : 96)
-gemm2_grouped_tn_kernel(const __grid_constant__ GroupedMaps maps, const GroupedParams gp) {
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_grouped_tn_kernel(const __grid_constant__ GroupedMaps maps, const GroupedParams gp) {
   constexpr int BN = 256;
-  using Cfg = Gemm2Cfg<BN, EW>;
+  using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align_1024(smem_raw);
   uint8_t* epi_stage = smem + Cfg::kPipeBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + EW * kEpiStageBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + kEpiWarps * kEpiStageBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tmem_full = empty_bar + Cfg::kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    for (int i = 0; i < gp.count; ++i) {
-      tma_prefetch_desc(&maps.a[i]);
-      tma_prefetch_desc(&maps.b[i]);
-    }
+  const int pi = grouped_find(gp, blockIdx.x);
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&maps.a[pi]);
+    tma_prefetch_desc(&maps.b[pi]);
   }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full[s], 1);
-      mbar_init(&tmem_empty[s], 2 * EW);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 2) tmem_alloc_2sm(tmem_holder, Cfg::kTmemCols);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
+  gemm_setup<BN>(full_bar, empty_bar);
   pdl_wait();
   pdl_launch_dependents();
 
-  if (warp == 0) {
-    // ------------------------------ TMA producer (both CTAs) ------------------------------
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int w = pair; w < gp.num_work; w += npairs) {
-        const int pi = grouped_find(gp, w);
-        const int lt = w - gp.pr[pi].tile_begin;
-        const int m0 = (lt / gp.pr[pi].tiles_n) * (2 * BM) + (int)rank * BM;
-        const int n0 = (lt % gp.pr[pi].tiles_n) * BN + (int)rank * (BN / 2);
-        const CUtensorMap* ta = &maps.a[pi];
-        const CUtensorMap* tb = &maps.b[pi];
-        for (int kb = 0; kb < gp.kblocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (leader) mbar_expect_tx(&full_bar[stage], 2 * Cfg::kStageBytes);
-          const uint32_t bar = mapa_u32(smem_u32(&full_bar[stage]), 0);
-          uint8_t* sa = smem + stage * Cfg::kStageBytes;
-          uint8_t* sb = sa + Cfg::kABytes;
-          const int k0 = kb * BK;
-#pragma unroll
-          for (int j = 0; j < BM / 64; ++j) tma_load_2d_2sm(sa + j * (BK * 128), ta, bar, m0 + 64 * j, k0);
-#pragma unroll
-          for (int j = 0; j < BN / 128; ++j) tma_load_2d_2sm(sb + j * (BK * 128), tb, bar, n0 + 64 * j, k0);
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer (leader CTA only) ------------------------------
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(2 * BM, BN, true, true);
-      constexpr uint32_t lbo = BK * 128, kstep = UMMA_K * 128;
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int w = pair; w < gp.num_work; w += npairs) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * Cfg::kAccStride;
-        for (int kb = 0; kb < gp.kblocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint32_t sb = sa + Cfg::kABytes;
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k)
-            umma_bf16_2sm(d_tmem, make_smem_desc(sa + k * kstep, lbo, 1024), make_smem_desc(sb + k * kstep, lbo, 1024),
-                          idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit_2sm(&empty_bar[stage]);
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_2sm(&tmem_full[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------ epilogue (both CTAs, own 128 rows) ------------------------------
-    GemmKernelParams q;
-    q.splits = 1; q.epilogue = B2_EPI_NONE; q.bias = nullptr; q.aux_in = nullptr; q.aux_out = nullptr;
-    q.partial = nullptr; q.dropout_p = 0.f; q.rng = nullptr; q.rng_site = 0; q.timing = nullptr; q.colsum = nullptr;
-    q.ld_aux_in = 0; q.ld_aux_out = 0; q.K = 0; q.tiles_m = 0; q.kblocks_per_split = 0; q.kblocks_total = 0;
-    DropCtx drop;
-    drop.k0 = 0; drop.k1 = 0; drop.step = 0; drop.site = 0; drop.thresh = 0; drop.scale = 1.f;
+  const GroupedProblem& pr = gp.pr[pi];
+  const int lt = blockIdx.x - pr.tile_begin;
+  const int m0 = (lt / pr.tiles_n) * BM;
+  const int n0 = (lt % pr.tiles_n) * BN;
+  gemm_mainloop<BN, true, true>(smem, full_bar, empty_bar, &maps.a[pi], &maps.b[pi], m0, n0, 0, gp.kblocks, warp,
+                                lane);
+  if (warp < 4) return;
+  uint8_t* stage = epi_stage + (warp - 4) * kEpiStageBytes;
+  if (gp.adamw) {
     // HF AdamW bias correction (as reduce_adamw_kernel): step_size = lr * sqrt(1 - b2^t) / (1 - b1^t)
     float step_size = gp.lr;
-    if (gp.adamw && gp.correct_bias) {
+    if (gp.correct_bias) {
       const long long t = *gp.step_counter + 1;
       const double bc1 = 1.0 - pow(gp.beta1_d, (double)t);
       const double bc2 = 1.0 - pow(gp.beta2_d, (double)t);
       step_size = (float)(gp.lr_d * sqrt(bc2) / bc1);
     }
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int w = pair; w < gp.num_work; w += npairs) {
-      const int pi = grouped_find(gp, w);
-      const int lt = w - gp.pr[pi].tile_begin;
-      q.M = gp.pr[pi].M; q.N = gp.pr[pi].N; q.tiles_n = gp.pr[pi].tiles_n; q.D = gp.pr[pi].D; q.ldd = gp.pr[pi].ldd;
-      const int m0 = (lt / gp.pr[pi].tiles_n) * (2 * BM) + (int)rank * BM;
-      const int n0 = (lt % gp.pr[pi].tiles_n) * BN;
-      if (gp.adamw)
-        epilogue_tile_adamw<EW>(gp.pr[pi], gp, step_size, tmem_base + acc * Cfg::kAccStride, warp, lane, m0, n0,
-                                epi_stage + (warp - 4) * kEpiStageBytes, &tmem_full[acc], acc_phase);
-      else
-      epilogue_tile<BN, EW>(q, drop, tmem_base + acc * Cfg::kAccStride, warp, lane, m0, n0, 0,
-                            epi_stage + (warp - 4) * kEpiStageBytes, &tmem_full[acc], acc_phase);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(&tmem_empty[acc]);
-        else mbar_arrive_remote(mapa_u32(smem_u32(&tmem_empty[acc]), 0));
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
+    epilogue_tile_adamw(pr, gp, step_size, reinterpret_cast<const float*>(smem), Cfg::kAccLd, warp, lane, m0, n0,
+                        stage);
+    return;
   }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, Cfg::kTmemCols);
-  }
+  GemmKernelParams q;
+  q.splits = 1; q.epilogue = B2_EPI_NONE; q.bias = nullptr; q.aux_in = nullptr; q.aux_out = nullptr;
+  q.partial = nullptr; q.dropout_p = 0.f; q.rng = nullptr; q.rng_site = 0; q.timing = nullptr; q.colsum = nullptr;
+  q.ld_aux_in = 0; q.ld_aux_out = 0; q.K = 0; q.tiles_m = 0; q.kblocks_per_split = 0; q.kblocks_total = 0;
+  q.M = pr.M; q.N = pr.N; q.tiles_n = pr.tiles_n; q.D = pr.D; q.ldd = pr.ldd;
+  DropCtx drop;
+  drop.k0 = 0; drop.k1 = 0; drop.step = 0; drop.site = 0; drop.thresh = 0; drop.scale = 1.f;
+  epilogue_tile<BN>(q, drop, reinterpret_cast<const float*>(smem), Cfg::kAccLd, warp, lane, m0, n0, 0, stage);
 }
 
 // sums split-K partials [splits][M][N] fp32 -> bf16 D
@@ -677,7 +382,7 @@ static int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    if (g_num_sms <= 0) g_num_sms = 132;
   }
   return g_num_sms;
 }
@@ -709,9 +414,9 @@ static int32_t launch_splitk_reduce(const b2_gemm_args_t& a, int splits, cudaStr
   return 0;
 }
 
-template <int BN, bool A_MN, bool B_MN, int EW>
+template <int BN, bool A_MN, bool B_MN>
 static int32_t launch_gemm(const b2_gemm_args_t& a, int splits, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, EW>;
+  using Cfg = GemmCfg<BN>;
   CUtensorMap ta, tb;
   int32_t st;
   if (!A_MN) st = get_tensor_map_2d(&ta, a.A, (uint64_t)a.M, (uint64_t)a.K, (uint64_t)a.lda * 2, BM, 64);
@@ -722,85 +427,51 @@ static int32_t launch_gemm(const b2_gemm_args_t& a, int splits, cudaStream_t str
   if (st) return st;
   GemmKernelParams p;
   fill_params(p, a, BM, BN, splits);
-  auto kern = gemm_bf16_kernel<BN, A_MN, B_MN, EW>;
+  auto kern = gemm_bf16_kernel<BN, A_MN, B_MN>;
   static bool attr_set = false;
   if (!attr_set) {
     B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set = true;
   }
-  const int work = p.tiles_m * p.tiles_n * p.splits;
-  const int grid = work < num_sms() ? work : num_sms();
-  B2_LAUNCH(kern, grid, gemm_threads(EW), Cfg::kSmemBytes, stream, ta, tb, p);
+  const int work = p.tiles_m * p.tiles_n * p.splits;   // one tile (or split-K slice of one) per CTA
+  B2_LAUNCH(kern, work, kGemmThreads, Cfg::kSmemBytes, stream, ta, tb, p);
   B2_CUDA(cudaGetLastError());
   count_launches(1);
   if (splits > 1 && a.epilogue != B2_EPI_ACCUM_F32) return launch_splitk_reduce(a, splits, stream);
   return 0;
 }
 
-template <int BN, bool A_MN, bool B_MN, int EW>
-static int32_t launch_gemm2(const b2_gemm_args_t& a, int splits, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg<BN, EW>;
-  CUtensorMap ta, tb;
-  int32_t st;
-  if (!A_MN) st = get_tensor_map_2d(&ta, a.A, (uint64_t)a.M, (uint64_t)a.K, (uint64_t)a.lda * 2, BM, 64);
-  else       st = get_tensor_map_2d(&ta, a.A, (uint64_t)a.K, (uint64_t)a.M, (uint64_t)a.lda * 2, BK, 64);
-  if (st) return st;
-  if (!B_MN) st = get_tensor_map_2d(&tb, a.B, (uint64_t)a.N, (uint64_t)a.K, (uint64_t)a.ldb * 2, BN / 2, 64);
-  else       st = get_tensor_map_2d(&tb, a.B, (uint64_t)a.K, (uint64_t)a.N, (uint64_t)a.ldb * 2, BK, 64);
-  if (st) return st;
-  GemmKernelParams p;
-  fill_params(p, a, 2 * BM, BN, splits);
-  auto kern = gemm2_bf16_kernel<BN, A_MN, B_MN, EW>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set = true;
-  }
-  const int work = p.tiles_m * p.tiles_n * p.splits;
-  const int max_pairs = num_sms() / 2;
-  const int pairs = work < max_pairs ? work : max_pairs;
-  B2_LAUNCH(kern, 2 * pairs, gemm_threads(EW), Cfg::kSmemBytes, stream, ta, tb, p);
-  B2_CUDA(cudaGetLastError());
-  count_launches(1);
-  if (splits > 1 && a.epilogue != B2_EPI_ACCUM_F32) return launch_splitk_reduce(a, splits, stream);
-  return 0;
-}
-
-// Kernel / tile-width / split-K choice.  Cost model per candidate: rounds of whole waves x per-k-block time, where
-// the k-block time is the larger of the tensor-pipe time and the L2->SM feed time (measured ceiling ~10 TB/s).
-struct Choice { int pair, bn, splits; };
+// Tile-width / split-K choice.  Cost model per candidate: waves of CTAs x per-k-block time, where the k-block time
+// is the larger of the tensor-pipe time (~2048 bf16 FMA per SM and cycle) and the L2->SM feed time.
+struct Choice { int bn, splits; };
 static Choice choose_config(const b2_gemm_args_t& a) {
   const int sms = num_sms();
   const int kblocks = (int)((a.K + BK - 1) / BK);
   const bool accum = a.epilogue == B2_EPI_ACCUM_F32;   // split-K slices add in place: no workspace, any split count
   const bool can_split = accum || ((a.epilogue == B2_EPI_NONE) && a.workspace != nullptr && a.bias == nullptr);
   double best = 1e30;
-  Choice c{0, 128, 1};
-  const double l2_bytes_per_cycle = 5500.0;   // ~10 TB/s at ~1.85 GHz, shared by the busy SMs
-  for (int pair = 0; pair <= 1; ++pair) {
-    const int bns[2] = {256, 128};
-    for (int bi = 0; bi < 2; ++bi) {
-      const int bn = bns[bi];
-      if (a.N % bn != 0 && (pair || bn != 128)) continue;
-      const int tile_m = pair ? 256 : 128;
-      const int tiles = (int)((a.M + tile_m - 1) / tile_m) * (int)((a.N + bn - 1) / bn);
-      const int slots = pair ? sms / 2 : sms;
-      const int max_s = can_split ? 8 : 1;
-      for (int s = 1; s <= max_s; s = accum ? s + 1 : s * 2) {
-        if (s > 1 && (kblocks / s < 8)) break;
-        if (s > 1 && !accum && (size_t)s * a.M * a.N * 4 > (size_t)a.workspace_bytes) break;
-        const int work = tiles * s;
-        const int rounds = (work + slots - 1) / slots;
-        const int busy_sms = (work < slots ? work : slots) * (pair ? 2 : 1);
-        const double mma_cycles = 128.0 * bn * 64 / 4096.0;                    // per SM, per k-block
-        const double bytes_per_sm = pair ? (128 + bn / 2) * 128.0 : (128 + bn) * 128.0;
-        const double feed_cycles = bytes_per_sm * busy_sms / l2_bytes_per_cycle;
-        const double kb_cycles = mma_cycles > feed_cycles ? mma_cycles : feed_cycles;
-        double t = rounds * ((double)((kblocks + s - 1) / s) * kb_cycles + 2500.0 /*prologue + epilogue tail*/);
-        if (s > 1 && !accum) t += 1500.0 + (double)s * a.M * a.N * 8 / 3000.0;  // partial write + reduce pass
-        if (s > 1 && accum) t += (double)(s - 1) * a.M * a.N * 4 / 3000.0;      // extra reduction traffic at L2
-        if (t < best) { best = t; c = Choice{pair, bn, s}; }
-      }
+  Choice c{128, 1};
+  const double l2_bytes_per_cycle = 3000.0;   // L2 -> SM bandwidth shared by the busy SMs, bytes per SM clock
+  const int bns[2] = {256, 128};
+  for (int bi = 0; bi < 2; ++bi) {
+    const int bn = bns[bi];
+    if (a.N % bn != 0 && bn != 128) continue;
+    const int tiles = (int)((a.M + BM - 1) / BM) * (int)((a.N + bn - 1) / bn);
+    const int max_s = can_split ? 8 : 1;
+    for (int s = 1; s <= max_s; s = accum ? s + 1 : s * 2) {
+      if (s > 1 && (kblocks / s < 8)) break;
+      if (s > 1 && !accum && (size_t)s * a.M * a.N * 4 > (size_t)a.workspace_bytes) break;
+      const int work = tiles * s;
+      const int rounds = (work + sms - 1) / sms;
+      const int busy_sms = work < sms ? work : sms;
+      const double mma_cycles = 128.0 * bn * 64 / 2048.0;                    // per SM, per k-block
+      const double bytes_per_sm = (128 + bn) * 128.0;
+      const double feed_cycles = bytes_per_sm * busy_sms / l2_bytes_per_cycle;
+      const double kb_cycles = mma_cycles > feed_cycles ? mma_cycles : feed_cycles;
+      double t = rounds * ((double)((kblocks + s - 1) / s) * kb_cycles + 2500.0 /*prologue + epilogue tail*/);
+      if (s > 1 && !accum) t += 1500.0 + (double)s * a.M * a.N * 8 / 3000.0;  // partial write + reduce pass
+      if (s > 1 && accum) t += (double)(s - 1) * a.M * a.N * 4 / 3000.0;      // extra reduction traffic at L2
+      if (t < best) { best = t; c = Choice{bn, s}; }
     }
   }
   return c;
@@ -809,18 +480,6 @@ static Choice choose_config(const b2_gemm_args_t& a) {
 }  // namespace b2
 
 using namespace b2;
-
-// Epilogue warps per CTA: 16 (640 threads x 96 registers: the CTA owns the SM's register file) or, with
-// B2_GEMM_EPI_WARPS=8, 8 (384 threads capped at 128 registers: a quarter of the register file stays free, so a
-// 256-thread block of a memory-bound kernel from another stream -- the AdamW update -- can be co-resident).
-static int gemm_epi_warps() {
-  static int v = 0;
-  if (v == 0) {
-    const char* e = getenv("B2_GEMM_EPI_WARPS");
-    v = (e != nullptr && atoi(e) == 8) ? 8 : 16;
-  }
-  return v;
-}
 
 extern "C" int32_t b2_gemm_bf16(const b2_gemm_args_t* a, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
@@ -848,17 +507,10 @@ extern "C" int32_t b2_gemm_bf16(const b2_gemm_args_t* a, void* stream_) {
   B2_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, "b2_gemm_bf16: dropout_p out of range");
 
   Choice c = choose_config(*a);
-  if (a->force_kernel == 1) c.pair = 0;
-  if (a->force_kernel == 2) c.pair = 1;
+  // force_kernel (1 / 2) selects between kernels on other builds; this one has a single GEMM kernel
   if (a->force_bn == 128 || a->force_bn == 256) {
-    B2_REQUIRE(a->N % a->force_bn == 0 || (a->force_bn == 128 && !c.pair), "b2_gemm_bf16: force_bn does not divide N");
+    B2_REQUIRE(a->N % a->force_bn == 0 || a->force_bn == 128, "b2_gemm_bf16: force_bn does not divide N");
     c.bn = a->force_bn;
-  }
-  if (c.pair) {
-    B2_REQUIRE(a->N % c.bn == 0, "b2_gemm_bf16: the CTA-pair kernel needs N %% %d == 0 (N=%lld)", c.bn,
-               (long long)a->N);
-  } else if (a->N % c.bn != 0 && c.bn != 128) {
-    c.bn = 128;
   }
   if (a->force_splits >= 1) {
     B2_REQUIRE(a->force_splits == 1 ||
@@ -871,26 +523,16 @@ extern "C" int32_t b2_gemm_bf16(const b2_gemm_args_t* a, void* stream_) {
   const bool a_mn = a->a_major == B2_MAJOR_MN, b_mn = a->b_major == B2_MAJOR_MN;
   B2_REQUIRE(!(a_mn && !b_mn), "b2_gemm_bf16: layout TT (A MN-major, B K-major) is not on the path");
 
-  const int epi_warps = gemm_epi_warps();
-#define B2_DISPATCH(FN, BN_, EW_)                                                      \
-  if (c.bn == BN_ && epi_warps == EW_) {                                               \
-    if (!a_mn && !b_mn) return FN<BN_, false, false, EW_>(*a, c.splits, stream);       \
-    if (!a_mn && b_mn) return FN<BN_, false, true, EW_>(*a, c.splits, stream);         \
-    return FN<BN_, true, true, EW_>(*a, c.splits, stream);                             \
+#define B2_DISPATCH(BN_)                                                          \
+  if (c.bn == BN_) {                                                              \
+    if (!a_mn && !b_mn) return launch_gemm<BN_, false, false>(*a, c.splits, stream); \
+    if (!a_mn && b_mn) return launch_gemm<BN_, false, true>(*a, c.splits, stream);   \
+    return launch_gemm<BN_, true, true>(*a, c.splits, stream);                       \
   }
-  if (c.pair) {
-    B2_DISPATCH(launch_gemm2, 128, 16)
-    B2_DISPATCH(launch_gemm2, 256, 16)
-    B2_DISPATCH(launch_gemm2, 128, 8)
-    B2_DISPATCH(launch_gemm2, 256, 8)
-  } else {
-    B2_DISPATCH(launch_gemm, 128, 16)
-    B2_DISPATCH(launch_gemm, 256, 16)
-    B2_DISPATCH(launch_gemm, 128, 8)
-    B2_DISPATCH(launch_gemm, 256, 8)
-  }
+  B2_DISPATCH(128)
+  B2_DISPATCH(256)
 #undef B2_DISPATCH
-  set_error("b2_gemm_bf16: no kernel for pair=%d BN=%d", c.pair, c.bn);
+  set_error("b2_gemm_bf16: no kernel for BN=%d", c.bn);
   return -2;
 }
 
@@ -907,13 +549,12 @@ static int32_t gemm_grouped_impl(const b2_gemm_args_t* args, int32_t count, cons
                 a.bias == nullptr && a.colsum_out == nullptr && a.N % 256 == 0 && a.K == args[0].K && a.M > 0 &&
                 a.K > 0 && a.A && a.B && a.D && a.K % 8 == 0 && a.lda % 8 == 0 && a.ldb % 8 == 0 &&
                 a.ldd % 8 == 0 && ((uintptr_t)a.A % 16 == 0) && ((uintptr_t)a.B % 16 == 0) &&
-                ((uintptr_t)a.D % 16 == 0) && a.force_kernel != 1 && a.force_splits <= 1 &&
+                ((uintptr_t)a.D % 16 == 0) && a.force_splits <= 1 &&
                 (a.force_bn == 0 || a.force_bn == 256);
   }
   if (targets != nullptr) {
     B2_REQUIRE(groupable, "b2_gemm_bf16_grouped_adamw: the problems do not fit the grouped kernel (TN layouts, plain "
                           "bf16 output, N %% 256 == 0, one K, at most %d)", kMaxGroup);
-    B2_REQUIRE(gemm_epi_warps() == 16, "b2_gemm_bf16_grouped_adamw: needs the 16-warp epilogue build");
     B2_REQUIRE(hp != nullptr && step_counter != nullptr, "b2_gemm_bf16_grouped_adamw: null optimizer arguments");
     B2_REQUIRE(hp->grad_scale == nullptr && hp->found_inf == nullptr,
                "b2_gemm_bf16_grouped_adamw: GradScaler state is not supported on the fused path");
@@ -949,7 +590,7 @@ static int32_t gemm_grouped_impl(const b2_gemm_args_t* args, int32_t count, cons
       g.w = targets[i].master; g.m = targets[i].exp_avg; g.v = targets[i].exp_avg_sq;
       g.shadow = (__nv_bfloat16*)targets[i].shadow; g.decay = targets[i].decay ? 1 : 0;
     }
-    work += (int)((a.M + 2 * BM - 1) / (2 * BM)) * g.tiles_n;
+    work += (int)((a.M + BM - 1) / BM) * g.tiles_n;
   }
   gp.adamw = targets != nullptr ? 1 : 0;
   gp.correct_bias = 0; gp.lr = gp.beta1 = gp.beta2 = gp.one_minus_beta1 = gp.one_minus_beta2 = gp.eps = gp.lr_wd = 0.f;
@@ -966,22 +607,13 @@ static int32_t gemm_grouped_impl(const b2_gemm_args_t* args, int32_t count, cons
   }
   for (int i = count; i < kMaxGroup; ++i) { gp.pr[i] = gp.pr[0]; gp.pr[i].tile_begin = 0x7fffffff; maps.a[i] = maps.a[0]; maps.b[i] = maps.b[0]; }
   gp.num_work = work;
-  const int max_pairs = num_sms() / 2;
-  const int pairs = work < max_pairs ? work : max_pairs;
   static bool attr_set = false;
   if (!attr_set) {
-    B2_CUDA(cudaFuncSetAttribute(gemm2_grouped_tn_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 Gemm2Cfg<256, 16>::kSmemBytes));
-    B2_CUDA(cudaFuncSetAttribute(gemm2_grouped_tn_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 Gemm2Cfg<256, 8>::kSmemBytes));
+    B2_CUDA(cudaFuncSetAttribute(gemm_grouped_tn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 GemmCfg<256>::kSmemBytes));
     attr_set = true;
   }
-  if (gemm_epi_warps() == 8) {
-    B2_LAUNCH(gemm2_grouped_tn_kernel<8>, 2 * pairs, gemm_threads(8), (Gemm2Cfg<256, 8>::kSmemBytes), stream, maps, gp);
-  } else {
-    B2_LAUNCH(gemm2_grouped_tn_kernel<16>, 2 * pairs, gemm_threads(16), (Gemm2Cfg<256, 16>::kSmemBytes), stream, maps,
-              gp);
-  }
+  B2_LAUNCH(gemm_grouped_tn_kernel, work, kGemmThreads, GemmCfg<256>::kSmemBytes, stream, maps, gp);
   B2_CUDA(cudaGetLastError());
   count_launches(1);
   return 0;

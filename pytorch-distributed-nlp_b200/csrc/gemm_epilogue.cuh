@@ -1,12 +1,11 @@
-// GEMM epilogue: TMEM accumulator -> registers -> fused element-wise math -> HBM, with COALESCED global traffic.
+// GEMM epilogue: fp32 accumulator tile (shared memory) -> fused element-wise math -> HBM, with COALESCED global traffic.
 //
-// tcgen05.ld (32x32b) hands every thread one accumulator ROW.  Storing rows straight from registers makes each
-// warp-wide 16-byte store touch 32 different 128-byte lines (one per row): the first profiles showed the epilogue,
-// not the tensor pipe, bounding every K=768 GEMM (~8k store wavefronts per 128x256 bf16 tile vs 6.1k MMA cycles).
-// Here each epilogue warp owns a 4 KB shared-memory staging tile (32 rows x 128 B, 16-byte chunks XOR-swizzled by
-// row & 7 so both access patterns are bank-conflict free).  Rows go registers -> staging -> global with every
-// warp-wide access covering 4 rows x 128 contiguous bytes (4 full lines); auxiliary inputs (residual, saved
-// pre-activation) take the same path in reverse.
+// The mainloop leaves the [128 x BN] fp32 accumulator in shared memory (wgmma fragments written out row-major), and
+// every epilogue thread then owns one accumulator ROW.  Storing rows straight from registers would make each
+// warp-wide 16-byte store touch 32 different 128-byte lines (one per row).  Here each epilogue warp owns a 4 KB
+// shared-memory staging tile (32 rows x 128 B, 16-byte chunks XOR-swizzled by row & 7 so both access patterns are
+// bank-conflict free).  Rows go registers -> staging -> global with every warp-wide access covering 4 rows x 128
+// contiguous bytes (4 full lines); auxiliary inputs (residual, saved pre-activation) take the same path in reverse.
 #pragma once
 #include "common.cuh"
 #include "../../include/b2_ddp_bert.h"
@@ -23,15 +22,9 @@ struct GemmKernelParams {
   __nv_bfloat16* aux_out; long long ld_aux_out;
   float* partial;  // split-K fp32 partials [splits][M][N]
   float dropout_p; const unsigned long long* rng; unsigned rng_site;
-  long long* timing;  // optional [gridDim.x][8] clock64 stamps (profiling aid, see tools/gemm_timeline.py)
+  long long* timing;  // unused by the H100 kernels (ABI field)
   float* colsum;      // optional fp32 [N]: += column sums of the bf16 output (bias gradient of the producing layer)
 };
-
-#ifdef __CUDACC__
-__device__ __forceinline__ void stamp(const GemmKernelParams& p, int slot) {
-  if (p.timing != nullptr) p.timing[(size_t)blockIdx.x * 8 + slot] = clock64();
-}
-#endif
 
 constexpr int kEpiStageBytes = 32 * 128;   // per epilogue warp
 
@@ -93,6 +86,15 @@ __device__ __forceinline__ void tile_g2s_async(uint8_t* stage, const uint8_t* g,
 }
 __device__ __forceinline__ void tile_async_wait() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
+// 32 consecutive fp32 accumulator columns of this thread's row (shared memory, 16-byte aligned)
+__device__ __forceinline__ void acc_ld32(const float* a, uint32_t (&v)[32]) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const uint4 t = *reinterpret_cast<const uint4*>(a + 4 * k);
+    v[4 * k] = t.x; v[4 * k + 1] = t.y; v[4 * k + 2] = t.z; v[4 * k + 3] = t.w;
+  }
+}
+
 // 32 bf16 columns (4 chunks, starting at chunk c0) of this thread's own row (row == lane) <-> 32 fp32 registers
 template <int CH>
 __device__ __forceinline__ void row_write32(uint8_t* stage, int lane, int c0, const float (&f)[32]) {
@@ -114,26 +116,24 @@ __device__ __forceinline__ void row_read32(uint8_t* stage, int lane, int c0, flo
   }
 }
 
-// EW epilogue warps drain one [128 rows x BN cols] accumulator: warp -> (TMEM lane quarter, column group).  With
-// EW = 16 every SM sub-partition runs four epilogue warps instead of two: the epilogue of a single-wave GEMM is fully
-// exposed (no next tile to hide behind) and that of the GELU GEMMs is longer than their K = 768 mainloop, so epilogue
-// latency is step time.  All math happens in passes of 32 columns (32 + 32 live registers) to fit 96 registers/thread.
-template <int BN, int EW>
-__device__ __forceinline__ void epilogue_tile(const GemmKernelParams& p, const DropCtx& drop, uint32_t tmem_acc,
-                                              int warp, int lane, int m_base, int n0, int split, uint8_t* stage,
-                                              uint64_t* acc_bar, uint32_t acc_phase) {
+// The 8 epilogue warps (4 .. 11) drain one [128 rows x BN cols] accumulator: warp -> (row quarter, column half),
+// thread -> one row.  All math happens in passes of 32 columns (32 + 32 live registers).
+constexpr int kEpiWarps = 8;
+template <int BN>
+__device__ __forceinline__ void epilogue_tile(const GemmKernelParams& p, const DropCtx& drop, const float* acc,
+                                              int acc_ld, int warp, int lane, int m_base, int n0, int split,
+                                              uint8_t* stage) {
   static_assert(BN == 128 || BN == 256, "tile widths on the path");
-  static_assert(EW == 8 || EW == 16, "epilogue warp counts on the path");
-  constexpr int kColsPerWarp = BN / (EW / 4);                 // 128, 64 or 32
-  constexpr int WT = kColsPerWarp >= 64 ? 64 : 32;            // bf16 staging-tile width (columns)
+  constexpr int kColsPerWarp = BN / 2;                        // 64 or 128
+  constexpr int WT = 64;                                      // bf16 staging-tile width (columns)
   constexpr int CH = WT / 8;                                  // 16-byte chunks per staged bf16 row
-  const int quarter = warp & 3;           // TMEM lane quarter this warp may touch
-  const int cgrp = (warp - 4) >> 2;       // column group
+  const int quarter = warp & 3;           // row quarter
+  const int cgrp = (warp - 4) >> 2;       // column half
   const int row0 = m_base + quarter * 32;
   const int rows_valid = p.M - row0;      // <= 0: nothing to write; >= 32: full tile
   const int m = row0 + lane;
   const int nw = n0 + cgrp * kColsPerWarp;
-  const uint32_t taddr = tmem_acc + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(cgrp * kColsPerWarp);
+  const float* arow = acc + (size_t)(quarter * 32 + lane) * acc_ld + cgrp * kColsPerWarp;
 
   if (p.epilogue == B2_EPI_PARTIAL_F32 || p.epilogue == B2_EPI_RESIDUAL_F32 || p.epilogue == B2_EPI_ACCUM_F32) {
     // ---- fp32 outputs: 32 columns (128 bytes) per group ----
@@ -154,17 +154,14 @@ __device__ __forceinline__ void epilogue_tile(const GemmKernelParams& p, const D
                           p.ld_aux_in * 4, lane, rows_valid);
     };
     prefetch(0);
-    mbar_wait(acc_bar, acc_phase);
-    tc_fence_after();
 #pragma unroll 1
     for (int c = 0; c < kColsPerWarp / 32; ++c) {
       const int n = nw + c * 32;
       uint32_t v[32];
-      tmem_ld32(taddr + c * 32, v);
-      tmem_ld_wait();
+      acc_ld32(arow + c * 32, v);
       if (n < p.N && rows_valid > 0) {
         if (!no_aux) {
-          if (c > 0) prefetch(c);   // group 0 was requested before the accumulator wait
+          if (c > 0) prefetch(c);
           tile_async_wait();
           __syncwarp();
 #pragma unroll
@@ -199,15 +196,13 @@ __device__ __forceinline__ void epilogue_tile(const GemmKernelParams& p, const D
       tile_g2s_async<CH>(stage, reinterpret_cast<const uint8_t*>(p.aux_in + (size_t)row0 * p.ld_aux_in + n),
                          p.ld_aux_in * 2, lane, rows_valid);
   };
-  prefetch(0);   // residual / saved pre-activation tile: independent of the accumulator, fetched under the mainloop
-  mbar_wait(acc_bar, acc_phase);
-  tc_fence_after();
+  prefetch(0);   // residual / saved pre-activation tile
 #pragma unroll 1
   for (int t = 0; t < kColsPerWarp / WT; ++t) {
     const int n = nw + t * WT;
     const bool active = n < p.N && rows_valid > 0;
     if (has_aux && active) {
-      if (t > 0) prefetch(t);   // tile 0 was requested before the accumulator wait
+      if (t > 0) prefetch(t);
       tile_async_wait();
       __syncwarp();
     }
@@ -216,8 +211,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmKernelParams& p, const D
       float f[32];
       {
         uint32_t v[32];
-        tmem_ld32(taddr + t * WT + h * 32, v);   // warp-collective: issued whether or not this warp stores
-        tmem_ld_wait();
+        acc_ld32(arow + t * WT + h * 32, v);
 #pragma unroll
         for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
       }

@@ -3,67 +3,47 @@
 //
 // Why a kernel of its own.
 //  * precision: with separate kernels the pre-LayerNorm sum z and the LayerNorm output both travelled through HBM as
-//    bf16, i.e. the RESIDUAL STREAM was rounded to bf16 four times per layer.  Measured on config A (and reproduced on
-//    the CPU by injecting exactly those roundings into the fp32 oracle): the gradient error of the attention query / key
-//    projections then grows with depth, 1.3e-2 in layer 0 -> 3.1e-2 in layer 11, where stock torch bf16 autocast --
-//    which keeps the stream in fp32 and rounds only GEMM operands -- stays at 1.0-1.4e-2.  Here z never leaves the
-//    SM before it is normalised (fp32 accumulator + fp32 residual -> statistics -> y), the residual comes in as fp32
-//    and the LayerNorm output leaves both as bf16 (the next GEMM's operand) and as fp32 (the next block's residual).
+//    bf16, i.e. the RESIDUAL STREAM was rounded to bf16 four times per layer; the gradient error of the attention
+//    query / key projections then grows with depth, where stock torch bf16 autocast -- which keeps the stream in fp32
+//    and rounds only GEMM operands -- does not.  Here z never leaves the SM before it is normalised (fp32 accumulator
+//    + fp32 residual -> statistics -> y), the residual comes in as fp32 and the LayerNorm output leaves both as bf16
+//    (the next GEMM's operand) and as fp32 (the next block's residual).
 //  * launches: one kernel instead of two per site, 24 sites per step.
-// LayerNorm needs full rows, and a row of 768 / 1024 fp32 accumulators does not fit one CTA's 512 TMEM columns -- so
-// the row is spread over a CLUSTER of PAIRS CTA pairs (tcgen05 cta_group::2, the same 256 x 256 pair tile as
-// gemm2_bf16_kernel): pair p owns columns [256 p, 256 p + 256), all pairs share the same 256 rows; PAIRS = 3 for
-// hidden 768 (cluster of 6), 4 for hidden 1024 (cluster of 8).  (A first version used four 192-wide pairs for hidden
-// 768: measured 15 co-resident 8-CTA clusters on this part, one short of the 16 row blocks of batch 32 x 128 -> two
-// waves, 31 us instead of 16.)
-//
-// Per CTA (128 rows x 256 columns, accumulator in TMEM):
-//   warp 0   TMA producer (this CTA's 128 A rows + its half of the pair's B tile; completion credited to the pair
-//            leader's mbarrier)          warp 1   MMA issuer (pair leader only)         warp 2   TMEM allocator
-//   warps 4-19  epilogue, warp -> (TMEM lane quarter, column group of 64), thread -> one row:
-//     under the mainloop: the warp's fp32 residual tile arrives by TMA, and every thread draws the Philox keep bits of
-//             its 64 elements (they do not depend on the accumulator: ~850 instructions per thread off the tail)
-//     pass 1  z = (acc + bias -> dropout) + residual in fp32, kept in shared memory (the residual tile is overwritten
-//             in place); bf16(z) stored to D for the backward; per-row partial statistics over the warp's 64 columns
-//             (mean, M2 = sum (z - mean)^2) written into the `stats` pad of every CTA that holds the same rows --
-//             distributed shared memory
-//     wait on the CTA's statistics barrier (st.async transaction bytes of all 4 PAIRS partials of its 128 rows)
-//     pass 2  every thread merges the 4 PAIRS partials of its row (Chan's parallel-variance formula: exact two-pass
-//             statistics, no E[x^2] - mean^2 cancellation), normalises its staged z in place, stores y as bf16 and fp32;
-//             mean / rstd (fp32, what the LayerNorm backward reads) are written by the first pair's first column group
-//   Every tile that crosses the SM boundary in the epilogue (fp32 residual in; bf16 z, bf16 y, fp32 y out) is one TMA
-//   box of 32 rows x 128 bytes issued by one lane, in the 128-byte swizzle stage_ptr<8> already uses (an fp32 [M, N]
-//   tensor is described to TMA as bf16 [M, 2N]).  The per-lane cp.async / ld.shared + st.global copies they replace
-//   were ~1 700 of the ~4 200 instructions an epilogue warp issued (ncu, profiles/r02_gemm_ln_epilogue.md), on a
-//   kernel whose tail is issue-bound: four epilogue warps per scheduler.
+// LayerNorm needs full rows, and a row of 768 / 1024 fp32 accumulators does not fit one CTA's registers next to the
+// operand ring -- so the row is spread over a CLUSTER of N / 256 CTAs (3 for hidden 768, 4 for hidden 1024): CTA
+// rank c owns columns [256 c, 256 c + 256) of the cluster's 128 rows and runs the GEMM mainloop of gemm.cu on them
+// (TMA producer warp, two wgmma consumer warpgroups, fp32 tile left in shared memory).  The epilogue then works a
+// row per warp, 8 columns per lane (coalesced global traffic, one Philox call per lane and row):
+//   pass 1  z = (acc + bias -> dropout) + residual in fp32, kept in shared memory in place of the accumulator;
+//           bf16(z) stored to D for the backward; the row's partial statistics over the CTA's 256 columns (mean,
+//           M2 = sum (z - mean)^2) are written into the `stats` pad of every CTA of the cluster (distributed shared
+//           memory), then one cluster barrier
+//   pass 2  every warp merges the partials of its rows (Chan's parallel-variance formula: exact two-pass statistics,
+//           no E[x^2] - mean^2 cancellation), normalises the staged z and stores y as bf16 and fp32; mean / rstd (fp32,
+//           what the LayerNorm backward reads) are written by rank 0
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
-#include "pair.cuh"
 #include "../../include/b2_ddp_bert.h"
 
 namespace b2 {
 
-constexpr int kLnBM = 128, kLnBK = 64, kLnUmmaK = 16;
-constexpr int kLnBN = 256;                       // columns per CTA pair
-constexpr int kLnEW = 16;                        // epilogue warps
-constexpr int kLnThreads = (4 + kLnEW) * 32;     // 640
-// (value-dependent arguments, as in gemm.cu: nvcc rejects __launch_bounds__ next to __maxnreg__ only when both are
-// non-dependent constants)
-template <int PAIRS> constexpr int gemm_ln_threads() { return PAIRS > 0 ? kLnThreads : 0; }
+constexpr int kLnBM = 128, kLnBK = 64, kLnWgmmaK = 16;
+constexpr int kLnBN = 256;                       // columns per CTA
+constexpr int kLnThreads = 384;                  // producer warpgroup + two consumer warpgroups
+constexpr int kLnEpiWarps = 8;                   // warps 4-11
 
-template <int PAIRS>   // CTA pairs per cluster = 256-column tiles per row: 3 (hidden 768) or 4 (hidden 1024)
+template <int CL>   // CTAs per cluster = 256-column tiles per row: 3 (hidden 768) or 4 (hidden 1024)
 struct GemmLnCfg {
-  static constexpr int kCluster = 2 * PAIRS;
-  static constexpr int kABytes = kLnBM * kLnBK * 2;            // this CTA's 128 A rows
-  static constexpr int kBBytes = (kLnBN / 2) * kLnBK * 2;      // this CTA's half of the pair's B tile
-  static constexpr int kStageBytes = kABytes + kBBytes;        // 32 KB
+  static constexpr int kCluster = CL;
+  static constexpr int kABytes = kLnBM * kLnBK * 2;
+  static constexpr int kBBytes = kLnBN * kLnBK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;        // 48 KB
   static constexpr int kStages = 4;
-  static constexpr int kTmemCols = 256;
-  static constexpr int kPipeBytes = kStages * kStageBytes;     // 128 KB: after the last MMA, 8 KB of epilogue scratch per warp
-  static constexpr int kStatsBytes = 4 * PAIRS * kLnBM * 8;    // [pair][column group][row] float2
-  static constexpr int kParamBytes = kLnEW * 3 * 64 * 4;       // per epilogue warp: bias, gamma, beta of its 64 columns, fp32
-  static constexpr int kSmemBytes = kPipeBytes + kLnEW * kEpiStageBytes + kStatsBytes + kParamBytes + 1024 /*align*/ + 512;
-  static_assert(kPipeBytes >= kLnEW * 2 * kEpiStageBytes, "epilogue scratch lives in the drained operand ring");
+  static constexpr int kPipeBytes = kStages * kStageBytes;
+  static constexpr int kAccLd = kLnBN + 4;                     // fp32 row pitch of the accumulator / z tile
+  static constexpr int kStatsBytes = CL * kLnBM * 8;           // [rank][row] float2 (mean, M2)
+  static constexpr int kSmemBytes = kPipeBytes + kStatsBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(kLnBM * kAccLd * 4 <= kPipeBytes, "the accumulator tile lives in the drained operand ring");
 };
 
 struct GemmLnParams {
@@ -76,353 +56,193 @@ struct GemmLnParams {
   __nv_bfloat16* Y; long long ldy;                 // LayerNorm output, bf16 [M, N]: the next GEMM's operand
   float* Yf; long long ldyf;                       // LayerNorm output, fp32 [M, N]: the next block's residual (or null)
   float* mean; float* rstd;                        // fp32 [M]
-  long long* timing;                               // optional [gridDim.x][8] clock64 stamps of the first epilogue warp
 };
-__device__ __forceinline__ void ln_stamp(const GemmLnParams& p, int slot) {
-  if (p.timing != nullptr) p.timing[(size_t)blockIdx.x * 8 + slot] = clock64();
-}
 
 __device__ __forceinline__ void unpack8(const uint4& t, float (&f)[8]) {
   f[0] = bf16_lo(t.x); f[1] = bf16_hi(t.x); f[2] = bf16_lo(t.y); f[3] = bf16_hi(t.y);
   f[4] = bf16_lo(t.z); f[5] = bf16_hi(t.z); f[6] = bf16_lo(t.w); f[7] = bf16_hi(t.w);
 }
 
-template <int PAIRS>
-__global__ void __cluster_dims__(2 * PAIRS, 1, 1) __launch_bounds__(gemm_ln_threads<PAIRS>())
-    __maxnreg__(PAIRS > 0 ? 96 : 64)
+template <int CL>
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(kLnThreads, 1)
 gemm_ln_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-               const __grid_constant__ CUtensorMap tmap_r /* fp32 residual */,
-               const __grid_constant__ CUtensorMap tmap_d /* bf16 z */,
-               const __grid_constant__ CUtensorMap tmap_y /* bf16 y */,
-               const __grid_constant__ CUtensorMap tmap_yf /* fp32 y (unused when p.Yf is null) */,
                const GemmLnParams p) {
-  using Cfg = GemmLnCfg<PAIRS>;
+  using Cfg = GemmLnCfg<CL>;
   constexpr int BN = kLnBN;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align_1024(smem_raw);
-  uint8_t* epi_stage = smem + Cfg::kPipeBytes;
-  float2* stats = reinterpret_cast<float2*>(epi_stage + kLnEW * kEpiStageBytes);
-  float* ptab_all = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(stats) + Cfg::kStatsBytes);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(ptab_all) + Cfg::kParamBytes);
+  float2* stats = reinterpret_cast<float2*>(smem + Cfg::kPipeBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kPipeBytes + Cfg::kStatsBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tmem_full = empty_bar + Cfg::kStages;
-  uint64_t* res_bar = tmem_full + 1;                  // [epilogue warp][residual half]: TMA completion
-  uint64_t* stats_bar = res_bar + 2 * kLnEW;          // transaction barrier: all 4 PAIRS partials of every row are in
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(stats_bar + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const bool stamper = warp == 4 && lane == 0;        // profiling aid (tools/gemm_ln_probe.py --timeline)
-  if (stamper) ln_stamp(p, 0);                        // 0: kernel entry
-  const uint32_t rank = cluster_ctarank();            // 0 .. 2 PAIRS - 1
-  const uint32_t parity = rank & 1u;                  // which 128 of the pair's 256 rows
-  const uint32_t lead_rank = rank & ~1u;              // the pair's leader CTA
-  const bool leader = parity == 0;
-  const int pair = (int)(rank >> 1);                  // column tile of this pair
-  const int row_block = blockIdx.x / Cfg::kCluster;
-  const int m0 = row_block * (2 * kLnBM) + (int)parity * kLnBM;
-  const int n_tile = pair * BN;
+  const uint32_t rank = cluster_ctarank();            // 0 .. CL - 1: column tile of this CTA
+  const int m0 = (blockIdx.x / CL) * kLnBM;
+  const int n_tile = (int)rank * BN;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-    tma_prefetch_desc(&tmap_r);
-    tma_prefetch_desc(&tmap_d);
-    tma_prefetch_desc(&tmap_y);
-    tma_prefetch_desc(&tmap_yf);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kLnEpiWarps);
     }
-    mbar_init(tmem_full, 1);
-    for (int i = 0; i < 2 * kLnEW; ++i) mbar_init(&res_bar[i], 1);
-    mbar_init(stats_bar, 1);
     fence_mbar_init();
-    // armed before the opening cluster barrier, i.e. before any CTA of the cluster can post a partial
-    mbar_expect_tx(stats_bar, (uint32_t)Cfg::kStatsBytes);
   }
-  if (warp == 2) tmem_alloc_2sm(tmem_holder, Cfg::kTmemCols);
-  tc_fence_before();
-  cluster_sync_all();   // barrier inits + TMEM allocation visible cluster-wide; every CTA of the cluster is running
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
+  __syncthreads();
   // PDL: nothing above touches global data
   pdl_wait();
   pdl_launch_dependents();
-  if (stamper) ln_stamp(p, 1);                        // 1: barriers + TMEM set up, cluster running, predecessor done
 
   if (warp == 0) {
-    // ------------------------------ TMA producer (every CTA) ------------------------------
+    // ------------------------------ TMA producer ------------------------------
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
-      const int nb = n_tile + (int)parity * (BN / 2);
       for (int kb = 0; kb < p.kblocks; ++kb) {
         mbar_wait(&empty_bar[stage], phase ^ 1);
-        if (leader) mbar_expect_tx(&full_bar[stage], 2 * Cfg::kStageBytes);
-        const uint32_t bar = mapa_u32(smem_u32(&full_bar[stage]), lead_rank);
+        mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
         uint8_t* sa = smem + stage * Cfg::kStageBytes;
-        uint8_t* sb = sa + Cfg::kABytes;
-        tma_load_2d_2sm(sa, &tmap_a, bar, kb * kLnBK, m0);     // box {64 k, 128 rows}
-        tma_load_2d_2sm(sb, &tmap_b, bar, kb * kLnBK, nb);     // box {64 k, 128 rows}
+        tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * kLnBK, m0);                 // box {64 k, 128 rows}
+        tma_load_2d(sa + Cfg::kABytes, &tmap_b, &full_bar[stage], kb * kLnBK, n_tile);   // box {64 k, 256 rows}
         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
       }
-      // The two ring stages the MMAs release first (those of k-blocks kblocks-4 and kblocks-3) take the second
-      // residual halves of the 16 epilogue warps while the last MMAs still run: issued by the epilogue warps
-      // themselves once the accumulator is complete, these 64 KB of TMA traffic sat in front of pass 1.
-      for (int t = 0; t < 2; ++t) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        for (int e = 8 * t; e < 8 * t + 8; ++e) {      // epilogue warp e: rows q = e & 3, column group e >> 2
-          const int erow0 = m0 + (e & 3) * 32;
-          if (erow0 < p.M) {
-            uint64_t* rb = &res_bar[2 * e + 1];
-            mbar_expect_tx(rb, kEpiStageBytes);
-            tma_load_2d(smem + stage * Cfg::kStageBytes + (e & 7) * kEpiStageBytes, &tmap_r, rb,
-                        2 * (n_tile + (e >> 2) * (BN / 4) + 32), erow0);
-          }
-        }
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer (pair leaders) ------------------------------
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(2 * kLnBM, BN, false, false);
-      const uint16_t pair_mask = (uint16_t)(3u << lead_rank);
-      int stage = 0; uint32_t phase = 0;
-      for (int kb = 0; kb < p.kblocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint32_t sb = sa + Cfg::kABytes;
-#pragma unroll
-        for (int k = 0; k < kLnBK / kLnUmmaK; ++k)
-          umma_bf16_2sm(tmem_base, make_smem_desc(sa + k * kLnUmmaK * 2, 16, 1024),
-                        make_smem_desc(sb + k * kLnUmmaK * 2, 16, 1024), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-        umma_commit_2sm(&empty_bar[stage], pair_mask);
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-      }
-      umma_commit_2sm(tmem_full, pair_mask);
     }
   } else if (warp >= 4) {
-    // ------------------------------ epilogue ------------------------------
-    // warp -> (TMEM lane quarter q, column group cg of 64); thread -> one row.  Three 4 KB tiles per warp:
-    //   zA, zB  fp32, columns [0, 32) / [32, 64) of the warp's block: residual in -> z (fp32, unrounded) -> y (fp32)
-    //   hb      bf16, all 64 columns: z on its way to D, then y on its way to Y
-    // zA is the warp's dedicated staging tile (its residual arrives under the mainloop); zB and hb live in the operand
-    // ring: zB in the two stages released first (filled by the producer warp, above), hb in the two released last;
-    // ring, which is dead once the accumulator barrier has fired (all MMAs complete, every TMA write consumed).
-    constexpr int CW = BN / 4;          // 64 columns per warp
-    const DropCtx drop = make_drop_ctx(p.rng, p.rng_site, p.dropout_p);
-    uint8_t* zA = epi_stage + (warp - 4) * kEpiStageBytes;
-    const int ew = warp - 4;
-    uint8_t* zB = smem + ((p.kblocks + (ew >> 3)) % Cfg::kStages) * Cfg::kStageBytes + (ew & 7) * kEpiStageBytes;
-    uint8_t* hb = smem + ((p.kblocks + 2 + (ew >> 3)) % Cfg::kStages) * Cfg::kStageBytes + (ew & 7) * kEpiStageBytes;
-    const int q = warp & 3, cg = (warp - 4) >> 2;
-    const int row_l = q * 32 + lane;                  // row inside this CTA's 128
-    const int row0 = m0 + q * 32;
-    const int rows_valid = p.M - row0;                // <= 0: nothing of this warp is stored
-    const int m = row0 + lane;
-    const int nw = n_tile + cg * CW;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(cg * CW);
-    const bool active = rows_valid > 0;               // warp-uniform; an inactive warp computes on stale tiles, stores nothing
-    uint64_t* rbarA = &res_bar[2 * (warp - 4)];
-    uint64_t* rbarB = rbarA + 1;
-
-    if (lane == 0 && active) {                        // residual columns [nw, nw + 32): rows past M arrive as zeros
-      mbar_expect_tx(rbarA, kEpiStageBytes);
-      tma_load_2d(zA, &tmap_r, rbarA, 2 * nw, row0);
+    // ------------------------------ wgmma consumers ------------------------------
+    const int wg = (warp - 4) >> 2;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0, prev = -1; uint32_t phase = 0;
+    for (int kb = 0; kb < p.kblocks; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes) + wg * 8192;
+      const uint32_t sb = smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kLnBK / kLnWgmmaK; ++k)
+        wgmma_bf16<BN, 0, 0>(acc, make_smem_desc(sa + k * kLnWgmmaK * 2, 16, 1024),
+                             make_smem_desc(sb + k * kLnWgmmaK * 2, 16, 1024), (kb > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
     }
-    // bias / gamma / beta of the warp's 64 columns, widened to fp32 once per warp (every lane needs the same values:
-    // 2 broadcast LDS.128 per 8 columns instead of an LDG and 8 unpacks, in the two passes that bound this kernel)
-    float* ptab = ptab_all + ew * (3 * 64);
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    named_barrier_sync(1, kLnEpiWarps * 32);   // the ring is dead: the accumulator tile may overwrite it
+    float* zs = reinterpret_cast<float*>(smem);
     {
-      const uint32_t tb = *reinterpret_cast<const uint32_t*>(p.bias + nw + 2 * lane);
-      const uint32_t tg = *reinterpret_cast<const uint32_t*>(p.gamma + nw + 2 * lane);
-      const uint32_t te = *reinterpret_cast<const uint32_t*>(p.beta + nw + 2 * lane);
-      *reinterpret_cast<float2*>(ptab + 2 * lane) = make_float2(bf16_lo(tb), bf16_hi(tb));
-      *reinterpret_cast<float2*>(ptab + 64 + 2 * lane) = make_float2(bf16_lo(tg), bf16_hi(tg));
-      *reinterpret_cast<float2*>(ptab + 128 + 2 * lane) = make_float2(bf16_lo(te), bf16_hi(te));
-    }
-    __syncwarp();
-    // dropout decisions of this thread's 64 elements, drawn while the mainloop runs: bit 8 k + i of keep_lo (k < 4) /
-    // keep_hi (k >= 4) <=> element nw + 8 k + i of row m is kept
-    uint32_t keep_lo = 0, keep_hi = 0;
+      const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      const int c = 2 * (lane & 3);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      keep_lo |= dropout_keep8(drop, (unsigned long long)m * p.N + nw + 8 * k) << (8 * k);
-      keep_hi |= dropout_keep8(drop, (unsigned long long)m * p.N + nw + 32 + 8 * k) << (8 * k);
-    }
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    if (stamper) ln_stamp(p, 2);                      // 2: accumulator complete
-    float sum = 0.f;
-    uint32_t vv[2][16];                 // accumulator columns of step j / j + 1: the next load flies under the math
-    tmem_ld16(taddr, vv[0]);
-#pragma unroll
-    for (int j = 0; j < CW / 16; ++j) {
-      tmem_ld_wait();
-      if (j + 1 < CW / 16) tmem_ld16(taddr + (j + 1) * 16, vv[(j + 1) & 1]);
-      const uint32_t (&v)[16] = vv[j & 1];
-      if (active) {
-        if (j == 0) mbar_wait(rbarA, 0);        // the first residual half has landed
-        else if (j == 2) mbar_wait(rbarB, 0);   // ... and the second
+      for (int j = 0; j < BN / 8; ++j) {
+        *reinterpret_cast<float2*>(zs + (size_t)r * Cfg::kAccLd + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(zs + (size_t)(r + 8) * Cfg::kAccLd + 8 * j + c) =
+            make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
-      uint8_t* zt = j < 2 ? zA : zB;
-      const uint32_t keep_j = (j < 2 ? keep_lo : keep_hi) >> ((j & 1) * 16);
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        const int col = nw + j * 16 + c * 8;
+    }
+    named_barrier_sync(1, kLnEpiWarps * 32);
+
+    // ---- pass 1: warp e takes rows e, e + 8, ...; lane l columns [8 l, 8 l + 8) of the CTA's 256 ----
+    const int ew = warp - 4;
+    const int col = n_tile + 8 * lane;
+    const DropCtx drop = make_drop_ctx(p.rng, p.rng_site, p.dropout_p);
+    float b8[8];
+    unpack8(*reinterpret_cast<const uint4*>(p.bias + col), b8);
+#pragma unroll 1
+    for (int r = ew; r < kLnBM; r += kLnEpiWarps) {
+      const int m = m0 + r;
+      float2 st = make_float2(0.f, 0.f);
+      if (m < p.M) {                                  // warp-uniform
+        float* zr = zs + (size_t)r * Cfg::kAccLd + 8 * lane;
+        const float4 a0 = *reinterpret_cast<const float4*>(zr), a1 = *reinterpret_cast<const float4*>(zr + 4);
+        const float* rp = p.resid + (size_t)m * p.ld_resid + col;
+        const float4 r0 = *reinterpret_cast<const float4*>(rp), r1 = *reinterpret_cast<const float4*>(rp + 4);
+        const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+        const float res[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+        const uint32_t keep = dropout_keep8(drop, (unsigned long long)m * p.N + col);
         float f[8];
-        const float4 bl = *reinterpret_cast<const float4*>(ptab + j * 16 + c * 8);
-        const float4 bh = *reinterpret_cast<const float4*>(ptab + j * 16 + c * 8 + 4);
-        const float b8[8] = {bl.x, bl.y, bl.z, bl.w, bh.x, bh.y, bh.z, bh.w};
-        const uint32_t keep = keep_j >> (c * 8);
-        uint4* r0 = stage_ptr<8>(zt, lane, ((j & 1) * 2 + c) * 2);         // 4 fp32 columns per 16-byte chunk
-        uint4* r1 = stage_ptr<8>(zt, lane, ((j & 1) * 2 + c) * 2 + 1);
-        const uint4 ra = *r0, rb = *r1;
-        const float r[8] = {__uint_as_float(ra.x), __uint_as_float(ra.y), __uint_as_float(ra.z), __uint_as_float(ra.w),
-                            __uint_as_float(rb.x), __uint_as_float(rb.y), __uint_as_float(rb.z), __uint_as_float(rb.w)};
+        float sum = 0.f;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          f[i] = __uint_as_float(v[c * 8 + i]) + b8[i];
-          // (two roundings, as the unfused reference sequence dropout(...) + residual; an FFMA here moves the noisy
-          // query / key gradient norms of bert-large's last layers by more than a percent against the fixture)
-          f[i] = (((keep >> i) & 1u) ? f[i] * drop.scale : 0.f) + r[i];
+          f[i] = a[i] + b8[i];
+          // (two roundings, as the unfused reference sequence dropout(...) + residual)
+          f[i] = (((keep >> i) & 1u) ? f[i] * drop.scale : 0.f) + res[i];
           sum += f[i];
         }
-        *r0 = make_uint4(__float_as_uint(f[0]), __float_as_uint(f[1]), __float_as_uint(f[2]), __float_as_uint(f[3]));
-        *r1 = make_uint4(__float_as_uint(f[4]), __float_as_uint(f[5]), __float_as_uint(f[6]), __float_as_uint(f[7]));
+        *reinterpret_cast<float4*>(zr) = make_float4(f[0], f[1], f[2], f[3]);
+        *reinterpret_cast<float4*>(zr + 4) = make_float4(f[4], f[5], f[6], f[7]);
         uint4 o;
         o.x = pack_bf16(f[0], f[1]); o.y = pack_bf16(f[2], f[3]); o.z = pack_bf16(f[4], f[5]); o.w = pack_bf16(f[6], f[7]);
-        *stage_ptr<8>(hb, lane, j * 2 + c) = o;          // bf16 z for the backward
+        *reinterpret_cast<uint4*>(p.D + (size_t)m * p.ldd + col) = o;          // bf16 z for the backward
+        // partial statistics of the UNROUNDED z over this CTA's 256 columns (two passes over registers)
+        const float mean_l = warp_sum(sum) * (1.0f / BN);
+        float m2 = 0.f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) m2 = fmaf(f[i] - mean_l, f[i] - mean_l, m2);
+        st = make_float2(mean_l, warp_sum(m2));
       }
+      if (lane < CL) st_cluster_f32x2(mapa_u32(smem_u32(&stats[rank * kLnBM + r]), (uint32_t)lane), st.x, st.y);
     }
-    // partial statistics of the UNROUNDED z over this warp's 64 columns: two passes over the staged fp32 row
-    const float mean_l = sum * (1.0f / CW);
-    float m2_l = 0.f;
-#pragma unroll
-    for (int c = 0; c < 16; ++c) {
-      const uint4 t = *stage_ptr<8>(c < 8 ? zA : zB, lane, c & 7);
-      const float d0 = __uint_as_float(t.x) - mean_l, d1 = __uint_as_float(t.y) - mean_l,
-                  d2 = __uint_as_float(t.z) - mean_l, d3 = __uint_as_float(t.w) - mean_l;
-      m2_l = fmaf(d0, d0, m2_l); m2_l = fmaf(d1, d1, m2_l); m2_l = fmaf(d2, d2, m2_l); m2_l = fmaf(d3, d3, m2_l);
-    }
-    {
-      const uint32_t slot = smem_u32(&stats[(pair * 4 + cg) * kLnBM + row_l]);
-#pragma unroll
-      const uint32_t sbar = smem_u32(stats_bar);
-      // st.async: the 8 bytes and their complete_tx on the receiver's barrier travel together -- no release fence (a
-      // MEMBAR.ALL.GPU under barrier.cluster.arrive.release) and no cluster-wide barrier in the middle of the epilogue
-#pragma unroll
-      for (int dp = 0; dp < PAIRS; ++dp) {
-        const uint32_t dst = (uint32_t)(2 * dp) + parity;
-        asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];" ::"r"(
-                         mapa_u32(slot, dst)),
-                     "f"(mean_l), "f"(m2_l), "r"(mapa_u32(sbar, dst))
-                     : "memory");
-      }
-    }
-    fence_proxy_async_smem();          // this lane's staged bf16 z -> visible to the TMA engine
-    __syncwarp();
-    if (lane == 0 && active) {
-      tma_store_2d(&tmap_d, hb, nw, row0);             // rows past M are clipped by the hardware
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    }
-    if (stamper) ln_stamp(p, 3);                      // 3: pass 1 done, partial statistics posted
-    mbar_wait(stats_bar, 0);
-    if (stamper) ln_stamp(p, 4);                      // 4: every partial of this row block has arrived
-    // merge the 4 PAIRS partials of this row (equal counts CW): mean = avg(mean_i), M2 = sum M2_i + CW sum (mean_i - mean)^2
+  }
+  // every partial of every row of the cluster has been posted (release) and is visible (acquire); the producer
+  // warpgroup takes part, as every thread of the cluster must
+  cluster_sync_all();
+  if (warp < 4) return;   // no CTA touches another's shared memory after the barrier: each may exit on its own
+
+  // ---- pass 2 ----
+  const int ew = warp - 4;
+  const int col = n_tile + 8 * lane;
+  float g8[8], e8[8];
+  unpack8(*reinterpret_cast<const uint4*>(p.gamma + col), g8);
+  unpack8(*reinterpret_cast<const uint4*>(p.beta + col), e8);
+  const float* zs = reinterpret_cast<const float*>(smem);
+#pragma unroll 1
+  for (int r = ew; r < kLnBM; r += kLnEpiWarps) {
+    const int m = m0 + r;
+    if (m >= p.M) break;                              // rows ascend: the rest of this warp's rows are past M too
+    // merge the CL partials of this row (equal counts BN): mean = avg(mean_i), M2 = sum M2_i + BN sum (mean_i - mean)^2
     float mean = 0.f;
 #pragma unroll
-    for (int i = 0; i < 4 * PAIRS; ++i) mean += stats[i * kLnBM + row_l].x;
-    mean *= 1.0f / (4 * PAIRS);
+    for (int i = 0; i < CL; ++i) mean += stats[i * kLnBM + r].x;
+    mean *= 1.0f / CL;
     float m2 = 0.f;
 #pragma unroll
-    for (int i = 0; i < 4 * PAIRS; ++i) {
-      const float2 t = stats[i * kLnBM + row_l];
+    for (int i = 0; i < CL; ++i) {
+      const float2 t = stats[i * kLnBM + r];
       const float d = t.x - mean;
-      m2 += t.y + (float)CW * d * d;
+      m2 += t.y + (float)BN * d * d;
     }
     const float rstd = rsqrtf(m2 / (float)p.N + p.eps);
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // hb has been read out (z -> D)
-    __syncwarp();
-#pragma unroll 1
-    for (int c = 0; c < 8; ++c) {          // 8 columns per step: two fp32 chunks, one bf16 chunk
-      if (c == 4) {                        // first fp32 half finished: on its way while the second is normalised
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0 && active && p.Yf != nullptr) {
-          tma_store_2d(&tmap_yf, zA, 2 * nw, row0);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-      }
-      const int col = nw + c * 8;
-      uint8_t* zt = c < 4 ? zA : zB;
-      const float4 gl = *reinterpret_cast<const float4*>(ptab + 64 + c * 8);
-      const float4 gh = *reinterpret_cast<const float4*>(ptab + 64 + c * 8 + 4);
-      const float4 el = *reinterpret_cast<const float4*>(ptab + 128 + c * 8);
-      const float4 eh = *reinterpret_cast<const float4*>(ptab + 128 + c * 8 + 4);
-      const float g[8] = {gl.x, gl.y, gl.z, gl.w, gh.x, gh.y, gh.z, gh.w};
-      const float b[8] = {el.x, el.y, el.z, el.w, eh.x, eh.y, eh.z, eh.w};
-      uint4* r0 = stage_ptr<8>(zt, lane, (c & 3) * 2);
-      uint4* r1 = stage_ptr<8>(zt, lane, (c & 3) * 2 + 1);
-      const uint4 ra = *r0, rb = *r1;
-      float f[8] = {__uint_as_float(ra.x), __uint_as_float(ra.y), __uint_as_float(ra.z), __uint_as_float(ra.w),
-                    __uint_as_float(rb.x), __uint_as_float(rb.y), __uint_as_float(rb.z), __uint_as_float(rb.w)};
+    const float* zr = zs + (size_t)r * Cfg::kAccLd + 8 * lane;
+    const float4 z0 = *reinterpret_cast<const float4*>(zr), z1 = *reinterpret_cast<const float4*>(zr + 4);
+    float f[8] = {z0.x, z0.y, z0.z, z0.w, z1.x, z1.y, z1.z, z1.w};
 #pragma unroll
-      for (int i = 0; i < 8; ++i) f[i] = (f[i] - mean) * rstd * g[i] + b[i];
-      *r0 = make_uint4(__float_as_uint(f[0]), __float_as_uint(f[1]), __float_as_uint(f[2]), __float_as_uint(f[3]));
-      *r1 = make_uint4(__float_as_uint(f[4]), __float_as_uint(f[5]), __float_as_uint(f[6]), __float_as_uint(f[7]));
-      uint4 o;
-      o.x = pack_bf16(f[0], f[1]); o.y = pack_bf16(f[2], f[3]); o.z = pack_bf16(f[4], f[5]); o.w = pack_bf16(f[6], f[7]);
-      *stage_ptr<8>(hb, lane, c) = o;
+    for (int i = 0; i < 8; ++i) f[i] = (f[i] - mean) * rstd * g8[i] + e8[i];
+    uint4 o;
+    o.x = pack_bf16(f[0], f[1]); o.y = pack_bf16(f[2], f[3]); o.z = pack_bf16(f[4], f[5]); o.w = pack_bf16(f[6], f[7]);
+    *reinterpret_cast<uint4*>(p.Y + (size_t)m * p.ldy + col) = o;
+    if (p.Yf != nullptr) {
+      float* yf = p.Yf + (size_t)m * p.ldyf + col;
+      *reinterpret_cast<float4*>(yf) = make_float4(f[0], f[1], f[2], f[3]);
+      *reinterpret_cast<float4*>(yf + 4) = make_float4(f[4], f[5], f[6], f[7]);
     }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (stamper) ln_stamp(p, 5);                      // 5: pass 2 done
-    if (pair == 0 && cg == 0 && lane < rows_valid) {
+    if (rank == 0 && lane == 0) {
       p.mean[m] = mean;
       p.rstd[m] = rstd;
     }
-    if (lane == 0 && active) {
-      tma_store_2d(&tmap_y, hb, nw, row0);
-      if (p.Yf != nullptr) tma_store_2d(&tmap_yf, zB, 2 * (nw + 32), row0);
-      // the tiles stay put until the engine has read them; the writes themselves complete with the grid (what the next
-      // kernel's griddepcontrol.wait / stream order observes), as with plain st.global
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    }
-    // closing cluster barrier, split around the TMA drain: it carries no data (every st.async this CTA is owed has
-    // landed before pass 2, every commit before that) -- it only keeps each CTA's shared memory and TMEM alive while a
-    // partner may still touch them, so the arrive needs no release fence and its latency overlaps the tile reads
-    tc_fence_before();
-    __syncwarp();
-    asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");
-    if (lane == 0 && active) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    __syncwarp();
-    if (stamper) ln_stamp(p, 6);                      // 6: output tiles read out of shared memory
-  }
-  if (warp < 4) {      // producer, MMA issuer, allocator, spare: straight to the closing barrier
-    tc_fence_before();
-    __syncwarp();
-    asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");
-  }
-  // no CTA may exit (or free TMEM) while a partner can still multicast-commit into it or write its stats pad
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-  if (stamper) ln_stamp(p, 7);                        // 7: whole cluster drained
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, Cfg::kTmemCols);
   }
 }
 
-template <int PAIRS>
+template <int CL>
 static int32_t gemm_ln_prepare() {
   static int state = 0;    // 0 = not yet, 1 = ready, -1 = failed
   if (state == 0) {
-    auto kern = gemm_ln_kernel<PAIRS>;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmLnCfg<PAIRS>::kSmemBytes) !=
+    auto kern = gemm_ln_kernel<CL>;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmLnCfg<CL>::kSmemBytes) !=
         cudaSuccess) {
       (void)cudaGetLastError();
       state = -1;
@@ -433,54 +253,40 @@ static int32_t gemm_ln_prepare() {
   return state;
 }
 
-template <int PAIRS>
+template <int CL>
 static int32_t gemm_ln_max_clusters() {
-  if (gemm_ln_prepare<PAIRS>() != 1) return 0;
+  if (gemm_ln_prepare<CL>() != 1) return 0;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(GemmLnCfg<PAIRS>::kCluster);
+  cfg.gridDim = dim3(GemmLnCfg<CL>::kCluster);
   cfg.blockDim = dim3(kLnThreads);
-  cfg.dynamicSmemBytes = GemmLnCfg<PAIRS>::kSmemBytes;
+  cfg.dynamicSmemBytes = GemmLnCfg<CL>::kSmemBytes;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = GemmLnCfg<PAIRS>::kCluster;
+  attr[0].val.clusterDim.x = GemmLnCfg<CL>::kCluster;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, gemm_ln_kernel<PAIRS>, &cfg) != cudaSuccess) {
+  if (cudaOccupancyMaxActiveClusters(&n, gemm_ln_kernel<CL>, &cfg) != cudaSuccess) {
     (void)cudaGetLastError();
     return 0;
   }
   return n;
 }
 
-template <int PAIRS>
+template <int CL>
 static int32_t launch_gemm_ln(const b2_gemm_args_t& a, const void* gamma, const void* beta, float eps, void* y,
                               int64_t ldy, float* y_f32, int64_t ldyf, float* mean, float* rstd,
                               cudaStream_t stream) {
-  using Cfg = GemmLnCfg<PAIRS>;
-  B2_REQUIRE(gemm_ln_prepare<PAIRS>() == 1, "b2_gemm_ln_fwd: cannot reserve %d bytes of shared memory",
+  using Cfg = GemmLnCfg<CL>;
+  B2_REQUIRE(gemm_ln_prepare<CL>() == 1, "b2_gemm_ln_fwd: cannot reserve %d bytes of shared memory",
              Cfg::kSmemBytes);
   CUtensorMap ta, tb;
   int32_t st = get_tensor_map_2d(&ta, a.A, (uint64_t)a.M, (uint64_t)a.K, (uint64_t)a.lda * 2, kLnBM, 64);
   if (st) return st;
-  st = get_tensor_map_2d(&tb, a.B, (uint64_t)a.N, (uint64_t)a.K, (uint64_t)a.ldb * 2, kLnBN / 2, 64);
+  st = get_tensor_map_2d(&tb, a.B, (uint64_t)a.N, (uint64_t)a.K, (uint64_t)a.ldb * 2, kLnBN, 64);
   if (st) return st;
-  // epilogue tiles: boxes of 32 rows x 128 bytes (64 bf16 / 32 fp32 columns; fp32 tensors as bf16 [M, 2 N])
-  CUtensorMap tr, td, ty, tyf;
-  st = get_tensor_map_2d(&tr, a.aux_in, (uint64_t)a.M, (uint64_t)a.N * 2, (uint64_t)a.ld_aux_in * 4, 32, 64);
-  if (st) return st;
-  st = get_tensor_map_2d(&td, a.D, (uint64_t)a.M, (uint64_t)a.N, (uint64_t)a.ldd * 2, 32, 64);
-  if (st) return st;
-  st = get_tensor_map_2d(&ty, y, (uint64_t)a.M, (uint64_t)a.N, (uint64_t)ldy * 2, 32, 64);
-  if (st) return st;
-  if (y_f32 != nullptr) {
-    st = get_tensor_map_2d(&tyf, y_f32, (uint64_t)a.M, (uint64_t)a.N * 2, (uint64_t)ldyf * 4, 32, 64);
-    if (st) return st;
-  } else {
-    tyf = tr;
-  }
   GemmLnParams p;
   p.M = (int)a.M; p.N = (int)a.N; p.kblocks = (int)((a.K + kLnBK - 1) / kLnBK);
   p.D = (__nv_bfloat16*)a.D; p.ldd = a.ldd;
@@ -489,9 +295,8 @@ static int32_t launch_gemm_ln(const b2_gemm_args_t& a, const void* gamma, const 
   p.dropout_p = a.dropout_p; p.rng = (const unsigned long long*)a.rng_state; p.rng_site = a.rng_site;
   p.gamma = (const __nv_bfloat16*)gamma; p.beta = (const __nv_bfloat16*)beta; p.eps = eps;
   p.Y = (__nv_bfloat16*)y; p.ldy = ldy; p.Yf = y_f32; p.ldyf = ldyf; p.mean = mean; p.rstd = rstd;
-  p.timing = (long long*)a.debug_timing;
-  const int row_blocks = (int)((a.M + 2 * kLnBM - 1) / (2 * kLnBM));
-  B2_LAUNCH(gemm_ln_kernel<PAIRS>, Cfg::kCluster * row_blocks, kLnThreads, Cfg::kSmemBytes, stream, ta, tb, tr, td, ty, tyf, p);
+  const int row_blocks = (int)((a.M + kLnBM - 1) / kLnBM);
+  B2_LAUNCH(gemm_ln_kernel<CL>, Cfg::kCluster * row_blocks, kLnThreads, Cfg::kSmemBytes, stream, ta, tb, p);
   B2_CUDA(cudaGetLastError());
   count_launches(1);
   return 0;

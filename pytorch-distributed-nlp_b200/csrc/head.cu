@@ -147,8 +147,8 @@ __global__ void __launch_bounds__(256) ce_fwd_bwd_kernel(const float* __restrict
 // ---- backward ----
 // k1: one thread per (b, j): dpd = sum_c dlogits[b,c] Wc[c,j] -> d_pooled = mask*scale*dpd -> d_pre = d_pooled*(1 -
 //     pooled^2) (fp32 scratch [batch, H]); also pm[b,j] = dropout(pooled)[b,j] (second fp32 scratch plane) for k1b.
-//     grid = (ceil(H/256), batch).  (A first version looped over the batch inside 3 blocks: 28 us of pure latency at
-//     the head of the backward critical path.)
+//     grid = (ceil(H/256), batch).  (Looping over the batch inside a few blocks is pure latency at the head of the
+//     backward critical path.)
 __global__ void __launch_bounds__(256) head_bwd_k1(const float* __restrict__ dlogits,
                                                   const __nv_bfloat16* __restrict__ pooled, int batch, int H,
                                                   const __nv_bfloat16* __restrict__ Wc, int C, float dropout_p,

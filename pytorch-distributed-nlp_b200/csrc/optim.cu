@@ -94,21 +94,15 @@ __global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWPara
 }
 
 // ---- single-GPU background form ------------------------------------------------------------------------------------
-// Measured (B2_DEBUG_SKIP_ADAMW): on one GPU the 0.49 ms of optimizer kernels are exposed almost in full, although they
-// run on their own stream under the backward pass -- a 256-thread x 64-register block cannot become resident on an SM
-// whose 64 K registers are held by a 640-thread x 96-register GEMM CTA (61 440), so the update only ever runs in the
-// gaps between GEMM kernels.  This variant is shaped to fit BESIDE such a CTA: 128 threads x 32 registers = the 4 096
-// registers that are left, no shared memory, and the same shared-memory carve-out preference as the GEMM kernels
-// (an SM is not re-partitioned while it has resident CTAs).  Blocks are short-lived (8 vectors of 4 elements per
-// thread) so they never hold an SM back from a kernel that needs all of it (the attention kernels).  Same arithmetic,
-// statement for statement, as reduce_adamw_kernel with world == 1; the bias-corrected step size is computed once per
-// step by adamw_prepare_kernel (double pow, as the host would) instead of in every block.
-// Measured (tools/coresidency_probe.py: a GEMM loop on one stream, the update of all 102 M parameters on another):
-// the blocks do become co-resident, but one 128-thread block per SM keeps only ~7 KB in flight: 27 % of the update
-// hides under the GEMMs (the 256-thread form: none -- it even costs 20 % more than running the two back to back);
-// in the training step +1.2 % (7 987 -> 8 085 samples/s).  Asking the L2 for the operands of a later block first
-// (cp.async.bulk.prefetch.L2, no registers held) was tried and measured worse (19 % hidden): the co-resident blocks are
-// bound by the latency of their own dependent load -> sqrt -> divide -> store chain, not by HBM queue depth.
+// On one GPU the optimizer kernels run on their own stream under the backward pass, but a 256-thread x 64-register
+// block cannot become resident on an SM whose registers are held by a GEMM CTA, so the update only runs in the gaps
+// between GEMM kernels.  This variant is shaped to fit beside such a CTA: 128 threads x 32 registers, no shared
+// memory, and the same shared-memory carve-out preference as the GEMM kernels (an SM is not re-partitioned while it
+// has resident CTAs).  Blocks are short-lived (8 vectors of 4 elements per thread) so they never hold an SM back from
+// a kernel that needs all of it (the attention kernels).  Same arithmetic, statement for statement, as
+// reduce_adamw_kernel with world == 1; the bias-corrected step size is computed once per step by adamw_prepare_kernel
+// (double pow, as the host would) instead of in every block.  The co-resident blocks are bound by the latency of their
+// own dependent load -> sqrt -> divide -> store chain, not by HBM queue depth.
 struct SlimParams {
   const __nv_bfloat16* grads; __nv_bfloat16* shadow;
   float* master; float* m; float* v;
@@ -268,7 +262,7 @@ extern "C" int32_t b2_bucket_reduce_adamw(const void* const* peer_grads, void* c
   p.skip = hp->skip_flags;
   const long long nvec = (end - begin) >> 3;
   long long blocks = (nvec + 255) / 256;
-  const long long cap = 148 * 8;
+  const long long cap = 132 * 8;   // 8 blocks per SM of an H100
   if (blocks > cap) blocks = cap;
   B2_LAUNCH(reduce_adamw_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream_, p);
   B2_CUDA(cudaGetLastError());

@@ -170,9 +170,8 @@ class DistributedDataParallel(nn.Module):
             self._slices = self._make_slices()
             # staging for the DMA form of the exchange: my slice of every bucket as held by each peer
             # transport form of the exchange: the fused peer-HBM kernel (default) or copy-engine DMA + local reduce.
-            # Round 1 measured the DMA form ahead (60.0 k vs 58.7 k samples/s on 8 B200); with the step body on a
-            # high-priority stream the exchange kernels no longer hold SMs the GEMM chain is waiting for, and the
-            # kernel form wins clearly: 66.0 k vs 54.6 k samples/s on 8 B200 (config A), 14.4 k vs 11.9 k (config C)
+            # With the step body on a high-priority stream the exchange kernels do not hold SMs the GEMM chain is
+            # waiting for, which favours the kernel form; B2_DDP_DMA=1 selects the copy-engine form (A/B switch)
             self.dma = os.environ.get("B2_DDP_DMA", "0") == "1"
             self._stage_off, off = [], 0
             for (sb, se) in self._slices:

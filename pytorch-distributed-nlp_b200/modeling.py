@@ -1,4 +1,4 @@
-"""Drop-in ``BertForSequenceClassification`` whose forward/backward run on the sm_100a kernels of libb2ddpbert.so.
+"""Drop-in ``BertForSequenceClassification`` whose forward/backward run on the sm_90a kernels of libb2ddpbert.so.
 
 Mirrors the surface `multi-gpu-distributed-cls.py` uses (reference lines in brackets):
   * ``BertConfig(..., num_labels=6)`` / ``BertForSequenceClassification.from_pretrained(path, config=config)`` [:336-338]
@@ -457,19 +457,18 @@ class _Engine:
         self.opt_stream = torch.cuda.Stream(device=self.dev)
         self.accum_dgrad = os.environ.get("B2_ACCUM_DGRAD", "1") != "0"
         self.grouped_wgrad = os.environ.get("B2_GROUPED_WGRAD", "1") != "0"
-        # experimental, off: measured 4.17 ms/step vs 3.94 with the separate per-bucket AdamW launches -- the epilogue's
-        # optimizer-state round trips (one 4 KB staging tile per warp) keep too few bytes in flight; see DESIGN.md 4.3
+        # experimental, off: the epilogue's optimizer-state round trips (one 4 KB staging tile per warp) keep too few
+        # bytes in flight to beat the separate per-bucket AdamW launches; see DESIGN.md
         self.fused_adamw = os.environ.get("B2_FUSED_ADAMW", "0") == "1"
         self.fused_adamw_active = False
         # cache of the forward's attention-dropout decisions for the backward (1 bit per (b, h, q, k), bit-exact against
-        # the Philox replica): neutral in round 1 (3.96 vs 3.95 ms/step), +1.4 % now that the step body runs on a
-        # high-priority stream (8 232 vs 8 117 samples/s, two A/B pairs in one run) -> on by default, B2_ATTN_KEEP_BITS=0
-        # regenerates the masks in the backward instead
+        # the Philox replica): the backward reads them instead of regenerating Philox; B2_ATTN_KEEP_BITS=0 regenerates
+        # the masks in the backward instead
         self.attn_keep_bits = os.environ.get("B2_ATTN_KEEP_BITS", "1") != "0"
         self.use_wgrad_stream = os.environ.get("B2_WGRAD_STREAM", "1") != "0"
         # dense + bias + dropout + residual + LayerNorm as ONE cluster kernel (b2_gemm_ln_fwd) for the two N = hidden
         # GEMMs of a layer, when the hidden size has a row-cluster tiling (768, 1024) and the device can co-schedule
-        # the 8-CTA clusters; otherwise (and with B2_FUSED_LN=0) the GEMM epilogue + separate LayerNorm launch
+        # the 3- / 4-CTA clusters; otherwise (and with B2_FUSED_LN=0) the GEMM epilogue + separate LayerNorm launch
         self.fused_ln = (os.environ.get("B2_FUSED_LN", "1") != "0" and self.H in (768, 1024) and
                          int(L.load().b2_gemm_ln_max_clusters(self.H)) > 0)
         # fp32 accumulators for the bias gradients that kernels produce as a side effect of their epilogues (QKV bias

@@ -100,17 +100,15 @@ class AdamW(torch.optim.Optimizer):
     # ---- pipelined update (FusedTrainStep / PackedTrainStep on one GPU) ------------------------------------------------
     def enable_pipelining(self):
         """Called by the captured train steps.  Measured (B2_DEBUG_SKIP_ADAMW): launched under the backward pass, the
-        0.49 ms of optimizer kernels are exposed almost in full -- the backward keeps every SM busy with GEMM CTAs that
-        own the whole register file.  The forward pass does not: its two dense + LayerNorm launches per layer occupy 96
-        of the 148 SMs.  So the update of step i is applied at the beginning of step i + 1: bucket by bucket in FORWARD
+        optimizer kernels are exposed almost in full -- the backward keeps every SM busy with GEMM CTAs that own the
+        whole register file.  The forward pass does not: its two dense + LayerNorm launches per layer leave SMs idle.  So the update of step i is applied at the beginning of step i + 1: bucket by bucket in FORWARD
         order on the optimizer stream (lowest priority), layer l of the forward waiting only for bucket l's event.
         Nothing is skipped: every captured step applies one full update (the previous step's), `state_dict()`, an eager
         forward, an evaluation step and `optimizer.step()` first flush what is pending, and the arithmetic (operands,
         order, step count) is exactly that of the unpipelined step."""
         model = self._model
-        # Measured (config A, one B200): 8 013 samples/s pipelined vs 8 123 unpipelined -- under the forward the update
-        # time-slices with the GEMM CTAs just as it does under the backward, and a layer that has to wait for its
-        # bucket's event stalls the critical path.  Correct (tests/test_model.py::test_pipelined_adamw_is_the_same_
+        # Under the forward the update time-slices with the GEMM CTAs just as it does under the backward, and a layer
+        # that has to wait for its bucket's event stalls the critical path.  Correct (tests/test_model.py::test_pipelined_adamw_is_the_same_
         # training run) but slower: opt-in only (B2_PIPELINED_ADAMW=1).
         if (os.environ.get("B2_PIPELINED_ADAMW", "0") != "1" or model._ddp is not None or self._amp_seen or
                 getattr(model._engine, "fused_adamw", False)):

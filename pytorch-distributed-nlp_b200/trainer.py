@@ -1,4 +1,4 @@
-"""The reference's ``Trainer`` / ``Args`` surface (multi-gpu-distributed-cls.py:113-257) on the B200 step.
+"""The reference's ``Trainer`` / ``Args`` surface (multi-gpu-distributed-cls.py:113-257) on the H100 step.
 
 Same methods, same argument meaning: ``on_step`` [:126-137], ``loss_reduce`` [:139-143], ``output_reduce`` [:145-155],
 ``train`` [:157-197], ``dev`` [:199-220], ``test`` [:222-239].  Differences, all on the hot path's periphery:
@@ -71,8 +71,7 @@ class _StagedGraphStep:
         self._h2d_done = None
         # The step body -- the critical chain of forward / dgrad kernels -- is issued (and captured) on a HIGH-priority
         # stream, so that when an SM frees up the block scheduler hands it to the critical path before the
-        # weight-gradient / optimizer streams (default, i.e. lowest, priority): measured 7 990 -> 8 093 samples/s on
-        # config A.  B2_STEP_PRIORITY=0 restores the plain current stream (A/B switch).
+        # weight-gradient / optimizer streams (default, i.e. lowest, priority).  B2_STEP_PRIORITY=0 restores the plain current stream (A/B switch).
         self._prio_stream = None
         if os.environ.get("B2_STEP_PRIORITY", "1") != "0":
             self._prio_stream = torch.cuda.Stream(device=dev, priority=-1)

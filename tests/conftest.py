@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a GPU machine)")
     # the C-ABI library is built in-tree; build it if a checkout has none yet (nvcc cross-compiles without a GPU)
     # CPU oracle runs: a container that shows 100+ CPUs but is throttled to a few thrashes when torch spawns one thread
     # per visible CPU -- use the affinity mask capped by the cgroup quota (oracle/cpu_step.usable_cores)

@@ -1,10 +1,10 @@
-"""Context number (SURVEY.md §8d, last row): the reference's loop body in stock torch eager on ONE B200 -- HF
+"""Context number (SURVEY.md §8d, last row): the reference's loop body in stock torch eager on ONE GPU -- HF
 BertForSequenceClassification (eager attention, as transformers 4.28.1 computes it), the restated HF AdamW run the
 way the original runs it (a python loop of per-tensor ops), cuBLAS/cuDNN kernels, no graph.  Three precisions:
 fp32 (what multi-gpu-distributed-cls.py runs), TF32 matmuls, bf16 autocast (what the -amp scripts run, minus the
 GradScaler).  NOT a pytest module (no test_ prefix), not part of bench.py's contract; run it by hand:
 
-    gpurun -- 'python tests/context_torch_eager.py > gpurun_out/torch_eager.json'
+    python tests/context_torch_eager.py > torch_eager.json
 
 Lives under tests/ because it drives oracle/ code (test infrastructure); nothing in the product imports it.
 """
@@ -54,7 +54,7 @@ def run(mode):
 
 
 if __name__ == "__main__":
-    res = {"what": "stock torch-eager HF BERT-base step on one B200 (context, SURVEY 8d)", "batch": BATCH, "seq": SEQ,
+    res = {"what": "stock torch-eager HF BERT-base step on one GPU (context, SURVEY 8d)", "batch": BATCH, "seq": SEQ,
            "steps": STEPS, "warmup": WARM, "torch": torch.__version__, "runs": [run(m) for m in
                                                                               ("fp32", "tf32", "bf16_autocast")]}
     print(json.dumps(res))

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM through the C ABI vs a torch fp32 matmul of the same bf16 operands (GPU)."""
+"""wgmma GEMM through the C ABI vs a torch fp32 matmul of the same bf16 operands (GPU)."""
 import pytest
 import torch
 
@@ -41,7 +41,8 @@ def _check(got, ref, tol=2e-2):
     assert err <= tol * scale, "max err %.4g vs scale %.4g" % (err, scale)
 
 
-# (kernel, bn): 1 = single-CTA 128 x bn tiles, 2 = CTA-pair (cta_group::2) 256 x bn tiles
+# (kernel, bn): force_kernel is a kernel choice of the ABI; this build has one GEMM kernel (128 x bn tiles), so both
+# values must give the same results
 KERNELS = [(1, 128), (1, 256), (2, 128), (2, 256)]
 
 
@@ -79,7 +80,7 @@ def test_tn_wgrad(cuda_dev, kernel, bn, splits):
 
 
 def test_pair_kernel_many_tiles_per_pair(cuda_dev):
-    """persistent loop + TMEM double buffering of the CTA-pair kernel: 16 x 12 = 192 tiles over 74 pairs"""
+    """more tiles than SMs: 32 x 12 = 384 tiles of 128 x 256 over 132 SMs"""
     M, N, K = 4096, 3072, 768
     torch.manual_seed(8)
     A, B, bias = _rand((M, K), cuda_dev), _rand((N, K), cuda_dev, 0.05), _rand((N,), cuda_dev)
@@ -285,12 +286,12 @@ def test_grouped_weight_gradients_with_fused_adamw(cuda_dev):
                                    (1000, 768, 768), (200, 1024, 136), (8192, 768, 768)])
 @pytest.mark.parametrize("p", [0.0, 0.1])
 def test_gemm_layernorm_cluster_kernel(cuda_dev, shape, p):
-    """b2_gemm_ln_fwd: dense + bias + dropout + fp32 residual + LayerNorm over a cluster of N / 256 CTA pairs (row
+    """b2_gemm_ln_fwd: dense + bias + dropout + fp32 residual + LayerNorm over a cluster of N / 256 CTAs (row
     statistics through distributed shared memory) vs torch fp32 on the same operands and the same Philox mask:
       D     == bf16 of the fp32 sum z (what the backward reads)               -- to one bf16 rounding
       y_f32 == LayerNorm(z) computed from the UNROUNDED z                     -- to fp32 summation-order accuracy
       y     == bf16(y_f32) exactly;  mean / rstd of the unrounded z
-    Covers both cluster shapes (N = 768 -> 3 pairs, N = 1024 -> 4 pairs), K = 768..4096, a ragged last row block, a K
+    Covers both cluster shapes (N = 768 -> 3 CTAs, N = 1024 -> 4 CTAs), K = 768..4096, a ragged last row block, a K
     tail, and more row blocks than clusters fit at once (M = 8192)."""
     M, N, K = shape
     dev = cuda_dev

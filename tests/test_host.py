@@ -230,11 +230,11 @@ def test_fused_adamw_skip_flags_cover_exactly_the_encoder_matrices():
                                                           2 * cfg.hidden_size * cfg.intermediate_size)
 
 
-def test_sass_carries_tcgen05_tmem_and_tma():
-    """what the compiler actually emitted for sm_100a (cuobjdump -sass of the in-tree library): the GEMM and attention
-    kernels issue tcgen05.mma (UTCHMMA), drain TMEM with tcgen05.ld (LDTM), commit to mbarriers (UTCBAR), allocate TMEM
-    (UTCATOMSWS) and move tiles with TMA (UTMALDG; UTMASTG for the attention stores); the CTA-pair kernels synchronise
-    the cluster (UCGABAR_*).  mma.sync / wgmma-era mnemonics (HMMA) must not appear in them."""
+def test_sass_carries_wgmma_and_tma():
+    """what the compiler actually emitted for sm_90a (cuobjdump -sass of the in-tree library): the GEMM and attention
+    kernels issue warpgroup MMAs (HGMMA), move tiles with TMA (UTMALDG; UTMASTG for the attention stores) and wait on
+    mbarriers (SYNCS); the LayerNorm-fused GEMM synchronises its cluster (UCGABAR_*).  mma.sync (HMMA) must not appear
+    in them."""
     import shutil
     import subprocess
     exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
@@ -256,14 +256,13 @@ def test_sass_carries_tcgen05_tmem_and_tma():
         assert hit, "no kernel matching %s in the library" % fragment
         return hit
 
-    for frag in ("gemm2_bf16_kernel", "gemm_bf16_kernel", "gemm2_grouped_tn_kernel"):
+    for frag in ("gemm_bf16_kernel", "gemm_grouped_tn_kernel", "gemm_ln_kernel"):
         for o in ops(frag):
-            assert {"UTCHMMA", "UTMALDG", "LDTM", "UTCBAR", "UTCATOMSWS"} <= o, (frag, sorted(o))
+            assert {"HGMMA", "UTMALDG", "SYNCS"} <= o, (frag, sorted(o))
             assert "HMMA" not in o
-    for frag in ("gemm2_bf16_kernel", "gemm2_grouped_tn_kernel"):
-        for o in ops(frag):
-            assert "UCGABAR_ARV" in o and "UCGABAR_WAIT" in o          # cta_group::2 pairs
+    for o in ops("gemm_ln_kernel"):
+        assert "UCGABAR_ARV" in o and "UCGABAR_WAIT" in o
     for frag in ("attention_fwd_kernel", "attention_fwd128_kernel", "attention_bwd_kernel"):
         for o in ops(frag):
-            assert {"UTCHMMA", "UTMALDG", "UTMASTG", "LDTM", "UTCBAR"} <= o, (frag, sorted(o))
+            assert {"HGMMA", "UTMALDG", "UTMASTG", "SYNCS"} <= o, (frag, sorted(o))
             assert "HMMA" not in o

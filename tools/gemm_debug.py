@@ -1,4 +1,4 @@
-"""Diagnostics for the tcgen05 GEMM (run on the GPU box when a test_gemm case fails): per-layout error statistics and
+"""Diagnostics for the wgmma GEMM (run on the GPU box when a test_gemm case fails): per-layout error statistics and
 a k-slice probe (A non-zero only in one 16-wide k-step) that localises descriptor / swizzle mistakes."""
 import sys
 import os

@@ -1,12 +1,12 @@
-"""Summarises an `ncu --csv` metric log of one training step into per-kernel evidence (profiles/rNN_ncu_counters.json):
-tensor-pipe utilisation for the tcgen05 kernels, DRAM bytes and achieved GB/s for the memory-bound ones.
+"""Summarises an `ncu --csv` metric log of one training step into per-kernel evidence (JSON on stdout):
+tensor-pipe utilisation for the wgmma kernels, DRAM bytes and achieved GB/s for the memory-bound ones.
 
     ncu --metrics gpu__time_duration.sum,sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_elapsed,\\
 sm__pipe_tensor_subpipe_hmma_cycles_active.avg.pct_of_peak_sustained_elapsed,\\
 sm__ops_path_tensor_op_hmma_src_bf16_dst_fp32.sum,dram__bytes_read.sum,dram__bytes_write.sum \\
         --clock-control none -s <first launch of the step> -c <launches per step> --csv --log-file counters.csv \\
         python tools/profile_step.py 3
-    python tools/ncu_counters.py counters.csv [peaks.json] > profiles/r02_ncu_counters.json
+    python tools/ncu_counters.py counters.csv [peaks.json] > ncu_counters.json
 Times under ncu are cold-cache and serialised: shares and per-launch counters are the evidence, not the absolute step.
 """
 import csv
