@@ -171,6 +171,10 @@ int32_t b2_colsum(const void* x, int64_t rows, int64_t cols, int64_t ldx, void* 
 /*   qkv  bf16 [batch*seq, 3*hidden]  (Q | K | V column blocks, heads of 64 inside each)                    */
 /*   mask int64 [batch, seq] of {0,1} as produced by the reference Collate, or NULL (= all ones)            */
 /*   ctx  bf16 [batch*seq, hidden]    lse fp32 [batch, heads, seq]                                          */
+/*   lse  natural-log log-sum-exp of each query row's masked, scaled scores, for the backward.  A row with no */
+/*        visible key (all-zero mask row) gets finfo(fp32).min * ln2 (~ -2.4e38, below -1e38 as no row with  */
+/*        a visible key can be): HF's softmax is uniform there (every score is finfo.min), ctx = mean of V,  */
+/*        and the backward recognises the value and gives every key P = 1/seq.                               */
 /*   keep_bits  NULL, or uint64 [batch, heads, seq, seq/64]: cache of the forward's dropout decisions; used  */
 /*              (written by fwd, read by bwd instead of regenerating Philox) when seq == 128 and dropout_p > 0,*/
 /*              ignored otherwise.  Pass the same buffer to both calls of a step, or NULL to both.            */

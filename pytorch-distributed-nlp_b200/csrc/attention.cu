@@ -38,6 +38,7 @@ __device__ __forceinline__ void st_pair(uint8_t* lo, uint8_t* hi, int row, int c
 struct AttnParams {
   int batch, seq, heads, hidden;  // hidden = heads * 64
   float scale;                    // 1/sqrt(64)
+  float neg_log2_seq;             // -log2(seq): backward exponent of a row with no visible key (row_masked_x)
   float dropout_p; const unsigned long long* rng; unsigned rng_site;
   const long long* mask;          // [batch, seq] or null
   __nv_bfloat16* ctx;             // fwd out [tokens, hidden]
@@ -88,6 +89,15 @@ template <bool kSeg>
 __device__ __forceinline__ bool key_masked(const uint32_t (&mw)[4], int seg_word, int col) {
   if (kSeg) return col < (seg_word & 0xffff) || col >= (seg_word >> 16);
   return (mw[col >> 5] >> (col & 31)) & 1u;
+}
+// Backward: the log2-domain exponent of a masked key of a query row whose log2 LSE is lse2.  A row with no visible key
+// (an all-zero attention_mask row) has all scores equal to finfo.min in HF, so its softmax is uniform.  The forward
+// gets that right (m = kMaskBias, every p = 1, l = seq) and stores lse = (kMaskBias + log2 seq) ln2, in which log2 seq
+// is lost to rounding: exp2(kMaskBias - lse2) would be 0, not 1/seq.  Such an lse2 (~kMaskBias) is far below that of
+// any row with a visible key (>= its largest finite score), so the row is recognised here and every key gets
+// P = 1/seq.  One select per row, nothing in the per-key loop.
+__device__ __forceinline__ float row_masked_x(float lse2, float neg_log2_seq) {
+  return lse2 < 0.5f * kMaskBias ? neg_log2_seq : kMaskBias - lse2;
 }
 // Column sums over the 128 rows of an m64n64 accumulator pair (one warpgroup per 64 rows), added into out[0, 64)
 __device__ __forceinline__ void frag_colsum64(const float (&f)[32], int lane, float* out) {
@@ -243,7 +253,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_fwd_kernel(const __g
   for (int u = 0; u < 2; ++u) {
     const float l_tot = quad_sum(l_run[u]);
     inv_l[u] = 1.0f / l_tot;
-    if (p.lse != nullptr && fr.t == 0)
+    if (p.lse != nullptr && fr.t == 0)   // no visible key: m = kMaskBias, lse ~ kMaskBias * ln2 (see row_masked_x)
       p.lse[((size_t)b * p.heads + h) * p.seq + qb * 128 + fr.r + 8 * u] = (m_run[u] + log2f(l_tot)) * kLn2;
   }
 #pragma unroll
@@ -374,7 +384,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attention_fwd128_kernel(const 
   for (int u = 0; u < 2; ++u) {
     const float l_tot = quad_sum(l_loc[u]);
     inv_l[u] = 1.0f / l_tot;
-    if (p.lse != nullptr && fr.t == 0)
+    if (p.lse != nullptr && fr.t == 0)   // see attention_fwd_kernel
       p.lse[((size_t)b * p.heads + h) * 128 + fr.r + 8 * u] = (m_new[u] + log2f(l_tot)) * kLn2;
   }
   wgmma_wait<0>();
@@ -496,7 +506,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
       }
       s_delta[tid] = delta;
     }
-    float lse2[2], delta[2];
+    float lse2[2], xm[2], delta[2];
     unsigned long long kept[2][2];
     const bool have_bits = kOneQ && p.keep_bits != nullptr;
     uint32_t keep[2][16];
@@ -516,7 +526,10 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
     wgmma_fence_regs(dp);
     __syncthreads();   // delta is in; O has been read and every product has read V: P may overwrite both
 #pragma unroll
-    for (int u = 0; u < 2; ++u) delta[u] = s_delta[fr.r + 8 * u];
+    for (int u = 0; u < 2; ++u) {
+      delta[u] = s_delta[fr.r + 8 * u];
+      xm[u] = row_masked_x(lse2[u], p.neg_log2_seq);
+    }
 #pragma unroll
     for (int ii = 0; ii < 64; ii += 2) {
       const int u = Frag::hi(ii), c = fr.col(ii);
@@ -525,7 +538,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
       for (int e = 0; e < 2; ++e) {
         const int cc = c + e;
         float x = fmaf(s[ii + e], c2, -lse2[u]);
-        if (key_masked<kOneQ && kSeg>(mw, seg[u], cc)) x = kMaskBias - lse2[u];   // what score*c2 + (-3.4e38) rounds to
+        if (key_masked<kOneQ && kSeg>(mw, seg[u], cc)) x = xm[u];   // what score*c2 + (-3.4e38) rounds to (row_masked_x)
         const float pr = ex2_approx(x);
         const bool kp = have_bits ? ((kept[u][cc >> 6] >> (cc & 63)) & 1ull) : ((keep[u][cc >> 3] >> (cc & 7)) & 1u);
         pd[e] = kp ? pr * drop.scale : 0.f;
@@ -754,6 +767,7 @@ static int32_t attention_bwd_impl(const void* qkv, const int64_t* attention_mask
   AttnParams p{};
   p.batch = (int)batch; p.seq = (int)seq; p.heads = (int)heads; p.hidden = (int)hidden;
   p.scale = 0.125f;
+  p.neg_log2_seq = -log2f((float)seq);
   p.dropout_p = dropout_p; p.rng = (const unsigned long long*)rng_state; p.rng_site = rng_site;
   p.mask = (const long long*)attention_mask;
   p.seg = segments;

@@ -112,6 +112,48 @@ def oracle_masks(cfg, B, S, seed, step):
     return m
 
 
+def attn_keep_mask(B, nh, S, seed, step, site, p, device="cpu"):
+    """Attention-probability keep mask [B, nh, S, S] as the attention kernels draw it: element ((b*nh + h)*S + q)*S + k
+    of dropout site `site` (packed bins use the same index, with b the bin).  None when p == 0."""
+    if p <= 0:
+        return None
+    return torch.from_numpy(philox_keep_mask(B * nh * S * S, seed, step, site, p).reshape(B, nh, S, S)).to(device)
+
+
+def padded_visibility(mask, S):
+    """[B, S, S] bool: query q of sequence b sees key k iff mask[b, k] (mask None: every key)"""
+    if mask is None:
+        return None
+    return (mask != 0)[:, None, :].expand(mask.shape[0], S, S)
+
+
+def packed_visibility(segments):
+    """[bins, 128, 128] bool from the packed segment words (lo | hi << 16): row q sees keys lo(q) <= k < hi(q)"""
+    seg = segments.long()
+    lo, hi = (seg & 0xffff)[..., None], (seg >> 16)[..., None]
+    k = torch.arange(seg.shape[-1], device=seg.device)
+    return (k >= lo) & (k < hi)
+
+
+def attention_ref(qkv, vis, B, nh, keep=None, p=0.0):
+    """HF BertSelfAttention (eager) in float64: softmax(q k^T / 8 + (~vis) * finfo(fp32).min) -> dropout -> @ v.
+    qkv [B*S, 3*nh*64] (Q | K | V column blocks); vis [B, S, S] bool (vis[b, q, k]: query q may see key k) or None
+    (every key visible); keep [B, nh, S, S] or None.  Make qkv a float64 leaf to take gradients by autograd.
+    Returns ctx [B*S, nh*64] and the natural-log lse [B, nh, S] of the masked scores.  A row with no visible key has
+    all-equal scores (finfo.min absorbs them), so its softmax is uniform, as in HF."""
+    H = nh * 64
+    S = qkv.shape[0] // B
+    q, k, v = (qkv[:, i * H:(i + 1) * H].double().view(B, S, nh, 64).transpose(1, 2) for i in range(3))
+    s = (q @ k.transpose(-1, -2)) * 0.125
+    if vis is not None:
+        s = s + (~vis)[:, None].double() * torch.finfo(torch.float32).min
+    pr = torch.softmax(s, -1)
+    lse = torch.logsumexp(s, -1)
+    if keep is not None:
+        pr = pr * keep / (1 - p)
+    return (pr @ v).transpose(1, 2).reshape(B * S, H), lse
+
+
 # ---- comparisons --------------------------------------------------------------------------------------------------------
 def rel_l2(a, b):
     a, b = a.double().flatten(), b.double().flatten()

@@ -6,7 +6,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from parity import b2, philox_keep_mask, rel_l2
+from parity import attention_ref, attn_keep_mask, b2, padded_visibility, philox_keep_mask, rel_l2
 from pytorch_distributed_nlp_b200 import _lib as L
 
 pytestmark = pytest.mark.gpu
@@ -174,22 +174,10 @@ def test_embed_fwd_bwd(cuda_dev, p):
         assert rel_l2(d_b.float(), br.grad) < 1.5e-2
 
 
-def _attn_ref(qkv, mask, B, Sq, nh, keep=None, p=0.0):
-    H = nh * 64
-    q, k, v = (qkv[:, i * H:(i + 1) * H].view(B, Sq, nh, 64).transpose(1, 2) for i in range(3))
-    s = (q @ k.transpose(-1, -2)) * 0.125
-    if mask is not None:
-        s = s + (1.0 - mask[:, None, None, :].float()) * torch.finfo(torch.float32).min
-    pr = torch.softmax(s, -1)
-    lse = torch.logsumexp(s, -1)
-    if keep is not None:
-        pr = pr * keep / (1 - p)
-    return (pr @ v).transpose(1, 2).reshape(B * Sq, H), lse
-
-
 @pytest.mark.parametrize("Sq,masked,p,cache", [(128, False, 0.0, False), (128, True, 0.1, False), (128, True, 0.1, True),
                                                (128, False, 0.1, True), (256, True, 0.0, False),
-                                               (512, True, 0.1, True)])
+                                               (512, True, 0.1, True), (256, True, 0.1, False),
+                                               (512, False, 0.0, False)])
 def test_attention_fwd_bwd(cuda_dev, Sq, masked, p, cache):
     """cache: hand both calls a keep-bit buffer (the forward's dropout decisions, re-read by the backward at seq 128;
     ignored at other lengths) -- results must not depend on it"""
@@ -210,11 +198,9 @@ def test_attention_fwd_bwd(cuda_dev, Sq, masked, p, cache):
     L.call("b2_attention_fwd", qkv.data_ptr(), L.ptr(mask), B, Sq, nh, 64, p, rs.data_ptr(), 4, ctx.data_ptr(),
            lse.data_ptr(), L.ptr(kb), S())
     torch.cuda.synchronize()
-    keep = None
-    if p > 0:
-        keep = torch.from_numpy(philox_keep_mask(B * nh * Sq * Sq, 1234, 5, 4, p).reshape(B, nh, Sq, Sq)).to(dev)
-    qr = qkv.float().requires_grad_(True)
-    ref, lse_ref = _attn_ref(qr, mask, B, Sq, nh, keep, p)
+    keep = attn_keep_mask(B, nh, Sq, 1234, 5, 4, p, dev)
+    qr = qkv.double().requires_grad_(True)
+    ref, lse_ref = attention_ref(qr, padded_visibility(mask, Sq), B, nh, keep, p)
     assert (ctx.float() - ref).abs().max().item() < 3e-2
     assert (lse.view(B, nh, Sq) - lse_ref).abs().max().item() < 2e-2
 
@@ -231,7 +217,7 @@ def test_attention_fwd_bwd(cuda_dev, Sq, masked, p, cache):
         assert np.array_equal(got, keep.cpu().numpy().astype(bool))
     if dbias is not None:   # fused QKV bias gradient == column sums of what was written
         assert rel_l2(dbias, dqkv.float().sum(0)) < 1e-4
-    ref.backward(dctx.float())
+    ref.backward(dctx.double())
     for i, nm in enumerate("qkv"):
         e = rel_l2(dqkv[:, i * H:(i + 1) * H].float(), qr.grad[:, i * H:(i + 1) * H])
         assert e < 3e-2, "d%s rel err %.3g" % (nm, e)

@@ -41,6 +41,26 @@ def test_tiny_step_matches_oracle(cuda_dev, padded, dropout):
     assert worst <= TOL_GRAD_REL, sorted(rows, key=lambda r: -r[1])[:5]
 
 
+@pytest.mark.parametrize("dropout", [False, True])
+def test_tiny_step_with_all_padding_sample_matches_oracle(cuda_dev, dropout):
+    """one sample of the padded batch is all padding (attention_mask all zeros): HF gives its query rows a uniform
+    softmax over the keys, so its value / query / key gradients are not zero and must reach the weights"""
+    cfg = tiny_config() if dropout else tiny_config(hidden_dropout_prob=0.0, attention_probs_dropout_prob=0.0)
+    state = state_from_hf_init(cfg)
+    model = make_model(cfg, state, cuda_dev).train()
+    model._engine.seed_dropout(99, 7)
+    batch = bert_ref.synthetic_batch(cfg, 4, 128, 1000, padded=True)
+    batch["input_ids"][2] = 0
+    batch["attention_mask"][2] = 0
+    out, loss = _fwd_bwd(model, batch, cuda_dev)
+    masks = oracle_masks(cfg, 4, 128, 99, 7) if dropout else None
+    rl, rz, rg = bert_ref.loss_and_grads(state, cfg, batch, masks=masks)
+    assert abs(float(loss) - float(rl)) <= TOL_LOSS
+    assert float((out[1].detach().cpu() - rz).abs().max()) <= TOL_LOGITS
+    worst, rows = grad_report(model.grad_dict(), rg)
+    assert worst <= TOL_GRAD_REL, sorted(rows, key=lambda r: -r[1])[:5]
+
+
 @pytest.mark.parametrize("name,cfg_kw,batch,seq", [
     # BASELINE.json config B (bert-base, seq 512): the multi-block attention paths (online softmax rescale forward,
     # dQ accumulation across key blocks backward) and the padded tail blocks, at 2 layers
