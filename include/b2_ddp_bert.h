@@ -319,6 +319,23 @@ int32_t b2_adamw_background(const void* grads, void* shadow, float* master, floa
                             const uint8_t* decay_flags, int64_t begin, int64_t end, const b2_adamw_hparams_t* hp,
                             const float* step_size, void* stream);
 
+/* Gradient accumulation over the slice [begin, end) (element indices, multiples of 8) of the bf16 gradient space
+ * `grads` and its fp32 accumulator `accum` (both indexed from their base, 16-byte aligned).
+ *   replaces: torch's accumulation into `.grad` across backwards, and DDP's no_sync() skipping the Reducer
+ *   (SP/torch/nn/parallel/distributed.py `no_sync`, `require_backward_grad_sync`) for the micro-batches of a window.
+ *   mode   operation                               bytes / parameter
+ *   STORE  accum = f32(grads)                      6   (first pass of a window: the accumulator is never zeroed)
+ *   ADD    accum += f32(grads)                     10
+ *   FOLD   grads = bf16_rne(accum + f32(grads))    8   (the final pass: exchange / AdamW then read `grads`)
+ *   FLUSH  grads = bf16_rne(accum)                 6   (optimizer step with no final pass)
+ * inf / nan propagate.  Blocks of 128 threads x <= 32 registers, no shared memory: shaped like
+ * b2_adamw_background, to run per bucket beside the backward's GEMM CTAs.                                      */
+#define B2_ACCUM_STORE 0
+#define B2_ACCUM_ADD 1
+#define B2_ACCUM_FOLD 2
+#define B2_ACCUM_FLUSH 3
+int32_t b2_grad_accumulate(void* grads, float* accum, int64_t begin, int64_t end, int32_t mode, void* stream);
+
 /* ++step (AdamW t) and ++rng step (dropout stream) on the device: keeps CUDA-graph replays stateful.
  * found_inf (optional device fp32, see b2_adamw_hparams_t): non-zero leaves the AdamW step count untouched.   */
 int32_t b2_step_advance(int64_t* step_counter, void* rng_state, const float* found_inf, void* stream);

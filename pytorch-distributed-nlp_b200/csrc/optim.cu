@@ -151,6 +151,67 @@ adamw_slim_kernel(const SlimParams p) {
   }
 }
 
+// ---- gradient accumulation -----------------------------------------------------------------------------------------
+// One pass over [begin, end) of the bf16 gradient space and its fp32 accumulator (B2_ACCUM_* in the header).  It is
+// launched per bucket on the optimizer stream while the backward's GEMM CTAs hold the SMs, so it has the shape of
+// adamw_slim_kernel: 128 threads x <= 32 registers, no shared memory, the GEMMs' carve-out, short-lived blocks.  Each
+// thread handles kAccIters vectors of 8 elements (16 bytes of bf16, 2 x float4 of fp32).  inf / nan pass through.
+constexpr int kAccThreads = 128, kAccIters = 8;
+template <int MODE>
+__global__ void __maxnreg__(32)
+grad_accumulate_kernel(__nv_bfloat16* __restrict__ grads, float* __restrict__ accum, long long begin, long long nvec) {
+  pdl_wait();
+  pdl_launch_dependents();
+  long long i = (long long)blockIdx.x * (kAccThreads * kAccIters) + threadIdx.x;
+#pragma unroll 1
+  for (int it = 0; it < kAccIters; ++it, i += kAccThreads) {
+    if (i >= nvec) break;
+    const long long e = begin + (i << 3);
+    float4* a = reinterpret_cast<float4*>(accum + e);
+    uint4* g = reinterpret_cast<uint4*>(grads + e);
+    float f[8];
+    if (MODE != B2_ACCUM_FLUSH) {
+      const uint4 q = *g;
+      f[0] = bf16_lo(q.x); f[1] = bf16_hi(q.x); f[2] = bf16_lo(q.y); f[3] = bf16_hi(q.y);
+      f[4] = bf16_lo(q.z); f[5] = bf16_hi(q.z); f[6] = bf16_lo(q.w); f[7] = bf16_hi(q.w);
+    }
+    if (MODE != B2_ACCUM_STORE) {
+      const float4 a0 = a[0], a1 = a[1];
+      if (MODE == B2_ACCUM_FLUSH) {
+        f[0] = a0.x; f[1] = a0.y; f[2] = a0.z; f[3] = a0.w; f[4] = a1.x; f[5] = a1.y; f[6] = a1.z; f[7] = a1.w;
+      } else {
+        f[0] = a0.x + f[0]; f[1] = a0.y + f[1]; f[2] = a0.z + f[2]; f[3] = a0.w + f[3];
+        f[4] = a1.x + f[4]; f[5] = a1.y + f[5]; f[6] = a1.z + f[6]; f[7] = a1.w + f[7];
+      }
+    }
+    if (MODE == B2_ACCUM_STORE || MODE == B2_ACCUM_ADD) {
+      a[0] = make_float4(f[0], f[1], f[2], f[3]);
+      a[1] = make_float4(f[4], f[5], f[6], f[7]);
+    } else {
+      uint4 o;
+      o.x = pack_bf16(f[0], f[1]); o.y = pack_bf16(f[2], f[3]);
+      o.z = pack_bf16(f[4], f[5]); o.w = pack_bf16(f[6], f[7]);
+      *g = o;
+    }
+  }
+}
+
+template <int MODE>
+static int32_t launch_grad_accumulate(void* grads, float* accum, long long begin, long long nvec, cudaStream_t stream) {
+  static bool attr = false;
+  if (!attr) {   // same shared-memory carve-out as the GEMM CTAs it is meant to run beside
+    B2_CUDA(cudaFuncSetAttribute(grad_accumulate_kernel<MODE>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 cudaSharedmemCarveoutMaxShared));
+    attr = true;
+  }
+  const long long per_block = (long long)kAccThreads * kAccIters;
+  B2_LAUNCH(grad_accumulate_kernel<MODE>, (unsigned)((nvec + per_block - 1) / per_block), kAccThreads, 0, stream,
+            (__nv_bfloat16*)grads, accum, begin, nvec);
+  B2_CUDA(cudaGetLastError());
+  count_launches(1);
+  return 0;
+}
+
 // HF AdamW bias correction for the NEXT update: step_size = lr * sqrt(1 - b2^t) / (1 - b1^t), t = *step + 1
 __global__ void adamw_prepare_kernel(double lr, double beta1, double beta2, int correct_bias, const long long* step,
                                      float* step_size) {
@@ -311,6 +372,25 @@ extern "C" int32_t b2_adamw_background(const void* grads, void* shadow, float* m
   B2_CUDA(cudaGetLastError());
   count_launches(1);
   return 0;
+}
+
+extern "C" int32_t b2_grad_accumulate(void* grads, float* accum, int64_t begin, int64_t end, int32_t mode,
+                                      void* stream_) {
+  B2_REQUIRE(grads && accum, "grad_accumulate: null pointer");
+  B2_REQUIRE(((uintptr_t)grads % 16 == 0) && ((uintptr_t)accum % 16 == 0),
+             "grad_accumulate: 16-byte alignment required");
+  B2_REQUIRE(begin >= 0 && end >= begin && begin % 8 == 0 && end % 8 == 0,
+             "grad_accumulate: slice [%lld,%lld) must be 8-element aligned", (long long)begin, (long long)end);
+  B2_REQUIRE(mode >= B2_ACCUM_STORE && mode <= B2_ACCUM_FLUSH, "grad_accumulate: unknown mode %d", (int)mode);
+  if (end == begin) return 0;
+  const long long nvec = (end - begin) >> 3;
+  cudaStream_t s = (cudaStream_t)stream_;
+  switch (mode) {
+    case B2_ACCUM_STORE: return launch_grad_accumulate<B2_ACCUM_STORE>(grads, accum, begin, nvec, s);
+    case B2_ACCUM_ADD: return launch_grad_accumulate<B2_ACCUM_ADD>(grads, accum, begin, nvec, s);
+    case B2_ACCUM_FOLD: return launch_grad_accumulate<B2_ACCUM_FOLD>(grads, accum, begin, nvec, s);
+    default: return launch_grad_accumulate<B2_ACCUM_FLUSH>(grads, accum, begin, nvec, s);
+  }
 }
 
 extern "C" int32_t b2_step_advance(int64_t* step_counter, void* rng_state, const float* found_inf, void* stream_) {

@@ -203,6 +203,13 @@ class DistributedDataParallel(nn.Module):
     def forward(self, *args, **kwargs):
         return self.module(*args, **kwargs)
 
+    def no_sync(self):
+        """torch DDP's gradient-accumulation context (SP/torch/nn/parallel/distributed.py `no_sync`): backwards inside
+        it only add into a local fp32 accumulator; the next backward outside it folds the sum in before its exchange.
+        Unlike stock DDP, an optimizer.step() with no such backward exchanges the accumulated gradients too, so the
+        ranks cannot silently diverge.  See BertForSequenceClassification.no_sync."""
+        return self.module.no_sync()
+
     # ---- checkpoint surface ---------------------------------------------------------------------------------------------
     def load_state_dict(self, state_dict, strict=True, assign=False):
         """`model.load_state_dict(torch.load(ckpt))` on the WRAPPED model (multi-gpu-distributed-cls.py:357-363): keys
@@ -275,6 +282,14 @@ class DistributedDataParallel(nn.Module):
         if wg_event is not None:
             self._side.wait_event(wg_event)
         s = self._side.cuda_stream
+        op = eng._pass_op
+        if op is not None:
+            # gradient accumulation, on the local gradients of the whole bucket: an accumulating pass stops here (no
+            # barrier, no exchange); the final pass folds BEFORE the barrier, so peers read the window's sum
+            b, e, _label = self.module._layout.buckets[idx]
+            eng.accumulate_range(b, e, op, s)
+            if op != L.ACCUM_FOLD:
+                return
         self.comm.barrier(_SLOT_BUCKET0 + idx, s)
         self._exchange_update(opt, idx, s)
         if self._pending is None:

@@ -11,6 +11,7 @@ The arithmetic follows HF ``BertForSequenceClassification`` (SP/transformers/mod
 1077-1154, eager attention) in bf16 with fp32 accumulation/statistics; fp32 master weights stay the parameters
 the user sees.  There is no PyTorch fallback: without the CUDA library every call raises.
 """
+import contextlib
 import os
 from collections import OrderedDict
 
@@ -203,18 +204,28 @@ class _StepFn(torch.autograd.Function):
         eng = model._engine
         if d_logits is None and (d_loss is None or not ctx.has_loss):
             raise RuntimeError("backward reached the model without any gradient")
+        accumulate = model._no_sync
         if model._optimizer is not None:
-            # gradients are OVERWRITTEN by every backward (bf16 bucket space, zero_grad is a no-op): a second backward
-            # before optimizer.step() would silently drop the first one's gradients where torch would accumulate
+            # gradients are OVERWRITTEN by every backward outside no_sync() (bf16 bucket space, zero_grad is a no-op):
+            # a second one before optimizer.step() would silently drop the first one's gradients where torch would
+            # accumulate them
             if model._grads_live:
+                if accumulate:
+                    raise RuntimeError("backward() inside no_sync() after a backward outside it without "
+                                       "optimizer.step() in between: run the window's earlier passes inside no_sync()")
                 raise RuntimeError("backward() called twice without optimizer.step() in between: gradient "
                                    "accumulation is not supported on this path (gradients are overwritten, not summed)")
-            model._grads_live = True
+            if not accumulate:
+                model._grads_live = True
+        eng.start_pass(accumulate)
         eng.backward(d_logits, d_loss if ctx.has_loss else None)
+        eng.end_pass()
         model._notify_backward_done()
         # Gradients live in the engine's bf16 bucket space, not in `.grad`.  The anchor (classifier.bias) gets its
         # true gradient as a 6-float fp32 probe: it is the column sum of d_logits, so an inf/nan anywhere upstream
-        # of the model shows up in it -- which is what torch.cuda.amp.GradScaler's inf check needs to see.
+        # of the model shows up in it -- which is what torch.cuda.amp.GradScaler's inf check needs to see.  Autograd
+        # sums the probes of an accumulation window's backwards; the final one reads the folded window sum, so the
+        # probe is non-finite exactly when some pass of the window was.
         off, shape = ctx.model._layout.entries["classifier.bias"]
         n = 1
         for d in shape:
@@ -246,6 +257,22 @@ class BertForSequenceClassification(nn.Module):
         self._optimizer = None
         self._ddp = None
         self._grads_live = False     # an eager backward has produced gradients no optimizer.step() has consumed yet
+        self._no_sync = False        # inside no_sync(): backwards accumulate
+
+    @contextlib.contextmanager
+    def no_sync(self):
+        """Gradient accumulation, as ``DistributedDataParallel.no_sync()`` (SP/torch/nn/parallel/distributed.py): a
+        backward inside the context adds its gradients into a local fp32 accumulator -- no exchange, no update, no
+        barrier.  The first backward after it folds the accumulator into its own gradients, and ``optimizer.step()``
+        applies the sum as usual; a step with no such backward applies the accumulator alone (under DDP with world > 1
+        it also exchanges, where stock torch DDP would leave the ranks diverged).  Scale the loss by 1/k yourself for
+        the mean over k micro-batches.  Also available on the bare model, so one loop runs on 1 and N GPUs."""
+        prev = self._no_sync
+        self._no_sync = True
+        try:
+            yield
+        finally:
+            self._no_sync = prev
 
     # ---- module skeleton reproducing HF parameter paths -------------------------------------------------------
     def _build_skeleton(self):
@@ -417,14 +444,15 @@ class BertForSequenceClassification(nn.Module):
 
     # ---- test / tooling helpers -----------------------------------------------------------------------------------------
     def grad_dict(self):
-        """fp32 copies of the (bf16) gradients of the last backward, keyed by HF parameter name."""
+        """fp32 copies of what the next optimizer.step() would apply, keyed by HF parameter name: the (bf16) gradients of
+        the last backward, or inside an open accumulation window the fp32 accumulator."""
         if self._engine is None:
             raise RuntimeError("no engine (model not on CUDA)")
         out = OrderedDict()
-        g = self._engine.grads
+        g = self._engine.accum if self._engine.accum_live else self._engine.grads
         for name, p in self._params_by_name.items():
             off, shape = self._layout.entries[name]
-            out[name] = g[off:off + p.numel()].view(shape).float()
+            out[name] = g[off:off + p.numel()].view(shape).to(torch.float32, copy=True)
         return out
 
 
@@ -461,6 +489,15 @@ class _Engine:
         # bytes in flight to beat the separate per-bucket AdamW launches; see DESIGN.md
         self.fused_adamw = os.environ.get("B2_FUSED_ADAMW", "0") == "1"
         self.fused_adamw_active = False
+        # gradient accumulation (no_sync(), Trainer gradient_accumulation_steps): fp32 accumulator over the flat space,
+        # allocated on first use (local even under DDP); accum_in_use switches off the paths that update before a fold
+        # could happen (the fused-epilogue and the pipelined AdamW); accum_live = the accumulator holds gradients no
+        # fold / flush has consumed yet; _pass_op = the b2_grad_accumulate mode of the running backward (None: none)
+        self.accum = None
+        self.accum_in_use = False
+        self.accum_live = False
+        self._pass_op = None
+        self._pass_stream = None
         # cache of the forward's attention-dropout decisions for the backward (1 bit per (b, h, q, k), bit-exact against
         # the Philox replica): the backward reads them instead of regenerating Philox; B2_ATTN_KEEP_BITS=0 regenerates
         # the masks in the backward instead
@@ -512,6 +549,47 @@ class _Engine:
 
     def refresh_shadow(self):
         L.call("b2_cast_f32_to_bf16", L.ptr(self.model._flat), L.ptr(self.shadow), self.lay.total, self.stream())
+
+    # ---- gradient accumulation ----
+    def ensure_accum(self):
+        if self.accum is None:
+            self.accum = torch.empty(self.lay.total, dtype=torch.float32, device=self.dev)
+        self.accum_in_use = True
+
+    def accumulate_range(self, begin, end, op, stream):
+        L.call("b2_grad_accumulate", self.grads.data_ptr(), self.accum.data_ptr(), begin, end, op, stream)
+
+    def start_pass(self, accumulate):
+        """Sets the accumulation mode of the next backward: STORE / ADD into the accumulator (accumulate), FOLD it into
+        the gradients (the first plain backward after accumulating ones), or nothing."""
+        if accumulate:
+            self.ensure_accum()
+            self._pass_op = L.ACCUM_ADD if self.accum_live else L.ACCUM_STORE
+        else:
+            self._pass_op = L.ACCUM_FOLD if self.accum_live else None
+
+    def end_pass(self):
+        """After the backward: the whole-range accumulate / fold when no per-bucket launch did it, else the join of
+        the stream that ran them (the next backward overwrites `grads`, and whoever reads them next is on the main
+        stream); an accumulating pass also moves the dropout stream on, as optimizer.step() does for the final one."""
+        op, side = self._pass_op, self._pass_stream
+        self._pass_op, self._pass_stream = None, None
+        if op is None:
+            return
+        main = torch.cuda.current_stream(self.dev)
+        if side is None:
+            self.accumulate_range(0, self.lay.total, op, main.cuda_stream)
+        else:
+            main.wait_stream(side)
+        self.accum_live = op != L.ACCUM_FOLD
+        if op != L.ACCUM_FOLD:
+            L.call("b2_step_advance", None, L.ptr(self.rng), None, main.cuda_stream)
+
+    def flush_accum(self, stream):
+        """optimizer.step() with the window still open (no final backward): grads = bf16(accumulator)"""
+        if self.accum_live:
+            self.accumulate_range(0, self.lay.total, L.ACCUM_FLUSH, stream)
+            self.accum_live = False
 
     def seed_dropout(self, seed, step=0):
         L.call("b2_rng_seed", L.ptr(self.rng), int(seed), int(step), self.stream())
@@ -811,7 +889,15 @@ class _Engine:
         # 85 % of the parameters); the per-bucket AdamW launches then skip those vectors
         self.fused_adamw_active = bool(overlap_opt and self.grouped_wgrad and self.fused_adamw and
                                        getattr(opt, "grad_scale", None) is None and
-                                       not getattr(opt, "_amp_seen", False))
+                                       not getattr(opt, "_amp_seen", False) and not self.accum_in_use)
+        # Under an armed DDP exchange the side stream takes the weight-gradient dependencies bucket by bucket
+        # (ddp._bucket_ready) and optimizer.step() joins it
+        ddp_overlap = (hooks is not None and hooks.world > 1 and hooks.overlap and opt is not None and
+                       getattr(opt, "_armed", False))
+        # an accumulating / folding backward: per bucket on the stream that runs the update (armed), else one
+        # whole-range launch in end_pass()
+        if self._pass_op is not None and (overlap_opt or ddp_overlap):
+            self._pass_stream = hooks._side if ddp_overlap else self.opt_stream
 
         def bucket_ready(idx, wg_event=None):
             """bucket `idx` holds its final gradients once the main stream reaches this point (and `wg_event`,
@@ -826,8 +912,13 @@ class _Engine:
                 if wg_event is not None:
                     self.opt_stream.wait_event(wg_event)
                 b0, e0, _lbl = self.lay.buckets[idx]
-                opt.update_range(b0, e0, 1, 0, [self.grads.data_ptr()], [self.shadow.data_ptr()],
-                                 self.opt_stream.cuda_stream, background=(idx != 0))
+                os_ = self.opt_stream.cuda_stream
+                if self._pass_op is not None:
+                    self.accumulate_range(b0, e0, self._pass_op, os_)
+                    if self._pass_op != L.ACCUM_FOLD:
+                        return      # an accumulating pass: no update
+                opt.update_range(b0, e0, 1, 0, [self.grads.data_ptr()], [self.shadow.data_ptr()], os_,
+                                 background=(idx != 0))
                 opt._pending.add(idx)
 
         if not self.lay.head_in_last_layer:
@@ -939,10 +1030,8 @@ class _Engine:
         else:
             L.call("b2_embed_bwd_packed", *emb_in, ws["pos32"].data_ptr(), *emb_tail)
         # Whoever consumes the gradients next on the main stream (optimizer.step, grad_dict) must see the weight-gradient
-        # stream's work.  Under an armed DDP exchange the side stream has taken those dependencies bucket by bucket
-        # (ddp._bucket_ready) and optimizer.step() joins the side stream; in every other case join here.
-        ddp_overlap = (hooks is not None and hooks.world > 1 and hooks.overlap and opt is not None and
-                       getattr(opt, "_armed", False))
+        # stream's work.  Under an armed DDP exchange optimizer.step() (or end_pass) joins the side stream, which has
+        # taken those dependencies; in every other case join here.
         if side is not main and not ddp_overlap:
             for l in sorted(done)[:2]:       # the last two layers processed (0 and 1) may still be in flight
                 main.wait_event(done[l])

@@ -110,8 +110,10 @@ class AdamW(torch.optim.Optimizer):
         # Under the forward the update time-slices with the GEMM CTAs just as it does under the backward, and a layer
         # that has to wait for its bucket's event stalls the critical path.  Correct (tests/test_model.py::test_pipelined_adamw_is_the_same_
         # training run) but slower: opt-in only (B2_PIPELINED_ADAMW=1).
+        # (gradient accumulation folds the window into the gradients at the end of the final backward: an update
+        # deferred past it has nothing to gain and a window to get wrong)
         if (os.environ.get("B2_PIPELINED_ADAMW", "0") != "1" or model._ddp is not None or self._amp_seen or
-                getattr(model._engine, "fused_adamw", False)):
+                getattr(model._engine, "fused_adamw", False) or getattr(model._engine, "accum_in_use", False)):
             return False
         self._pipelined = True
         self._armed = False          # no per-bucket launches under the backward
@@ -268,6 +270,8 @@ class AdamW(torch.optim.Optimizer):
         eng = model._engine
         if eng is None:
             raise RuntimeError("optimizer.step(): the model is not on CUDA")
+        # every pass of an accumulation window ran inside no_sync(): apply the accumulator (torch applies its .grad)
+        eng.flush_accum(torch.cuda.current_stream(eng.dev).cuda_stream)
         if model._ddp is not None and model._ddp.world > 1:
             model._ddp._optimizer_step(self)
         else:

@@ -9,6 +9,7 @@ Same methods, same argument meaning: ``on_step`` [:126-137], ``loss_reduce`` [:1
   * ``loss_reduce`` / ``output_reduce`` go through the peer-memory kernels when the model is the b200 DDP wrapper;
   * ``train`` uses :class:`FusedTrainStep` (the whole step captured in one CUDA graph) when ``args.fused`` is set.
 """
+import contextlib
 import os
 import time
 
@@ -38,6 +39,8 @@ class Args:
     fused = True          # capture fwd + bwd + exchange + AdamW in one CUDA graph
     pack = False          # pack the valid prefixes of the padded [B, 128] batches into 128-token bins (packing.py): the
                           # reference pads every row to max_seq_len although real rows average 18 tokens [:76]
+    gradient_accumulation_steps = 1   # k > 1: one optimizer step per k batches, each batch's loss scaled by 1/k (the
+                                      # HF Trainer / DeepSpeed name; fabric-cls.py's grad_accumulation)
     log_every = 1         # the reference prints every step (forces a D2H sync per step)
     total_step = 0
 
@@ -66,8 +69,11 @@ class _StagedGraphStep:
         self.loss_out = torch.zeros((), dtype=torch.float32, device=dev)
         self.h_loss = torch.zeros((), dtype=torch.float32).pin_memory()
         self.use_graph = use_graph
-        self.graph = None
-        self._warm = 0
+        self.graph = None         # the graph of the optimizer-step body (the only one without accumulation)
+        self._graphs = {}         # role -> graph, role = (final pass, window already holds gradients), see run_device
+        self._warm = {}
+        self._role = (True, False)
+        self.accum_steps = 1
         self._h2d_done = None
         # The step body -- the critical chain of forward / dgrad kernels -- is issued (and captured) on a HIGH-priority
         # stream, so that when an SM frees up the block scheduler hands it to the critical path before the
@@ -116,48 +122,74 @@ class _StagedGraphStep:
             self._body()
         cur.wait_stream(self._prio_stream)
 
-    def run_device(self):
-        """The step with inputs already staged on the device (bench `value` path)."""
-        self._run_device()
+    def run_device(self, final=True):
+        """The step with inputs already staged on the device (bench `value` path).  final=False: a micro-batch of a
+        gradient-accumulation window (forward, backward, accumulate; no optimizer step)."""
         opt = getattr(self, "opt", None)
-        if opt is not None and opt._pipelined:
-            opt._deferred_pending = True      # (a graph replay runs no Python: keep the host-side flag current)
+        # the body's accumulation mode (STORE / ADD / FOLD / none) follows from these two, and a graph replay runs no
+        # Python: one graph per combination, and the host-side flags are kept current here
+        self._role = (final, opt is not None and self.eng.accum_live)
+        self._run_device()
+        if opt is not None:
+            self.eng.accum_live = not final
+            if opt._pipelined:
+                opt._deferred_pending = True
 
     def _run_device(self):
         if not self.use_graph:
             self._run_body()
             return
-        if self.graph is None:
-            if self._warm < 2:
+        role = self._role
+        g = self._graphs.get(role)
+        if g is None:
+            if self._warm.get(role, 0) < 2:
                 # eager warm-up: first launches set kernel attributes, DDP arms its overlap path
                 self._run_body()
-                self._warm += 1
+                self._warm[role] = self._warm.get(role, 0) + 1
                 return
             torch.cuda.synchronize(self.eng.dev)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 self._run_body()
-            self.graph = g
-            self.graph.replay()
-            return
-        self.graph.replay()
+            self._graphs[role] = g
+            if role[0]:
+                self.graph = g
+        g.replay()
+
+    def _arm(self, optimizer, accum_steps):
+        self.opt = optimizer
+        self.accum_steps = accum_steps
+        if accum_steps > 1:
+            self.eng.ensure_accum()       # before enable_pipelining, and outside any capture
+        # the fused step owns backward + optimizer: per-bucket AdamW (and, under DDP, the peer exchange) may start
+        # while backward is still running
+        optimizer._armed = True
+        optimizer.enable_pipelining()     # one GPU: the update moves under the NEXT step's forward (optim.py)
 
     def _train_body(self, forward):
-        """forward(weight_events) -> (logits, loss): the common part of the captured train steps"""
+        """forward(weight_events) -> (logits, loss): the common part of the captured train steps.  A micro-batch body
+        (self._role[0] False) accumulates its gradients and bumps the dropout stream instead of stepping; the final
+        body folds the window in before the update."""
         eng, opt = self.eng, self.opt
+        final = self._role[0]
         events = opt.apply_pending(in_step=True) if opt._pipelined else None     # step i-1's update, see optim.py
         logits, loss = forward(events)
         B, S, mask, p_h, p_a, p_c, packed = eng._saved
         eng._saved = None
         Bo = B if packed is None else packed[1].numel()
         ws = eng.workspace(B, S, Bo)
+        if self.accum_steps > 1:
+            ws["dloss_logits"].mul_(1.0 / self.accum_steps)     # what an eager loop does with loss / k
         # d(loss)/d(logits) was produced by the CE kernel: the reference's criterion(logits, label) [:169]
+        eng.start_pass(not final)
         eng._backward_from_dlogits(ws["dloss_logits"], B, S, mask, p_h, p_a, p_c, packed)
-        if opt._pipelined:
-            opt.mark_grads_pending()
-            torch.cuda.current_stream(eng.dev).wait_stream(eng.opt_stream)   # (step counter bump of the applied update)
-        else:
-            opt.step()
+        eng.end_pass()
+        if final:
+            if opt._pipelined:
+                opt.mark_grads_pending()
+                torch.cuda.current_stream(eng.dev).wait_stream(eng.opt_stream)  # (step counter bump of the applied update)
+            else:
+                opt.step()
         self.loss_out.copy_(loss)
 
     def loss_to_host(self):
@@ -169,15 +201,12 @@ class _StagedGraphStep:
 class FusedTrainStep(_StagedGraphStep):
     """One training step == one CUDA-graph replay: H2D of the batch, embeddings -> 12 layers -> head -> CE, the full
     backward, the peer-HBM gradient exchange fused with AdamW, and the device-side step/RNG bump.  Semantically the body
-    of the reference loop [:166-176] without the host round trips."""
+    of the reference loop [:166-176] without the host round trips.  accum_steps = k > 1: gradient accumulation over k
+    micro-batches, the loss scaled by 1/k; call with final=False for the first k - 1 of a window."""
 
-    def __init__(self, model, optimizer, batch_size, seq_len, use_graph=True):
+    def __init__(self, model, optimizer, batch_size, seq_len, use_graph=True, accum_steps=1):
         super().__init__(model, batch_size, seq_len, use_graph)
-        self.opt = optimizer
-        # the fused step owns backward + optimizer: per-bucket AdamW (and, under DDP, the peer exchange) may start
-        # while backward is still running
-        optimizer._armed = True
-        optimizer.enable_pipelining()     # one GPU: the update moves under the NEXT step's forward (optim.py)
+        self._arm(optimizer, accum_steps)
         self.kernel_launches = None
 
     # the step body, expressed only with stream-ordered work (capturable)
@@ -186,11 +215,11 @@ class FusedTrainStep(_StagedGraphStep):
         self._train_body(lambda ev: self.eng.forward(self.d_ids, self.d_tt, self.d_mask, self.d_lab, training=True,
                                                      need_backward=True, weight_events=ev))
 
-    def __call__(self, batch_data):
+    def __call__(self, batch_data, final=True):
         """batch_data: the dict the reference Collate yields (host int64 tensors).  Returns the device loss scalar
-        (local rank's mean CE, like `loss` at [:169])."""
+        (local rank's mean CE, like `loss` at [:169]; unscaled under accumulation)."""
         self.stage(batch_data)
-        self.run_device()
+        self.run_device(final)
         return self.loss_out
 
 
@@ -199,7 +228,7 @@ class PackedTrainStep(_StagedGraphStep):
     instance (staging buffers + CUDA graph) per bin count; the Trainer keeps a small cache of them, since the number of
     bins a batch packs into varies with its lengths."""
 
-    def __init__(self, model, optimizer, bins, batch, use_graph=True):
+    def __init__(self, model, optimizer, bins, batch, use_graph=True, accum_steps=1):
         super().__init__(model, bins, 128, use_graph)
         dev = self.eng.dev
         self.bins, self.batch = bins, batch
@@ -210,9 +239,7 @@ class PackedTrainStep(_StagedGraphStep):
         z = lambda *sh: torch.zeros(*sh, dtype=torch.int64, device=dev)
         self.d_pos, self.d_cls, self.d_lab = z(bins, 128), z(batch), z(batch)
         self.d_seg = torch.zeros(bins, 128, dtype=torch.int32, device=dev)
-        self.opt = optimizer
-        optimizer._armed = True
-        optimizer.enable_pipelining()
+        self._arm(optimizer, accum_steps)
 
     def _unstage(self):
         n, st = self.bins * 128, self.d_stage
@@ -245,9 +272,9 @@ class PackedTrainStep(_StagedGraphStep):
         self._train_body(lambda ev: self.eng.forward(self.d_ids, self.d_tt, None, self.d_lab, training=True,
                                                      need_backward=True, packed=packed, weight_events=ev))
 
-    def __call__(self, packed, label):
+    def __call__(self, packed, label, final=True):
         self.stage(packed, label)
-        self.run_device()
+        self.run_device(final)
         return self.loss_out
 
 
@@ -287,6 +314,7 @@ class Trainer:
         self._scaler = None
         self._fused_eval = {}
         self._pin = {}
+        self._micro = 0       # batches of the open gradient-accumulation window
 
     def _to_device(self, batch_data):
         dev = _unwrap(self.model)._engine.dev
@@ -340,43 +368,70 @@ class Trainer:
         return outputs.clone(), targets.clone()
 
     def train_step(self, batch_data):
-        """One step of the reference loop body [:166-176]; returns the rank-averaged loss (device scalar)."""
+        """One step of the reference loop body [:166-176]; returns the rank-averaged loss (device scalar).  With
+        args.gradient_accumulation_steps = k > 1 a call is one micro-batch: the first k - 1 of a window accumulate
+        (inside no_sync() on the eager paths), the k-th also steps the optimizer; every loss is scaled by 1/k
+        (fabric-cls.py:150-157) and the returned loss is the unscaled micro-batch loss."""
+        k = max(1, int(getattr(self.args, "gradient_accumulation_steps", 1)))
+        first, final = self._micro == 0, self._micro >= k - 1
+        self._micro = 0 if final else self._micro + 1
         if getattr(self.args, "fused", True) and getattr(self.args, "pack", False) and \
                 batch_data["input_ids"].shape[1] == 128 and not batch_data["input_ids"].is_cuda:
             from .packing import pack_batch
             packed = pack_batch(batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"])
             key = (packed["bins"], batch_data["input_ids"].shape[0])
-            if key not in self._packed:
+            if key not in self._packed or self._packed[key].accum_steps != k:
                 if len(self._packed) >= 16:           # bound the graph cache: drop the oldest entry
                     self._packed.pop(next(iter(self._packed)))
-                self._packed[key] = PackedTrainStep(self.model, self.optimizer, key[0], key[1])
+                self._packed[key] = PackedTrainStep(self.model, self.optimizer, key[0], key[1], accum_steps=k)
             self.model.train()
-            loss = self._packed[key](packed, batch_data["label"])
+            loss = self._packed[key](packed, batch_data["label"], final)
         elif getattr(self.args, "fused", True):
             B, S = batch_data["input_ids"].shape
-            if self._fused is None or (self._fused.B, self._fused.S) != (B, S):
-                self._fused = FusedTrainStep(self.model, self.optimizer, B, S)
+            if self._fused is None or (self._fused.B, self._fused.S, self._fused.accum_steps) != (B, S, k):
+                self._fused = FusedTrainStep(self.model, self.optimizer, B, S, accum_steps=k)
             self.model.train()
-            loss = self._fused(batch_data)
+            loss = self._fused(batch_data, final)
         elif getattr(self.args, "use_amp", False):
             # the -amp scripts' loop body (multi-gpu-distributed-mp-amp-cls.py:166-171), scaler created once
             if self._scaler is None:
                 self._scaler = torch.amp.GradScaler("cuda")
             self.model.train()
-            with torch.autocast("cuda"):
+            with self._window(final):
+                with torch.autocast("cuda"):
+                    logits, label = self.on_step(batch_data)
+                    loss = self.criterion(logits, label)
+                self._scaler.scale(loss / k if k > 1 else loss).backward()
+            if final:
+                self._scaler.step(self.optimizer)
+                self._scaler.update()
+        else:
+            self.model.train()
+            with self._window(final):
                 logits, label = self.on_step(batch_data)
                 loss = self.criterion(logits, label)
-            self._scaler.scale(loss).backward()
+                if first:
+                    self.optimizer.zero_grad()
+                (loss / k if k > 1 else loss).backward()
+            if final:
+                self.optimizer.step()
+        return self.loss_reduce(loss.detach())
+
+    def _window(self, final):
+        """the eager loops' micro-batches run inside no_sync(), the final one of a window outside it"""
+        return contextlib.nullcontext() if final else self.model.no_sync()
+
+    def close_window(self):
+        """Steps the optimizer on a partial accumulation window (end of an epoch, as HF Trainer does); the 1/k scale
+        stays.  No-op when no window is open."""
+        if self._micro == 0:
+            return
+        self._micro = 0
+        if self._scaler is not None and not getattr(self.args, "fused", True):
             self._scaler.step(self.optimizer)
             self._scaler.update()
         else:
-            self.model.train()
-            logits, label = self.on_step(batch_data)
-            loss = self.criterion(logits, label)
-            self.optimizer.zero_grad()
-            loss.backward()
             self.optimizer.step()
-        return self.loss_reduce(loss.detach())
 
     def train(self, train_loader, dev_loader=None, train_sampler=None):
         gloabl_step = 1
@@ -406,6 +461,7 @@ class Trainer:
                                 # rank 0 alone, as in the reference [:190-192]: under DDP state_dict() pulls the fp32
                                 # slices other ranks own out of their HBM one-sidedly (ddp.py::_gather_master)
                                 torch.save(self.model.state_dict(), self.args.ckpt_path)
+            self.close_window()
         if self.args.local_rank == 0:
             end = time.time()
             print("耗时：{}分钟".format((end - start) / 60))
