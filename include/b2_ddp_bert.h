@@ -28,7 +28,7 @@ extern "C" {
 /* ------------------------------------------------------------------------------------------------------ */
 const char* b2_last_error(void);
 int32_t b2_abi_version(void);             /* bumped when a struct below changes */
-#define B2_ABI_VERSION 18
+#define B2_ABI_VERSION 19
 int64_t b2_launch_count(void);            /* kernels launched by this library so far (process-wide) */
 
 /* ------------------------------------------------------------------------------------------------------ */
@@ -274,27 +274,7 @@ typedef struct b2_adamw_hparams {
   /* optional DEVICE pointer to the GradScaler's fp32 inf/nan indicator: a non-zero value skips the update (and the
    * step count), as GradScaler.step() skips optimizer.step().  NULL = always update.                            */
   const float* found_inf;
-  /* optional DEVICE uint8 per 8-element vector (indexed like decay_flags): non-zero = this vector was already
-   * updated elsewhere (b2_gemm_bf16_grouped_adamw) and is skipped.  NULL = update everything in [begin, end).     */
-  const uint8_t* skip_flags;
 } b2_adamw_hparams_t;
-
-/* The layer's weight gradients AND their HF-AdamW update in one launch (single-GPU step: no exchange between the
- * gradient and the update): b2_gemm_bf16_grouped whose epilogue, for every output element, rounds the gradient to
- * bf16 (still written to D_i), updates exp_avg / exp_avg_sq / the fp32 master weight of the same element in place
- * and writes the bf16 shadow weight.  targets[i] addresses the optimizer state of problem i's [M_i, N_i] block
- * (row pitch = args[i].ldd elements); decay != 0 applies hp->weight_decay.  Same arithmetic as
- * b2_bucket_reduce_adamw; hp->grad_scale / found_inf must be NULL.  The problems must be groupable (see
- * b2_gemm_bf16_grouped) -- this entry point fails instead of falling back.                                       */
-typedef struct b2_fused_adamw_target {
-  float* master;
-  float* exp_avg;
-  float* exp_avg_sq;
-  void* shadow; /* bf16 */
-  int32_t decay;
-} b2_fused_adamw_target_t;
-int32_t b2_gemm_bf16_grouped_adamw(const b2_gemm_args_t* args, const b2_fused_adamw_target_t* targets, int32_t count,
-                                   const b2_adamw_hparams_t* hp, const int64_t* step_counter, void* stream);
 
 /* Fused update of one contiguous slice [begin, end) (element indices, multiples of 8) of the flat parameter
  * space.  world == 1: grads read from `grad_local`.  world > 1: element-wise mean over `peer_grads[0..world)`

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2ddpbert.so")
-ABI_VERSION = 18
+ABI_VERSION = 19
 
 MAJOR_K, MAJOR_MN = 0, 1
 EPI_NONE, EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_DROPOUT_RESIDUAL, EPI_RESIDUAL, EPI_GELU_BWD = 0, 1, 2, 3, 4, 5
@@ -35,19 +35,13 @@ class GemmArgs(C.Structure):
 
 class AdamWHParams(C.Structure):
     _fields_ = [("lr", f64), ("beta1", f64), ("beta2", f64), ("eps", f64), ("weight_decay", f64),
-                ("correct_bias", i32), ("grad_scale", vp), ("found_inf", vp), ("skip_flags", vp)]
-
-
-class FusedAdamWTarget(C.Structure):
-    _fields_ = [("master", vp), ("exp_avg", vp), ("exp_avg_sq", vp), ("shadow", vp), ("decay", i32)]
+                ("correct_bias", i32), ("grad_scale", vp), ("found_inf", vp)]
 
 
 # name -> argtypes; every function returns int32 status unless listed in _SPECIAL
 _SIGNATURES = {
     "b2_gemm_bf16": [C.POINTER(GemmArgs), vp],
     "b2_gemm_bf16_grouped": [C.POINTER(GemmArgs), i32, vp],
-    "b2_gemm_bf16_grouped_adamw": [C.POINTER(GemmArgs), C.POINTER(FusedAdamWTarget), i32, C.POINTER(AdamWHParams), vp,
-                                   vp],
     "b2_gemm_ln_fwd": [C.POINTER(GemmArgs), vp, vp, f32, vp, i64, vp, i64, vp, vp, vp],
     "b2_embed_fwd": [vp, vp, i64, i64, vp, vp, vp, vp, vp, i64, i64, i64, f32, f32, vp, u32, vp, vp, vp, vp, vp, vp,
                      vp, vp],

@@ -15,14 +15,6 @@ namespace b2 {
 static thread_local char g_err[1024] = "";
 static std::atomic<long long> g_launches{0};
 void count_launches(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B2_PDL");
-    v = (e != nullptr && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
 
 void set_error(const char* fmt, ...) {
   va_list ap;

@@ -638,15 +638,6 @@ constexpr int kFwdSmem = 5 * TILE_BYTES + 128 + 1024;
 constexpr int kFwd128Smem = 3 * TILE_BYTES + 64 + 1024;
 constexpr int kBwdSmem = 8 * TILE_BYTES + 64 + 512 + 1024;
 
-// B2_ATTN_FWD128=0 keeps seq == 128 on the general forward kernel (A/B measurements)
-static bool fwd128_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B2_ATTN_FWD128");
-    v = (e != nullptr && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
 constexpr int kBwdSmemOneQ = 7 * TILE_BYTES + 64 + 512 + 1024;
 
 static int32_t check_attn_shapes(const char* who, int64_t batch, int64_t seq, int64_t heads, int64_t head_dim) {
@@ -669,7 +660,7 @@ static int32_t attention_fwd_impl(const void* qkv, const int64_t* attention_mask
                                   uint64_t* keep_bits, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   B2_REQUIRE(qkv && ctx, "attention_fwd: null pointer");
-  B2_REQUIRE(segments == nullptr || (seq == 128 && fwd128_enabled()),
+  B2_REQUIRE(segments == nullptr || seq == 128,
              "attention_fwd: packed bins are 128 tokens long (seq=%lld)", (long long)seq);
   int32_t st = check_attn_shapes("attention_fwd", batch, seq, heads, head_dim);
   if (st) return st;
@@ -686,7 +677,7 @@ static int32_t attention_fwd_impl(const void* qkv, const int64_t* attention_mask
   p.seg = segments;
   p.ctx = (__nv_bfloat16*)ctx; p.lse = lse;
   // the keep-bit cache exists for the seq == 128 kernel pair only (and only when there is dropout to remember)
-  p.keep_bits = (seq == 128 && dropout_p > 0.f && fwd128_enabled()) ? (unsigned long long*)keep_bits : nullptr;
+  p.keep_bits = (seq == 128 && dropout_p > 0.f) ? (unsigned long long*)keep_bits : nullptr;
   static bool attr = false;
   if (!attr) {
     B2_CUDA(cudaFuncSetAttribute(attention_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmem));
@@ -696,7 +687,7 @@ static int32_t attention_fwd_impl(const void* qkv, const int64_t* attention_mask
   st = get_tensor_map_2d(&tm_ctx, ctx, (uint64_t)tokens, (uint64_t)hidden, (uint64_t)(hidden * 2), 128, 64);
   if (st) return st;
   dim3 grid((unsigned)(seq / 128), (unsigned)heads, (unsigned)batch);
-  if (seq == 128 && fwd128_enabled()) {
+  if (seq == 128) {
     static bool attr128 = false;
     if (!attr128) {
       B2_CUDA(cudaFuncSetAttribute(attention_fwd128_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -778,7 +769,7 @@ static int32_t attention_bwd_impl(const void* qkv, const int64_t* attention_mask
   B2_REQUIRE(dbias_accum == nullptr || seq == 128,
              "attention_bwd: the fused QKV bias gradient covers seq == 128 (longer sequences: use b2_colsum)");
   p.dbias = dbias_accum;
-  p.keep_bits = (seq == 128 && dropout_p > 0.f && fwd128_enabled()) ? (unsigned long long*)keep_bits : nullptr;
+  p.keep_bits = (seq == 128 && dropout_p > 0.f) ? (unsigned long long*)keep_bits : nullptr;
   if (p.dq_accum) B2_CUDA(cudaMemsetAsync(p.dq_accum, 0, (size_t)tokens * hidden * 4, stream));
   static bool attr = false;
   if (!attr) {

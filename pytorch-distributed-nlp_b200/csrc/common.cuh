@@ -43,7 +43,6 @@ int32_t get_tensor_map_2d(CUtensorMap* out, const void* base, uint64_t rows, uin
 // kernel launch: cudaLaunchKernelEx with the programmatic-stream-serialization attribute (PDL), so that back-to-back
 // kernels of a step (318 per step, captured in one CUDA graph) overlap launch latency with the predecessor's tail
 // ----------------------------------------------------------------------------------------------
-bool pdl_enabled();
 template <typename... KArgs, typename... Args>
 inline void launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
                           Args&&... args) {
@@ -54,7 +53,7 @@ inline void launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);   // errors surface via cudaGetLastError()

@@ -174,125 +174,12 @@ constexpr int kMaxGroup = 4;
 struct GroupedProblem {
   int M, N, tiles_n, tile_begin;   // tile_begin: first global work index of this problem
   __nv_bfloat16* D; long long ldd;
-  // fused AdamW (optional): optimizer state holding the same [M, N] elements with the same row pitch
-  float* w; float* m; float* v; __nv_bfloat16* shadow; int decay;
 };
 struct GroupedParams {
   int count, num_work, kblocks;
   GroupedProblem pr[kMaxGroup];
-  // fused HF-AdamW (adamw != 0): the weight gradient never makes a round trip through HBM before the update
-  int adamw, correct_bias;
-  float lr, beta1, beta2, one_minus_beta1, one_minus_beta2, eps, lr_wd;
-  double lr_d, beta1_d, beta2_d;
-  const long long* step_counter;
 };
 
-// Epilogue of the grouped weight-gradient kernel with the optimizer fused in (single-GPU training step): the fp32
-// accumulator is rounded to bf16 (exactly the gradient the unfused path stores and reads back), then exp_avg,
-// exp_avg_sq and the fp32 master weight of the same elements make one round trip each through the warp's staging
-// tile (coalesced 128-byte rows in, update, coalesced rows out), and the bf16 shadow weight and the bf16 gradient
-// are written.  Same arithmetic, statement for statement, as reduce_adamw_kernel (csrc/optim.cu).  The extra
-// ~26 bytes per parameter move in the GEMM's epilogue instead of in a separate HBM-bound kernel.
-__device__ __forceinline__ void epilogue_tile_adamw(const GroupedProblem& pr, const GroupedParams& gp, float step_size,
-                                                    const float* acc, int acc_ld, int warp, int lane, int m_base,
-                                                    int n0, uint8_t* stage) {
-  constexpr int BN = 256;
-  constexpr int kColsPerWarp = BN / 2;
-  const int quarter = warp & 3, cgrp = (warp - 4) >> 2;
-  const int row0 = m_base + quarter * 32;
-  const int rows_valid = pr.M - row0;
-  const int nw = n0 + cgrp * kColsPerWarp;
-  const float* arow = acc + (size_t)(quarter * 32 + lane) * acc_ld + cgrp * kColsPerWarp;
-  const bool any = rows_valid > 0;
-  auto fetch = [&](const float* base, int n) {
-    tile_g2s_async<8>(stage, reinterpret_cast<const uint8_t*>(base + (size_t)row0 * pr.ldd + n), pr.ldd * 4, lane,
-                      rows_valid);
-  };
-  auto put = [&](float* base, int n) {
-    tile_s2g<8>(stage, reinterpret_cast<uint8_t*>(base + (size_t)row0 * pr.ldd + n), pr.ldd * 4, lane, rows_valid);
-  };
-  if (any && nw < pr.N) fetch(pr.m, nw);   // first exp_avg tile
-#pragma unroll 1
-  for (int c = 0; c < kColsPerWarp / 32; ++c) {
-    const int n = nw + c * 32;
-    float g[32];
-    {
-      uint32_t v[32];
-      acc_ld32(arow + c * 32, v);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) g[j] = __uint_as_float(v[j]);
-    }
-    if (!(any && n < pr.N)) continue;
-    // the gradient as the rest of the system sees it: bf16
-#pragma unroll
-    for (int j = 0; j < 32; j += 2) (void)pack_bf16_round(g[j], g[j + 1]);
-    float u[32];   // exp_avg (new), then the update direction, then the new weight
-    if (c > 0) fetch(pr.m, n);
-    tile_async_wait();
-    __syncwarp();
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      uint4* q = stage_ptr<8>(stage, lane, k);
-      const uint4 t = *q;
-      u[4 * k + 0] = __uint_as_float(t.x) * gp.beta1 + g[4 * k + 0] * gp.one_minus_beta1;
-      u[4 * k + 1] = __uint_as_float(t.y) * gp.beta1 + g[4 * k + 1] * gp.one_minus_beta1;
-      u[4 * k + 2] = __uint_as_float(t.z) * gp.beta1 + g[4 * k + 2] * gp.one_minus_beta1;
-      u[4 * k + 3] = __uint_as_float(t.w) * gp.beta1 + g[4 * k + 3] * gp.one_minus_beta1;
-      *q = make_uint4(__float_as_uint(u[4 * k]), __float_as_uint(u[4 * k + 1]), __float_as_uint(u[4 * k + 2]),
-                      __float_as_uint(u[4 * k + 3]));
-    }
-    __syncwarp();
-    put(pr.m, n);
-    __syncwarp();
-    fetch(pr.v, n);
-    tile_async_wait();
-    __syncwarp();
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      uint4* q = stage_ptr<8>(stage, lane, k);
-      const uint4 t = *q;
-      float vv[4] = {__uint_as_float(t.x), __uint_as_float(t.y), __uint_as_float(t.z), __uint_as_float(t.w)};
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float gk = g[4 * k + i];
-        vv[i] = vv[i] * gp.beta2 + gk * gk * gp.one_minus_beta2;
-        u[4 * k + i] = u[4 * k + i] / (sqrtf(vv[i]) + gp.eps);
-      }
-      *q = make_uint4(__float_as_uint(vv[0]), __float_as_uint(vv[1]), __float_as_uint(vv[2]), __float_as_uint(vv[3]));
-    }
-    __syncwarp();
-    put(pr.v, n);
-    __syncwarp();
-    fetch(pr.w, n);
-    tile_async_wait();
-    __syncwarp();
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      uint4* q = stage_ptr<8>(stage, lane, k);
-      const uint4 t = *q;
-      float ww[4] = {__uint_as_float(t.x), __uint_as_float(t.y), __uint_as_float(t.z), __uint_as_float(t.w)};
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        ww[i] = ww[i] - step_size * u[4 * k + i];
-        if (pr.decay) ww[i] = ww[i] - gp.lr_wd * ww[i];
-        u[4 * k + i] = ww[i];
-      }
-      *q = make_uint4(__float_as_uint(ww[0]), __float_as_uint(ww[1]), __float_as_uint(ww[2]), __float_as_uint(ww[3]));
-    }
-    __syncwarp();
-    put(pr.w, n);
-    __syncwarp();
-    // bf16 outputs (64-byte rows): the shadow weight the next forward reads, and the gradient itself
-    row_write32<4>(stage, lane, 0, u);
-    __syncwarp();
-    tile_s2g<4>(stage, reinterpret_cast<uint8_t*>(pr.shadow + (size_t)row0 * pr.ldd + n), pr.ldd * 2, lane, rows_valid);
-    __syncwarp();
-    row_write32<4>(stage, lane, 0, g);
-    __syncwarp();
-    tile_s2g<4>(stage, reinterpret_cast<uint8_t*>(pr.D + (size_t)row0 * pr.ldd + n), pr.ldd * 2, lane, rows_valid);
-    __syncwarp();
-  }
-}
 struct GroupedMaps {
   CUtensorMap a[kMaxGroup], b[kMaxGroup];
 };
@@ -332,19 +219,6 @@ gemm_grouped_tn_kernel(const __grid_constant__ GroupedMaps maps, const GroupedPa
                                 lane);
   if (warp < 4) return;
   uint8_t* stage = epi_stage + (warp - 4) * kEpiStageBytes;
-  if (gp.adamw) {
-    // HF AdamW bias correction (as reduce_adamw_kernel): step_size = lr * sqrt(1 - b2^t) / (1 - b1^t)
-    float step_size = gp.lr;
-    if (gp.correct_bias) {
-      const long long t = *gp.step_counter + 1;
-      const double bc1 = 1.0 - pow(gp.beta1_d, (double)t);
-      const double bc2 = 1.0 - pow(gp.beta2_d, (double)t);
-      step_size = (float)(gp.lr_d * sqrt(bc2) / bc1);
-    }
-    epilogue_tile_adamw(pr, gp, step_size, reinterpret_cast<const float*>(smem), Cfg::kAccLd, warp, lane, m0, n0,
-                        stage);
-    return;
-  }
   GemmKernelParams q;
   q.splits = 1; q.epilogue = B2_EPI_NONE; q.bias = nullptr; q.aux_in = nullptr; q.aux_out = nullptr;
   q.partial = nullptr; q.dropout_p = 0.f; q.rng = nullptr; q.rng_site = 0; q.timing = nullptr; q.colsum = nullptr;
@@ -536,8 +410,7 @@ extern "C" int32_t b2_gemm_bf16(const b2_gemm_args_t* a, void* stream_) {
   return -2;
 }
 
-static int32_t gemm_grouped_impl(const b2_gemm_args_t* args, int32_t count, const b2_fused_adamw_target_t* targets,
-                                 const b2_adamw_hparams_t* hp, const int64_t* step_counter, void* stream_) {
+extern "C" int32_t b2_gemm_bf16_grouped(const b2_gemm_args_t* args, int32_t count, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   B2_REQUIRE(args != nullptr && count >= 1, "b2_gemm_bf16_grouped: no problems");
   // the one-launch path covers what the weight-gradient step needs: TN layouts, plain bf16 output, 256-wide tiles,
@@ -551,18 +424,6 @@ static int32_t gemm_grouped_impl(const b2_gemm_args_t* args, int32_t count, cons
                 a.ldd % 8 == 0 && ((uintptr_t)a.A % 16 == 0) && ((uintptr_t)a.B % 16 == 0) &&
                 ((uintptr_t)a.D % 16 == 0) && a.force_splits <= 1 &&
                 (a.force_bn == 0 || a.force_bn == 256);
-  }
-  if (targets != nullptr) {
-    B2_REQUIRE(groupable, "b2_gemm_bf16_grouped_adamw: the problems do not fit the grouped kernel (TN layouts, plain "
-                          "bf16 output, N %% 256 == 0, one K, at most %d)", kMaxGroup);
-    B2_REQUIRE(hp != nullptr && step_counter != nullptr, "b2_gemm_bf16_grouped_adamw: null optimizer arguments");
-    B2_REQUIRE(hp->grad_scale == nullptr && hp->found_inf == nullptr,
-               "b2_gemm_bf16_grouped_adamw: GradScaler state is not supported on the fused path");
-    for (int i = 0; i < count; ++i)
-      B2_REQUIRE(targets[i].master && targets[i].exp_avg && targets[i].exp_avg_sq && targets[i].shadow &&
-                     ((uintptr_t)targets[i].master % 16 == 0) && ((uintptr_t)targets[i].exp_avg % 16 == 0) &&
-                     ((uintptr_t)targets[i].exp_avg_sq % 16 == 0) && ((uintptr_t)targets[i].shadow % 16 == 0),
-                 "b2_gemm_bf16_grouped_adamw: null / misaligned optimizer state for problem %d", i);
   }
   if (!groupable) {
     for (int i = 0; i < count; ++i) {
@@ -585,25 +446,7 @@ static int32_t gemm_grouped_impl(const b2_gemm_args_t* args, int32_t count, cons
     GroupedProblem& g = gp.pr[i];
     g.M = (int)a.M; g.N = (int)a.N; g.tiles_n = (int)(a.N / 256); g.tile_begin = work;
     g.D = (__nv_bfloat16*)a.D; g.ldd = a.ldd;
-    g.w = nullptr; g.m = nullptr; g.v = nullptr; g.shadow = nullptr; g.decay = 0;
-    if (targets != nullptr) {
-      g.w = targets[i].master; g.m = targets[i].exp_avg; g.v = targets[i].exp_avg_sq;
-      g.shadow = (__nv_bfloat16*)targets[i].shadow; g.decay = targets[i].decay ? 1 : 0;
-    }
     work += (int)((a.M + BM - 1) / BM) * g.tiles_n;
-  }
-  gp.adamw = targets != nullptr ? 1 : 0;
-  gp.correct_bias = 0; gp.lr = gp.beta1 = gp.beta2 = gp.one_minus_beta1 = gp.one_minus_beta2 = gp.eps = gp.lr_wd = 0.f;
-  gp.lr_d = gp.beta1_d = gp.beta2_d = 0.0; gp.step_counter = nullptr;
-  if (targets != nullptr) {   // same roundings as b2_bucket_reduce_adamw
-    gp.lr_d = hp->lr; gp.beta1_d = hp->beta1; gp.beta2_d = hp->beta2;
-    gp.lr = (float)hp->lr; gp.beta1 = (float)hp->beta1; gp.beta2 = (float)hp->beta2;
-    gp.one_minus_beta1 = (float)(1.0 - hp->beta1); gp.one_minus_beta2 = (float)(1.0 - hp->beta2);
-    gp.eps = (float)hp->eps; gp.lr_wd = (float)(hp->lr * hp->weight_decay);
-    gp.correct_bias = hp->correct_bias;
-    gp.step_counter = (const long long*)step_counter;
-    if (!(hp->weight_decay > 0.0))
-      for (int i = 0; i < count; ++i) gp.pr[i].decay = 0;
   }
   for (int i = count; i < kMaxGroup; ++i) { gp.pr[i] = gp.pr[0]; gp.pr[i].tile_begin = 0x7fffffff; maps.a[i] = maps.a[0]; maps.b[i] = maps.b[0]; }
   gp.num_work = work;
@@ -617,15 +460,4 @@ static int32_t gemm_grouped_impl(const b2_gemm_args_t* args, int32_t count, cons
   B2_CUDA(cudaGetLastError());
   count_launches(1);
   return 0;
-}
-
-extern "C" int32_t b2_gemm_bf16_grouped(const b2_gemm_args_t* args, int32_t count, void* stream_) {
-  return gemm_grouped_impl(args, count, nullptr, nullptr, nullptr, stream_);
-}
-
-extern "C" int32_t b2_gemm_bf16_grouped_adamw(const b2_gemm_args_t* args, const b2_fused_adamw_target_t* targets,
-                                              int32_t count, const b2_adamw_hparams_t* hp,
-                                              const int64_t* step_counter, void* stream_) {
-  B2_REQUIRE(targets != nullptr, "b2_gemm_bf16_grouped_adamw: null targets");
-  return gemm_grouped_impl(args, count, targets, hp, step_counter, stream_);
 }

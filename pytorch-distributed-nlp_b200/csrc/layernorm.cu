@@ -396,15 +396,6 @@ static int num_sms() {
   }
   return n;
 }
-// B2_LN_BWD_PAIR=0 falls back to the one-warp-per-row kernel (A/B measurements)
-static bool ln_bwd_pair() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B2_LN_BWD_PAIR");
-    v = (e != nullptr && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
 
 int32_t launch_layernorm_bwd(const void* dy, const void* dy_add, const void* x, const float* mean, const float* rstd,
                              const void* gamma, int64_t rows, int64_t hidden, float dropout_p, const void* rng,
@@ -429,7 +420,7 @@ int32_t launch_layernorm_bwd(const void* dy, const void* dy_add, const void* x, 
     else B2_LAUNCH((layernorm_bwd_kernel<VPL_, false, false>), nblocks, 256, 0, stream, B2_LN_ARGS);                  \
     break;
   B2_REQUIRE(dy_f32 || !dx_f32, "layernorm_bwd: fp32 dx with bf16 dy is not on the path");
-  const bool paired = dy_f32 && dx_f32 && mode == 0 && dy_add == nullptr && dx_drop != nullptr && ln_bwd_pair();
+  const bool paired = dy_f32 && dx_f32 && mode == 0 && dy_add == nullptr && dx_drop != nullptr;
   if (paired) {
     // one resident 512-thread block per SM: a single wave, rows strided over the whole grid
     if (nblocks > num_sms()) nblocks = num_sms();

@@ -30,7 +30,6 @@ struct ReduceAdamWParams {
   const long long* step_counter;
   const float* grad_scale;   // optional device scalar (GradScaler): gradients are divided by it
   const float* found_inf;    // optional device scalar (GradScaler): non-zero skips the update
-  const uint8_t* skip;       // optional per-vector flags: already updated by the fused wgrad epilogue
 };
 
 __global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWParams p) {
@@ -51,7 +50,6 @@ __global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWPara
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec;
        i += (long long)gridDim.x * blockDim.x) {
     const long long e = p.begin + (i << 3);
-    if (p.skip != nullptr && p.skip[e >> 3]) continue;
     float g[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 #pragma unroll
     for (int r = 0; r < MAX_WORLD; ++r) {
@@ -320,7 +318,6 @@ extern "C" int32_t b2_bucket_reduce_adamw(const void* const* peer_grads, void* c
   p.step_counter = (const long long*)step_counter;
   p.grad_scale = hp->grad_scale;
   p.found_inf = hp->found_inf;
-  p.skip = hp->skip_flags;
   const long long nvec = (end - begin) >> 3;
   long long blocks = (nvec + 255) / 256;
   const long long cap = 132 * 8;   // 8 blocks per SM of an H100
@@ -348,8 +345,8 @@ extern "C" int32_t b2_adamw_background(const void* grads, void* shadow, float* m
              "adamw_background: null pointer");
   B2_REQUIRE(begin >= 0 && end >= begin && begin % 8 == 0 && end % 8 == 0,
              "adamw_background: slice [%lld,%lld) must be 8-element aligned", (long long)begin, (long long)end);
-  B2_REQUIRE(hp->grad_scale == nullptr && hp->found_inf == nullptr && hp->skip_flags == nullptr,
-             "adamw_background: GradScaler state / skip flags are handled by b2_bucket_reduce_adamw");
+  B2_REQUIRE(hp->grad_scale == nullptr && hp->found_inf == nullptr,
+             "adamw_background: GradScaler state is handled by b2_bucket_reduce_adamw");
   if (end == begin) return 0;
   static bool attr = false;
   if (!attr) {   // same shared-memory carve-out as the GEMM CTAs it is meant to run beside

@@ -405,8 +405,6 @@ class BertForSequenceClassification(nn.Module):
         return torch.nn.modules.module._IncompatibleKeys(missing, unexpected)
 
     def state_dict(self, *args, **kwargs):
-        if self._optimizer is not None:
-            self._optimizer.flush_pending()      # a pipelined train step may still owe its update
         if self._ddp is not None:
             self._ddp._gather_master()
         return super().state_dict(*args, **kwargs)
@@ -421,8 +419,6 @@ class BertForSequenceClassification(nn.Module):
                                "there is no CPU path.")
         if input_ids is None:
             raise ValueError("input_ids is required")
-        if self._optimizer is not None:
-            self._optimizer.flush_pending()      # a pipelined train step may still owe its update
         packed = None
         if segments is not None or cls_index is not None:
             if position_ids is None or segments is None or cls_index is None:
@@ -483,31 +479,19 @@ class _Engine:
         self._saved = None
         self.wgrad_stream = torch.cuda.Stream(device=self.dev)
         self.opt_stream = torch.cuda.Stream(device=self.dev)
-        self.accum_dgrad = os.environ.get("B2_ACCUM_DGRAD", "1") != "0"
-        self.grouped_wgrad = os.environ.get("B2_GROUPED_WGRAD", "1") != "0"
-        # experimental, off: the epilogue's optimizer-state round trips (one 4 KB staging tile per warp) keep too few
-        # bytes in flight to beat the separate per-bucket AdamW launches; see DESIGN.md
-        self.fused_adamw = os.environ.get("B2_FUSED_ADAMW", "0") == "1"
-        self.fused_adamw_active = False
         # gradient accumulation (no_sync(), Trainer gradient_accumulation_steps): fp32 accumulator over the flat space,
-        # allocated on first use (local even under DDP); accum_in_use switches off the paths that update before a fold
-        # could happen (the fused-epilogue and the pipelined AdamW); accum_live = the accumulator holds gradients no
-        # fold / flush has consumed yet; _pass_op = the b2_grad_accumulate mode of the running backward (None: none)
+        # allocated on first use (local even under DDP); accum_in_use = some backward has accumulated into it;
+        # accum_live = the accumulator holds gradients no fold / flush has consumed yet; _pass_op = the
+        # b2_grad_accumulate mode of the running backward (None: none)
         self.accum = None
         self.accum_in_use = False
         self.accum_live = False
         self._pass_op = None
         self._pass_stream = None
-        # cache of the forward's attention-dropout decisions for the backward (1 bit per (b, h, q, k), bit-exact against
-        # the Philox replica): the backward reads them instead of regenerating Philox; B2_ATTN_KEEP_BITS=0 regenerates
-        # the masks in the backward instead
-        self.attn_keep_bits = os.environ.get("B2_ATTN_KEEP_BITS", "1") != "0"
-        self.use_wgrad_stream = os.environ.get("B2_WGRAD_STREAM", "1") != "0"
         # dense + bias + dropout + residual + LayerNorm as ONE cluster kernel (b2_gemm_ln_fwd) for the two N = hidden
         # GEMMs of a layer, when the hidden size has a row-cluster tiling (768, 1024) and the device can co-schedule
-        # the 3- / 4-CTA clusters; otherwise (and with B2_FUSED_LN=0) the GEMM epilogue + separate LayerNorm launch
-        self.fused_ln = (os.environ.get("B2_FUSED_LN", "1") != "0" and self.H in (768, 1024) and
-                         int(L.load().b2_gemm_ln_max_clusters(self.H)) > 0)
+        # the 3- / 4-CTA clusters; otherwise the GEMM epilogue + separate LayerNorm launch
+        self.fused_ln = self.H in (768, 1024) and int(L.load().b2_gemm_ln_max_clusters(self.H)) > 0
         # fp32 accumulators for the bias gradients that kernels produce as a side effect of their epilogues (QKV bias
         # from attention backward, intermediate bias from the GELU' dgrad): per layer [3H | I]; one finishing launch
         # per step turns them into bf16 gradients and re-zeroes them
@@ -622,8 +606,7 @@ class _Engine:
             "layers": [
                 {"qkv": e(M, 3 * H), "ctx": e(M, H), "lse": e(B * self.heads * S, dtype=f32),
                  # attention-dropout decisions of the forward, 1 bit per (b, h, q, k): read back by the backward
-                 "keep": (e(B * self.heads * S * (S // 64), dtype=torch.int64)
-                          if (S == 128 and self.attn_keep_bits) else None),
+                 "keep": e(B * self.heads * S * (S // 64), dtype=torch.int64) if S == 128 else None,
                  "z1": e(M, H),
                  "x1": e(M, H), "mean1": e(M, dtype=f32), "rstd1": e(M, dtype=f32), "u": e(M, I), "h": e(M, I),
                  "z2": e(M, H), "x2": e(M, H), "mean2": e(M, dtype=f32), "rstd2": e(M, dtype=f32),
@@ -634,8 +617,8 @@ class _Engine:
             "dlogits": e(Bo, self.C, dtype=f32), "dloss_logits": e(Bo, self.C, dtype=f32),
             # gradient of the residual stream: fp32 (12 layers of residual adds would otherwise each round it to bf16);
             # dzd / dz1d are the bf16 (dropout-masked) copies the tensor cores consume
-            "dxA": e(M, H, dtype=f32), "dxB": e(M, H, dtype=f32), "dz": e(M, H, dtype=f32),
-            "dz1": e(M, H, dtype=f32), "emb_dx": e(M, H), "dctx": e(M, H), "head_scratch": e(2 * Bo, H, dtype=f32),
+            "dxA": e(M, H, dtype=f32), "dxB": e(M, H, dtype=f32),
+            "emb_dx": e(M, H), "dctx": e(M, H), "head_scratch": e(2 * Bo, H, dtype=f32),
             # operands of the weight-gradient GEMMs, double-buffered by layer parity (see _backward_from_dlogits)
             "dzd": [e(M, H), e(M, H)], "dz1d": [e(M, H), e(M, H)], "dU": [e(M, I), e(M, I)],
             "dqkv": [e(M, 3 * H), e(M, 3 * H)],
@@ -665,9 +648,7 @@ class _Engine:
             a.workspace, a.workspace_bytes = self.split_ws.data_ptr(), self.split_ws.numel()
         else:
             a.workspace, a.workspace_bytes = None, 0
-        a.force_bn = int(os.environ.get("B2_FORCE_BN", "0"))
-        a.force_splits = 0
-        a.force_kernel = int(os.environ.get("B2_FORCE_KERNEL", "0"))
+        a.force_bn = a.force_splits = a.force_kernel = 0
         a.debug_timing = None
         a.colsum_out = colsum
         if defer is not None:
@@ -701,12 +682,9 @@ class _Engine:
         L.call("b2_layernorm_fwd", z, gamma, beta, M, H, eps, y, mean, rstd, s)
 
     # ---- forward --------------------------------------------------------------------------------------------------------
-    def forward(self, input_ids, token_type_ids, attention_mask, labels, training, need_backward, packed=None,
-                weight_events=None):
+    def forward(self, input_ids, token_type_ids, attention_mask, labels, training, need_backward, packed=None):
         """packed: None, or (position_ids int64 [bins, 128], segments int32 [bins, 128], cls_index int64 [batch]) --
-        the rows of `input_ids` are then 128-token bins produced by packing.pack_batch, not sequences.
-        weight_events: None, or one event per bucket (forward order) after which that bucket's bf16 weights are
-        current (pipelined optimizer, optim.AdamW.apply_pending): each is awaited right before its first use."""
+        the rows of `input_ids` are then 128-token bins produced by packing.pack_batch, not sequences."""
         cfg, H, I = self.cfg, self.H, self.I
         if input_ids.dim() != 2:
             raise ValueError("input_ids must be [batch, seq]")
@@ -750,9 +728,6 @@ class _Engine:
         w = self.w
         KM, MN = L.MAJOR_K, L.MAJOR_MN
 
-        cur = torch.cuda.current_stream(self.dev)
-        if weight_events is not None:
-            cur.wait_event(weight_events[0])
         emb_w = (w("bert.embeddings.word_embeddings.weight"), w("bert.embeddings.position_embeddings.weight"),
                  w("bert.embeddings.token_type_embeddings.weight"), w("bert.embeddings.LayerNorm.weight"),
                  w("bert.embeddings.LayerNorm.bias"))
@@ -769,8 +744,6 @@ class _Engine:
         for l in range(self.nl):
             a = ws["layers"][l]
             pre = "bert.encoder.layer.%d." % l
-            if weight_events is not None:
-                cur.wait_event(weight_events[1 + l])
             self.gemm(M, 3 * H, H, x.data_ptr(), H, KM, w(pre + "attention.self.query.weight"), H, KM,
                       a["qkv"].data_ptr(), 3 * H, L.EPI_BIAS, bias=w(pre + "attention.self.query.bias"))
             if packed is None:
@@ -794,8 +767,6 @@ class _Engine:
                 w(pre + "output.LayerNorm.bias"), a["z2"].data_ptr(), a["x2"].data_ptr(), L.ptr(a["x2f"]),
                 a["mean2"].data_ptr(), a["rstd2"].data_ptr())
             x, xf = a["x2"], a["x2f"]
-        if weight_events is not None:
-            cur.wait_event(weight_events[-1])         # the head's bucket (the last layer's, or its own)
         head_w = (w("bert.pooler.dense.weight"), w("bert.pooler.dense.bias"), w("classifier.weight"),
                   w("classifier.bias"))
         if packed is None:
@@ -856,40 +827,25 @@ class _Engine:
         # data gradient (d_hidden) on the main stream; the four head parameter gradients on the weight-gradient stream
         # (they belong to the last layer's bucket, whose readiness waits for that stream's marker of the layer anyway).
         # A model without encoder layers announces its head bucket right away: keep everything on one stream there.
-        main0 = torch.cuda.current_stream(self.dev)
-        head_side = self.wgrad_stream if (self.use_wgrad_stream and self.nl > 0) else main0
-        if head_side is not main0:
+        main = torch.cuda.current_stream(self.dev)
+        side = self.wgrad_stream
+        if self.nl > 0:
             # the side stream may still be busy with the previous step's tail; it must also not overtake this step
-            head_side.wait_stream(main0)
+            side.wait_stream(main)
         L.call("b2_head_bwd_split", dl.data_ptr(), x_last.data_ptr(), ws["pooled"].data_ptr(),
                None if packed is None else packed[1].data_ptr(), M, Bo, S, H, w("bert.pooler.dense.weight"),
                w("classifier.weight"), self.C, p_c, rng, 1 + 3 * self.nl, *head_g, ws["dxA"].data_ptr(), 1,
-               ws["head_scratch"].data_ptr(), s, None if head_side is main0 else head_side.cuda_stream)
+               ws["head_scratch"].data_ptr(), s, side.cuda_stream if self.nl > 0 else None)
         dx, dx_other = ws["dxA"], ws["dxB"]
         # Weight gradients are off the critical path (only the optimizer consumes them): they run on a second stream,
         # overlapping the dgrad / LayerNorm / attention chain of the main stream.  Their A operands (dzd, dU, dz1d,
         # dqkv) are double-buffered by layer parity; the main stream may reuse a buffer set only after the weight
         # gradients of the layer two steps earlier have drained (done[l + 2]).
-        main = torch.cuda.current_stream(self.dev)
-        side = self.wgrad_stream if self.use_wgrad_stream else main
         ss = side.cuda_stream
         done = {}
 
-        def fork():
-            if side is not main:
-                ev = torch.cuda.Event()
-                ev.record(main)
-                side.wait_event(ev)
-
-        # (head bucket is announced right after these helpers are defined)
         opt = self.model._optimizer
         overlap_opt = hooks is None and opt is not None and getattr(opt, "_armed", False)
-        # single GPU, optimizer armed by the fused step, no GradScaler: the encoder weight matrices are updated in the
-        # epilogue of the grouped weight-gradient GEMM itself (no gradient round trip, no separate HBM-bound pass over
-        # 85 % of the parameters); the per-bucket AdamW launches then skip those vectors
-        self.fused_adamw_active = bool(overlap_opt and self.grouped_wgrad and self.fused_adamw and
-                                       getattr(opt, "grad_scale", None) is None and
-                                       not getattr(opt, "_amp_seen", False) and not self.accum_in_use)
         # Under an armed DDP exchange the side stream takes the weight-gradient dependencies bucket by bucket
         # (ddp._bucket_ready) and optimizer.step() joins it
         ddp_overlap = (hooks is not None and hooks.world > 1 and hooks.overlap and opt is not None and
@@ -929,47 +885,35 @@ class _Engine:
             pre = "bert.encoder.layer.%d." % l
             st = l & 1
             dzd, dU, dz1d, dqkv = ws["dzd"][st], ws["dU"][st], ws["dz1d"][st], ws["dqkv"][st]
-            if side is not main and (l + 2) in done:
+            if (l + 2) in done:
                 main.wait_event(done[l + 2])
             # --- BertOutput: LN2 backward (+ dropout mask, bias grad), FFN2 wgrad/dgrad(+GELU')
             acc_l = self.bias_acc.data_ptr() + 4 * l * self.acc_per_layer
             # column sums (d_gamma, d_beta, d_bias) are added into this layer's fp32 accumulators by the kernel itself
             L.call("b2_layernorm_bwd_accum", dx.data_ptr(), a["z2"].data_ptr(), a["mean2"].data_ptr(),
                    a["rstd2"].data_ptr(), w(pre + "output.LayerNorm.weight"), M, H, p_h, rng, 3 + 3 * l,
-                   (dx_other if self.accum_dgrad else ws["dz"]).data_ptr(), dzd.data_ptr(),
-                   acc_l + 4 * (3 * H + I), s)
-            # the layer's four weight gradients: launched one by one on the side stream, or (grouped_wgrad) collected
-            # and issued as ONE persistent launch once the last operand (dqkv) exists
-            wgrads = [] if self.grouped_wgrad else None
-            if wgrads is None:
-                fork()
+                   dx_other.data_ptr(), dzd.data_ptr(), acc_l + 4 * (3 * H + I), s)
+            # the layer's four weight gradients: collected here and issued as ONE launch on the side stream once the
+            # last operand (dqkv) exists
+            wgrads = []
             self.gemm(H, I, M, dzd.data_ptr(), H, MN, a["h"].data_ptr(), I, MN, g(pre + "output.dense.weight"), I,
-                      split=True, stream=ss, defer=wgrads)
+                      split=True, defer=wgrads)
             # dU = (dY2 W2) * gelu'(u); its column sums (= intermediate bias gradient) accumulate in the same epilogue
             self.gemm(M, I, H, dzd.data_ptr(), H, KM, w(pre + "output.dense.weight"), I, MN, dU.data_ptr(), I,
                       L.EPI_GELU_BWD, aux_in=a["u"].data_ptr(), ld_aux_in=I, colsum=acc_l + 4 * 3 * H)
             # --- BertIntermediate
-            if wgrads is None:
-                fork()
             self.gemm(I, H, M, dU.data_ptr(), I, MN, a["x1"].data_ptr(), H, MN,
-                      g(pre + "intermediate.dense.weight"), H, split=True, stream=ss, defer=wgrads)
-            # dX1 = dZ2 + dU W1.  accum_dgrad: LayerNorm backward left dZ2 (fp32) in dx_other and the GEMM adds into
-            # it (split-K slices reduce in place at L2), else the epilogue reads dZ2 as an auxiliary tile
-            if self.accum_dgrad:
-                self.gemm(M, H, I, dU.data_ptr(), I, KM, w(pre + "intermediate.dense.weight"), H, MN,
-                          dx_other.data_ptr(), H, L.EPI_ACCUM_F32)
-            else:
-                self.gemm(M, H, I, dU.data_ptr(), I, KM, w(pre + "intermediate.dense.weight"), H, MN,
-                          dx_other.data_ptr(), H, L.EPI_RESIDUAL_F32, aux_in=ws["dz"].data_ptr(), ld_aux_in=H)
+                      g(pre + "intermediate.dense.weight"), H, split=True, defer=wgrads)
+            # dX1 = dZ2 + dU W1: LayerNorm backward left dZ2 (fp32) in dx_other and the GEMM adds into it (split-K
+            # slices reduce in place at L2)
+            self.gemm(M, H, I, dU.data_ptr(), I, KM, w(pre + "intermediate.dense.weight"), H, MN,
+                      dx_other.data_ptr(), H, L.EPI_ACCUM_F32)
             # --- BertSelfOutput
             L.call("b2_layernorm_bwd_accum", dx_other.data_ptr(), a["z1"].data_ptr(), a["mean1"].data_ptr(),
                    a["rstd1"].data_ptr(), w(pre + "attention.output.LayerNorm.weight"), M, H, p_h, rng, 2 + 3 * l,
-                   (dx if self.accum_dgrad else ws["dz1"]).data_ptr(), dz1d.data_ptr(),
-                   acc_l + 4 * (6 * H + I), s)
-            if wgrads is None:
-                fork()
+                   dx.data_ptr(), dz1d.data_ptr(), acc_l + 4 * (6 * H + I), s)
             self.gemm(H, H, M, dz1d.data_ptr(), H, MN, a["ctx"].data_ptr(), H, MN,
-                      g(pre + "attention.output.dense.weight"), H, split=True, stream=ss, defer=wgrads)
+                      g(pre + "attention.output.dense.weight"), H, split=True, defer=wgrads)
             self.gemm(M, H, H, dz1d.data_ptr(), H, KM, w(pre + "attention.output.dense.weight"), H, MN,
                       ws["dctx"].data_ptr(), H)
             # --- BertSelfAttention
@@ -984,39 +928,29 @@ class _Engine:
             if S != 128:   # long-sequence parity configs: separate column-sum pass into the same accumulator slot
                 L.call("b2_colsum", dqkv.data_ptr(), M, 3 * H, 3 * H, g(pre + "attention.self.query.bias"),
                        scratch, scratch_bytes, s)
-            fork()
             self.gemm(3 * H, H, M, dqkv.data_ptr(), 3 * H, MN, x_in.data_ptr(), H, MN,
-                      g(pre + "attention.self.query.weight"), H, split=True, stream=ss, defer=wgrads)
-            if wgrads is not None:
-                # 108 full-K 256x256 tiles (BERT-base) in two waves of one kernel instead of four small split-K GEMMs
-                # and their reduce kernels; largest problems first
-                wgrads.sort(key=lambda t: -(t.M * t.N))
-                if self.fused_adamw_active:
-                    hp = opt.hparams()
-                    hp.skip_flags = None
-                    arr = (L.GemmArgs * len(wgrads))(*wgrads)
-                    L.call("b2_gemm_bf16_grouped_adamw", arr, opt.fused_targets(wgrads), len(wgrads), hp,
-                           L.ptr(opt._state()["step"]), ss)
-                else:
-                    self.gemm_grouped(wgrads, ss)
+                      g(pre + "attention.self.query.weight"), H, split=True, defer=wgrads)
+            # fork: the side stream waits for every operand of the layer's weight gradients
+            ev = torch.cuda.Event()
+            ev.record(main)
+            side.wait_event(ev)
+            # 108 full-K 256x256 tiles (BERT-base) in two waves of one kernel instead of four small split-K GEMMs and
+            # their reduce kernels; largest problems first
+            wgrads.sort(key=lambda t: -(t.M * t.N))
+            self.gemm_grouped(wgrads, ss)
             # fp32 accumulators -> bf16 bias gradients of this layer (and re-arm them); for S != 128 the QKV segment's
             # accumulator is unused (zero) and must not overwrite the colsum result: finish only the intermediate one.
-            # Every kernel that adds into this layer's accumulators is behind the fork() above, and only the optimizer /
+            # Every kernel that adds into this layer's accumulators is behind the fork above, and only the optimizer /
             # exchange reads the result: the launch rides the weight-gradient stream, off the critical path.
             spl = self.segs_per_layer
             seg0 = spl * l if S == 128 else spl * l + 1
             L.call("b2_accum_finish", self.bias_acc.data_ptr(), self.grads.data_ptr(),
                    self.bias_segs.data_ptr() + 24 * seg0, spl * (l + 1) - seg0, max(3 * H, I), ss)
-            if side is not main:
-                done[l] = torch.cuda.Event()
-                done[l].record(side)
-            if self.accum_dgrad:
-                self.gemm(M, H, 3 * H, dqkv.data_ptr(), 3 * H, KM, w(pre + "attention.self.query.weight"), H, MN,
-                          dx.data_ptr(), H, L.EPI_ACCUM_F32)
-            else:
-                self.gemm(M, H, 3 * H, dqkv.data_ptr(), 3 * H, KM, w(pre + "attention.self.query.weight"), H, MN,
-                          dx.data_ptr(), H, L.EPI_RESIDUAL_F32, aux_in=ws["dz1"].data_ptr(), ld_aux_in=H)
-            bucket_ready(1 + l, done.get(l))   # complete only with this layer's weight gradients
+            done[l] = torch.cuda.Event()
+            done[l].record(side)
+            self.gemm(M, H, 3 * H, dqkv.data_ptr(), 3 * H, KM, w(pre + "attention.self.query.weight"), H, MN,
+                      dx.data_ptr(), H, L.EPI_ACCUM_F32)
+            bucket_ready(1 + l, done[l])   # complete only with this layer's weight gradients
         emb_in = (dx.data_ptr(), 1, ws["emb_pre"].data_ptr(), ws["emb_mean"].data_ptr(), ws["emb_rstd"].data_ptr(),
                   w("bert.embeddings.LayerNorm.weight"), ws["ids32"].data_ptr(), ws["tt32"].data_ptr())
         emb_tail = (B, S, H, cfg.vocab_size, cfg.type_vocab_size,
@@ -1032,7 +966,7 @@ class _Engine:
         # Whoever consumes the gradients next on the main stream (optimizer.step, grad_dict) must see the weight-gradient
         # stream's work.  Under an armed DDP exchange optimizer.step() (or end_pass) joins the side stream, which has
         # taken those dependencies; in every other case join here.
-        if side is not main and not ddp_overlap:
+        if not ddp_overlap:
             for l in sorted(done)[:2]:       # the last two layers processed (0 and 1) may still be in flight
                 main.wait_event(done[l])
         bucket_ready(0)

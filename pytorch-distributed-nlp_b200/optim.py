@@ -65,14 +65,6 @@ class AdamW(torch.optim.Optimizer):
         self._dev_state = None
         self._armed = False      # set by FusedTrainStep: per-bucket updates may start during backward
         self._pending = set()    # buckets already updated (on the engine's optimizer stream) in this step
-        self._background = os.environ.get("B2_ADAMW_BACKGROUND", "1") != "0"   # one-GPU update shaped to co-reside
-        # pipelined form (one GPU, captured steps only; see apply_pending): the update of step i runs at the START of
-        # step i + 1, bucket by bucket in forward order on the low-priority optimizer stream, while the forward pass
-        # works its way up the layers
-        self._pipelined = False
-        self._deferred_pending = False
-        self._amp_seen = False   # a GradScaler drives this optimizer: the scale is only known inside step(), so
-                                 # per-bucket updates must not start during backward
         self._model._optimizer = self
 
     # -- device state (fp32 moments, step counter) ------------------------------------------------------------------
@@ -88,119 +80,19 @@ class AdamW(torch.optim.Optimizer):
                 "exp_avg_sq": torch.zeros(n, dtype=torch.float32, device=eng.dev),
                 "step": torch.zeros(1, dtype=torch.int64, device=eng.dev),
                 "step_size": torch.zeros(1, dtype=torch.float32, device=eng.dev),   # see b2_adamw_prepare
-                # pipelined form: 1.0 = the gradient space holds nothing that is not applied yet (the update kernels
-                # treat it like GradScaler's found_inf: non-zero -> skip), 0.0 = gradients of the last backward pending
-                "no_grads": torch.ones(1, dtype=torch.float32, device=eng.dev),
                 "decay": self._decay_flags_cpu.to(eng.dev),
-                "skip": self._fused_skip_flags().to(eng.dev),
             }
             self._prepare(eng.stream())
         return self._dev_state
 
-    # ---- pipelined update (FusedTrainStep / PackedTrainStep on one GPU) ------------------------------------------------
-    def enable_pipelining(self):
-        """Called by the captured train steps.  Measured (B2_DEBUG_SKIP_ADAMW): launched under the backward pass, the
-        optimizer kernels are exposed almost in full -- the backward keeps every SM busy with GEMM CTAs that own the
-        whole register file.  The forward pass does not: its two dense + LayerNorm launches per layer leave SMs idle.  So the update of step i is applied at the beginning of step i + 1: bucket by bucket in FORWARD
-        order on the optimizer stream (lowest priority), layer l of the forward waiting only for bucket l's event.
-        Nothing is skipped: every captured step applies one full update (the previous step's), `state_dict()`, an eager
-        forward, an evaluation step and `optimizer.step()` first flush what is pending, and the arithmetic (operands,
-        order, step count) is exactly that of the unpipelined step."""
-        model = self._model
-        # Under the forward the update time-slices with the GEMM CTAs just as it does under the backward, and a layer
-        # that has to wait for its bucket's event stalls the critical path.  Correct (tests/test_model.py::test_pipelined_adamw_is_the_same_
-        # training run) but slower: opt-in only (B2_PIPELINED_ADAMW=1).
-        # (gradient accumulation folds the window into the gradients at the end of the final backward: an update
-        # deferred past it has nothing to gain and a window to get wrong)
-        if (os.environ.get("B2_PIPELINED_ADAMW", "0") != "1" or model._ddp is not None or self._amp_seen or
-                getattr(model._engine, "fused_adamw", False) or getattr(model._engine, "accum_in_use", False)):
-            return False
-        self._pipelined = True
-        self._armed = False          # no per-bucket launches under the backward
-        return True
-
-    def apply_pending(self, in_step):
-        """Applies the gradients of the last backward if they have not been applied yet (device flag, so the same
-        captured nodes serve the first replay, where nothing is pending).  in_step: launched from a train step body
-        on the optimizer stream, returns one event per bucket (forward order); else: on the current stream."""
-        st = self._state()
-        model = self._model
-        eng = model._engine
-        main = torch.cuda.current_stream(eng.dev)
-        stream = eng.opt_stream if in_step else main
-        if in_step:
-            ev0 = torch.cuda.Event()
-            ev0.record(main)
-            stream.wait_event(ev0)
-        hp = self.hparams()
-        hp.grad_scale, hp.skip_flags = None, None
-        hp.found_inf = st["no_grads"].data_ptr()
-        gptr, sptr = L.ptr_array([eng.grads.data_ptr()]), L.ptr_array([eng.shadow.data_ptr()])
-        events = []
-        for (b0, e0, _lbl) in model._layout.buckets:
-            L.call("b2_bucket_reduce_adamw", gptr, sptr, 1, 0, L.ptr(model._flat), L.ptr(st["exp_avg"]),
-                   L.ptr(st["exp_avg_sq"]), L.ptr(st["decay"]), b0, e0, hp, L.ptr(st["step"]), stream.cuda_stream)
-            if in_step:
-                ev = torch.cuda.Event()
-                ev.record(stream)
-                events.append(ev)
-        L.call("b2_step_advance", L.ptr(st["step"]), None, st["no_grads"].data_ptr(), stream.cuda_stream)
-        self._prepare(stream.cuda_stream)
-        return events
-
-    def mark_grads_pending(self):
-        """end of a pipelined step body: the gradient space now holds an unapplied backward; bump the dropout stream"""
-        st = self._state()
-        eng = self._model._engine
-        s = eng.stream()
-        L.call("b2_zero", st["no_grads"].data_ptr(), 4, s)
-        L.call("b2_step_advance", None, L.ptr(eng.rng), None, s)
-        self._deferred_pending = True
-
     def flush_pending(self):
-        """applies a pending pipelined update now (on the current stream): called before anything reads the weights or
-        overwrites the gradients outside a pipelined step body"""
-        if not self._deferred_pending:
-            return
-        self._deferred_pending = False
-        self.apply_pending(in_step=False)
-        self._dev_state["no_grads"].fill_(1.0)
+        """No-op: every update is applied within the step that produced its gradients, so none is ever left pending.
+        Kept for callers that flush before reading the weights."""
 
     def _prepare(self, stream):
         """bias-corrected step size of the NEXT update -> device float (read by the background kernel)"""
         st = self._dev_state
         L.call("b2_adamw_prepare", self.hparams(), L.ptr(st["step"]), L.ptr(st["step_size"]), stream)
-
-    def _fused_skip_flags(self):
-        """uint8 per 8-element vector: 1 for the encoder weight matrices, which the single-GPU fused step updates in the
-        epilogue of the grouped weight-gradient GEMM (b2_gemm_bf16_grouped_adamw); the per-bucket update skips them."""
-        lay = self._model._layout
-        flags = torch.zeros(lay.total // 8, dtype=torch.uint8)
-        for l in range(self._model.config.num_hidden_layers):
-            pre = "bert.encoder.layer.%d." % l
-            for nm in ("attention.self.query.weight", "attention.self.key.weight", "attention.self.value.weight",
-                       "attention.output.dense.weight", "intermediate.dense.weight", "output.dense.weight"):
-                off, shape = lay.entries[pre + nm]
-                flags[off // 8:(off + shape[0] * shape[1]) // 8] = 1
-        return flags
-
-    def fused_targets(self, problems):
-        """b2_fused_adamw_target_t array for weight-gradient problems whose D pointers lie in the engine's bf16 gradient
-        space: the optimizer state of the same elements."""
-        st = self._state()
-        model = self._model
-        eng = model._engine
-        gbase = eng.grads.data_ptr()
-        arr = (L.FusedAdamWTarget * len(problems))()
-        decay = self._decay_flags_cpu
-        for i, pr in enumerate(problems):
-            off = (pr.D - gbase) // 2
-            arr[i].master = model._flat.data_ptr() + 4 * off
-            arr[i].exp_avg = st["exp_avg"].data_ptr() + 4 * off
-            arr[i].exp_avg_sq = st["exp_avg_sq"].data_ptr() + 4 * off
-            arr[i].shadow = eng.shadow.data_ptr() + 2 * off
-            arr[i].decay = int(decay[off // 8])
-        return arr
 
     def hparams(self):
         g = self.param_groups[0]
@@ -213,10 +105,6 @@ class AdamW(torch.optim.Optimizer):
         if gs is not None and (gs.dtype != torch.float32 or not gs.is_cuda):
             raise TypeError("grad_scale must be a CUDA fp32 scalar (torch.cuda.amp.GradScaler's)")
         hp.found_inf = self._found_inf_ptr()
-        eng = self._model._engine
-        st = self._dev_state
-        hp.skip_flags = (st["skip"].data_ptr() if (st is not None and getattr(eng, "fused_adamw_active", False))
-                         else None)
         return hp
 
     def _found_inf_ptr(self):
@@ -245,8 +133,7 @@ class AdamW(torch.optim.Optimizer):
         st = self._state()
         hp = self.hparams()
         model = self._model
-        if (background and world == 1 and self._background and hp.grad_scale is None and hp.found_inf is None and
-                hp.skip_flags is None):
+        if background and world == 1 and hp.grad_scale is None and hp.found_inf is None:
             # one GPU: the form that fits beside the GEMM CTAs (csrc/optim.cu, adamw_slim_kernel)
             L.call("b2_adamw_background", peer_grads[0], peer_shadow[0], L.ptr(model._flat), L.ptr(st["exp_avg"]),
                    L.ptr(st["exp_avg_sq"]), L.ptr(st["decay"]), begin, end, hp, L.ptr(st["step_size"]), stream)
@@ -263,9 +150,6 @@ class AdamW(torch.optim.Optimizer):
     @torch.no_grad()
     def step(self, closure=None):
         loss = closure() if closure is not None else None
-        self.flush_pending()
-        if getattr(self, "grad_scale", None) is not None:
-            self._amp_seen = True
         model = self._model
         eng = model._engine
         if eng is None:

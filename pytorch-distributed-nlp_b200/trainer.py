@@ -10,7 +10,6 @@ Same methods, same argument meaning: ``on_step`` [:126-137], ``loss_reduce`` [:1
   * ``train`` uses :class:`FusedTrainStep` (the whole step captured in one CUDA graph) when ``args.fused`` is set.
 """
 import contextlib
-import os
 import time
 
 import numpy as np
@@ -77,10 +76,8 @@ class _StagedGraphStep:
         self._h2d_done = None
         # The step body -- the critical chain of forward / dgrad kernels -- is issued (and captured) on a HIGH-priority
         # stream, so that when an SM frees up the block scheduler hands it to the critical path before the
-        # weight-gradient / optimizer streams (default, i.e. lowest, priority).  B2_STEP_PRIORITY=0 restores the plain current stream (A/B switch).
-        self._prio_stream = None
-        if os.environ.get("B2_STEP_PRIORITY", "1") != "0":
-            self._prio_stream = torch.cuda.Stream(device=dev, priority=-1)
+        # weight-gradient / optimizer streams (default, i.e. lowest, priority).
+        self._prio_stream = torch.cuda.Stream(device=dev, priority=-1)
 
     def _unstage(self):
         n = self.B * self.S
@@ -113,9 +110,6 @@ class _StagedGraphStep:
         self._h2d_done.record(torch.cuda.current_stream(self.eng.dev))
 
     def _run_body(self):
-        if self._prio_stream is None:
-            self._body()
-            return
         cur = torch.cuda.current_stream(self.eng.dev)
         self._prio_stream.wait_stream(cur)
         with torch.cuda.stream(self._prio_stream):
@@ -132,8 +126,6 @@ class _StagedGraphStep:
         self._run_device()
         if opt is not None:
             self.eng.accum_live = not final
-            if opt._pipelined:
-                opt._deferred_pending = True
 
     def _run_device(self):
         if not self.use_graph:
@@ -160,20 +152,18 @@ class _StagedGraphStep:
         self.opt = optimizer
         self.accum_steps = accum_steps
         if accum_steps > 1:
-            self.eng.ensure_accum()       # before enable_pipelining, and outside any capture
+            self.eng.ensure_accum()       # outside any capture
         # the fused step owns backward + optimizer: per-bucket AdamW (and, under DDP, the peer exchange) may start
         # while backward is still running
         optimizer._armed = True
-        optimizer.enable_pipelining()     # one GPU: the update moves under the NEXT step's forward (optim.py)
 
     def _train_body(self, forward):
-        """forward(weight_events) -> (logits, loss): the common part of the captured train steps.  A micro-batch body
+        """forward() -> (logits, loss): the common part of the captured train steps.  A micro-batch body
         (self._role[0] False) accumulates its gradients and bumps the dropout stream instead of stepping; the final
         body folds the window in before the update."""
         eng, opt = self.eng, self.opt
         final = self._role[0]
-        events = opt.apply_pending(in_step=True) if opt._pipelined else None     # step i-1's update, see optim.py
-        logits, loss = forward(events)
+        logits, loss = forward()
         B, S, mask, p_h, p_a, p_c, packed = eng._saved
         eng._saved = None
         Bo = B if packed is None else packed[1].numel()
@@ -185,11 +175,7 @@ class _StagedGraphStep:
         eng._backward_from_dlogits(ws["dloss_logits"], B, S, mask, p_h, p_a, p_c, packed)
         eng.end_pass()
         if final:
-            if opt._pipelined:
-                opt.mark_grads_pending()
-                torch.cuda.current_stream(eng.dev).wait_stream(eng.opt_stream)  # (step counter bump of the applied update)
-            else:
-                opt.step()
+            opt.step()
         self.loss_out.copy_(loss)
 
     def loss_to_host(self):
@@ -212,8 +198,8 @@ class FusedTrainStep(_StagedGraphStep):
     # the step body, expressed only with stream-ordered work (capturable)
     def _body(self):
         self._unstage()
-        self._train_body(lambda ev: self.eng.forward(self.d_ids, self.d_tt, self.d_mask, self.d_lab, training=True,
-                                                     need_backward=True, weight_events=ev))
+        self._train_body(lambda: self.eng.forward(self.d_ids, self.d_tt, self.d_mask, self.d_lab, training=True,
+                                                  need_backward=True))
 
     def __call__(self, batch_data, final=True):
         """batch_data: the dict the reference Collate yields (host int64 tensors).  Returns the device loss scalar
@@ -269,8 +255,8 @@ class PackedTrainStep(_StagedGraphStep):
     def _body(self):
         self._unstage()
         packed = (self.d_pos, self.d_seg, self.d_cls)
-        self._train_body(lambda ev: self.eng.forward(self.d_ids, self.d_tt, None, self.d_lab, training=True,
-                                                     need_backward=True, packed=packed, weight_events=ev))
+        self._train_body(lambda: self.eng.forward(self.d_ids, self.d_tt, None, self.d_lab, training=True,
+                                                  need_backward=True, packed=packed))
 
     def __call__(self, packed, label, final=True):
         self.stage(packed, label)
@@ -295,8 +281,6 @@ class FusedEvalStep(_StagedGraphStep):
         self.loss_out.copy_(loss)
 
     def __call__(self, batch_data):
-        if self.model._optimizer is not None:
-            self.model._optimizer.flush_pending()     # a pipelined train step may still owe its update
         self.stage(batch_data)
         self.run_device()
         return self.logits_out, self.d_lab, self.loss_out

@@ -240,48 +240,6 @@ def test_grouped_weight_gradients(cuda_dev, shapes):
         _check(D, A.float().t() @ B.float())
 
 
-def test_grouped_weight_gradients_with_fused_adamw(cuda_dev):
-    """b2_gemm_bf16_grouped_adamw: gradient (bf16, still written) + HF-AdamW on the same elements in the epilogue,
-    against the restated HF update applied to the reference gradient"""
-    K, lr, wd, t_prev = 1024, 3e-3, 0.01, 4
-    shapes = [(768, 512), (256, 768)]
-    probs = [_tn_problem(m, n, K, cuda_dev, 60 + i) for i, (m, n) in enumerate(shapes)]
-    arr = (L.GemmArgs * len(probs))(*[p[0] for p in probs])
-    tg = (L.FusedAdamWTarget * len(probs))()
-    state = []
-    for i, (m, n) in enumerate(shapes):
-        torch.manual_seed(80 + i)
-        w = torch.randn(m, n, device=cuda_dev) * 0.05
-        ea = torch.randn(m, n, device=cuda_dev) * 0.01
-        es = torch.rand(m, n, device=cuda_dev) * 1e-3
-        sh = torch.zeros(m, n, dtype=torch.bfloat16, device=cuda_dev)
-        state.append((w.clone(), ea.clone(), es.clone(), w, ea, es, sh))
-        tg[i].master, tg[i].exp_avg, tg[i].exp_avg_sq, tg[i].shadow = w.data_ptr(), ea.data_ptr(), es.data_ptr(), \
-            sh.data_ptr()
-        tg[i].decay = 1 if i == 0 else 0
-    hp = L.AdamWHParams()
-    hp.lr, hp.beta1, hp.beta2, hp.eps, hp.weight_decay, hp.correct_bias = lr, 0.9, 0.999, 1e-6, wd, 1
-    hp.grad_scale, hp.found_inf, hp.skip_flags = None, None, None
-    step = torch.tensor([t_prev], dtype=torch.int64, device=cuda_dev)
-    L.call("b2_gemm_bf16_grouped_adamw", arr, tg, len(probs), hp, step.data_ptr(),
-           torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    for i, ((_a, A, B, D), (w0, m0, v0, w, ea, es, sh)) in enumerate(zip(probs, state)):
-        _check(D, A.float().t() @ B.float())
-        g = D.float()                                   # the update must use exactly the bf16 gradient it stored
-        t = t_prev + 1
-        m1 = m0 * 0.9 + g * (1 - 0.9)
-        v1 = v0 * 0.999 + g * g * (1 - 0.999)
-        step_size = lr * (1 - 0.999 ** t) ** 0.5 / (1 - 0.9 ** t)
-        w1 = w0 - step_size * (m1 / (v1.sqrt() + 1e-6))
-        if i == 0:
-            w1 = w1 - lr * wd * w1
-        assert float((ea - m1).abs().max()) <= 1e-6 * float(m1.abs().max()) + 1e-9, i
-        assert float((es - v1).abs().max()) <= 1e-5 * float(v1.abs().max()) + 1e-12, i
-        assert float((w - w1).abs().max()) <= 2e-6, i
-        assert torch.equal(sh, w.to(torch.bfloat16)), i
-
-
 @pytest.mark.parametrize("shape", [(4096, 768, 768), (4096, 768, 3072), (2048, 1024, 1024), (2048, 1024, 4096),
                                    (1000, 768, 768), (200, 1024, 136), (8192, 768, 768)])
 @pytest.mark.parametrize("p", [0.0, 0.1])

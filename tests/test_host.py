@@ -207,29 +207,6 @@ def test_bench_b200_arm_fails_loudly_without_a_gpu():
     assert r.returncode != 0 and "no CPU fallback" in r.stderr and r.stdout.strip() == ""
 
 
-def test_fused_adamw_skip_flags_cover_exactly_the_encoder_matrices():
-    """the vectors the (experimental) fused weight-gradient epilogue updates itself -- and the per-bucket AdamW launch
-    must then skip -- are the six weight matrices of every encoder layer, nothing else"""
-    class A:
-        weight_decay, learning_rate = 0.01, 3e-5
-    cfg = tiny_config()
-    m = b2.BertForSequenceClassification(cfg)
-    opt = b2.build_optimizer(m, A)
-    flags = opt._fused_skip_flags()
-    want = torch.zeros_like(flags)
-    for n, (off, shape) in m._layout.entries.items():
-        is_enc_matrix = n.startswith("bert.encoder.layer.") and n.endswith(".weight") and "LayerNorm" not in n
-        numel = 1
-        for d in shape:
-            numel *= d
-        if is_enc_matrix:
-            assert numel % 8 == 0
-            want[off // 8:(off + numel) // 8] = 1
-    assert torch.equal(flags, want)
-    assert int(flags.sum()) * 8 == cfg.num_hidden_layers * (4 * cfg.hidden_size ** 2 +
-                                                          2 * cfg.hidden_size * cfg.intermediate_size)
-
-
 def test_sass_carries_wgmma_and_tma():
     """what the compiler actually emitted for sm_90a (cuobjdump -sass of the in-tree library): the GEMM and attention
     kernels issue warpgroup MMAs (HGMMA), move tiles with TMA (UTMALDG; UTMASTG for the attention stores) and wait on

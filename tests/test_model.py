@@ -163,43 +163,6 @@ def test_tiny_trajectory_eager_and_fused(cuda_dev):
         assert float((sd[k].double() - sd2[k].double()).abs().max()) <= 2e-5, k
 
 
-def test_pipelined_adamw_is_the_same_training_run(cuda_dev, monkeypatch):
-    """B2_PIPELINED_ADAMW=1 (opt-in experiment: the update of step i runs at the start of step i + 1, under the forward
-    pass): same losses and, once the pending update is flushed by state_dict(), the same weights as the default step;
-    an evaluation step in between sees the updated weights."""
-    cfg = tiny_config(hidden_dropout_prob=0.0, attention_probs_dropout_prob=0.0)
-    state = state_from_hf_init(cfg)
-    batches = [bert_ref.synthetic_batch(cfg, 4, 128, 2600 + i, padded=(i % 2 == 1)) for i in range(6)]
-
-    class A:
-        weight_decay, learning_rate = 0.01, 3e-5
-
-    def run(pipelined):
-        monkeypatch.setenv("B2_PIPELINED_ADAMW", "1" if pipelined else "0")
-        model = make_model(cfg, state, cuda_dev).train()
-        opt = b2.build_optimizer(model, A)
-        step = b2.FusedTrainStep(model, opt, 4, 128)
-        assert opt._pipelined == pipelined
-        losses, ev_logits = [], None
-        for i, b in enumerate(batches):
-            step(b)
-            losses.append(step.loss_to_host())
-            if i == 3:      # evaluation between two steps: must see the weights AFTER step 3's update
-                ev = b2.FusedEvalStep(model, 4, 128)
-                ev_logits = ev(batches[0])[0].clone()
-                model.train()
-        return losses, ev_logits, {k: v.clone() for k, v in model.state_dict().items()}, int(opt._state()["step"])
-
-    l0, e0, w0, t0 = run(False)
-    l1, e1, w1, t1 = run(True)
-    assert t0 == t1 == len(batches)
-    for a, c in zip(l0, l1):
-        assert abs(a - c) <= 5e-5, (l0, l1)
-    assert float((e0 - e1).abs().max()) <= 1e-3
-    for k in w0:
-        assert float((w0[k].double() - w1[k].double()).abs().max()) <= 2e-5, k
-
-
 def test_amp_script_loop_with_gradscaler(cuda_dev):
     """The -amp scripts' loop (multi-gpu-distributed-mp-amp-cls.py:166-171: autocast, scaler.scale(loss).backward(),
     scaler.step(optimizer), scaler.update(), and no zero_grad) runs unchanged and lands where the plain loop lands:

@@ -8,7 +8,7 @@ Edges, kernel by kernel:
   head.cu      pooler groups of 8 rows with a ragged last group, packed cls rows (unsorted, the last row of the last
                bin); b2_head_bwd_split with fp32 / bf16 d_hidden on one stream and on a second stream; the mean
                cross-entropy beyond one 256-thread block's first sweep, with ignored labels and logits near +-80.
-  optim.cu     the mean over 1-8 peer gradient buffers, shadow fan-out with NULL entries, slices, skip flags,
+  optim.cu     the mean over 1-8 peer gradient buffers, shadow fan-out with NULL entries, slices,
                GradScaler scale / found_inf, a grid-stride loop that wraps; the background form on a ragged slice;
                the fp32 -> bf16 bias-gradient finish with the engine's segment table; the two casts.
   layernorm.cu the warp-pair backward at the engine's row counts (the operand ring and the row-sum exchange wrap),
@@ -611,10 +611,10 @@ def test_ce_fwd_bwd(cuda_dev, B, C, with_grad):
 # ======================================================================================================================
 # C. Optimizer
 # ======================================================================================================================
-def hparams(lr=1e-2, wd=0.01, correct_bias=1, scale=None, found_inf=None, skip=None):
+def hparams(lr=1e-2, wd=0.01, correct_bias=1, scale=None, found_inf=None):
     hp = L.AdamWHParams()
     hp.lr, hp.beta1, hp.beta2, hp.eps, hp.weight_decay, hp.correct_bias = lr, 0.9, 0.999, 1e-6, wd, correct_bias
-    hp.grad_scale, hp.found_inf, hp.skip_flags = L.ptr(scale), L.ptr(found_inf), L.ptr(skip)
+    hp.grad_scale, hp.found_inf = L.ptr(scale), L.ptr(found_inf)
     return hp
 
 
@@ -717,13 +717,13 @@ def test_reduce_adamw_world(cuda_dev, world):
     check_reduce(run, ref, sel, "reduce world=%d" % world)
 
 
-REDUCE_EDGES = ["wrap", "slice", "skip", "no_bias_correction", "no_weight_decay", "scale_1000"]
+REDUCE_EDGES = ["wrap", "slice", "no_bias_correction", "no_weight_decay", "scale_1000"]
 
 
 @pytest.mark.parametrize("case", REDUCE_EDGES)
 def test_reduce_adamw_edges(cuda_dev, case):
     dev = cuda_dev
-    world = {"wrap": 2, "slice": 3, "skip": 2, "no_bias_correction": 4, "no_weight_decay": 1, "scale_1000": 3}[case]
+    world = {"wrap": 2, "slice": 3, "no_bias_correction": 4, "no_weight_decay": 1, "scale_1000": 3}[case]
     # "wrap": more vectors than the capped grid (132 x 8 blocks of 256 threads) covers in one sweep, ragged tail
     n = (3 << 20) + 8 * 13 if case == "wrap" else 8 * 20011
     run = ReduceRun(dev, world, n, seed=len(case))
@@ -731,14 +731,9 @@ def test_reduce_adamw_edges(cuda_dev, case):
     lr, wd, cb = 1e-2, (0.0 if case == "no_weight_decay" else 0.01), (0 if case == "no_bias_correction" else 1)
     if case == "no_weight_decay":
         run.decay.fill_(1)
-    skip = None
-    if case == "skip":
-        skip = (torch.rand(n // 8, device=dev, generator=run.gen) < 0.25).to(torch.uint8)
     scale = torch.tensor([1000.0], device=dev) if case == "scale_1000" else None
     vec = torch.zeros(n // 8, dtype=torch.bool, device=dev)
     vec[begin // 8: end // 8] = True
-    if skip is not None:
-        vec &= skip == 0
     sel_mask = vec.repeat_interleave(8)
     sel = sel_mask.nonzero()[:, 0]
     before = run.state()
@@ -746,12 +741,12 @@ def test_reduce_adamw_edges(cuda_dev, case):
                    extra=2 if scale is not None else 0)
     for _ in range(3):
         grads = run.grads(1000.0 if scale is not None else 1.0)
-        run.call(grads, hparams(lr, wd, cb, scale=scale, skip=skip), begin, end)
+        run.call(grads, hparams(lr, wd, cb, scale=scale), begin, end)
         g = sum(x.double() for x in grads) / world
         ref.step(g / 1000.0 if scale is not None else g)
     torch.cuda.synchronize()
     check_reduce(run, ref, sel, "reduce " + case)
-    for a, b in zip(before, run.state()):         # everything outside the slice / flagged vectors: bit for bit
+    for a, b in zip(before, run.state()):         # everything outside the slice: bit for bit
         assert torch.equal(a[~sel_mask], b[~sel_mask]), case
 
 
