@@ -28,7 +28,7 @@ extern "C" {
 /* ------------------------------------------------------------------------------------------------------ */
 const char* b2_last_error(void);
 int32_t b2_abi_version(void);             /* bumped when a struct below changes */
-#define B2_ABI_VERSION 19
+#define B2_ABI_VERSION 20
 int64_t b2_launch_count(void);            /* kernels launched by this library so far (process-wide) */
 
 /* ------------------------------------------------------------------------------------------------------ */
@@ -274,6 +274,13 @@ typedef struct b2_adamw_hparams {
   /* optional DEVICE pointer to the GradScaler's fp32 inf/nan indicator: a non-zero value skips the update (and the
    * step count), as GradScaler.step() skips optimizer.step().  NULL = always update.                            */
   const float* found_inf;
+  /* gradient-norm clipping (torch.nn.utils.clip_grad_norm_, HF TrainingArguments.max_grad_norm) as optional fields
+   * rather than separate entry points.  clip_coef: optional DEVICE fp32 scalar from b2_grad_norm_finalize; the
+   * gradient is multiplied by it before the moments.  grad_f32 (b2_bucket_reduce_adamw only): optional DEVICE fp32
+   * mean gradient of the slice [begin, end), indexed from begin (the stash of b2_grad_reduce_sumsq), read instead of
+   * the peers' bf16 gradients.  NULL = today's update, bit for bit.                                                */
+  const float* clip_coef;
+  const float* grad_f32;
 } b2_adamw_hparams_t;
 
 /* Fused update of one contiguous slice [begin, end) (element indices, multiples of 8) of the flat parameter
@@ -315,6 +322,32 @@ int32_t b2_adamw_background(const void* grads, void* shadow, float* master, floa
 #define B2_ACCUM_FOLD 2
 #define B2_ACCUM_FLUSH 3
 int32_t b2_grad_accumulate(void* grads, float* accum, int64_t begin, int64_t end, int32_t mode, void* stream);
+
+/* Gradient-norm clipping (torch.nn.utils.clip_grad_norm_ with norm_type 2, torch 2.11 `clip_grads_with_norm_`).  No
+ * parameter may move until the norm of the whole (DDP-mean) gradient is known, so a clipped step runs in three phases:
+ * reduce (+ partial sums of squares) per bucket slice, one finalize, then the update with hparams.clip_coef.
+ *
+ * Reduce phase over [begin, end) (multiples of 8).  world > 1: rank-order fp32 sum of the slice over
+ * `peer_grads[0..world)` times 1/world -- the gradient b2_bucket_reduce_adamw would use -- stored into `stash`
+ * (fp32 [end - begin], indexed from begin, 16-byte aligned).  world 1: reads peer_grads[0], stash must be NULL.
+ * Each warp writes the sum of squares of the gradients it saw to its own fp64 slot of `partials`:
+ * B2_SUMSQ_SLOTS(end - begin) slots, every one written.  No atomics: bit-reproducible.  Blocks of 128 threads x
+ * <= 32 registers, no shared memory: shaped to run per bucket beside the backward's GEMM CTAs.
+ * bytes / parameter: 2 * world in, 4 out (world 1: 2 in).                                                          */
+#define B2_SUMSQ_SLOTS(n) (4 * (((n) + 8191) / 8192))
+int32_t b2_grad_reduce_sumsq(const void* const* peer_grads, int32_t world, float* stash, int64_t begin, int64_t end,
+                             double* partials, void* stream);
+/* Norm finalize: sums partials[0..nslots) in a fixed order (fp64).  world > 1: the ranks' totals are then added in rank
+ * order through peer memory (b2_scalar_allreduce_mean on `slot`, x world): bit-identical on every rank.  Writes
+ *   *total_norm = sqrt(sum) / *grad_scale (grad_scale optional: the norm of the unscaled gradients)
+ *   *clip_coef  = min(1, max_norm / (*total_norm + 1e-6)); a non-finite norm propagates as in torch (NaN stays NaN)
+ *   *skip       (optional) = 1 if *found_inf (optional) is non-zero, or a grad_scale is given and the norm is not
+ *                 finite (GradScaler's inf check over every gradient); else 0.  Use it as the update's found_inf.
+ * world 1: one launch; peer_scratch / peer_flags / epoch may be NULL.                                            */
+int32_t b2_grad_norm_finalize(const double* partials, int64_t nslots, float* const* peer_scratch,
+                              void* const* peer_flags, int32_t world, int32_t rank, int32_t slot, uint32_t* epoch,
+                              float max_norm, const float* grad_scale, const float* found_inf, float* total_norm,
+                              float* clip_coef, float* skip, void* stream);
 
 /* ++step (AdamW t) and ++rng step (dropout stream) on the device: keeps CUDA-graph replays stateful.
  * found_inf (optional device fp32, see b2_adamw_hparams_t): non-zero leaves the AdamW step count untouched.   */

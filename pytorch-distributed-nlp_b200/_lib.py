@@ -8,13 +8,20 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2ddpbert.so")
-ABI_VERSION = 19
+ABI_VERSION = 20
 
 MAJOR_K, MAJOR_MN = 0, 1
 EPI_NONE, EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_DROPOUT_RESIDUAL, EPI_RESIDUAL, EPI_GELU_BWD = 0, 1, 2, 3, 4, 5
 EPI_RESIDUAL_F32 = 6
 EPI_ACCUM_F32 = 7
 ACCUM_STORE, ACCUM_ADD, ACCUM_FOLD, ACCUM_FLUSH = 0, 1, 2, 3     # b2_grad_accumulate modes
+
+
+def sumsq_slots(n):
+    """B2_SUMSQ_SLOTS: partial-sum slots b2_grad_reduce_sumsq writes for a slice of n elements"""
+    return 4 * ((n + 8191) // 8192)
+
+
 IPC_HANDLE_BYTES = 64
 FLAG_SLOTS = 64
 
@@ -35,7 +42,8 @@ class GemmArgs(C.Structure):
 
 class AdamWHParams(C.Structure):
     _fields_ = [("lr", f64), ("beta1", f64), ("beta2", f64), ("eps", f64), ("weight_decay", f64),
-                ("correct_bias", i32), ("grad_scale", vp), ("found_inf", vp)]
+                ("correct_bias", i32), ("grad_scale", vp), ("found_inf", vp),
+                ("clip_coef", vp), ("grad_f32", vp)]
 
 
 # name -> argtypes; every function returns int32 status unless listed in _SPECIAL
@@ -75,6 +83,8 @@ _SIGNATURES = {
     "b2_adamw_prepare": [C.POINTER(AdamWHParams), vp, vp, vp],
     "b2_adamw_background": [vp, vp, vp, vp, vp, vp, i64, i64, C.POINTER(AdamWHParams), vp, vp],
     "b2_grad_accumulate": [vp, vp, i64, i64, i32, vp],
+    "b2_grad_reduce_sumsq": [C.POINTER(vp), i32, vp, i64, i64, vp, vp],
+    "b2_grad_norm_finalize": [vp, i64, C.POINTER(vp), C.POINTER(vp), i32, i32, i32, vp, f32, vp, vp, vp, vp, vp, vp],
     "b2_step_advance": [vp, vp, vp, vp],
     "b2_rng_seed": [vp, u64, u64, vp],
     "b2_cast_f32_to_bf16": [vp, vp, i64, vp],

@@ -30,12 +30,16 @@ struct ReduceAdamWParams {
   const long long* step_counter;
   const float* grad_scale;   // optional device scalar (GradScaler): gradients are divided by it
   const float* found_inf;    // optional device scalar (GradScaler): non-zero skips the update
+  const float* clip_coef;    // optional device scalar (gradient clipping): gradients are multiplied by it
+  const float* grad_f32;     // optional fp32 mean gradient of [begin, end), indexed from begin: read instead of peers
 };
 
 __global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWParams p) {
   pdl_wait();               // PDL: predecessors complete + visible before any global access
   pdl_launch_dependents();  // let the next kernel in the stream begin launching
   if (p.found_inf != nullptr && *p.found_inf != 0.f) return;   // GradScaler saw inf/nan: this step is skipped
+  // x * 1.0f is exact: without a coefficient the update is today's, bit for bit
+  const float coef = p.clip_coef != nullptr ? *p.clip_coef : 1.0f;
   // HF AdamW bias correction: step_size = lr * sqrt(1 - b2^t) / (1 - b1^t), t = steps taken including this one
   const long long t = *p.step_counter + 1;
   float step_size = p.lr;
@@ -44,20 +48,27 @@ __global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWPara
     const double bc2 = 1.0 - pow(p.beta2_d, (double)t);
     step_size = (float)(p.lr_d * sqrt(bc2) / bc1);
   }
-  // mean over ranks; with a GradScaler also the unscale (a power of two: exact)
-  const float inv_world = (p.grad_scale != nullptr ? 1.0f / *p.grad_scale : 1.0f) / (float)p.world;
+  // mean over ranks (unless grad_f32 already holds it); with a GradScaler also the unscale (a power of two: exact)
+  const float inv_world = (p.grad_scale != nullptr ? 1.0f / *p.grad_scale : 1.0f) /
+                          (p.grad_f32 != nullptr ? 1.0f : (float)p.world);
   const long long nvec = (p.end - p.begin) >> 3;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec;
        i += (long long)gridDim.x * blockDim.x) {
     const long long e = p.begin + (i << 3);
     float g[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (p.grad_f32 != nullptr) {
+      const float4 a0 = *reinterpret_cast<const float4*>(p.grad_f32 + (e - p.begin));
+      const float4 a1 = *reinterpret_cast<const float4*>(p.grad_f32 + (e - p.begin) + 4);
+      g[0] = a0.x; g[1] = a0.y; g[2] = a0.z; g[3] = a0.w; g[4] = a1.x; g[5] = a1.y; g[6] = a1.z; g[7] = a1.w;
+    } else {
 #pragma unroll
-    for (int r = 0; r < MAX_WORLD; ++r) {
-      if (r < p.world) {
-        // peer-mapped pointer: plain 16-byte global load; the address aperture routes it over NVLink
-        const uint4 q = *reinterpret_cast<const uint4*>(p.grads[r] + e);
-        g[0] += bf16_lo(q.x); g[1] += bf16_hi(q.x); g[2] += bf16_lo(q.y); g[3] += bf16_hi(q.y);
-        g[4] += bf16_lo(q.z); g[5] += bf16_hi(q.z); g[6] += bf16_lo(q.w); g[7] += bf16_hi(q.w);
+      for (int r = 0; r < MAX_WORLD; ++r) {
+        if (r < p.world) {
+          // peer-mapped pointer: plain 16-byte global load; the address aperture routes it over NVLink
+          const uint4 q = *reinterpret_cast<const uint4*>(p.grads[r] + e);
+          g[0] += bf16_lo(q.x); g[1] += bf16_hi(q.x); g[2] += bf16_lo(q.y); g[3] += bf16_hi(q.y);
+          g[4] += bf16_lo(q.z); g[5] += bf16_hi(q.z); g[6] += bf16_lo(q.w); g[7] += bf16_hi(q.w);
+        }
       }
     }
     const bool decay = p.has_wd && p.decay[e >> 3];
@@ -69,7 +80,7 @@ __global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWPara
     float vv[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      const float gk = g[k] * inv_world;
+      const float gk = g[k] * inv_world * coef;
       mm[k] = mm[k] * p.beta1 + gk * p.one_minus_beta1;
       vv[k] = vv[k] * p.beta2 + gk * gk * p.one_minus_beta2;
       const float denom = sqrtf(vv[k]) + p.eps;
@@ -109,6 +120,7 @@ struct SlimParams {
   float beta1, beta2, one_minus_beta1, one_minus_beta2, eps, lr_wd;
   int has_wd;
   const float* step_size;
+  const float* clip_coef;   // optional (gradient clipping): gradients are multiplied by it
 };
 constexpr int kSlimThreads = 128, kSlimIters = 8;
 template <int DUMMY>
@@ -117,6 +129,7 @@ adamw_slim_kernel(const SlimParams p) {
   pdl_wait();
   pdl_launch_dependents();
   const float step_size = *p.step_size;
+  const float coef = p.clip_coef != nullptr ? *p.clip_coef : 1.0f;   // x * 1.0f is exact
   long long i = (long long)blockIdx.x * (kSlimThreads * kSlimIters) + threadIdx.x;
 #pragma unroll 1
   for (int it = 0; it < kSlimIters; ++it, i += kSlimThreads) {
@@ -127,7 +140,8 @@ adamw_slim_kernel(const SlimParams p) {
     float4 mm = *reinterpret_cast<const float4*>(p.m + e);
     float4 vv = *reinterpret_cast<const float4*>(p.v + e);
     const bool decay = p.has_wd && p.decay[e >> 3];
-    const float g0 = bf16_lo(q.x), g1 = bf16_hi(q.x), g2 = bf16_lo(q.y), g3 = bf16_hi(q.y);
+    const float g0 = bf16_lo(q.x) * coef, g1 = bf16_hi(q.x) * coef, g2 = bf16_lo(q.y) * coef,
+                g3 = bf16_hi(q.y) * coef;
     mm.x = mm.x * p.beta1 + g0 * p.one_minus_beta1; vv.x = vv.x * p.beta2 + g0 * g0 * p.one_minus_beta2;
     mm.y = mm.y * p.beta1 + g1 * p.one_minus_beta1; vv.y = vv.y * p.beta2 + g1 * g1 * p.one_minus_beta2;
     mm.z = mm.z * p.beta1 + g2 * p.one_minus_beta1; vv.z = vv.z * p.beta2 + g2 * g2 * p.one_minus_beta2;
@@ -208,6 +222,101 @@ static int32_t launch_grad_accumulate(void* grads, float* accum, long long begin
   B2_CUDA(cudaGetLastError());
   count_launches(1);
   return 0;
+}
+
+// ---- gradient-norm clipping ----------------------------------------------------------------------------------------
+// Reduce phase of a clipped step over [begin, end): world > 1 reads the slice from every peer, sums in fp32 in rank
+// order, multiplies by 1/world and stores the mean into the fp32 stash (the update reads it back instead of the
+// peers); world 1 only reads.  Every warp writes the sum of squares of the (mean) gradients it saw into its own fp64
+// slot: no atomics, so the norm is bit-reproducible.  At world 1 it runs per bucket under the backward, so it has the
+// shape of grad_accumulate_kernel: 128 threads x <= 32 registers, no shared memory, short-lived blocks.
+struct SumsqParams {
+  const __nv_bfloat16* grads[MAX_WORLD];
+  int world;
+  float inv_world;
+  float* stash;        // world > 1: fp32 [end - begin], indexed from begin
+  double* partials;    // B2_SUMSQ_SLOTS(end - begin) slots, 4 per block
+  long long begin, nvec;
+};
+constexpr int kSqThreads = 128, kSqIters = 8;
+static_assert(kSqThreads * kSqIters * 8 == 8192 && kSqThreads / 32 == 4, "B2_SUMSQ_SLOTS in the header");
+__global__ void __maxnreg__(32) grad_reduce_sumsq_kernel(const SumsqParams p) {
+  pdl_wait();
+  pdl_launch_dependents();
+  long long i = (long long)blockIdx.x * (kSqThreads * kSqIters) + threadIdx.x;
+  double acc = 0.0;
+#pragma unroll 1
+  for (int it = 0; it < kSqIters; ++it, i += kSqThreads) {
+    if (i >= p.nvec) break;
+    const long long e = p.begin + (i << 3);
+    float g[8];
+    if (p.world == 1) {
+      const uint4 q = *reinterpret_cast<const uint4*>(p.grads[0] + e);
+      g[0] = bf16_lo(q.x); g[1] = bf16_hi(q.x); g[2] = bf16_lo(q.y); g[3] = bf16_hi(q.y);
+      g[4] = bf16_lo(q.z); g[5] = bf16_hi(q.z); g[6] = bf16_lo(q.w); g[7] = bf16_hi(q.w);
+    } else {
+      // the sum of reduce_adamw_kernel, from +0 in rank order: the stash holds exactly the gradient it would use
+#pragma unroll
+      for (int k = 0; k < 8; ++k) g[k] = 0.f;
+#pragma unroll
+      for (int r = 0; r < MAX_WORLD; ++r) {
+        if (r < p.world) {
+          const uint4 q = *reinterpret_cast<const uint4*>(p.grads[r] + e);
+          g[0] += bf16_lo(q.x); g[1] += bf16_hi(q.x); g[2] += bf16_lo(q.y); g[3] += bf16_hi(q.y);
+          g[4] += bf16_lo(q.z); g[5] += bf16_hi(q.z); g[6] += bf16_lo(q.w); g[7] += bf16_hi(q.w);
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < 8; ++k) g[k] *= p.inv_world;
+      float4* s = reinterpret_cast<float4*>(p.stash + (e - p.begin));
+      s[0] = make_float4(g[0], g[1], g[2], g[3]);
+      s[1] = make_float4(g[4], g[5], g[6], g[7]);
+    }
+    float sq = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) sq = fmaf(g[k], g[k], sq);
+    acc += (double)sq;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) p.partials[blockIdx.x * (kSqThreads / 32) + (threadIdx.x >> 5)] = acc;
+}
+
+constexpr int kFinThreads = 1024;
+// Norm finalize: sum the slots in a fixed order (fp64).  mode 0: world 1, the norm of these slots.  mode 1: write this
+// rank's share of the sum of squares to *total_norm (then exchanged, see b2_grad_norm_finalize).  mode 2: start from the
+// rank mean of the shares in *clip_coef (x world).  Then total_norm = sqrt(sum) [/ grad_scale] and torch's coefficient.
+__global__ void grad_norm_finalize_kernel(const double* __restrict__ partials, long long nslots, int mode, int world,
+                                          float max_norm, const float* grad_scale, const float* found_inf,
+                                          float* total_norm, float* clip_coef, float* skip) {
+  pdl_wait();
+  pdl_launch_dependents();
+  __shared__ double red[kFinThreads];
+  double s = 0.0;
+  if (mode != 2) {
+    for (long long i = threadIdx.x; i < nslots; i += blockDim.x) s += partials[i];
+    red[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = kFinThreads / 2; o > 0; o >>= 1) {
+      if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+      __syncthreads();
+    }
+    s = red[0];
+  }
+  if (threadIdx.x != 0) return;
+  if (mode == 1) {
+    *total_norm = (float)s;
+    return;
+  }
+  if (mode == 2) s = (double)*clip_coef * (double)world;   // identical on every rank: the mean is
+  float norm = (float)sqrt(s);
+  if (grad_scale != nullptr) norm = norm / *grad_scale;
+  // torch.nn.utils.clip_grads_with_norm_: clamp(max_norm / (total_norm + 1e-6), max=1); a NaN norm stays NaN
+  const float q = max_norm / (norm + 1e-6f);
+  *total_norm = norm;
+  *clip_coef = q > 1.0f ? 1.0f : q;
+  if (skip != nullptr)
+    *skip = ((found_inf != nullptr && *found_inf != 0.f) || (grad_scale != nullptr && !isfinite(norm))) ? 1.f : 0.f;
 }
 
 // HF AdamW bias correction for the NEXT update: step_size = lr * sqrt(1 - b2^t) / (1 - b1^t), t = *step + 1
@@ -318,6 +427,9 @@ extern "C" int32_t b2_bucket_reduce_adamw(const void* const* peer_grads, void* c
   p.step_counter = (const long long*)step_counter;
   p.grad_scale = hp->grad_scale;
   p.found_inf = hp->found_inf;
+  p.clip_coef = hp->clip_coef;
+  p.grad_f32 = hp->grad_f32;
+  B2_REQUIRE((uintptr_t)p.grad_f32 % 16 == 0, "bucket_reduce_adamw: grad_f32 must be 16-byte aligned");
   const long long nvec = (end - begin) >> 3;
   long long blocks = (nvec + 255) / 256;
   const long long cap = 132 * 8;   // 8 blocks per SM of an H100
@@ -345,8 +457,8 @@ extern "C" int32_t b2_adamw_background(const void* grads, void* shadow, float* m
              "adamw_background: null pointer");
   B2_REQUIRE(begin >= 0 && end >= begin && begin % 8 == 0 && end % 8 == 0,
              "adamw_background: slice [%lld,%lld) must be 8-element aligned", (long long)begin, (long long)end);
-  B2_REQUIRE(hp->grad_scale == nullptr && hp->found_inf == nullptr,
-             "adamw_background: GradScaler state is handled by b2_bucket_reduce_adamw");
+  B2_REQUIRE(hp->grad_scale == nullptr && hp->found_inf == nullptr && hp->grad_f32 == nullptr,
+             "adamw_background: GradScaler state and fp32 sources are handled by b2_bucket_reduce_adamw");
   if (end == begin) return 0;
   static bool attr = false;
   if (!attr) {   // same shared-memory carve-out as the GEMM CTAs it is meant to run beside
@@ -363,6 +475,7 @@ extern "C" int32_t b2_adamw_background(const void* grads, void* shadow, float* m
   p.eps = (float)hp->eps; p.lr_wd = (float)(hp->lr * hp->weight_decay);
   p.has_wd = hp->weight_decay > 0.0 ? 1 : 0;
   p.step_size = step_size;
+  p.clip_coef = hp->clip_coef;
   const long long per_block = (long long)kSlimThreads * kSlimIters;
   const long long blocks = (p.nvec4 + per_block - 1) / per_block;
   B2_LAUNCH(adamw_slim_kernel<1>, (unsigned)blocks, kSlimThreads, 0, (cudaStream_t)stream_, p);
@@ -388,6 +501,71 @@ extern "C" int32_t b2_grad_accumulate(void* grads, float* accum, int64_t begin, 
     case B2_ACCUM_FOLD: return launch_grad_accumulate<B2_ACCUM_FOLD>(grads, accum, begin, nvec, s);
     default: return launch_grad_accumulate<B2_ACCUM_FLUSH>(grads, accum, begin, nvec, s);
   }
+}
+
+extern "C" int32_t b2_grad_reduce_sumsq(const void* const* peer_grads, int32_t world, float* stash, int64_t begin,
+                                        int64_t end, double* partials, void* stream_) {
+  B2_REQUIRE(peer_grads && partials, "grad_reduce_sumsq: null pointer");
+  B2_REQUIRE(world >= 1 && world <= MAX_WORLD, "grad_reduce_sumsq: world=%d", world);
+  B2_REQUIRE((world == 1) == (stash == nullptr), "grad_reduce_sumsq: the fp32 stash is required at world > 1 only");
+  B2_REQUIRE(begin >= 0 && end >= begin && begin % 8 == 0 && end % 8 == 0,
+             "grad_reduce_sumsq: slice [%lld,%lld) must be 8-element aligned", (long long)begin, (long long)end);
+  B2_REQUIRE((uintptr_t)stash % 16 == 0, "grad_reduce_sumsq: 16-byte alignment required");
+  if (end == begin) return 0;
+  SumsqParams p;
+  for (int r = 0; r < MAX_WORLD; ++r) {
+    p.grads[r] = r < world ? (const __nv_bfloat16*)peer_grads[r] : nullptr;
+    if (r < world) B2_REQUIRE(p.grads[r], "grad_reduce_sumsq: null peer pointer for rank %d", r);
+  }
+  p.world = world;
+  p.inv_world = 1.0f / (float)world;
+  p.stash = stash;
+  p.partials = partials;
+  p.begin = begin;
+  p.nvec = (end - begin) >> 3;
+  static bool attr = false;
+  if (!attr) {   // same shared-memory carve-out as the GEMM CTAs it is meant to run beside
+    B2_CUDA(cudaFuncSetAttribute(grad_reduce_sumsq_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 cudaSharedmemCarveoutMaxShared));
+    attr = true;
+  }
+  const long long per_block = (long long)kSqThreads * kSqIters;
+  B2_LAUNCH(grad_reduce_sumsq_kernel, (unsigned)((p.nvec + per_block - 1) / per_block), kSqThreads, 0,
+            (cudaStream_t)stream_, p);
+  B2_CUDA(cudaGetLastError());
+  count_launches(1);
+  return 0;
+}
+
+extern "C" int32_t b2_grad_norm_finalize(const double* partials, int64_t nslots, float* const* peer_scratch,
+                                         void* const* peer_flags, int32_t world, int32_t rank, int32_t slot,
+                                         uint32_t* epoch, float max_norm, const float* grad_scale,
+                                         const float* found_inf, float* total_norm, float* clip_coef, float* skip,
+                                         void* stream_) {
+  B2_REQUIRE(partials && nslots >= 0 && total_norm && clip_coef, "grad_norm_finalize: bad args");
+  B2_REQUIRE(world >= 1 && world <= MAX_WORLD && rank >= 0 && rank < world, "grad_norm_finalize: world=%d rank=%d",
+             world, rank);
+  cudaStream_t s = (cudaStream_t)stream_;
+  if (world == 1) {
+    B2_LAUNCH(grad_norm_finalize_kernel, 1, kFinThreads, 0, s, partials, (long long)nslots, 0, 1, max_norm, grad_scale,
+              found_inf, total_norm, clip_coef, skip);
+    B2_CUDA(cudaGetLastError());
+    count_launches(1);
+    return 0;
+  }
+  // this rank's share -> *total_norm; rank-order mean of the shares -> *clip_coef; then the norm from that mean
+  B2_LAUNCH(grad_norm_finalize_kernel, 1, kFinThreads, 0, s, partials, (long long)nslots, 1, world, max_norm, grad_scale,
+            found_inf, total_norm, clip_coef, skip);
+  B2_CUDA(cudaGetLastError());
+  count_launches(1);
+  const int32_t st = b2_scalar_allreduce_mean(total_norm, clip_coef, peer_scratch, peer_flags, world, rank, slot,
+                                              epoch, stream_);
+  if (st) return st;
+  B2_LAUNCH(grad_norm_finalize_kernel, 1, kFinThreads, 0, s, partials, (long long)nslots, 2, world, max_norm, grad_scale,
+            found_inf, total_norm, clip_coef, skip);
+  B2_CUDA(cudaGetLastError());
+  count_launches(1);
+  return 0;
 }
 
 extern "C" int32_t b2_step_advance(int64_t* step_counter, void* rng_state, const float* found_inf, void* stream_) {

@@ -85,6 +85,7 @@ class PeerComm:
         self.alloc("flags", L.FLAG_SLOTS * self.world * 4)
         self.alloc("scalar", 2 * self.world * 4)
         self.alloc("scalar_inf", 2 * self.world * 4)
+        self.alloc("scalar_clip", 2 * self.world * 4)
 
     def alloc(self, name, nbytes):
         """Collective: every rank allocates `nbytes` under `name` and maps every peer's copy."""
@@ -123,7 +124,7 @@ class PeerComm:
 
 
 # flag slots
-_SLOT_GRADS_READY, _SLOT_UPDATE_DONE, _SLOT_LOSS, _SLOT_GATHER, _SLOT_INF, _SLOT_BUCKET0 = 0, 1, 2, 3, 4, 8
+_SLOT_GRADS_READY, _SLOT_UPDATE_DONE, _SLOT_LOSS, _SLOT_GATHER, _SLOT_INF, _SLOT_CLIP, _SLOT_BUCKET0 = 0, 1, 2, 3, 4, 5, 8
 _GATHER_SLOT_BYTES = 64 << 10     # per-rank capacity of the two eval-gather buffers (grown on demand)
 
 
@@ -291,36 +292,50 @@ class DistributedDataParallel(nn.Module):
             if op != L.ACCUM_FOLD:
                 return
         self.comm.barrier(_SLOT_BUCKET0 + idx, s)
-        self._exchange_update(opt, idx, s)
+        if opt._clip is not None:
+            opt._clip_reduce(idx, self._grad_sources(idx, s), s)   # a clipped step: the update waits for the norm
+        else:
+            self._exchange_update(opt, idx, s)
         if self._pending is None:
             self._pending = set()
         self._pending.add(idx)
+
+    def _grad_sources(self, idx, s):
+        """every rank's bf16 gradients of my slice of bucket `idx`, as the reduce kernels read them: the peers' mapped
+        buffers (kernel form), or in the DMA form local staging copies filled by copy-engine transfers on `s`"""
+        sb, se = self._slices[idx]
+        peers_g = self.comm.peers["grads"]
+        if not self.dma or idx == 0 or se <= sb:
+            return list(peers_g)
+        g_ptrs = []
+        for r in range(self.world):
+            if r == self.rank:
+                g_ptrs.append(peers_g[r])
+                continue
+            st = self._stage.data_ptr() + self._stage_off[idx][r]
+            L.call("b2_copy_async", st, peers_g[r] + 2 * sb, 2 * (se - sb), s)
+            g_ptrs.append(st - 2 * sb)        # the kernel indexes base + absolute element index
+        return g_ptrs
 
     def _exchange_update(self, opt, idx, s):
         """Mean over ranks + HF-AdamW on my slice of bucket `idx` + delivery of the new bf16 weights to every rank.
         Kernel form (default): the reduce kernel loads the peers' slices / stores the peers' shadows itself through the
         mapped pointers -- one launch per bucket does the one-shot peer-HBM reduction, the fp32 cast, the partitioned
         AdamW and the delivery of the new weights.  DMA form (B2_DDP_DMA=1, every bucket but the last one produced):
-        the transfers are copy-engine copies over NVLink and the reduce kernel works on local memory only."""
+        the transfers are copy-engine copies over NVLink and the reduce kernel works on local memory only.  In a
+        clipped step the mean is already in the clip stash (the reduce phase made it): no peer gradient is read."""
         sb, se = self._slices[idx]
         if se <= sb:
             return
         peers_g, peers_s = self.comm.peers["grads"], self.comm.peers["shadow"]
+        stash = opt._clip_stash_ptr(idx) if opt._clip is not None else None
         if not self.dma or idx == 0:
-            opt.update_range(sb, se, self.world, self.rank, peers_g, peers_s, s)
+            opt.update_range(sb, se, self.world, self.rank, peers_g, peers_s, s, grad_f32=stash)
             return
         nbytes = 2 * (se - sb)
-        g_ptrs, s_ptrs = [], []
-        for r in range(self.world):
-            if r == self.rank:
-                g_ptrs.append(peers_g[r])
-                s_ptrs.append(peers_s[r])
-                continue
-            st = self._stage.data_ptr() + self._stage_off[idx][r]
-            L.call("b2_copy_async", st, peers_g[r] + 2 * sb, nbytes, s)
-            g_ptrs.append(st - 2 * sb)        # the kernel indexes base + absolute element index
-            s_ptrs.append(None)
-        opt.update_range(sb, se, self.world, self.rank, g_ptrs, s_ptrs, s)
+        g_ptrs = list(peers_g) if stash is not None else self._grad_sources(idx, s)
+        s_ptrs = [peers_s[r] if r == self.rank else None for r in range(self.world)]
+        opt.update_range(sb, se, self.world, self.rank, g_ptrs, s_ptrs, s, grad_f32=stash)
         mine = peers_s[self.rank] + 2 * sb
         for r in range(self.world):
             if r != self.rank:
@@ -350,7 +365,19 @@ class DistributedDataParallel(nn.Module):
         main = torch.cuda.current_stream(eng.dev)
         nb = len(self.module._layout.buckets)
         done = self._pending or set()
-        if len(done) == nb:
+        if opt._clip is not None:
+            # a clipped step: the hooks (or clip_grad_norm_) ran the reduce phase; the finalize and every update follow
+            if done:
+                ev = torch.cuda.Event()
+                ev.record(self._side)
+                main.wait_event(ev)
+            s = main.cuda_stream
+            opt._clip_before_update(s)
+            for idx in range(nb):
+                self._exchange_update(opt, idx, s)
+            self.comm.barrier(_SLOT_UPDATE_DONE, s)
+            opt.advance(s)
+        elif len(done) == nb:
             # everything was launched from the backward hooks: just join
             s = self._side.cuda_stream
             self.comm.barrier(_SLOT_UPDATE_DONE, s)
@@ -373,6 +400,16 @@ class DistributedDataParallel(nn.Module):
             opt.advance(s)
         self._pending = None
         self._master_stale = True
+
+    def _clip_reduce_rest(self, opt, s):
+        """the reduce phase, on `s`, of every bucket no backward hook has reduced, behind the barrier that makes every
+        rank's gradients final"""
+        todo = [idx for idx in range(len(self.module._layout.buckets)) if idx not in opt._clip["reduced"]]
+        if not todo:
+            return
+        self.comm.barrier(_SLOT_GRADS_READY, s)
+        for idx in todo:
+            opt._clip_reduce(idx, self._grad_sources(idx, s), s)
 
     def _gather_master(self):
         """fp32 masters are updated slice-wise by their owner ranks.  Re-assemble them on THIS rank by pulling every

@@ -873,8 +873,13 @@ class _Engine:
                     self.accumulate_range(b0, e0, self._pass_op, os_)
                     if self._pass_op != L.ACCUM_FOLD:
                         return      # an accumulating pass: no update
-                opt.update_range(b0, e0, 1, 0, [self.grads.data_ptr()], [self.shadow.data_ptr()], os_,
-                                 background=(idx != 0))
+                if opt._clip is not None:
+                    # a clipped step: only the reduce phase hides under the backward; no bucket may move before the
+                    # norm of the whole gradient is known (optimizer.step() finalizes and updates)
+                    opt._clip_reduce(idx, [self.grads.data_ptr()], os_)
+                else:
+                    opt.update_range(b0, e0, 1, 0, [self.grads.data_ptr()], [self.shadow.data_ptr()], os_,
+                                     background=(idx != 0))
                 opt._pending.add(idx)
 
         if not self.lay.head_in_last_layer:

@@ -65,6 +65,10 @@ class AdamW(torch.optim.Optimizer):
         self._dev_state = None
         self._armed = False      # set by FusedTrainStep: per-bucket updates may start during backward
         self._pending = set()    # buckets already updated (on the engine's optimizer stream) in this step
+        # gradient clipping: _clip = the clipped step in progress (None: the next step does not clip), _clip_buf = its
+        # device buffers, kept across steps (captured graphs replay on them)
+        self._clip = None
+        self._clip_buf = None
         self._model._optimizer = self
 
     # -- device state (fp32 moments, step counter) ------------------------------------------------------------------
@@ -105,9 +109,17 @@ class AdamW(torch.optim.Optimizer):
         if gs is not None and (gs.dtype != torch.float32 or not gs.is_cuda):
             raise TypeError("grad_scale must be a CUDA fp32 scalar (torch.cuda.amp.GradScaler's)")
         hp.found_inf = self._found_inf_ptr()
+        if self._clip is not None and self._clip["final"]:
+            hp.clip_coef = self._clip_buf["coef"].data_ptr()
         return hp
 
     def _found_inf_ptr(self):
+        """what skips the update: the GradScaler's flag, or in a clipped step the finalize's (which includes it)"""
+        if self._clip is not None and self._clip["final"]:
+            return self._clip_buf["skip"].data_ptr()
+        return self._scaler_found_inf_ptr()
+
+    def _scaler_found_inf_ptr(self):
         fi = getattr(self, "found_inf", None)         # GradScaler: 0-dim fp32 tensor (or int 0 when nothing was checked)
         if isinstance(fi, torch.Tensor):
             if fi.dtype != torch.float32 or not fi.is_cuda:
@@ -123,17 +135,19 @@ class AdamW(torch.optim.Optimizer):
         self._model._params_by_name["classifier.bias"].grad = None
         return None
 
-    def update_range(self, begin, end, world, rank, peer_grads, peer_shadow, stream, background=False):
+    def update_range(self, begin, end, world, rank, peer_grads, peer_shadow, stream, background=False, grad_f32=None):
         """Fused (mean over peers +) HF-AdamW on flat elements [begin, end).  background=True (one GPU, the update of
         a bucket launched while the backward pass is still running): the form shaped to run beside the GEMM CTAs;
         with nothing left to hide behind (the last bucket, or a plain optimizer.step()) the 256-thread kernel is the
-        faster one (5.2 vs 3.6 TB/s alone)."""
+        faster one (5.2 vs 3.6 TB/s alone).  In a clipped step the gradient is multiplied by the clip coefficient;
+        grad_f32: the fp32 mean gradient of the slice (the clip stash) to read instead of the peers' bf16 gradients."""
         if os.environ.get("B2_DEBUG_SKIP_ADAMW") == "1":
             return      # MEASUREMENT ONLY (how much of the optimizer is exposed in the step): weights are not updated
         st = self._state()
         hp = self.hparams()
+        hp.grad_f32 = grad_f32
         model = self._model
-        if background and world == 1 and hp.grad_scale is None and hp.found_inf is None:
+        if background and world == 1 and hp.grad_scale is None and hp.found_inf is None and grad_f32 is None:
             # one GPU: the form that fits beside the GEMM CTAs (csrc/optim.cu, adamw_slim_kernel)
             L.call("b2_adamw_background", peer_grads[0], peer_shadow[0], L.ptr(model._flat), L.ptr(st["exp_avg"]),
                    L.ptr(st["exp_avg_sq"]), L.ptr(st["decay"]), begin, end, hp, L.ptr(st["step_size"]), stream)
@@ -146,6 +160,103 @@ class AdamW(torch.optim.Optimizer):
         st = self._state()
         L.call("b2_step_advance", L.ptr(st["step"]), L.ptr(self._model._engine.rng), self._found_inf_ptr(), stream)
         self._prepare(stream)
+
+    # -- gradient-norm clipping: reduce (+ partial sums of squares) per bucket, one norm, then the update -----------------
+    def _clip_ranges(self):
+        """(world, rank, [(begin, end)] per bucket): the bucket slices this rank reduces and updates"""
+        ddp = self._model._ddp
+        if ddp is not None and ddp.world > 1:
+            return ddp.world, ddp.rank, list(ddp._slices)
+        return 1, 0, [(b, e) for (b, e, _label) in self._model._layout.buckets]
+
+    def _clip_arm(self, max_norm):
+        """Starts a clipped step: from here until step() no bucket is updated before the norm of the whole gradient is
+        known.  The device buffers (and, under DDP, the fp32 stash of this rank's slices) are allocated on first use."""
+        if self._clip is not None:
+            raise RuntimeError("clip_grad_norm_() called twice before optimizer.step(): the gradients of this step are "
+                               "already clipped")
+        max_norm = float(max_norm)
+        if not max_norm > 0.0:
+            raise ValueError("max_norm must be positive (got %r)" % max_norm)
+        world, rank, ranges = self._clip_ranges()
+        dev = self._model._engine.dev
+        key = (world, rank, tuple(ranges), dev)
+        if self._clip_buf is None or self._clip_buf["key"] != key:
+            slot_off, stash_off, ns, nst = [], [], 0, 0
+            for (b, e) in ranges:
+                slot_off.append(ns)
+                stash_off.append(nst)
+                ns += L.sumsq_slots(max(0, e - b))
+                nst += max(0, e - b)
+            f32 = dict(dtype=torch.float32, device=dev)
+            self._clip_buf = {
+                "key": key, "ranges": ranges, "slot_off": slot_off, "stash_off": stash_off, "nslots": ns,
+                "partials": torch.zeros(max(ns, 1), dtype=torch.float64, device=dev),
+                "stash": torch.empty(max(nst, 8), **f32) if world > 1 else None,   # 4 B x total / world
+                "norm": torch.zeros((), **f32), "coef": torch.ones((), **f32), "skip": torch.zeros((), **f32),
+            }
+        self._clip = {"max_norm": max_norm, "reduced": set(), "final": False}
+
+    def _clip_stash_ptr(self, idx):
+        buf = self._clip_buf
+        return None if buf["stash"] is None else buf["stash"].data_ptr() + 4 * buf["stash_off"][idx]
+
+    def _clip_reduce(self, idx, peer_grads, stream):
+        """reduce phase of bucket `idx`: this rank's slice, read from `peer_grads` (one per rank)"""
+        buf = self._clip_buf
+        b, e = buf["ranges"][idx]
+        if e > b:
+            L.call("b2_grad_reduce_sumsq", L.ptr_array(peer_grads), len(peer_grads), self._clip_stash_ptr(idx), b, e,
+                   buf["partials"].data_ptr() + 8 * buf["slot_off"][idx], stream)
+        self._clip["reduced"].add(idx)
+
+    def _clip_finalize(self, stream):
+        """the norm and the coefficient (collective under DDP).  Inside a GradScaler step it divides by the scale, so the
+        norm is that of the unscaled gradients, and a non-finite norm skips the step like GradScaler's inf check."""
+        buf, world, rank = self._clip_buf, 1, 0
+        scratch = flags = epoch = None
+        slot = 0
+        ddp = self._model._ddp
+        if ddp is not None and ddp.world > 1:
+            from .ddp import _SLOT_CLIP
+            world, rank, slot = ddp.world, ddp.rank, _SLOT_CLIP
+            scratch = L.ptr_array(ddp.comm.peers["scalar_clip"])
+            flags = L.ptr_array(ddp.comm.peers["flags"])
+            epoch = ddp.comm.epoch_ptr(_SLOT_CLIP)
+        gs = getattr(self, "grad_scale", None)
+        L.call("b2_grad_norm_finalize", buf["partials"].data_ptr(), buf["nslots"], scratch, flags, world, rank, slot,
+               epoch, self._clip["max_norm"], L.ptr(gs), self._scaler_found_inf_ptr(), buf["norm"].data_ptr(),
+               buf["coef"].data_ptr(), buf["skip"].data_ptr(), stream)
+        self._clip["final"] = True
+
+    def _clip_before_update(self, stream):
+        """in step(): the reduce phase of every bucket no backward hook has reduced, then the finalize -- again when a
+        GradScaler hands over its scale, since the norm clip_grad_norm_ returned was that of the scaled gradients"""
+        ddp = self._model._ddp
+        if ddp is not None and ddp.world > 1:
+            ddp._clip_reduce_rest(self, stream)
+        else:
+            eng = self._model._engine
+            for idx in range(len(self._model._layout.buckets)):
+                if idx not in self._clip["reduced"]:
+                    self._clip_reduce(idx, [eng.grads.data_ptr()], stream)
+        if not self._clip["final"] or getattr(self, "grad_scale", None) is not None:
+            self._clip_finalize(stream)
+
+    def clip_now(self, max_norm):
+        """The eager clip_grad_norm_: flush an open accumulation window, reduce every bucket, finalize; step() then runs
+        the update with the coefficient.  Returns the device norm buffer."""
+        model = self._model
+        eng = model._engine
+        ddp = model._ddp
+        if self._pending or (ddp is not None and ddp._pending):
+            raise RuntimeError("clip_grad_norm_(): this step's update already ran during backward (the optimizer is "
+                               "armed by a FusedTrainStep); clip through the captured step's max_grad_norm instead")
+        s = torch.cuda.current_stream(eng.dev).cuda_stream
+        eng.flush_accum(s)
+        self._clip_arm(max_norm)
+        self._clip_before_update(s)
+        return self._clip_buf["norm"]
 
     @torch.no_grad()
     def step(self, closure=None):
@@ -165,7 +276,11 @@ class AdamW(torch.optim.Optimizer):
                 ev = torch.cuda.Event()
                 ev.record(eng.opt_stream)
                 main.wait_event(ev)
-            if len(self._pending) == 0:
+            if self._clip is not None:
+                # the per-bucket launches of the backward were the reduce phase only
+                self._clip_before_update(s)
+                self.update_range(0, model._layout.total, 1, 0, [eng.grads.data_ptr()], [eng.shadow.data_ptr()], s)
+            elif len(self._pending) == 0:
                 self.update_range(0, model._layout.total, 1, 0, [eng.grads.data_ptr()], [eng.shadow.data_ptr()], s)
             else:
                 for idx, (b0, e0, _lbl) in enumerate(model._layout.buckets):
@@ -173,6 +288,7 @@ class AdamW(torch.optim.Optimizer):
                         self.update_range(b0, e0, 1, 0, [eng.grads.data_ptr()], [eng.shadow.data_ptr()], s)
             self._pending = set()
             self.advance(s)
+        self._clip = None
         model._grads_live = False
         # the inf-check probe has served its purpose (GradScaler reads it before calling step); the -amp scripts never
         # call zero_grad, so drop it here or it would accumulate
@@ -187,6 +303,49 @@ class AdamW(torch.optim.Optimizer):
             off, shape = self._model._layout.entries[name]
             out[name] = (st["exp_avg"][off:off + p.numel()].view(shape), st["exp_avg_sq"][off:off + p.numel()].view(shape))
         return out
+
+
+def clip_grad_norm_(parameters, max_norm, norm_type=2.0, error_if_nonfinite=False, foreach=None):
+    """``torch.nn.utils.clip_grad_norm_`` for a b200 model: call it between ``backward()`` and ``optimizer.step()``.
+
+    torch's own function cannot be used: the gradients live in the model's bf16 bucket space, not in ``.grad``, so it
+    would see only the 6-float probe on ``classifier.bias`` and clip nothing else.  This one computes the 2-norm of the
+    gradient the next ``optimizer.step()`` applies (an open ``no_sync()`` window is flushed first) and makes that step
+    multiply the gradient by ``min(1, max_norm / (norm + 1e-6))`` (torch's coefficient).
+
+    ``parameters`` must be every parameter of one b200 model (``model.parameters()``, wrapped or not).  Returns the
+    total norm as a 0-dim fp32 CUDA tensor without a host sync; ``error_if_nonfinite=True`` syncs and raises
+    ``RuntimeError`` on a non-finite norm, and the step is then not clipped.  ``foreach`` is accepted and ignored.
+
+    Under ``DistributedDataParallel`` with world > 1 it is the norm of the DDP-mean gradient, the one torch DDP clips,
+    and the call is collective: every rank must make it, and every rank gets the same norm bit for bit.  Under a
+    GradScaler step (the package Trainer's ``use_amp``) ``step()`` recomputes the norm from the unscaled gradients."""
+    if isinstance(parameters, torch.Tensor):
+        parameters = [parameters]
+    params = list(parameters)
+    if float(norm_type) != 2.0:
+        raise ValueError("clip_grad_norm_: only norm_type=2 is supported (got %r)" % (norm_type,))
+    owners = {id(getattr(p, "_b2_owner", None)) for p in params}
+    model = getattr(params[0], "_b2_owner", None) if params else None
+    if model is None or len(owners) != 1:
+        raise TypeError("clip_grad_norm_: the parameters must all belong to ONE b200 BertForSequenceClassification")
+    names = {p._b2_name for p in params}
+    if names != set(model._layout.entries):
+        raise ValueError("clip_grad_norm_: clipping covers the whole gradient of the model; pass every parameter "
+                         "(%d of %d were passed)" % (len(names), len(model._layout.entries)))
+    if model._engine is None:
+        raise RuntimeError("clip_grad_norm_: the model is not on CUDA (there is no CPU path): call model.cuda() first")
+    opt = model._optimizer
+    if opt is None:
+        raise RuntimeError("clip_grad_norm_: the clip is applied by the model's AdamW inside optimizer.step(); build "
+                           "the optimizer first")
+    norm = opt.clip_now(max_norm)
+    if error_if_nonfinite and not bool(torch.isfinite(norm)):
+        opt._clip = None
+        raise RuntimeError("The total norm of order 2.0 for gradients from `parameters` is non-finite, so it cannot be "
+                           "clipped. To disable this error and scale the gradients by the non-finite norm anyway, set "
+                           "`error_if_nonfinite=False`")
+    return norm.clone()
 
 
 def build_optimizer(model, args):

@@ -16,6 +16,7 @@ import numpy as np
 import torch
 
 from .ddp import DistributedDataParallel
+from .optim import clip_grad_norm_
 
 
 class Args:
@@ -40,6 +41,8 @@ class Args:
                           # reference pads every row to max_seq_len although real rows average 18 tokens [:76]
     gradient_accumulation_steps = 1   # k > 1: one optimizer step per k batches, each batch's loss scaled by 1/k (the
                                       # HF Trainer / DeepSpeed name; fabric-cls.py's grad_accumulation)
+    max_grad_norm = None  # clip the gradient's 2-norm to this before every optimizer step (HF TrainingArguments'
+                          # name); None or 0: no clipping
     log_every = 1         # the reference prints every step (forces a D2H sync per step)
     total_step = 0
 
@@ -73,6 +76,7 @@ class _StagedGraphStep:
         self._warm = {}
         self._role = (True, False)
         self.accum_steps = 1
+        self.max_grad_norm = None
         self._h2d_done = None
         # The step body -- the critical chain of forward / dgrad kernels -- is issued (and captured) on a HIGH-priority
         # stream, so that when an SM frees up the block scheduler hands it to the critical path before the
@@ -148,9 +152,10 @@ class _StagedGraphStep:
                 self.graph = g
         g.replay()
 
-    def _arm(self, optimizer, accum_steps):
+    def _arm(self, optimizer, accum_steps, max_grad_norm=None):
         self.opt = optimizer
         self.accum_steps = accum_steps
+        self.max_grad_norm = float(max_grad_norm) if max_grad_norm else None
         if accum_steps > 1:
             self.eng.ensure_accum()       # outside any capture
         # the fused step owns backward + optimizer: per-bucket AdamW (and, under DDP, the peer exchange) may start
@@ -171,6 +176,8 @@ class _StagedGraphStep:
         if self.accum_steps > 1:
             ws["dloss_logits"].mul_(1.0 / self.accum_steps)     # what an eager loop does with loss / k
         # d(loss)/d(logits) was produced by the CE kernel: the reference's criterion(logits, label) [:169]
+        if final and self.max_grad_norm is not None:
+            opt._clip_arm(self.max_grad_norm)     # the backward's per-bucket launches become the reduce phase
         eng.start_pass(not final)
         eng._backward_from_dlogits(ws["dloss_logits"], B, S, mask, p_h, p_a, p_c, packed)
         eng.end_pass()
@@ -188,11 +195,12 @@ class FusedTrainStep(_StagedGraphStep):
     """One training step == one CUDA-graph replay: H2D of the batch, embeddings -> 12 layers -> head -> CE, the full
     backward, the peer-HBM gradient exchange fused with AdamW, and the device-side step/RNG bump.  Semantically the body
     of the reference loop [:166-176] without the host round trips.  accum_steps = k > 1: gradient accumulation over k
-    micro-batches, the loss scaled by 1/k; call with final=False for the first k - 1 of a window."""
+    micro-batches, the loss scaled by 1/k; call with final=False for the first k - 1 of a window.  max_grad_norm:
+    clip the gradient's 2-norm before the update (see clip_grad_norm_); the norm is left in optimizer._clip_buf."""
 
-    def __init__(self, model, optimizer, batch_size, seq_len, use_graph=True, accum_steps=1):
+    def __init__(self, model, optimizer, batch_size, seq_len, use_graph=True, accum_steps=1, max_grad_norm=None):
         super().__init__(model, batch_size, seq_len, use_graph)
-        self._arm(optimizer, accum_steps)
+        self._arm(optimizer, accum_steps, max_grad_norm)
         self.kernel_launches = None
 
     # the step body, expressed only with stream-ordered work (capturable)
@@ -214,7 +222,7 @@ class PackedTrainStep(_StagedGraphStep):
     instance (staging buffers + CUDA graph) per bin count; the Trainer keeps a small cache of them, since the number of
     bins a batch packs into varies with its lengths."""
 
-    def __init__(self, model, optimizer, bins, batch, use_graph=True, accum_steps=1):
+    def __init__(self, model, optimizer, bins, batch, use_graph=True, accum_steps=1, max_grad_norm=None):
         super().__init__(model, bins, 128, use_graph)
         dev = self.eng.dev
         self.bins, self.batch = bins, batch
@@ -225,7 +233,7 @@ class PackedTrainStep(_StagedGraphStep):
         z = lambda *sh: torch.zeros(*sh, dtype=torch.int64, device=dev)
         self.d_pos, self.d_cls, self.d_lab = z(bins, 128), z(batch), z(batch)
         self.d_seg = torch.zeros(bins, 128, dtype=torch.int32, device=dev)
-        self._arm(optimizer, accum_steps)
+        self._arm(optimizer, accum_steps, max_grad_norm)
 
     def _unstage(self):
         n, st = self.bins * 128, self.d_stage
@@ -299,6 +307,8 @@ class Trainer:
         self._fused_eval = {}
         self._pin = {}
         self._micro = 0       # batches of the open gradient-accumulation window
+        self.last_grad_norm = None   # device scalar: the pre-clip gradient norm of the last optimizer step (HF's
+                                     # logged `grad_norm`); None when not clipping
 
     def _to_device(self, batch_data):
         dev = _unwrap(self.model)._engine.dev
@@ -357,6 +367,7 @@ class Trainer:
         (inside no_sync() on the eager paths), the k-th also steps the optimizer; every loss is scaled by 1/k
         (fabric-cls.py:150-157) and the returned loss is the unscaled micro-batch loss."""
         k = max(1, int(getattr(self.args, "gradient_accumulation_steps", 1)))
+        clip = self._max_grad_norm()
         first, final = self._micro == 0, self._micro >= k - 1
         self._micro = 0 if final else self._micro + 1
         if getattr(self.args, "fused", True) and getattr(self.args, "pack", False) and \
@@ -364,16 +375,18 @@ class Trainer:
             from .packing import pack_batch
             packed = pack_batch(batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"])
             key = (packed["bins"], batch_data["input_ids"].shape[0])
-            if key not in self._packed or self._packed[key].accum_steps != k:
+            if key not in self._packed or (self._packed[key].accum_steps, self._packed[key].max_grad_norm) != (k, clip):
                 if len(self._packed) >= 16:           # bound the graph cache: drop the oldest entry
                     self._packed.pop(next(iter(self._packed)))
-                self._packed[key] = PackedTrainStep(self.model, self.optimizer, key[0], key[1], accum_steps=k)
+                self._packed[key] = PackedTrainStep(self.model, self.optimizer, key[0], key[1], accum_steps=k,
+                                                    max_grad_norm=clip)
             self.model.train()
             loss = self._packed[key](packed, batch_data["label"], final)
         elif getattr(self.args, "fused", True):
             B, S = batch_data["input_ids"].shape
-            if self._fused is None or (self._fused.B, self._fused.S, self._fused.accum_steps) != (B, S, k):
-                self._fused = FusedTrainStep(self.model, self.optimizer, B, S, accum_steps=k)
+            if self._fused is None or (self._fused.B, self._fused.S, self._fused.accum_steps,
+                                       self._fused.max_grad_norm) != (B, S, k, clip):
+                self._fused = FusedTrainStep(self.model, self.optimizer, B, S, accum_steps=k, max_grad_norm=clip)
             self.model.train()
             loss = self._fused(batch_data, final)
         elif getattr(self.args, "use_amp", False):
@@ -387,6 +400,7 @@ class Trainer:
                     loss = self.criterion(logits, label)
                 self._scaler.scale(loss / k if k > 1 else loss).backward()
             if final:
+                self._clip(clip)        # no scaler.unscale_: step() takes the scale out of the norm
                 self._scaler.step(self.optimizer)
                 self._scaler.update()
         else:
@@ -398,8 +412,23 @@ class Trainer:
                     self.optimizer.zero_grad()
                 (loss / k if k > 1 else loss).backward()
             if final:
+                self._clip(clip)
                 self.optimizer.step()
+        if final:
+            self._note_grad_norm(clip)
         return self.loss_reduce(loss.detach())
+
+    def _max_grad_norm(self):
+        m = getattr(self.args, "max_grad_norm", None)
+        return float(m) if m else None
+
+    def _clip(self, clip):
+        if clip is not None:
+            clip_grad_norm_(self.model.parameters(), clip)
+
+    def _note_grad_norm(self, clip):
+        buf = self.optimizer._clip_buf
+        self.last_grad_norm = buf["norm"].clone() if clip is not None and buf is not None else None
 
     def _window(self, final):
         """the eager loops' micro-batches run inside no_sync(), the final one of a window outside it"""
@@ -411,11 +440,14 @@ class Trainer:
         if self._micro == 0:
             return
         self._micro = 0
+        clip = self._max_grad_norm()
+        self._clip(clip)
         if self._scaler is not None and not getattr(self.args, "fused", True):
             self._scaler.step(self.optimizer)
             self._scaler.update()
         else:
             self.optimizer.step()
+        self._note_grad_norm(clip)
 
     def train(self, train_loader, dev_loader=None, train_sampler=None):
         gloabl_step = 1
