@@ -28,7 +28,7 @@ extern "C" {
 /* ------------------------------------------------------------------------------------------------------ */
 const char* b2_last_error(void);
 int32_t b2_abi_version(void);             /* bumped when a struct below changes */
-#define B2_ABI_VERSION 20
+#define B2_ABI_VERSION 21
 int64_t b2_launch_count(void);            /* kernels launched by this library so far (process-wide) */
 
 /* ------------------------------------------------------------------------------------------------------ */
@@ -281,6 +281,11 @@ typedef struct b2_adamw_hparams {
    * the peers' bf16 gradients.  NULL = today's update, bit for bit.                                                */
   const float* clip_coef;
   const float* grad_f32;
+  /* optional DEVICE fp64 learning rate, read in place of `lr` by all three AdamW entry points: a captured training
+   * step refreshes it before every replay from the host's param_groups[0]["lr"], so a torch LR scheduler keeps
+   * working there.  lr * weight_decay is formed in double from it, as the host forms it from `lr`: a device value
+   * equal to `lr` gives the same bits.  NULL = `lr` by value.                                                  */
+  const double* lr_dev;
 } b2_adamw_hparams_t;
 
 /* Fused update of one contiguous slice [begin, end) (element indices, multiples of 8) of the flat parameter

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2ddpbert.so")
-ABI_VERSION = 20
+ABI_VERSION = 21
 
 MAJOR_K, MAJOR_MN = 0, 1
 EPI_NONE, EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_DROPOUT_RESIDUAL, EPI_RESIDUAL, EPI_GELU_BWD = 0, 1, 2, 3, 4, 5
@@ -43,7 +43,7 @@ class GemmArgs(C.Structure):
 class AdamWHParams(C.Structure):
     _fields_ = [("lr", f64), ("beta1", f64), ("beta2", f64), ("eps", f64), ("weight_decay", f64),
                 ("correct_bias", i32), ("grad_scale", vp), ("found_inf", vp),
-                ("clip_coef", vp), ("grad_f32", vp)]
+                ("clip_coef", vp), ("grad_f32", vp), ("lr_dev", vp)]
 
 
 # name -> argtypes; every function returns int32 status unless listed in _SPECIAL

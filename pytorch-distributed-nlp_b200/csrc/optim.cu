@@ -32,6 +32,8 @@ struct ReduceAdamWParams {
   const float* found_inf;    // optional device scalar (GradScaler): non-zero skips the update
   const float* clip_coef;    // optional device scalar (gradient clipping): gradients are multiplied by it
   const float* grad_f32;     // optional fp32 mean gradient of [begin, end), indexed from begin: read instead of peers
+  const double* lr_dev;      // optional device fp64 learning rate (a captured step's schedule): read instead of lr_d
+  double weight_decay_d;
 };
 
 __global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWParams p) {
@@ -40,13 +42,22 @@ __global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWPara
   if (p.found_inf != nullptr && *p.found_inf != 0.f) return;   // GradScaler saw inf/nan: this step is skipped
   // x * 1.0f is exact: without a coefficient the update is today's, bit for bit
   const float coef = p.clip_coef != nullptr ? *p.clip_coef : 1.0f;
+  // the learning rate from device memory: the same double arithmetic the host does on the by-value lr, so a device lr
+  // equal to the host value gives the same bits
+  double lr_d = p.lr_d;
+  float lr = p.lr, lr_wd = p.lr_wd;
+  if (p.lr_dev != nullptr) {
+    lr_d = *p.lr_dev;
+    lr = (float)lr_d;
+    lr_wd = (float)(lr_d * p.weight_decay_d);
+  }
   // HF AdamW bias correction: step_size = lr * sqrt(1 - b2^t) / (1 - b1^t), t = steps taken including this one
   const long long t = *p.step_counter + 1;
-  float step_size = p.lr;
+  float step_size = lr;
   if (p.correct_bias) {
     const double bc1 = 1.0 - pow(p.beta1_d, (double)t);
     const double bc2 = 1.0 - pow(p.beta2_d, (double)t);
-    step_size = (float)(p.lr_d * sqrt(bc2) / bc1);
+    step_size = (float)(lr_d * sqrt(bc2) / bc1);
   }
   // mean over ranks (unless grad_f32 already holds it); with a GradScaler also the unscale (a power of two: exact)
   const float inv_world = (p.grad_scale != nullptr ? 1.0f / *p.grad_scale : 1.0f) /
@@ -85,7 +96,7 @@ __global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWPara
       vv[k] = vv[k] * p.beta2 + gk * gk * p.one_minus_beta2;
       const float denom = sqrtf(vv[k]) + p.eps;
       w[k] = w[k] - step_size * (mm[k] / denom);
-      if (decay) w[k] = w[k] - p.lr_wd * w[k];
+      if (decay) w[k] = w[k] - lr_wd * w[k];
     }
     *reinterpret_cast<float4*>(p.master + e) = make_float4(w[0], w[1], w[2], w[3]);
     *reinterpret_cast<float4*>(p.master + e + 4) = make_float4(w[4], w[5], w[6], w[7]);
@@ -121,6 +132,8 @@ struct SlimParams {
   int has_wd;
   const float* step_size;
   const float* clip_coef;   // optional (gradient clipping): gradients are multiplied by it
+  const double* lr_dev;     // optional device fp64 learning rate: lr_wd is computed from it (step_size already is)
+  double weight_decay;
 };
 constexpr int kSlimThreads = 128, kSlimIters = 8;
 template <int DUMMY>
@@ -130,32 +143,39 @@ adamw_slim_kernel(const SlimParams p) {
   pdl_launch_dependents();
   const float step_size = *p.step_size;
   const float coef = p.clip_coef != nullptr ? *p.clip_coef : 1.0f;   // x * 1.0f is exact
+  const float lr_wd = p.lr_dev != nullptr ? (float)(*p.lr_dev * p.weight_decay) : p.lr_wd;
   long long i = (long long)blockIdx.x * (kSlimThreads * kSlimIters) + threadIdx.x;
 #pragma unroll 1
   for (int it = 0; it < kSlimIters; ++it, i += kSlimThreads) {
     if (i >= p.nvec4) break;
     const long long e = p.begin + (i << 2);
     const uint2 q = *reinterpret_cast<const uint2*>(p.grads + e);
-    float4 w = *reinterpret_cast<const float4*>(p.master + e);
     float4 mm = *reinterpret_cast<const float4*>(p.m + e);
     float4 vv = *reinterpret_cast<const float4*>(p.v + e);
-    const bool decay = p.has_wd && p.decay[e >> 3];
     const float g0 = bf16_lo(q.x) * coef, g1 = bf16_hi(q.x) * coef, g2 = bf16_lo(q.y) * coef,
                 g3 = bf16_hi(q.y) * coef;
     mm.x = mm.x * p.beta1 + g0 * p.one_minus_beta1; vv.x = vv.x * p.beta2 + g0 * g0 * p.one_minus_beta2;
     mm.y = mm.y * p.beta1 + g1 * p.one_minus_beta1; vv.y = vv.y * p.beta2 + g1 * g1 * p.one_minus_beta2;
     mm.z = mm.z * p.beta1 + g2 * p.one_minus_beta1; vv.z = vv.z * p.beta2 + g2 * g2 * p.one_minus_beta2;
     mm.w = mm.w * p.beta1 + g3 * p.one_minus_beta1; vv.w = vv.w * p.beta2 + g3 * g3 * p.one_minus_beta2;
-    w.x = w.x - step_size * (mm.x / (sqrtf(vv.x) + p.eps));
-    w.y = w.y - step_size * (mm.y / (sqrtf(vv.y) + p.eps));
-    w.z = w.z - step_size * (mm.z / (sqrtf(vv.z) + p.eps));
-    w.w = w.w - step_size * (mm.w / (sqrtf(vv.w) + p.eps));
-    if (decay) {
-      w.x = w.x - p.lr_wd * w.x; w.y = w.y - p.lr_wd * w.y; w.z = w.z - p.lr_wd * w.z; w.w = w.w - p.lr_wd * w.w;
-    }
-    *reinterpret_cast<float4*>(p.master + e) = w;
     *reinterpret_cast<float4*>(p.m + e) = mm;
     *reinterpret_cast<float4*>(p.v + e) = vv;
+    // the Adam direction first, then the master weights: fewer values live at once (no spills at 32 registers)
+    float4 u;
+    u.x = mm.x / (sqrtf(vv.x) + p.eps);
+    u.y = mm.y / (sqrtf(vv.y) + p.eps);
+    u.z = mm.z / (sqrtf(vv.z) + p.eps);
+    u.w = mm.w / (sqrtf(vv.w) + p.eps);
+    float4 w = *reinterpret_cast<const float4*>(p.master + e);
+    const bool decay = p.has_wd && p.decay[e >> 3];
+    w.x = w.x - step_size * u.x;
+    w.y = w.y - step_size * u.y;
+    w.z = w.z - step_size * u.z;
+    w.w = w.w - step_size * u.w;
+    if (decay) {
+      w.x = w.x - lr_wd * w.x; w.y = w.y - lr_wd * w.y; w.z = w.z - lr_wd * w.z; w.w = w.w - lr_wd * w.w;
+    }
+    *reinterpret_cast<float4*>(p.master + e) = w;
     uint2 o;
     o.x = pack_bf16(w.x, w.y);
     o.y = pack_bf16(w.z, w.w);
@@ -319,12 +339,14 @@ __global__ void grad_norm_finalize_kernel(const double* __restrict__ partials, l
     *skip = ((found_inf != nullptr && *found_inf != 0.f) || (grad_scale != nullptr && !isfinite(norm))) ? 1.f : 0.f;
 }
 
-// HF AdamW bias correction for the NEXT update: step_size = lr * sqrt(1 - b2^t) / (1 - b1^t), t = *step + 1
-__global__ void adamw_prepare_kernel(double lr, double beta1, double beta2, int correct_bias, const long long* step,
-                                     float* step_size) {
+// HF AdamW bias correction for the NEXT update: step_size = lr * sqrt(1 - b2^t) / (1 - b1^t), t = *step + 1; lr is
+// *lr_dev when that is set
+__global__ void adamw_prepare_kernel(double lr_arg, const double* lr_dev, double beta1, double beta2, int correct_bias,
+                                     const long long* step, float* step_size) {
   pdl_wait();
   pdl_launch_dependents();
   if (threadIdx.x == 0 && blockIdx.x == 0) {
+    const double lr = lr_dev != nullptr ? *lr_dev : lr_arg;
     double ss = lr;
     if (correct_bias) {
       const long long t = *step + 1;
@@ -429,6 +451,8 @@ extern "C" int32_t b2_bucket_reduce_adamw(const void* const* peer_grads, void* c
   p.found_inf = hp->found_inf;
   p.clip_coef = hp->clip_coef;
   p.grad_f32 = hp->grad_f32;
+  p.lr_dev = hp->lr_dev;
+  p.weight_decay_d = hp->weight_decay;
   B2_REQUIRE((uintptr_t)p.grad_f32 % 16 == 0, "bucket_reduce_adamw: grad_f32 must be 16-byte aligned");
   const long long nvec = (end - begin) >> 3;
   long long blocks = (nvec + 255) / 256;
@@ -443,8 +467,8 @@ extern "C" int32_t b2_bucket_reduce_adamw(const void* const* peer_grads, void* c
 extern "C" int32_t b2_adamw_prepare(const b2_adamw_hparams_t* hp, const int64_t* step_counter, float* step_size,
                                     void* stream_) {
   B2_REQUIRE(hp && step_counter && step_size, "adamw_prepare: null pointer");
-  B2_LAUNCH(adamw_prepare_kernel, 1, 32, 0, (cudaStream_t)stream_, hp->lr, hp->beta1, hp->beta2, hp->correct_bias,
-            (const long long*)step_counter, step_size);
+  B2_LAUNCH(adamw_prepare_kernel, 1, 32, 0, (cudaStream_t)stream_, hp->lr, hp->lr_dev, hp->beta1, hp->beta2,
+            hp->correct_bias, (const long long*)step_counter, step_size);
   B2_CUDA(cudaGetLastError());
   count_launches(1);
   return 0;
@@ -476,6 +500,8 @@ extern "C" int32_t b2_adamw_background(const void* grads, void* shadow, float* m
   p.has_wd = hp->weight_decay > 0.0 ? 1 : 0;
   p.step_size = step_size;
   p.clip_coef = hp->clip_coef;
+  p.lr_dev = hp->lr_dev;
+  p.weight_decay = hp->weight_decay;
   const long long per_block = (long long)kSlimThreads * kSlimIters;
   const long long blocks = (p.nvec4 + per_block - 1) / per_block;
   B2_LAUNCH(adamw_slim_kernel<1>, (unsigned)blocks, kSlimThreads, 0, (cudaStream_t)stream_, p);

@@ -878,6 +878,8 @@ class _Engine:
                     # norm of the whole gradient is known (optimizer.step() finalizes and updates)
                     opt._clip_reduce(idx, [self.grads.data_ptr()], os_)
                 else:
+                    if not opt._pending:
+                        opt.prepare_background(os_)      # the step size of this step's lr
                     opt.update_range(b0, e0, 1, 0, [self.grads.data_ptr()], [self.shadow.data_ptr()], os_,
                                      background=(idx != 0))
                 opt._pending.add(idx)

@@ -69,6 +69,9 @@ class AdamW(torch.optim.Optimizer):
         # device buffers, kept across steps (captured graphs replay on them)
         self._clip = None
         self._clip_buf = None
+        # set by a captured train step for the duration of its body: the kernels read the lr from the device scalar
+        # the step refreshes before every replay (see hparams), not the value passed at launch / capture
+        self._lr_dev_on = False
         self._model._optimizer = self
 
     # -- device state (fp32 moments, step counter) ------------------------------------------------------------------
@@ -84,6 +87,7 @@ class AdamW(torch.optim.Optimizer):
                 "exp_avg_sq": torch.zeros(n, dtype=torch.float32, device=eng.dev),
                 "step": torch.zeros(1, dtype=torch.int64, device=eng.dev),
                 "step_size": torch.zeros(1, dtype=torch.float32, device=eng.dev),   # see b2_adamw_prepare
+                "lr": torch.zeros(1, dtype=torch.float64, device=eng.dev),           # a captured step's lr
                 "decay": self._decay_flags_cpu.to(eng.dev),
             }
             self._prepare(eng.stream())
@@ -98,6 +102,24 @@ class AdamW(torch.optim.Optimizer):
         st = self._dev_state
         L.call("b2_adamw_prepare", self.hparams(), L.ptr(st["step"]), L.ptr(st["step_size"]), stream)
 
+    def current_lr(self):
+        """The lr of the next update: param_groups' (a torch LR scheduler changes it between steps).  The update is
+        one kernel over every parameter, so the groups must agree; they may differ only in weight_decay."""
+        lr = self.param_groups[0]["lr"]
+        for g in self.param_groups[1:]:
+            if g["lr"] != lr:
+                raise ValueError("param groups have different learning rates (%s); the fused update applies one lr to "
+                                 "every parameter (a LambdaLR with one lambda per group can cause this)"
+                                 % ", ".join(repr(x["lr"]) for x in self.param_groups))
+        return float(lr)
+
+    def captured_hparams(self):
+        """The hyperparameters a captured step bakes into its graph (all but the lr, which it reads at every replay)"""
+        return {"betas": tuple(tuple(float(b) for b in g["betas"]) for g in self.param_groups),
+                "eps": tuple(float(g["eps"]) for g in self.param_groups),
+                "weight_decay": tuple(float(g["weight_decay"]) for g in self.param_groups),
+                "correct_bias": tuple(bool(g["correct_bias"]) for g in self.param_groups)}
+
     def hparams(self):
         g = self.param_groups[0]
         hp = L.AdamWHParams()
@@ -111,6 +133,8 @@ class AdamW(torch.optim.Optimizer):
         hp.found_inf = self._found_inf_ptr()
         if self._clip is not None and self._clip["final"]:
             hp.clip_coef = self._clip_buf["coef"].data_ptr()
+        if self._lr_dev_on:
+            hp.lr_dev = self._dev_state["lr"].data_ptr()
         return hp
 
     def _found_inf_ptr(self):
@@ -155,6 +179,12 @@ class AdamW(torch.optim.Optimizer):
         L.call("b2_bucket_reduce_adamw", L.ptr_array(peer_grads), L.ptr_array(peer_shadow), world, rank,
                L.ptr(model._flat), L.ptr(st["exp_avg"]), L.ptr(st["exp_avg_sq"]), L.ptr(st["decay"]), begin, end,
                hp, L.ptr(st["step"]), stream)
+
+    def prepare_background(self, stream):
+        """Before the first per-bucket background update of a step: the step size from the lr current now, not the
+        one of the previous step() (a scheduler has stepped since)"""
+        self._state()
+        self._prepare(stream)
 
     def advance(self, stream):
         st = self._state()
@@ -261,6 +291,7 @@ class AdamW(torch.optim.Optimizer):
     @torch.no_grad()
     def step(self, closure=None):
         loss = closure() if closure is not None else None
+        self.current_lr()
         model = self._model
         eng = model._engine
         if eng is None:

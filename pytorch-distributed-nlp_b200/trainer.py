@@ -8,8 +8,12 @@ Same methods, same argument meaning: ``on_step`` [:126-137], ``loss_reduce`` [:1
     inside the gradient exchange, and a host-blocking barrier only serialises forward/backward across ranks;
   * ``loss_reduce`` / ``output_reduce`` go through the peer-memory kernels when the model is the b200 DDP wrapper;
   * ``train`` uses :class:`FusedTrainStep` (the whole step captured in one CUDA graph) when ``args.fused`` is set.
+A learning-rate schedule is a host-side torch ``LRScheduler`` (passed as ``scheduler=`` like fabric-cls.py's Trainer, or
+built from ``Args.lr_scheduler_type``), stepped once per optimizer step on every path; the captured steps read the lr
+it sets at every replay.
 """
 import contextlib
+import math
 import time
 
 import numpy as np
@@ -17,6 +21,7 @@ import torch
 
 from .ddp import DistributedDataParallel
 from .optim import clip_grad_norm_
+from .schedules import get_scheduler, warmup_steps
 
 
 class Args:
@@ -43,6 +48,10 @@ class Args:
                                       # HF Trainer / DeepSpeed name; fabric-cls.py's grad_accumulation)
     max_grad_norm = None  # clip the gradient's 2-norm to this before every optimizer step (HF TrainingArguments'
                           # name); None or 0: no clipping
+    lr_scheduler_type = None   # HF TrainingArguments' names: "linear", "cosine", "constant", "constant_with_warmup";
+                               # None: a constant lr (HF's default is "linear")
+    warmup_steps = 0      # linear warmup from 0 over this many optimizer steps; when 0, ceil(warmup_ratio x total)
+    warmup_ratio = 0.0
     log_every = 1         # the reference prints every step (forces a D2H sync per step)
     total_step = 0
 
@@ -66,14 +75,14 @@ class _StagedGraphStep:
         z = lambda *s: torch.zeros(*s, dtype=torch.int64, device=dev)
         self.d_ids, self.d_tt, self.d_mask, self.d_lab = z(batch_size, seq_len), z(batch_size, seq_len), \
             z(batch_size, seq_len), z(batch_size)
-        self.h_stage = torch.empty(3 * batch_size * seq_len + batch_size, dtype=torch.int64).pin_memory()
-        self.d_stage = torch.empty_like(self.h_stage, device=dev)
+        self._alloc_stage(3 * batch_size * seq_len + batch_size)
         self.loss_out = torch.zeros((), dtype=torch.float32, device=dev)
         self.h_loss = torch.zeros((), dtype=torch.float32).pin_memory()
         self.use_graph = use_graph
         self.graph = None         # the graph of the optimizer-step body (the only one without accumulation)
         self._graphs = {}         # role -> graph, role = (final pass, window already holds gradients), see run_device
         self._warm = {}
+        self._graph_hp = {}       # role -> the optimizer hyperparameters its graph was captured with
         self._role = (True, False)
         self.accum_steps = 1
         self.max_grad_norm = None
@@ -94,6 +103,26 @@ class _StagedGraphStep:
     def _body(self):
         raise NotImplementedError
 
+    def _alloc_stage(self, n):
+        """pinned / device staging of n int64 for the batch (h_stage / d_stage), then one slot carrying
+        param_groups[0]["lr"] as float64 bits: both travel in the one H2D copy of stage()"""
+        self._h_stage_all = torch.zeros(n + 1, dtype=torch.int64).pin_memory()
+        self._d_stage_all = torch.zeros_like(self._h_stage_all, device=self.eng.dev)
+        self.h_stage, self.d_stage = self._h_stage_all[:n], self._d_stage_all[:n]
+
+    def _stage_lr(self):
+        opt = getattr(self, "opt", None)
+        if opt is not None:
+            self._h_stage_all[-1:].view(torch.float64).fill_(opt.current_lr())
+
+    def _h2d(self):
+        self._d_stage_all.copy_(self._h_stage_all, non_blocking=True)
+        self._h2d_done = torch.cuda.Event()
+        self._h2d_done.record(torch.cuda.current_stream(self.eng.dev))
+
+    def _unstage_lr(self):
+        self.opt._state()["lr"].copy_(self._d_stage_all[-1:].view(torch.float64))
+
     def stage(self, batch_data):
         """Host batch (the dict the reference Collate yields, int64 tensors) -> pinned staging -> async H2D."""
         n = self.B * self.S
@@ -109,9 +138,8 @@ class _StagedGraphStep:
         hs[n:2 * n].copy_(tt.reshape(-1))
         hs[2 * n:3 * n].copy_(mask.reshape(-1))
         hs[3 * n:3 * n + self.B].copy_(lab.reshape(-1))
-        self.d_stage.copy_(hs, non_blocking=True)
-        self._h2d_done = torch.cuda.Event()
-        self._h2d_done.record(torch.cuda.current_stream(self.eng.dev))
+        self._stage_lr()
+        self._h2d()
 
     def _run_body(self):
         cur = torch.cuda.current_stream(self.eng.dev)
@@ -148,9 +176,22 @@ class _StagedGraphStep:
             with torch.cuda.graph(g):
                 self._run_body()
             self._graphs[role] = g
+            if getattr(self, "opt", None) is not None:
+                self._graph_hp[role] = self.opt.captured_hparams()
             if role[0]:
                 self.graph = g
+        elif role in self._graph_hp:
+            self._check_hparams(self._graph_hp[role])
         g.replay()
+
+    def _check_hparams(self, captured):
+        """a replay reads the lr live; every other optimizer hyperparameter is the one the graph was captured with"""
+        now = self.opt.captured_hparams()
+        for field, was in captured.items():
+            if now[field] != was:
+                raise RuntimeError("%s: the optimizer's %s changed from %r to %r after the step was captured; the "
+                                   "captured step reads only the lr at each replay, so build a new %s to use it"
+                                   % (type(self).__name__, field, was, now[field], type(self).__name__))
 
     def _arm(self, optimizer, accum_steps, max_grad_norm=None):
         self.opt = optimizer
@@ -158,6 +199,10 @@ class _StagedGraphStep:
         self.max_grad_norm = float(max_grad_norm) if max_grad_norm else None
         if accum_steps > 1:
             self.eng.ensure_accum()       # outside any capture
+        # a valid lr in the device slot before any stage(): run_device() on inputs written straight into d_stage
+        # replays at the lr current when the step was built (or last staged)
+        self._stage_lr()
+        self._d_stage_all[-1:].copy_(self._h_stage_all[-1:])
         # the fused step owns backward + optimizer: per-bucket AdamW (and, under DDP, the peer exchange) may start
         # while backward is still running
         optimizer._armed = True
@@ -165,9 +210,17 @@ class _StagedGraphStep:
     def _train_body(self, forward):
         """forward() -> (logits, loss): the common part of the captured train steps.  A micro-batch body
         (self._role[0] False) accumulates its gradients and bumps the dropout stream instead of stepping; the final
-        body folds the window in before the update."""
+        body folds the window in before the update.  The staged lr goes to the optimizer's device lr first, and every
+        update (and step-size prepare) of the body reads it from there, so a replay applies the lr of its own step."""
+        self._unstage_lr()
+        self.opt._lr_dev_on = True
+        try:
+            self._train_pass(forward, self._role[0])
+        finally:
+            self.opt._lr_dev_on = False
+
+    def _train_pass(self, forward, final):
         eng, opt = self.eng, self.opt
-        final = self._role[0]
         logits, loss = forward()
         B, S, mask, p_h, p_a, p_c, packed = eng._saved
         eng._saved = None
@@ -228,8 +281,7 @@ class PackedTrainStep(_StagedGraphStep):
         self.bins, self.batch = bins, batch
         n = bins * 128
         # pinned staging: ids | token types | positions | segments (as int64) | cls rows | labels
-        self.h_stage = torch.empty(4 * n + 2 * batch, dtype=torch.int64).pin_memory()
-        self.d_stage = torch.empty_like(self.h_stage, device=dev)
+        self._alloc_stage(4 * n + 2 * batch)
         z = lambda *sh: torch.zeros(*sh, dtype=torch.int64, device=dev)
         self.d_pos, self.d_cls, self.d_lab = z(bins, 128), z(batch), z(batch)
         self.d_seg = torch.zeros(bins, 128, dtype=torch.int32, device=dev)
@@ -256,9 +308,8 @@ class PackedTrainStep(_StagedGraphStep):
         hs[3 * n:4 * n].copy_(packed["segments"].reshape(-1))
         hs[4 * n:4 * n + self.batch].copy_(packed["cls_index"])
         hs[4 * n + self.batch:4 * n + 2 * self.batch].copy_(label.reshape(-1))
-        self.d_stage.copy_(hs, non_blocking=True)
-        self._h2d_done = torch.cuda.Event()
-        self._h2d_done.record(torch.cuda.current_stream(self.eng.dev))
+        self._stage_lr()
+        self._h2d()
 
     def _body(self):
         self._unstage()
@@ -295,7 +346,11 @@ class FusedEvalStep(_StagedGraphStep):
 
 
 class Trainer:
-    def __init__(self, args, config, model, criterion, optimizer):
+    def __init__(self, args, config, model, criterion, optimizer, scheduler=None):
+        """scheduler: a torch LR scheduler of `optimizer` (fabric-cls.py's Trainer argument), stepped once per optimizer
+        step; it takes precedence over args.lr_scheduler_type"""
+        if scheduler is not None and getattr(scheduler, "optimizer", None) is not optimizer:
+            raise ValueError("the scheduler must belong to the Trainer's optimizer")
         self.args = args
         self.config = config          # (the reference's `self.config = config,` stores a 1-tuple by accident, :121)
         self.model = model
@@ -309,6 +364,25 @@ class Trainer:
         self._micro = 0       # batches of the open gradient-accumulation window
         self.last_grad_norm = None   # device scalar: the pre-clip gradient norm of the last optimizer step (HF's
                                      # logged `grad_norm`); None when not clipping
+        self.lr_scheduler = scheduler
+
+    def num_training_steps(self, train_loader):
+        """optimizer steps train() takes: epochs x ceil(batches / k).  HF Trainer floors batches / k; this Trainer
+        also steps the partial window at the end of an epoch (close_window), so a linear schedule reaches 0 exactly
+        after the last step."""
+        k = max(1, int(getattr(self.args, "gradient_accumulation_steps", 1)))
+        return int(self.args.epochs) * math.ceil(len(train_loader) / k)
+
+    def create_scheduler(self, num_training_steps):
+        """HF Trainer.create_scheduler: builds self.lr_scheduler from args.lr_scheduler_type / warmup_steps /
+        warmup_ratio, unless a scheduler was passed or built already.  Returns it (None: a constant lr)."""
+        name = getattr(self.args, "lr_scheduler_type", None)
+        if self.lr_scheduler is None and name is not None:
+            warm = warmup_steps(num_training_steps, getattr(self.args, "warmup_steps", 0),
+                                getattr(self.args, "warmup_ratio", 0.0))
+            self.lr_scheduler = get_scheduler(name, self.optimizer, num_warmup_steps=warm,
+                                              num_training_steps=num_training_steps)
+        return self.lr_scheduler
 
     def _to_device(self, batch_data):
         dev = _unwrap(self.model)._engine.dev
@@ -367,6 +441,9 @@ class Trainer:
         (inside no_sync() on the eager paths), the k-th also steps the optimizer; every loss is scaled by 1/k
         (fabric-cls.py:150-157) and the returned loss is the unscaled micro-batch loss."""
         k = max(1, int(getattr(self.args, "gradient_accumulation_steps", 1)))
+        if self.lr_scheduler is None and getattr(self.args, "lr_scheduler_type", None) is not None:
+            raise RuntimeError("args.lr_scheduler_type is set but no scheduler was built: call "
+                               "trainer.create_scheduler(num_training_steps) first (train() does)")
         clip = self._max_grad_norm()
         first, final = self._micro == 0, self._micro >= k - 1
         self._micro = 0 if final else self._micro + 1
@@ -382,6 +459,8 @@ class Trainer:
                                                     max_grad_norm=clip)
             self.model.train()
             loss = self._packed[key](packed, batch_data["label"], final)
+            if final:
+                self._scheduler_step()      # after the replay: the next stage() reads the new lr
         elif getattr(self.args, "fused", True):
             B, S = batch_data["input_ids"].shape
             if self._fused is None or (self._fused.B, self._fused.S, self._fused.accum_steps,
@@ -389,6 +468,8 @@ class Trainer:
                 self._fused = FusedTrainStep(self.model, self.optimizer, B, S, accum_steps=k, max_grad_norm=clip)
             self.model.train()
             loss = self._fused(batch_data, final)
+            if final:
+                self._scheduler_step()
         elif getattr(self.args, "use_amp", False):
             # the -amp scripts' loop body (multi-gpu-distributed-mp-amp-cls.py:166-171), scaler created once
             if self._scaler is None:
@@ -401,8 +482,7 @@ class Trainer:
                 self._scaler.scale(loss / k if k > 1 else loss).backward()
             if final:
                 self._clip(clip)        # no scaler.unscale_: step() takes the scale out of the norm
-                self._scaler.step(self.optimizer)
-                self._scaler.update()
+                self._scaler_step()
         else:
             self.model.train()
             with self._window(final):
@@ -414,9 +494,27 @@ class Trainer:
             if final:
                 self._clip(clip)
                 self.optimizer.step()
+                self._scheduler_step()
         if final:
             self._note_grad_norm(clip)
         return self.loss_reduce(loss.detach())
+
+    def _scheduler_step(self):
+        if self.lr_scheduler is not None:
+            self.lr_scheduler.step()
+
+    def _scaler_step(self):
+        """GradScaler step + update; the scheduler steps only if the optimizer ran (HF Trainer 4.28: the scale did
+        not drop).  Reading the scale is one host sync per step, on this eager path only."""
+        if self.lr_scheduler is None:
+            self._scaler.step(self.optimizer)
+            self._scaler.update()
+            return
+        scale_before = self._scaler.get_scale()
+        self._scaler.step(self.optimizer)
+        self._scaler.update()
+        if scale_before <= self._scaler.get_scale():
+            self.lr_scheduler.step()
 
     def _max_grad_norm(self):
         m = getattr(self.args, "max_grad_norm", None)
@@ -443,10 +541,10 @@ class Trainer:
         clip = self._max_grad_norm()
         self._clip(clip)
         if self._scaler is not None and not getattr(self.args, "fused", True):
-            self._scaler.step(self.optimizer)
-            self._scaler.update()
+            self._scaler_step()
         else:
             self.optimizer.step()
+            self._scheduler_step()
         self._note_grad_norm(clip)
 
     def train(self, train_loader, dev_loader=None, train_sampler=None):
@@ -454,6 +552,8 @@ class Trainer:
         best_acc = 0.
         if self.args.local_rank == 0:
             start = time.time()
+        if self.lr_scheduler is None and getattr(self.args, "lr_scheduler_type", None) is not None:
+            self.create_scheduler(self.num_training_steps(train_loader))
         for epoch in range(1, self.args.epochs + 1):
             if train_sampler is not None:
                 train_sampler.set_epoch(epoch)
