@@ -28,7 +28,7 @@ extern "C" {
 /* ------------------------------------------------------------------------------------------------------ */
 const char* b2_last_error(void);
 int32_t b2_abi_version(void);             /* bumped when a struct below changes */
-#define B2_ABI_VERSION 21
+#define B2_ABI_VERSION 22
 int64_t b2_launch_count(void);            /* kernels launched by this library so far (process-wide) */
 
 /* ------------------------------------------------------------------------------------------------------ */
@@ -201,6 +201,22 @@ int32_t b2_head_fwd(const void* hidden_states /* bf16 [batch*seq, hidden] */, in
 /* mean cross-entropy and d(loss)/d(logits); labels int64 [batch]; loss_scale multiplies dlogits (DDP: 1)    */
 int32_t b2_ce_fwd_bwd(const float* logits, const int64_t* labels, int64_t batch, int64_t num_labels,
                       float* loss /* scalar */, float* dlogits /* [batch, num_labels] or NULL */, void* stream);
+/* the losses of HF's three problem types and the options of torch's CrossEntropyLoss, all with reduction "mean":   */
+/*   B2_LOSS_CE   CrossEntropyLoss(weight, ignore_index, label_smoothing)   labels int64 [batch]                    */
+/*   B2_LOSS_MSE  MSELoss()                                                  labels fp32 [batch, num_labels]         */
+/*   B2_LOSS_BCE  BCEWithLogitsLoss(pos_weight)                              labels fp32 [batch, num_labels]         */
+/* CE with the defaults (no weight, ignore_index -100, no smoothing) computes exactly what b2_ce_fwd_bwd does.      */
+/* A degenerate CE batch (every row ignored, or zero total weight) gives loss nan and dlogits 0.                    */
+enum { B2_LOSS_CE = 0, B2_LOSS_MSE = 1, B2_LOSS_BCE = 2 };
+typedef struct b2_loss_params {
+  const float* weight;       /* CE: device fp32 [num_labels] class weights, or NULL                              */
+  const float* pos_weight;   /* BCE: device fp32 [num_labels], or NULL                                           */
+  int64_t ignore_index;      /* CE: rows with this label count for nothing (torch's default -100)                */
+  float label_smoothing;     /* CE: in [0, 1]                                                                    */
+} b2_loss_params_t;
+int32_t b2_loss_fwd_bwd(const float* logits, const void* labels, int64_t batch, int64_t num_labels, int32_t mode,
+                        const b2_loss_params_t* params /* NULL: the defaults */, float* loss /* scalar */,
+                        float* dlogits /* [batch, num_labels] or NULL */, void* stream);
 /* backward of b2_head_fwd: from dlogits to d(hidden_states[:,0]) and the four head parameter grads (bf16)  */
 int32_t b2_head_bwd(const float* dlogits, const void* hidden_states, const void* pooled, int64_t batch,
                     int64_t seq, int64_t hidden, const void* pool_w, const void* cls_w, int64_t num_labels,

@@ -10,6 +10,7 @@ from .ddp import DistributedDataParallel
 from .synthetic import REFERENCE_LENGTH_HISTOGRAM, reference_length_batch, synthetic_batch
 from .packing import pack_batch
 from .schedules import get_scheduler
+from .losses import PROBLEM_TYPES, Loss, infer_problem_type, loss_from_criterion
 from .trainer import Args, FusedEvalStep, FusedTrainStep, PackedTrainStep, Trainer
 
 
@@ -26,5 +27,5 @@ def set_seed(seed=123):
 
 
 __all__ = ["BertConfig", "BertForSequenceClassification", "SequenceClassifierOutput", "AdamW", "build_optimizer", "clip_grad_norm_",
-           "DistributedDataParallel", "Args", "Trainer", "FusedTrainStep", "FusedEvalStep", "PackedTrainStep", "pack_batch", "get_scheduler", "synthetic_batch", "reference_length_batch", "REFERENCE_LENGTH_HISTOGRAM", "set_seed", "bert_base_config",
+           "DistributedDataParallel", "Args", "Trainer", "FusedTrainStep", "FusedEvalStep", "PackedTrainStep", "pack_batch", "get_scheduler", "Loss", "PROBLEM_TYPES", "infer_problem_type", "loss_from_criterion", "synthetic_batch", "reference_length_batch", "REFERENCE_LENGTH_HISTOGRAM", "set_seed", "bert_base_config",
            "bert_large_config", "chinese_bert_wwm_ext_config"]

@@ -8,13 +8,14 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2ddpbert.so")
-ABI_VERSION = 21
+ABI_VERSION = 22
 
 MAJOR_K, MAJOR_MN = 0, 1
 EPI_NONE, EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_DROPOUT_RESIDUAL, EPI_RESIDUAL, EPI_GELU_BWD = 0, 1, 2, 3, 4, 5
 EPI_RESIDUAL_F32 = 6
 EPI_ACCUM_F32 = 7
 ACCUM_STORE, ACCUM_ADD, ACCUM_FOLD, ACCUM_FLUSH = 0, 1, 2, 3     # b2_grad_accumulate modes
+LOSS_CE, LOSS_MSE, LOSS_BCE = 0, 1, 2                            # b2_loss_fwd_bwd modes
 
 
 def sumsq_slots(n):
@@ -46,6 +47,10 @@ class AdamWHParams(C.Structure):
                 ("clip_coef", vp), ("grad_f32", vp), ("lr_dev", vp)]
 
 
+class LossParams(C.Structure):
+    _fields_ = [("weight", vp), ("pos_weight", vp), ("ignore_index", i64), ("label_smoothing", f32)]
+
+
 # name -> argtypes; every function returns int32 status unless listed in _SPECIAL
 _SIGNATURES = {
     "b2_gemm_bf16": [C.POINTER(GemmArgs), vp],
@@ -66,6 +71,7 @@ _SIGNATURES = {
     "b2_accum_finish": [vp, vp, vp, i64, i64, vp],
     "b2_head_fwd": [vp, i64, i64, i64, vp, vp, vp, vp, i64, f32, vp, u32, vp, vp, vp],
     "b2_ce_fwd_bwd": [vp, vp, i64, i64, vp, vp, vp],
+    "b2_loss_fwd_bwd": [vp, vp, i64, i64, i32, C.POINTER(LossParams), vp, vp, vp],
     "b2_head_bwd": [vp, vp, vp, i64, i64, i64, vp, vp, i64, f32, vp, u32, vp, vp, vp, vp, vp, i32, vp, vp],
     # packed-bin variants (include/b2_ddp_bert.h, "packed bins")
     "b2_embed_fwd_packed": [vp, vp, vp, i64, i64, i64, vp, vp, vp, vp, vp, i64, i64, i64, f32, f32, vp, u32, vp, vp, vp,

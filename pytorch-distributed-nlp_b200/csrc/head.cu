@@ -85,63 +85,150 @@ __global__ void __launch_bounds__(256) classifier_fwd_kernel(const __nv_bfloat16
   if (lane == 0) logits[o] = s + __bfloat162float(bc[c]);
 }
 
-// mean CE over the batch + dlogits = (softmax - onehot) / batch.  One block, one thread per sample (strided).
-__global__ void __launch_bounds__(256) ce_fwd_bwd_kernel(const float* __restrict__ logits,
-                                                        const long long* __restrict__ labels, int batch, int C,
-                                                        float* __restrict__ loss, float* __restrict__ dlogits) {
+// The loss loss_fwd_bwd_kernel computes, fixed at compile time.  CE_PLAIN is CrossEntropyLoss() with torch's defaults
+// compiled in (ignore_index -100, no class weights, no smoothing): the reference's criterion
+// (multi-gpu-distributed-cls.py:343), run by b2_ce_fwd_bwd and the default training step.
+enum LossKind { CE_PLAIN, CE, MSE, BCE };
+
+// Mean loss + dlogits = d(loss)/d(logits), fp32 [batch, C].  One block, rows strided over the threads, reductions in a
+// fixed order through shared memory (no atomics): a graph replay gives the same bits.  torch 2.11's formulas:
+//   CE   CrossEntropyLoss(weight=w, ignore_index, label_smoothing=eps), reduction "mean": each row whose label y is not
+//        ignore_index adds (1 - eps) w[y] (lse - z[y]) + eps / C * sum_c w[c] (lse - z[c]), and the sum is divided by
+//        W = sum of those rows' w[y] (w = 1 without weights: W = their count).  Any other label outside [0, C) is an
+//        error (torch raises a device-side assert: here a message + trap).  W == 0 (every row ignored, or zero weights):
+//        the loss is nan (0 / 0, as torch) and dlogits are 0.
+//   MSE  MSELoss(): mean over batch x C of (z - t)^2.
+//   BCE  BCEWithLogitsLoss(pos_weight=pw): mean over batch x C of (1 - t) z - lw logsigmoid(z), lw = 1 + (pw[c] - 1) t;
+//        gradient lw sigmoid(z) - pw[c] t, as torch's backward.
+// labels: int64 [batch] (CE); targets: fp32 [batch, C] (MSE, BCE).
+template <int KIND>
+__global__ void __launch_bounds__(256) loss_fwd_bwd_kernel(const float* __restrict__ logits,
+                                                          const long long* __restrict__ labels, int batch, int C,
+                                                          float* __restrict__ loss, float* __restrict__ dlogits,
+                                                          const float* __restrict__ targets, b2_loss_params_t prm) {
   pdl_wait();               // PDL: predecessors complete + visible before any global access
   pdl_launch_dependents();  // let the next kernel in the stream begin launching
-  // torch.nn.CrossEntropyLoss semantics (multi-gpu-distributed-cls.py:343, defaults): labels equal to ignore_index
-  // (-100) contribute nothing and the mean runs over the other samples; any other label outside [0, C) is an error
-  // (torch raises a device-side assert: here a message + trap)
   __shared__ float red[256];
   __shared__ int cnt[256];
-  int valid = 0;
-  for (int b = threadIdx.x; b < batch; b += blockDim.x) {
-    const long long y = labels[b];
-    if (y == -100) continue;
-    if (y < 0 || y >= C) {
-      printf("b2 ce_fwd_bwd: label %lld of sample %d is outside [0, %d) (and is not ignore_index -100)\n", y, b, C);
-      __trap();
+  if constexpr (KIND == MSE || KIND == BCE) {
+    const float* __restrict__ pw = KIND == BCE ? prm.pos_weight : nullptr;
+    const float n = (float)batch * (float)C;
+    const float inv = 1.0f / n;
+    float local = 0.f;
+    for (int b = threadIdx.x; b < batch; b += blockDim.x) {
+      for (int c = 0; c < C; ++c) {
+        const size_t i = (size_t)b * C + c;
+        const float z = logits[i], t = targets[i];
+        float l, d;
+        if constexpr (KIND == MSE) {
+          const float e = z - t;
+          l = e * e;
+          d = 2.f * e;
+        } else {
+          const float p = pw != nullptr ? pw[c] : 1.f;
+          const float lw = pw != nullptr ? (p - 1.f) * t + 1.f : 1.f;
+          const float log_sig = fminf(z, 0.f) - log1pf(expf(-fabsf(z)));
+          l = (1.f - t) * z - lw * log_sig;
+          d = lw / (1.f + expf(-z)) - p * t;
+        }
+        local += l;
+        if (dlogits != nullptr) dlogits[i] = d * inv;
+      }
     }
-    ++valid;
-  }
-  cnt[threadIdx.x] = valid;
-  __syncthreads();
-  for (int s = blockDim.x / 2; s > 0; s >>= 1) {
-    if ((int)threadIdx.x < s) cnt[threadIdx.x] += cnt[threadIdx.x + s];
+    red[threadIdx.x] = local;
     __syncthreads();
-  }
-  const int n_valid = cnt[0];
-  const float inv = n_valid > 0 ? 1.0f / (float)n_valid : 0.f;
-  float local = 0.f;
-  for (int b = threadIdx.x; b < batch; b += blockDim.x) {
-    const float* z = logits + (size_t)b * C;
-    const long long y = labels[b];
-    if (y == -100) {
-      if (dlogits != nullptr)
-        for (int c = 0; c < C; ++c) dlogits[(size_t)b * C + c] = 0.f;
-      continue;
+    for (int s = blockDim.x / 2; s > 0; s >>= 1) {
+      if ((int)threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+      __syncthreads();
     }
-    float mx = -INFINITY;
-    for (int c = 0; c < C; ++c) mx = fmaxf(mx, z[c]);
-    float se = 0.f;
-    for (int c = 0; c < C; ++c) se += expf(z[c] - mx);
-    const float lse = mx + logf(se);
-    local += lse - z[y];
-    if (dlogits != nullptr) {
-      for (int c = 0; c < C; ++c)
-        dlogits[(size_t)b * C + c] = (expf(z[c] - lse) - (c == (int)y ? 1.f : 0.f)) * inv;
+    if (threadIdx.x == 0) *loss = red[0] / n;
+  } else {
+    // CE_PLAIN folds the options to constants: the weight and smoothing terms below compile away
+    constexpr bool plain = KIND == CE_PLAIN;
+    const long long ignore = plain ? -100ll : prm.ignore_index;
+    const float* __restrict__ w = plain ? nullptr : prm.weight;
+    const float eps = plain ? 0.f : prm.label_smoothing;
+    int valid = 0;
+    float wsum = 0.f;
+    for (int b = threadIdx.x; b < batch; b += blockDim.x) {
+      const long long y = labels[b];
+      if (y == ignore) continue;
+      if (y < 0 || y >= C) {
+        printf("b2 cross-entropy: label %lld of sample %d is outside [0, %d) and is not the ignore_index\n", y, b, C);
+        __trap();
+      }
+      ++valid;
+      if (w != nullptr) wsum += w[y];
     }
-  }
-  red[threadIdx.x] = local;
-  __syncthreads();
-  for (int s = blockDim.x / 2; s > 0; s >>= 1) {
-    if ((int)threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+    cnt[threadIdx.x] = valid;
     __syncthreads();
+    for (int s = blockDim.x / 2; s > 0; s >>= 1) {
+      if ((int)threadIdx.x < s) cnt[threadIdx.x] += cnt[threadIdx.x + s];
+      __syncthreads();
+    }
+    const int n_valid = cnt[0];
+    bool ok = n_valid > 0;
+    float inv = ok ? 1.0f / (float)n_valid : 0.f;
+    if (w != nullptr) {   // the weighted mean divides by the sum of the counted rows' weights
+      red[threadIdx.x] = wsum;
+      __syncthreads();
+      for (int s = blockDim.x / 2; s > 0; s >>= 1) {
+        if ((int)threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+        __syncthreads();
+      }
+      const float W = red[0];
+      __syncthreads();    // every thread has read red[0] before the loss reduction reuses it
+      ok = W != 0.f;
+      inv = ok ? 1.0f / W : 0.f;
+    }
+    float local = 0.f;
+    for (int b = threadIdx.x; b < batch; b += blockDim.x) {
+      const float* z = logits + (size_t)b * C;
+      const long long y = labels[b];
+      if (y == ignore) {
+        if (dlogits != nullptr)
+          for (int c = 0; c < C; ++c) dlogits[(size_t)b * C + c] = 0.f;
+        continue;
+      }
+      float mx = -INFINITY;
+      for (int c = 0; c < C; ++c) mx = fmaxf(mx, z[c]);
+      float se = 0.f;
+      for (int c = 0; c < C; ++c) se += expf(z[c] - mx);
+      const float lse = mx + logf(se);
+      const float wy = w != nullptr ? w[y] : 1.f;
+      float l = lse - z[y];
+      if (w != nullptr) l *= wy;
+      float sw = (float)C;    // sum of the class weights (C without weights)
+      if (eps != 0.f) {
+        float sm = 0.f;
+        if (w != nullptr) sw = 0.f;
+        for (int c = 0; c < C; ++c) {
+          const float wc = w != nullptr ? w[c] : 1.f;
+          sm += wc * (lse - z[c]);
+          if (w != nullptr) sw += wc;
+        }
+        l = (1.f - eps) * l + eps / (float)C * sm;
+      }
+      local += l;
+      if (dlogits != nullptr) {
+        for (int c = 0; c < C; ++c) {
+          const float p = expf(z[c] - lse);
+          float d = p - (c == (int)y ? 1.f : 0.f);
+          if (w != nullptr) d *= wy;
+          if (eps != 0.f) d = (1.f - eps) * d + eps / (float)C * (sw * p - (w != nullptr ? w[c] : 1.f));
+          dlogits[(size_t)b * C + c] = d * inv;
+        }
+      }
+    }
+    red[threadIdx.x] = local;
+    __syncthreads();
+    for (int s = blockDim.x / 2; s > 0; s >>= 1) {
+      if ((int)threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+      __syncthreads();
+    }
+    // nothing counted: torch returns nan (0 / 0)
+    if (threadIdx.x == 0) *loss = ok ? red[0] * inv : __int_as_float(0x7fc00000);
   }
-  // all samples ignored: torch returns nan (0 / 0)
-  if (threadIdx.x == 0) *loss = n_valid > 0 ? red[0] * inv : __int_as_float(0x7fc00000);
 }
 
 // ---- backward ----
@@ -295,8 +382,47 @@ extern "C" int32_t b2_ce_fwd_bwd(const float* logits, const int64_t* labels, int
                                  float* loss, float* dlogits, void* stream_) {
   B2_REQUIRE(logits && labels && loss, "ce_fwd_bwd: null pointer");
   B2_REQUIRE(batch > 0 && num_labels > 0, "ce_fwd_bwd: empty batch");
-  B2_LAUNCH(ce_fwd_bwd_kernel, 1, 256, 0, (cudaStream_t)stream_, logits, (const long long*)labels, (int)batch,
-                                                          (int)num_labels, loss, dlogits);
+  const b2_loss_params_t none = {nullptr, nullptr, -100, 0.f};
+  B2_LAUNCH(loss_fwd_bwd_kernel<CE_PLAIN>, 1, 256, 0, (cudaStream_t)stream_, logits, (const long long*)labels,
+            (int)batch, (int)num_labels, loss, dlogits, (const float*)nullptr, none);
+  B2_CUDA(cudaGetLastError());
+  count_launches(1);
+  return 0;
+}
+
+extern "C" int32_t b2_loss_fwd_bwd(const float* logits, const void* labels, int64_t batch, int64_t num_labels,
+                                   int32_t mode, const b2_loss_params_t* params, float* loss, float* dlogits,
+                                   void* stream_) {
+  B2_REQUIRE(logits && labels && loss, "loss_fwd_bwd: null pointer");
+  B2_REQUIRE(batch > 0 && num_labels > 0, "loss_fwd_bwd: empty batch");
+  B2_REQUIRE(batch * num_labels <= (1ll << 30), "loss_fwd_bwd: batch x num_labels = %lld is too large",
+             (long long)(batch * num_labels));
+  const b2_loss_params_t p = params != nullptr ? *params : b2_loss_params_t{nullptr, nullptr, -100, 0.f};
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const long long* y = (const long long*)labels;
+  const float* t = (const float*)labels;
+  const int B = (int)batch, C = (int)num_labels;
+  if (mode == B2_LOSS_CE) {
+    B2_REQUIRE(p.pos_weight == nullptr, "loss_fwd_bwd: pos_weight applies to BCE only");
+    B2_REQUIRE(p.label_smoothing >= 0.f && p.label_smoothing <= 1.f,
+               "loss_fwd_bwd: label_smoothing=%g must be in [0, 1]", (double)p.label_smoothing);
+    // CrossEntropyLoss() runs the kernel b2_ce_fwd_bwd runs, so its bits do not depend on the entry point
+    if (p.weight == nullptr && p.ignore_index == -100 && p.label_smoothing == 0.f)
+      B2_LAUNCH(loss_fwd_bwd_kernel<CE_PLAIN>, 1, 256, 0, stream, logits, y, B, C, loss, dlogits, (const float*)nullptr,
+                p);
+    else
+      B2_LAUNCH(loss_fwd_bwd_kernel<CE>, 1, 256, 0, stream, logits, y, B, C, loss, dlogits, (const float*)nullptr, p);
+  } else if (mode == B2_LOSS_MSE) {
+    B2_REQUIRE(p.weight == nullptr && p.pos_weight == nullptr, "loss_fwd_bwd: MSE takes no weights");
+    B2_LAUNCH(loss_fwd_bwd_kernel<MSE>, 1, 256, 0, stream, logits, (const long long*)nullptr, B, C, loss, dlogits, t,
+              p);
+  } else if (mode == B2_LOSS_BCE) {
+    B2_REQUIRE(p.weight == nullptr, "loss_fwd_bwd: BCE takes pos_weight, not weight");
+    B2_LAUNCH(loss_fwd_bwd_kernel<BCE>, 1, 256, 0, stream, logits, (const long long*)nullptr, B, C, loss, dlogits, t,
+              p);
+  } else {
+    B2_REQUIRE(false, "loss_fwd_bwd: unknown mode %d", (int)mode);
+  }
   B2_CUDA(cudaGetLastError());
   count_launches(1);
   return 0;

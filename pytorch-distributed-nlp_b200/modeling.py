@@ -19,6 +19,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib as L
+from .losses import PROBLEM_TYPES, infer_problem_type, problem_type_loss
 
 
 class BertConfig:
@@ -28,7 +29,7 @@ class BertConfig:
                  intermediate_size=3072, hidden_act="gelu", hidden_dropout_prob=0.1,
                  attention_probs_dropout_prob=0.1, max_position_embeddings=512, type_vocab_size=2,
                  initializer_range=0.02, layer_norm_eps=1e-12, pad_token_id=0, num_labels=2,
-                 classifier_dropout=None, **kwargs):
+                 classifier_dropout=None, problem_type=None, **kwargs):
         self.vocab_size = vocab_size
         self.hidden_size = hidden_size
         self.num_hidden_layers = num_hidden_layers
@@ -44,6 +45,9 @@ class BertConfig:
         self.pad_token_id = pad_token_id
         self.num_labels = num_labels
         self.classifier_dropout = classifier_dropout
+        if problem_type is not None and problem_type not in PROBLEM_TYPES:
+            raise ValueError("problem_type=%r: expected None or one of %s" % (problem_type, PROBLEM_TYPES))
+        self.problem_type = problem_type    # HF's: None is inferred from the first labels (losses.py)
         for k, v in kwargs.items():
             setattr(self, k, v)
 
@@ -258,6 +262,7 @@ class BertForSequenceClassification(nn.Module):
         self._ddp = None
         self._grads_live = False     # an eager backward has produced gradients no optimizer.step() has consumed yet
         self._no_sync = False        # inside no_sync(): backwards accumulate
+        self._pt_loss = None         # (problem_type, losses.Loss) of the in-model loss
 
     @contextlib.contextmanager
     def no_sync(self):
@@ -433,6 +438,18 @@ class BertForSequenceClassification(nn.Module):
         logits, loss = self._engine.forward(input_ids, token_type_ids, attention_mask, labels,
                                             training=self.training, need_backward=False, packed=packed)
         return SequenceClassifierOutput(loss=None if loss is None else loss.clone(), logits=logits.clone())
+
+    def _problem_type_loss(self, labels):
+        """The loss of `labels = ...` (HF BertForSequenceClassification.forward): config.problem_type's, inferred from
+        these labels and stored on the config when it is None"""
+        cfg = self.config
+        pt = getattr(cfg, "problem_type", None)
+        if pt is None:
+            pt = infer_problem_type(self.num_labels, labels)
+            cfg.problem_type = pt
+        if self._pt_loss is None or self._pt_loss[0] != pt:
+            self._pt_loss = (pt, problem_type_loss(pt, self.num_labels))
+        return self._pt_loss[1]
 
     def _notify_backward_done(self):
         if self._ddp is not None:
@@ -682,9 +699,11 @@ class _Engine:
         L.call("b2_layernorm_fwd", z, gamma, beta, M, H, eps, y, mean, rstd, s)
 
     # ---- forward --------------------------------------------------------------------------------------------------------
-    def forward(self, input_ids, token_type_ids, attention_mask, labels, training, need_backward, packed=None):
+    def forward(self, input_ids, token_type_ids, attention_mask, labels, training, need_backward, packed=None,
+                loss_fn=None):
         """packed: None, or (position_ids int64 [bins, 128], segments int32 [bins, 128], cls_index int64 [batch]) --
-        the rows of `input_ids` are then 128-token bins produced by packing.pack_batch, not sequences."""
+        the rows of `input_ids` are then 128-token bins produced by packing.pack_batch, not sequences.
+        loss_fn: the losses.Loss of `labels` (None: the model's problem-type loss, HF's in-model loss)."""
         cfg, H, I = self.cfg, self.H, self.I
         if input_ids.dim() != 2:
             raise ValueError("input_ids must be [batch, seq]")
@@ -713,8 +732,12 @@ class _Engine:
             if t is not None:
                 if t.device != self.dev:
                     raise RuntimeError("%s is on %s, model on %s" % (nm, t.device, self.dev))
-                if t.dtype != torch.int64:
+                if t is not labels and t.dtype != torch.int64:
                     raise TypeError("%s must be int64 (as the reference Collate produces)" % nm)
+        if labels is not None:
+            if loss_fn is None:
+                loss_fn = self.model._problem_type_loss(labels)
+            labels = loss_fn.device_labels(labels, Bo)
         ws = self.workspace(B, S, Bo)
         M = B * S
         s = self.stream()
@@ -777,11 +800,8 @@ class _Engine:
                    1 + 3 * self.nl, ws["pooled"].data_ptr(), ws["logits"].data_ptr(), s)
         loss = None
         if labels is not None:
-            lab = labels.contiguous().view(-1)
-            if lab.numel() != Bo:
-                raise ValueError("labels must be [batch]")
-            L.call("b2_ce_fwd_bwd", ws["logits"].data_ptr(), lab.data_ptr(), Bo, self.C, ws["loss"].data_ptr(),
-                   ws["dloss_logits"].data_ptr() if need_backward else None, s)
+            loss_fn.launch(ws["logits"].data_ptr(), labels, Bo, ws["loss"].data_ptr(),
+                           ws["dloss_logits"].data_ptr() if need_backward else None, s)
             loss = ws["loss"]
         if need_backward:
             self._saved = (B, S, mask, p_h, p_a, p_c, None if packed is None else (segs, cls_rows))

@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 from .ddp import DistributedDataParallel
+from .losses import criterion_key, infer_problem_type, loss_from_criterion, problem_type_loss
 from .optim import clip_grad_norm_
 from .schedules import get_scheduler, warmup_steps
 
@@ -60,11 +61,24 @@ def _unwrap(model):
     return model.module if isinstance(model, DistributedDataParallel) else model
 
 
+def step_loss(model, criterion=None):
+    """The losses.Loss a captured step computes: `criterion`'s when it is one the device kernel reproduces (else
+    ValueError), and with no criterion the model's problem-type loss -- single-label cross-entropy when the config has
+    no problem_type and more than one label (the step then stages int64 labels, as the reference's Collate yields)."""
+    m = _unwrap(model)
+    if criterion is not None:
+        return loss_from_criterion(criterion, m.num_labels, m._engine.dev if m._engine is not None else None)
+    pt = getattr(m.config, "problem_type", None)
+    if pt is None:
+        pt = "regression" if m.num_labels == 1 else "single_label_classification"
+    return problem_type_loss(pt, m.num_labels)
+
+
 class _StagedGraphStep:
     """Shared plumbing of the graph-captured steps: one pinned staging buffer for the four host tensors of a batch, one
     async H2D copy, two eager warm-up passes (first launches set kernel attributes), then capture + replay."""
 
-    def __init__(self, model, batch_size, seq_len, use_graph=True):
+    def __init__(self, model, batch_size, seq_len, use_graph=True, criterion=None):
         self.wrapper = model if isinstance(model, DistributedDataParallel) else None
         self.model = _unwrap(model)
         self.eng = self.model._engine
@@ -72,10 +86,12 @@ class _StagedGraphStep:
             raise RuntimeError("%s: model must be on CUDA" % type(self).__name__)
         dev = self.eng.dev
         self.B, self.S = batch_size, seq_len
+        self.loss_fn = step_loss(self.model, criterion)
+        self.criterion_key = criterion_key(criterion)
         z = lambda *s: torch.zeros(*s, dtype=torch.int64, device=dev)
-        self.d_ids, self.d_tt, self.d_mask, self.d_lab = z(batch_size, seq_len), z(batch_size, seq_len), \
-            z(batch_size, seq_len), z(batch_size)
-        self._alloc_stage(3 * batch_size * seq_len + batch_size)
+        self.d_ids, self.d_tt, self.d_mask = z(batch_size, seq_len), z(batch_size, seq_len), z(batch_size, seq_len)
+        self.d_lab, lab_slots = self._label_buffer(batch_size)
+        self._alloc_stage(3 * batch_size * seq_len + lab_slots)
         self.loss_out = torch.zeros((), dtype=torch.float32, device=dev)
         self.h_loss = torch.zeros((), dtype=torch.float32).pin_memory()
         self.use_graph = use_graph
@@ -92,13 +108,45 @@ class _StagedGraphStep:
         # weight-gradient / optimizer streams (default, i.e. lowest, priority).
         self._prio_stream = torch.cuda.Stream(device=dev, priority=-1)
 
+    def _label_buffer(self, rows):
+        """device labels of `rows` sequences for self.loss_fn, and the int64 staging slots they take: int64 [rows]
+        class indices, or fp32 [rows] / [rows, C] packed two to a slot"""
+        dev = self.eng.dev
+        shape = self.loss_fn.label_shape(rows)
+        if not self.loss_fn.float_labels:
+            return torch.zeros(shape, dtype=torch.int64, device=dev), rows
+        t = torch.zeros(shape, dtype=torch.float32, device=dev)
+        return t, (t.numel() + 1) // 2
+
+    def _stage_labels(self, hs, lab):
+        """host labels -> the label slots `hs` of the pinned staging buffer (fp32 labels bit for bit)"""
+        fn = self.loss_fn
+        if not fn.float_labels:
+            if lab.is_floating_point():
+                raise TypeError("%s was built for int64 class labels, got %s: pass a criterion (or config.problem_type)"
+                                " for float labels" % (type(self).__name__, lab.dtype))
+            hs.copy_(lab.reshape(-1))
+            return
+        try:
+            fn.check_labels(lab, self.d_lab.shape[0])
+        except (TypeError, ValueError) as e:
+            raise type(e)("%s was built for %s labels of shape %s: %s"
+                          % (type(self).__name__, "fp32", list(self.d_lab.shape), e)) from None
+        hs.view(torch.float32)[:self.d_lab.numel()].copy_(lab.reshape(-1))
+
+    def _unstage_labels(self, st):
+        if self.loss_fn.float_labels:
+            self.d_lab.view(-1).copy_(st.view(torch.float32)[:self.d_lab.numel()])
+        else:
+            self.d_lab.copy_(st)
+
     def _unstage(self):
         n = self.B * self.S
         st = self.d_stage
         self.d_ids.copy_(st[0:n].view(self.B, self.S))
         self.d_tt.copy_(st[n:2 * n].view(self.B, self.S))
         self.d_mask.copy_(st[2 * n:3 * n].view(self.B, self.S))
-        self.d_lab.copy_(st[3 * n:3 * n + self.B])
+        self._unstage_labels(st[3 * n:])
 
     def _body(self):
         raise NotImplementedError
@@ -137,7 +185,7 @@ class _StagedGraphStep:
         hs[0:n].copy_(ids.reshape(-1))
         hs[n:2 * n].copy_(tt.reshape(-1))
         hs[2 * n:3 * n].copy_(mask.reshape(-1))
-        hs[3 * n:3 * n + self.B].copy_(lab.reshape(-1))
+        self._stage_labels(hs[3 * n:], lab)
         self._stage_lr()
         self._h2d()
 
@@ -228,7 +276,7 @@ class _StagedGraphStep:
         ws = eng.workspace(B, S, Bo)
         if self.accum_steps > 1:
             ws["dloss_logits"].mul_(1.0 / self.accum_steps)     # what an eager loop does with loss / k
-        # d(loss)/d(logits) was produced by the CE kernel: the reference's criterion(logits, label) [:169]
+        # d(loss)/d(logits) was produced by the loss kernel: the reference's criterion(logits, label) [:169]
         if final and self.max_grad_norm is not None:
             opt._clip_arm(self.max_grad_norm)     # the backward's per-bucket launches become the reduce phase
         eng.start_pass(not final)
@@ -251,8 +299,9 @@ class FusedTrainStep(_StagedGraphStep):
     micro-batches, the loss scaled by 1/k; call with final=False for the first k - 1 of a window.  max_grad_norm:
     clip the gradient's 2-norm before the update (see clip_grad_norm_); the norm is left in optimizer._clip_buf."""
 
-    def __init__(self, model, optimizer, batch_size, seq_len, use_graph=True, accum_steps=1, max_grad_norm=None):
-        super().__init__(model, batch_size, seq_len, use_graph)
+    def __init__(self, model, optimizer, batch_size, seq_len, use_graph=True, accum_steps=1, max_grad_norm=None,
+                 criterion=None):
+        super().__init__(model, batch_size, seq_len, use_graph, criterion)
         self._arm(optimizer, accum_steps, max_grad_norm)
         self.kernel_launches = None
 
@@ -260,11 +309,12 @@ class FusedTrainStep(_StagedGraphStep):
     def _body(self):
         self._unstage()
         self._train_body(lambda: self.eng.forward(self.d_ids, self.d_tt, self.d_mask, self.d_lab, training=True,
-                                                  need_backward=True))
+                                                  need_backward=True, loss_fn=self.loss_fn))
 
     def __call__(self, batch_data, final=True):
-        """batch_data: the dict the reference Collate yields (host int64 tensors).  Returns the device loss scalar
-        (local rank's mean CE, like `loss` at [:169]; unscaled under accumulation)."""
+        """batch_data: the dict the reference Collate yields (host int64 tensors; fp32 labels for regression and
+        multi-label).  Returns the device loss scalar (local rank's mean loss, like `loss` at [:169]; unscaled under
+        accumulation)."""
         self.stage(batch_data)
         self.run_device(final)
         return self.loss_out
@@ -275,15 +325,17 @@ class PackedTrainStep(_StagedGraphStep):
     instance (staging buffers + CUDA graph) per bin count; the Trainer keeps a small cache of them, since the number of
     bins a batch packs into varies with its lengths."""
 
-    def __init__(self, model, optimizer, bins, batch, use_graph=True, accum_steps=1, max_grad_norm=None):
-        super().__init__(model, bins, 128, use_graph)
+    def __init__(self, model, optimizer, bins, batch, use_graph=True, accum_steps=1, max_grad_norm=None,
+                 criterion=None):
+        super().__init__(model, bins, 128, use_graph, criterion)
         dev = self.eng.dev
         self.bins, self.batch = bins, batch
         n = bins * 128
         # pinned staging: ids | token types | positions | segments (as int64) | cls rows | labels
-        self._alloc_stage(4 * n + 2 * batch)
+        self.d_lab, lab_slots = self._label_buffer(batch)
+        self._alloc_stage(4 * n + batch + lab_slots)
         z = lambda *sh: torch.zeros(*sh, dtype=torch.int64, device=dev)
-        self.d_pos, self.d_cls, self.d_lab = z(bins, 128), z(batch), z(batch)
+        self.d_pos, self.d_cls = z(bins, 128), z(batch)
         self.d_seg = torch.zeros(bins, 128, dtype=torch.int32, device=dev)
         self._arm(optimizer, accum_steps, max_grad_norm)
 
@@ -294,11 +346,11 @@ class PackedTrainStep(_StagedGraphStep):
         self.d_pos.copy_(st[2 * n:3 * n].view(self.bins, 128))
         self.d_seg.copy_(st[3 * n:4 * n].view(self.bins, 128))          # int64 -> int32
         self.d_cls.copy_(st[4 * n:4 * n + self.batch])
-        self.d_lab.copy_(st[4 * n + self.batch:4 * n + 2 * self.batch])
+        self._unstage_labels(st[4 * n + self.batch:])
 
     def stage(self, packed, label):
         n, hs = self.bins * 128, self.h_stage
-        if packed["bins"] != self.bins or label.numel() != self.batch:
+        if packed["bins"] != self.bins or label.shape[0] != self.batch:
             raise ValueError("PackedTrainStep was built for %d bins / %d sequences" % (self.bins, self.batch))
         if self._h2d_done is not None:
             self._h2d_done.synchronize()
@@ -307,7 +359,7 @@ class PackedTrainStep(_StagedGraphStep):
         hs[2 * n:3 * n].copy_(packed["position_ids"].reshape(-1))
         hs[3 * n:4 * n].copy_(packed["segments"].reshape(-1))
         hs[4 * n:4 * n + self.batch].copy_(packed["cls_index"])
-        hs[4 * n + self.batch:4 * n + 2 * self.batch].copy_(label.reshape(-1))
+        self._stage_labels(hs[4 * n + self.batch:], label)
         self._stage_lr()
         self._h2d()
 
@@ -315,7 +367,7 @@ class PackedTrainStep(_StagedGraphStep):
         self._unstage()
         packed = (self.d_pos, self.d_seg, self.d_cls)
         self._train_body(lambda: self.eng.forward(self.d_ids, self.d_tt, None, self.d_lab, training=True,
-                                                  need_backward=True, packed=packed))
+                                                  need_backward=True, packed=packed, loss_fn=self.loss_fn))
 
     def __call__(self, packed, label, final=True):
         self.stage(packed, label)
@@ -325,17 +377,18 @@ class PackedTrainStep(_StagedGraphStep):
 
 class FusedEvalStep(_StagedGraphStep):
     """The reference's eval body (`on_step` + `criterion` under `no_grad`, [:204-208] / [:228-229]) as one CUDA-graph
-    replay: H2D of the batch, the dropout-free forward, mean CE.  Returns device tensors that are overwritten by the
-    next call (the callers below consume them before staging the next batch)."""
+    replay: H2D of the batch, the dropout-free forward, the mean loss of `criterion` (None: the model's problem-type
+    loss).  Returns device tensors that are overwritten by the next call (the callers below consume them before
+    staging the next batch)."""
 
-    def __init__(self, model, batch_size, seq_len, use_graph=True):
-        super().__init__(model, batch_size, seq_len, use_graph)
+    def __init__(self, model, batch_size, seq_len, use_graph=True, criterion=None):
+        super().__init__(model, batch_size, seq_len, use_graph, criterion)
         self.logits_out = torch.zeros(batch_size, self.model.num_labels, dtype=torch.float32, device=self.eng.dev)
 
     def _body(self):
         self._unstage()
         logits, loss = self.eng.forward(self.d_ids, self.d_tt, self.d_mask, self.d_lab, training=False,
-                                        need_backward=False)
+                                        need_backward=False, loss_fn=self.loss_fn)
         self.logits_out.copy_(logits)
         self.loss_out.copy_(loss)
 
@@ -405,25 +458,73 @@ class Trainer:
             self._pin[key][1] = ev
         return out
 
-    def on_step(self, batch_data):
+    def _forward(self, batch_data):
+        """on_step's model call: (output, device label)"""
         d = self._to_device(batch_data)
         label = d["label"]
         output = self.model(input_ids=d["input_ids"], token_type_ids=d["token_type_ids"],
                             attention_mask=d["attention_mask"], labels=label)
+        return output, label
+
+    def on_step(self, batch_data):
+        output, label = self._forward(batch_data)
         logits = output[1]
         return logits, label
 
-    def eval_step(self, batch_data):
-        """`on_step` for the no-grad loops: the graph-captured forward when ``args.fused`` (one replay per batch instead
-        of ~100 eager launches), else the eager call.  Returns (logits, label) like `on_step`."""
+    def problem_type(self, label):
+        """the model's config.problem_type; when None, HF's rule applied to `label` (stored on the config, as the
+        model's first labelled forward does)"""
+        cfg = _unwrap(self.model).config
+        if getattr(cfg, "problem_type", None) is None:
+            cfg.problem_type = infer_problem_type(_unwrap(self.model).num_labels, label)
+        return cfg.problem_type
+
+    def compute_loss(self, logits, label, model_loss=None):
+        """the criterion on the logits (the reference's criterion(logits, label) [:169]); with one label and float
+        labels over the squeezed logits, as HF's regression.  No criterion: the model's own loss `model_loss`."""
+        if self.criterion is None:
+            if model_loss is None:
+                raise ValueError("Trainer has no criterion and the model returned no loss")
+            return model_loss
+        if _unwrap(self.model).num_labels == 1 and label.is_floating_point():
+            return self.criterion(logits.reshape(-1), label.reshape(-1))
+        return self.criterion(logits, label)
+
+    def _eager_loss(self, batch_data):
+        """the eager loops' forward + loss: on_step and the criterion, or with no criterion the model's own loss"""
+        if self.criterion is None:
+            output, _label = self._forward(batch_data)
+            return output[0]
+        logits, label = self.on_step(batch_data)
+        return self.compute_loss(logits, label)
+
+    def _eval_forward(self, batch_data):
+        """(logits, label, the model's loss) of a no-grad batch: the graph-captured forward when ``args.fused`` (one
+        replay per batch instead of ~100 eager launches), else the eager call"""
         if not getattr(self.args, "fused", True) or batch_data["input_ids"].is_cuda:
-            return self.on_step(batch_data)
+            output, label = self._forward(batch_data)
+            return output[1], label, output[0]
+        self.problem_type(batch_data["label"])
         B, S = batch_data["input_ids"].shape
-        key = (id(_unwrap(self.model)), B, S)     # `test` may swap the model [:222-224]
+        m = _unwrap(self.model)
+        key = (id(m), B, S, m.config.problem_type)     # `test` may swap the model [:222-224]
         if key not in self._fused_eval:
             self._fused_eval[key] = FusedEvalStep(self.model, B, S)
-        logits, label, _loss = self._fused_eval[key](batch_data)
+        return self._fused_eval[key](batch_data)
+
+    def eval_step(self, batch_data):
+        """`on_step` for the no-grad loops.  Returns (logits, label) like `on_step`."""
+        logits, label, _loss = self._eval_forward(batch_data)
         return logits, label
+
+    def _captured_loss_key(self, label):
+        """what a cached captured step must have been built for: the criterion's loss parameters, or with no
+        criterion the model's problem type.  An unset problem type is inferred from this batch's labels either way, as
+        the eager path's labelled forward does."""
+        problem_type = self.problem_type(label)
+        if self.criterion is None:
+            return None, problem_type
+        return criterion_key(self.criterion), None
 
     def loss_reduce(self, loss):
         if isinstance(self.model, DistributedDataParallel):
@@ -452,20 +553,26 @@ class Trainer:
             from .packing import pack_batch
             packed = pack_batch(batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"])
             key = (packed["bins"], batch_data["input_ids"].shape[0])
-            if key not in self._packed or (self._packed[key].accum_steps, self._packed[key].max_grad_norm) != (k, clip):
+            lkey = self._captured_loss_key(batch_data["label"])
+            if key not in self._packed or (self._packed[key].accum_steps, self._packed[key].max_grad_norm,
+                                           self._packed[key].loss_key) != (k, clip, lkey):
                 if len(self._packed) >= 16:           # bound the graph cache: drop the oldest entry
                     self._packed.pop(next(iter(self._packed)))
                 self._packed[key] = PackedTrainStep(self.model, self.optimizer, key[0], key[1], accum_steps=k,
-                                                    max_grad_norm=clip)
+                                                    max_grad_norm=clip, criterion=self.criterion)
+                self._packed[key].loss_key = lkey
             self.model.train()
             loss = self._packed[key](packed, batch_data["label"], final)
             if final:
                 self._scheduler_step()      # after the replay: the next stage() reads the new lr
         elif getattr(self.args, "fused", True):
             B, S = batch_data["input_ids"].shape
+            lkey = self._captured_loss_key(batch_data["label"])
             if self._fused is None or (self._fused.B, self._fused.S, self._fused.accum_steps,
-                                       self._fused.max_grad_norm) != (B, S, k, clip):
-                self._fused = FusedTrainStep(self.model, self.optimizer, B, S, accum_steps=k, max_grad_norm=clip)
+                                       self._fused.max_grad_norm, self._fused.loss_key) != (B, S, k, clip, lkey):
+                self._fused = FusedTrainStep(self.model, self.optimizer, B, S, accum_steps=k, max_grad_norm=clip,
+                                             criterion=self.criterion)
+                self._fused.loss_key = lkey
             self.model.train()
             loss = self._fused(batch_data, final)
             if final:
@@ -477,8 +584,7 @@ class Trainer:
             self.model.train()
             with self._window(final):
                 with torch.autocast("cuda"):
-                    logits, label = self.on_step(batch_data)
-                    loss = self.criterion(logits, label)
+                    loss = self._eager_loss(batch_data)
                 self._scaler.scale(loss / k if k > 1 else loss).backward()
             if final:
                 self._clip(clip)        # no scaler.unscale_: step() takes the scale out of the norm
@@ -486,8 +592,7 @@ class Trainer:
         else:
             self.model.train()
             with self._window(final):
-                logits, label = self.on_step(batch_data)
-                loss = self.criterion(logits, label)
+                loss = self._eager_loss(batch_data)
                 if first:
                     self.optimizer.zero_grad()
                 (loss / k if k > 1 else loss).backward()
@@ -586,26 +691,45 @@ class Trainer:
                 torch.save(self.model.state_dict(), self.args.ckpt_path)
 
     def dev(self, dev_loader):
+        """(summed rank-mean loss, metric) over the gathered rows.  The metric, higher is better: accuracy
+        (single-label), subset accuracy -- every column of (logits > 0) equal to (labels >= 0.5) -- (multi-label), or
+        the Pearson correlation of predictions and labels (regression)."""
         self.model.eval()
         correct_total = 0
         num_total = 0
         loss_total = 0.
+        reg_preds, reg_trues = [], []
+        problem_type = None
         with torch.no_grad():
             for step, batch_data in enumerate(dev_loader):
-                logits, label = self.eval_step(batch_data)
-                loss = self.criterion(logits, label)
+                logits, label, model_loss = self._eval_forward(batch_data)
+                problem_type = self.problem_type(label)
+                loss = self.compute_loss(logits, label, model_loss)
                 loss = self.loss_reduce(loss)
                 loss_total += loss
                 logits, label = self.output_reduce(logits, label)
                 logits = logits.detach().cpu().numpy()
+                if problem_type == "regression":
+                    reg_preds.append(logits.reshape(-1))
+                    reg_trues.append(label.reshape(-1).detach().cpu().numpy())
+                    continue
+                if problem_type == "multi_label_classification":
+                    label = label.detach().cpu().numpy()
+                    num_total += len(label)
+                    correct_total += ((logits > 0) == (label >= 0.5)).all(axis=1).sum()
+                    continue
                 label = label.view(-1).detach().cpu().numpy()
                 num_total += len(label)
                 preds = np.argmax(logits, axis=1).flatten()
                 correct_num = (preds == label).sum()
                 correct_total += correct_num
+        if problem_type == "regression":
+            return loss_total, float(np.corrcoef(np.concatenate(reg_preds), np.concatenate(reg_trues))[0, 1])
         return loss_total, correct_total / num_total
 
     def test(self, model, test_loader, labels):
+        """sklearn's classification_report over the gathered rows: of the argmax class (single-label) or of the
+        indicator arrays (logits > 0) against (labels >= 0.5) (multi-label).  Regression raises ValueError."""
         self.model = model
         self.model.eval()
         preds = []
@@ -613,12 +737,22 @@ class Trainer:
         with torch.no_grad():
             for step, batch_data in enumerate(test_loader):
                 logits, label = self.eval_step(batch_data)
+                problem_type = self.problem_type(label)
+                if problem_type == "regression":
+                    raise ValueError("test() prints a classification report, which does not apply to regression: "
+                                     "use dev() for the Pearson correlation")
                 logits, label = self.output_reduce(logits, label)
-                label = label.view(-1).detach().cpu().numpy().tolist()
                 logits = logits.detach().cpu().numpy()
+                if problem_type == "multi_label_classification":
+                    trues.append(label.detach().cpu().numpy() >= 0.5)
+                    preds.append(logits > 0)
+                    continue
+                label = label.view(-1).detach().cpu().numpy().tolist()
                 pred = np.argmax(logits, axis=1).flatten().tolist()
                 trues.extend(label)
                 preds.extend(pred)
+        if preds and isinstance(preds[0], np.ndarray):
+            trues, preds = np.concatenate(trues).astype(int), np.concatenate(preds).astype(int)
         from sklearn.metrics import classification_report
         report = classification_report(trues, preds, target_names=labels)
         return report
