@@ -327,6 +327,42 @@ int32_t b2_adamw_background(const void* grads, void* shadow, float* master, floa
                             const uint8_t* decay_flags, int64_t begin, int64_t end, const b2_adamw_hparams_t* hp,
                             const float* step_size, void* stream);
 
+/* SGD with momentum: torch.optim.SGD (torch 2.11 sgd.py::_single_tensor_sgd) as the same two fused forms.  The optional
+ * device fields mean exactly what they mean in b2_adamw_hparams_t.  Per element, with g the gradient AdamW would use
+ * (mean over ranks / grad_scale * clip_coef):
+ *   if maximize:     g = -g
+ *   if decay flag:   g = g + weight_decay * w                      (coupled L2, on the master before the update)
+ *   if momentum:     buf = g on the first applied step, else buf = momentum * buf + (1 - dampening) * g
+ *                    g = nesterov ? g + momentum * buf : buf
+ *   w = w + (-lr) * g;  shadow = bf16_rne(w)
+ * Each `a + alpha * b` is one fma, as torch's CUDA add is; `momentum * buf` is rounded on its own.  weight_decay,
+ * momentum, 1 - dampening and -lr are rounded to fp32 from the doubles (and -lr from *lr_dev the same way).
+ * `momentum_buffer` (fp32, indexed like master) is given exactly when momentum != 0; with momentum 0 it is neither
+ * read nor written.  `step_counter` (device int64, required with momentum) counts the applied steps since the buffer
+ * came into use: 0 = the buffer is initialised from g (torch's `momentum_buffer is None`).  b2_step_advance bumps it
+ * and leaves it alone on a skipped step.  A non-zero *found_inf leaves master, buffer and shadow untouched.
+ * bytes / parameter at world 1: 12 without momentum (2 gradient, 4 + 4 master, 2 shadow), 20 with it.        */
+typedef struct b2_sgd_hparams {
+  double lr, momentum, dampening, weight_decay; /* python doubles, rounded to fp32 the way torch rounds them */
+  int32_t nesterov, maximize;
+  const float* grad_scale;
+  const float* found_inf;
+  const float* clip_coef;
+  const float* grad_f32;
+  const double* lr_dev;
+} b2_sgd_hparams_t;
+
+/* Any world: the form of b2_bucket_reduce_adamw (mean over peer_grads, or grad_f32; shadow stores to every non-NULL
+ * peer_shadow[r]).                                                                                               */
+int32_t b2_bucket_reduce_sgd(const void* const* peer_grads, void* const* peer_shadow, int32_t world, int32_t rank,
+                             float* master, float* momentum_buffer, const uint8_t* decay_flags, int64_t begin,
+                             int64_t end, const b2_sgd_hparams_t* hp, const int64_t* step_counter, void* stream);
+/* world 1, no GradScaler state and no grad_f32: the form of b2_adamw_background (128 threads x <= 32 registers, no
+ * shared memory), to run per bucket beside the backward's GEMM CTAs.  Needs no prepare step.                    */
+int32_t b2_sgd_background(const void* grads, void* shadow, float* master, float* momentum_buffer,
+                          const uint8_t* decay_flags, int64_t begin, int64_t end, const b2_sgd_hparams_t* hp,
+                          const int64_t* step_counter, void* stream);
+
 /* Gradient accumulation over the slice [begin, end) (element indices, multiples of 8) of the bf16 gradient space
  * `grads` and its fp32 accumulator `accum` (both indexed from their base, 16-byte aligned).
  *   replaces: torch's accumulation into `.grad` across backwards, and DDP's no_sync() skipping the Reducer
@@ -370,8 +406,8 @@ int32_t b2_grad_norm_finalize(const double* partials, int64_t nslots, float* con
                               float max_norm, const float* grad_scale, const float* found_inf, float* total_norm,
                               float* clip_coef, float* skip, void* stream);
 
-/* ++step (AdamW t) and ++rng step (dropout stream) on the device: keeps CUDA-graph replays stateful.
- * found_inf (optional device fp32, see b2_adamw_hparams_t): non-zero leaves the AdamW step count untouched.   */
+/* ++step (AdamW t, SGD's applied-step count) and ++rng step (dropout stream) on the device: keeps CUDA-graph replays
+ * stateful.  found_inf (optional device fp32, see b2_adamw_hparams_t): non-zero leaves the step count untouched.  */
 int32_t b2_step_advance(int64_t* step_counter, void* rng_state, const float* found_inf, void* stream);
 int32_t b2_rng_seed(void* rng_state, uint64_t seed, uint64_t step, void* stream);
 

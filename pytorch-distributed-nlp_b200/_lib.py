@@ -47,6 +47,12 @@ class AdamWHParams(C.Structure):
                 ("clip_coef", vp), ("grad_f32", vp), ("lr_dev", vp)]
 
 
+class SGDHParams(C.Structure):
+    _fields_ = [("lr", f64), ("momentum", f64), ("dampening", f64), ("weight_decay", f64),
+                ("nesterov", i32), ("maximize", i32), ("grad_scale", vp), ("found_inf", vp),
+                ("clip_coef", vp), ("grad_f32", vp), ("lr_dev", vp)]
+
+
 class LossParams(C.Structure):
     _fields_ = [("weight", vp), ("pos_weight", vp), ("ignore_index", i64), ("label_smoothing", f32)]
 
@@ -88,6 +94,9 @@ _SIGNATURES = {
                                C.POINTER(AdamWHParams), vp, vp],
     "b2_adamw_prepare": [C.POINTER(AdamWHParams), vp, vp, vp],
     "b2_adamw_background": [vp, vp, vp, vp, vp, vp, i64, i64, C.POINTER(AdamWHParams), vp, vp],
+    "b2_bucket_reduce_sgd": [C.POINTER(vp), C.POINTER(vp), i32, i32, vp, vp, vp, i64, i64, C.POINTER(SGDHParams), vp,
+                             vp],
+    "b2_sgd_background": [vp, vp, vp, vp, vp, i64, i64, C.POINTER(SGDHParams), vp, vp],
     "b2_grad_accumulate": [vp, vp, i64, i64, i32, vp],
     "b2_grad_reduce_sumsq": [C.POINTER(vp), i32, vp, i64, i64, vp, vp],
     "b2_grad_norm_finalize": [vp, i64, C.POINTER(vp), C.POINTER(vp), i32, i32, i32, vp, f32, vp, vp, vp, vp, vp, vp],

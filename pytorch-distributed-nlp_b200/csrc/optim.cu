@@ -7,8 +7,9 @@
 //
 // Each rank owns a contiguous 1/world slice of every bucket: it reads that slice of the bf16 gradients straight
 // out of every peer's HBM (NVSwitch peer loads), sums in fp32 in fixed rank order, divides by world (DDP's mean),
-// applies the HF AdamW update to its fp32 master weights / moments, and stores the refreshed bf16 shadow weights
-// into every peer's weight buffer (NVSwitch peer stores).  world == 1 degenerates to a fused multi-tensor AdamW.
+// applies the optimizer update (HF AdamW, or torch SGD) to its fp32 master weights / state, and stores the refreshed
+// bf16 shadow weights into every peer's weight buffer (NVSwitch peer stores).  world == 1 degenerates to a fused
+// multi-tensor optimizer step.
 #include "common.cuh"
 #include "../../include/b2_ddp_bert.h"
 
@@ -16,49 +17,205 @@ namespace b2 {
 
 constexpr int MAX_WORLD = 8;
 
-struct ReduceAdamWParams {
+// ---- update rules --------------------------------------------------------------------------------------------------
+// The two kernel forms below (reduce_update_kernel: any world; slim_update_kernel: world 1, beside the backward) own the
+// gradient path every optimizer shares: the peer gather in rank order, 1/world and the GradScaler unscale, the clip
+// coefficient, the fp32 stash, the found_inf skip, the device lr and the delivery of the bf16 shadow weights.  They are
+// instantiated once per update rule.  A rule supplies
+//   Args                            its scalars (pre-rounded on the host) and state pointers
+//   Step reduce_step / slim_step    the per-launch values, from the device lr when lr_dev is set
+//   update8 (reduce form)           8 elements: loads master + state, updates, stores them, returns the new weights
+//   update4 (slim form)             4 elements, the same
+struct AdamWRule {
+  struct Args {
+    float* m; float* v;
+    // scalars pre-rounded on the host exactly as torch rounds the python doubles HF AdamW passes to its ATen ops
+    double lr_d, beta1_d, beta2_d, weight_decay_d;
+    float lr, beta1, beta2, one_minus_beta1, one_minus_beta2, eps, lr_wd;
+    int correct_bias;
+    const long long* step_counter;   // reduce form: t = *step_counter + 1
+    const float* step_size;          // slim form: the bias-corrected step size from adamw_prepare_kernel
+  };
+  struct Step { float step_size, lr_wd; };
+
+  static __device__ __forceinline__ Step reduce_step(const Args& a, const double* lr_dev) {
+    // the learning rate from device memory: the same double arithmetic the host does on the by-value lr, so a device
+    // lr equal to the host value gives the same bits
+    double lr_d = a.lr_d;
+    float lr = a.lr, lr_wd = a.lr_wd;
+    if (lr_dev != nullptr) {
+      lr_d = *lr_dev;
+      lr = (float)lr_d;
+      lr_wd = (float)(lr_d * a.weight_decay_d);
+    }
+    // HF AdamW bias correction: step_size = lr * sqrt(1 - b2^t) / (1 - b1^t), t = steps taken including this one
+    const long long t = *a.step_counter + 1;
+    float step_size = lr;
+    if (a.correct_bias) {
+      const double bc1 = 1.0 - pow(a.beta1_d, (double)t);
+      const double bc2 = 1.0 - pow(a.beta2_d, (double)t);
+      step_size = (float)(lr_d * sqrt(bc2) / bc1);
+    }
+    return {step_size, lr_wd};
+  }
+  static __device__ __forceinline__ Step slim_step(const Args& a, const double* lr_dev) {
+    return {*a.step_size, lr_dev != nullptr ? (float)(*lr_dev * a.weight_decay_d) : a.lr_wd};
+  }
+
+  template <class P>
+  static __device__ __forceinline__ void update8(const P& p, const Step& s, long long e, const float* g,
+                                                 float inv_world, float coef, bool decay, float* w) {
+    const Args& a = p.rule;
+    float4 w0 = *reinterpret_cast<const float4*>(p.master + e), w1 = *reinterpret_cast<const float4*>(p.master + e + 4);
+    float4 m0 = *reinterpret_cast<const float4*>(a.m + e), m1 = *reinterpret_cast<const float4*>(a.m + e + 4);
+    float4 v0 = *reinterpret_cast<const float4*>(a.v + e), v1 = *reinterpret_cast<const float4*>(a.v + e + 4);
+    w[0] = w0.x; w[1] = w0.y; w[2] = w0.z; w[3] = w0.w; w[4] = w1.x; w[5] = w1.y; w[6] = w1.z; w[7] = w1.w;
+    float mm[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
+    float vv[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const float gk = g[k] * inv_world * coef;
+      mm[k] = mm[k] * a.beta1 + gk * a.one_minus_beta1;
+      vv[k] = vv[k] * a.beta2 + gk * gk * a.one_minus_beta2;
+      const float denom = sqrtf(vv[k]) + a.eps;
+      w[k] = w[k] - s.step_size * (mm[k] / denom);
+      if (decay) w[k] = w[k] - s.lr_wd * w[k];
+    }
+    *reinterpret_cast<float4*>(p.master + e) = make_float4(w[0], w[1], w[2], w[3]);
+    *reinterpret_cast<float4*>(p.master + e + 4) = make_float4(w[4], w[5], w[6], w[7]);
+    *reinterpret_cast<float4*>(a.m + e) = make_float4(mm[0], mm[1], mm[2], mm[3]);
+    *reinterpret_cast<float4*>(a.m + e + 4) = make_float4(mm[4], mm[5], mm[6], mm[7]);
+    *reinterpret_cast<float4*>(a.v + e) = make_float4(vv[0], vv[1], vv[2], vv[3]);
+    *reinterpret_cast<float4*>(a.v + e + 4) = make_float4(vv[4], vv[5], vv[6], vv[7]);
+  }
+
+  template <class P>
+  static __device__ __forceinline__ float4 update4(const P& p, const Step& s, long long e, uint2 q, float coef) {
+    const Args& a = p.rule;
+    float4 mm = *reinterpret_cast<const float4*>(a.m + e);
+    float4 vv = *reinterpret_cast<const float4*>(a.v + e);
+    const float g0 = bf16_lo(q.x) * coef, g1 = bf16_hi(q.x) * coef, g2 = bf16_lo(q.y) * coef,
+                g3 = bf16_hi(q.y) * coef;
+    mm.x = mm.x * a.beta1 + g0 * a.one_minus_beta1; vv.x = vv.x * a.beta2 + g0 * g0 * a.one_minus_beta2;
+    mm.y = mm.y * a.beta1 + g1 * a.one_minus_beta1; vv.y = vv.y * a.beta2 + g1 * g1 * a.one_minus_beta2;
+    mm.z = mm.z * a.beta1 + g2 * a.one_minus_beta1; vv.z = vv.z * a.beta2 + g2 * g2 * a.one_minus_beta2;
+    mm.w = mm.w * a.beta1 + g3 * a.one_minus_beta1; vv.w = vv.w * a.beta2 + g3 * g3 * a.one_minus_beta2;
+    *reinterpret_cast<float4*>(a.m + e) = mm;
+    *reinterpret_cast<float4*>(a.v + e) = vv;
+    // the Adam direction first, then the master weights: fewer values live at once (no spills at 32 registers)
+    float4 u;
+    u.x = mm.x / (sqrtf(vv.x) + a.eps);
+    u.y = mm.y / (sqrtf(vv.y) + a.eps);
+    u.z = mm.z / (sqrtf(vv.z) + a.eps);
+    u.w = mm.w / (sqrtf(vv.w) + a.eps);
+    float4 w = *reinterpret_cast<const float4*>(p.master + e);
+    const bool decay = p.has_wd && p.decay[e >> 3];
+    w.x = w.x - s.step_size * u.x;
+    w.y = w.y - s.step_size * u.y;
+    w.z = w.z - s.step_size * u.z;
+    w.w = w.w - s.step_size * u.w;
+    if (decay) {
+      w.x = w.x - s.lr_wd * w.x; w.y = w.y - s.lr_wd * w.y; w.z = w.z - s.lr_wd * w.z; w.w = w.w - s.lr_wd * w.w;
+    }
+    *reinterpret_cast<float4*>(p.master + e) = w;
+    return w;
+  }
+};
+
+// torch.optim.SGD (torch 2.11 sgd.py::_single_tensor_sgd), per element.  Each `x.add(y, alpha=a)` of torch's CUDA ops
+// is one fma(a, y, x) and `buf.mul_(momentum)` a separately rounded product, so those are written out explicitly.
+struct SgdRule {
+  struct Args {
+    float* buf;                      // momentum buffer; NULL when momentum == 0 (then never read or written)
+    const long long* step_counter;   // applied steps since the buffer exists: 0 = torch's `momentum_buffer is None`
+    float neg_lr, momentum, one_minus_dampening, weight_decay;   // -lr, 1 - dampening: rounded as torch's alphas
+    int nesterov, maximize;
+  };
+  struct Step { float neg_lr; bool first; };
+
+  static __device__ __forceinline__ Step reduce_step(const Args& a, const double* lr_dev) {
+    return {lr_dev != nullptr ? (float)(-*lr_dev) : a.neg_lr, a.buf != nullptr && *a.step_counter == 0};
+  }
+  static __device__ __forceinline__ Step slim_step(const Args& a, const double* lr_dev) {
+    return reduce_step(a, lr_dev);
+  }
+
+  static __device__ __forceinline__ float rule(const Args& a, const Step& s, float g, float w, float& b, bool decay) {
+    if (a.maximize) g = -g;
+    if (decay) g = fmaf(a.weight_decay, w, g);                     // grad.add(param, alpha=weight_decay)
+    if (a.buf != nullptr) {
+      // first step: buf = grad.clone(); then buf.mul_(momentum).add_(grad, alpha=1 - dampening)
+      b = s.first ? g : fmaf(a.one_minus_dampening, g, __fmul_rn(b, a.momentum));
+      g = a.nesterov ? fmaf(a.momentum, b, g) : b;                 // grad.add(buf, alpha=momentum) : buf
+    }
+    return fmaf(s.neg_lr, g, w);                                   // param.add_(grad, alpha=-lr)
+  }
+
+  template <class P>
+  static __device__ __forceinline__ void update8(const P& p, const Step& s, long long e, const float* g,
+                                                 float inv_world, float coef, bool decay, float* w) {
+    const Args& a = p.rule;
+    const float4 w0 = *reinterpret_cast<const float4*>(p.master + e);
+    const float4 w1 = *reinterpret_cast<const float4*>(p.master + e + 4);
+    w[0] = w0.x; w[1] = w0.y; w[2] = w0.z; w[3] = w0.w; w[4] = w1.x; w[5] = w1.y; w[6] = w1.z; w[7] = w1.w;
+    float b[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (a.buf != nullptr && !s.first) {
+      const float4 b0 = *reinterpret_cast<const float4*>(a.buf + e), b1 = *reinterpret_cast<const float4*>(a.buf + e + 4);
+      b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) w[k] = rule(a, s, g[k] * inv_world * coef, w[k], b[k], decay);
+    *reinterpret_cast<float4*>(p.master + e) = make_float4(w[0], w[1], w[2], w[3]);
+    *reinterpret_cast<float4*>(p.master + e + 4) = make_float4(w[4], w[5], w[6], w[7]);
+    if (a.buf != nullptr) {
+      *reinterpret_cast<float4*>(a.buf + e) = make_float4(b[0], b[1], b[2], b[3]);
+      *reinterpret_cast<float4*>(a.buf + e + 4) = make_float4(b[4], b[5], b[6], b[7]);
+    }
+  }
+
+  template <class P>
+  static __device__ __forceinline__ float4 update4(const P& p, const Step& s, long long e, uint2 q, float coef) {
+    const Args& a = p.rule;
+    float4 w = *reinterpret_cast<const float4*>(p.master + e);
+    const bool decay = p.has_wd && p.decay[e >> 3];
+    float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (a.buf != nullptr && !s.first) b = *reinterpret_cast<const float4*>(a.buf + e);
+    w.x = rule(a, s, bf16_lo(q.x) * coef, w.x, b.x, decay);
+    w.y = rule(a, s, bf16_hi(q.x) * coef, w.y, b.y, decay);
+    w.z = rule(a, s, bf16_lo(q.y) * coef, w.z, b.z, decay);
+    w.w = rule(a, s, bf16_hi(q.y) * coef, w.w, b.w, decay);
+    if (a.buf != nullptr) *reinterpret_cast<float4*>(a.buf + e) = b;
+    *reinterpret_cast<float4*>(p.master + e) = w;
+    return w;
+  }
+};
+
+// ---- reduce form: any world ----------------------------------------------------------------------------------------
+template <class Rule>
+struct ReduceParams {
   const __nv_bfloat16* grads[MAX_WORLD];
   __nv_bfloat16* shadow[MAX_WORLD];
   int world;
-  float* master; float* m; float* v;
+  float* master;
   const uint8_t* decay;
   long long begin, end;  // element range, multiples of 8
-  // scalars pre-rounded on the host exactly as torch rounds the python doubles HF AdamW passes to its ATen ops
-  double lr_d, beta1_d, beta2_d;
-  float lr, beta1, beta2, one_minus_beta1, one_minus_beta2, eps, lr_wd;
-  int correct_bias, has_wd;
-  const long long* step_counter;
+  int has_wd;
   const float* grad_scale;   // optional device scalar (GradScaler): gradients are divided by it
   const float* found_inf;    // optional device scalar (GradScaler): non-zero skips the update
   const float* clip_coef;    // optional device scalar (gradient clipping): gradients are multiplied by it
   const float* grad_f32;     // optional fp32 mean gradient of [begin, end), indexed from begin: read instead of peers
-  const double* lr_dev;      // optional device fp64 learning rate (a captured step's schedule): read instead of lr_d
-  double weight_decay_d;
+  const double* lr_dev;      // optional device fp64 learning rate (a captured step's schedule): read instead of the lr
+  typename Rule::Args rule;
 };
 
-__global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWParams p) {
+template <class Rule>
+__global__ void __launch_bounds__(256) reduce_update_kernel(const ReduceParams<Rule> p) {
   pdl_wait();               // PDL: predecessors complete + visible before any global access
   pdl_launch_dependents();  // let the next kernel in the stream begin launching
   if (p.found_inf != nullptr && *p.found_inf != 0.f) return;   // GradScaler saw inf/nan: this step is skipped
-  // x * 1.0f is exact: without a coefficient the update is today's, bit for bit
+  // x * 1.0f is exact: without a coefficient the update is the unclipped one, bit for bit
   const float coef = p.clip_coef != nullptr ? *p.clip_coef : 1.0f;
-  // the learning rate from device memory: the same double arithmetic the host does on the by-value lr, so a device lr
-  // equal to the host value gives the same bits
-  double lr_d = p.lr_d;
-  float lr = p.lr, lr_wd = p.lr_wd;
-  if (p.lr_dev != nullptr) {
-    lr_d = *p.lr_dev;
-    lr = (float)lr_d;
-    lr_wd = (float)(lr_d * p.weight_decay_d);
-  }
-  // HF AdamW bias correction: step_size = lr * sqrt(1 - b2^t) / (1 - b1^t), t = steps taken including this one
-  const long long t = *p.step_counter + 1;
-  float step_size = lr;
-  if (p.correct_bias) {
-    const double bc1 = 1.0 - pow(p.beta1_d, (double)t);
-    const double bc2 = 1.0 - pow(p.beta2_d, (double)t);
-    step_size = (float)(lr_d * sqrt(bc2) / bc1);
-  }
+  const typename Rule::Step s = Rule::reduce_step(p.rule, p.lr_dev);
   // mean over ranks (unless grad_f32 already holds it); with a GradScaler also the unscale (a power of two: exact)
   const float inv_world = (p.grad_scale != nullptr ? 1.0f / *p.grad_scale : 1.0f) /
                           (p.grad_f32 != nullptr ? 1.0f : (float)p.world);
@@ -83,27 +240,8 @@ __global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWPara
       }
     }
     const bool decay = p.has_wd && p.decay[e >> 3];
-    float4 w0 = *reinterpret_cast<const float4*>(p.master + e), w1 = *reinterpret_cast<const float4*>(p.master + e + 4);
-    float4 m0 = *reinterpret_cast<const float4*>(p.m + e), m1 = *reinterpret_cast<const float4*>(p.m + e + 4);
-    float4 v0 = *reinterpret_cast<const float4*>(p.v + e), v1 = *reinterpret_cast<const float4*>(p.v + e + 4);
-    float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-    float mm[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
-    float vv[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const float gk = g[k] * inv_world * coef;
-      mm[k] = mm[k] * p.beta1 + gk * p.one_minus_beta1;
-      vv[k] = vv[k] * p.beta2 + gk * gk * p.one_minus_beta2;
-      const float denom = sqrtf(vv[k]) + p.eps;
-      w[k] = w[k] - step_size * (mm[k] / denom);
-      if (decay) w[k] = w[k] - lr_wd * w[k];
-    }
-    *reinterpret_cast<float4*>(p.master + e) = make_float4(w[0], w[1], w[2], w[3]);
-    *reinterpret_cast<float4*>(p.master + e + 4) = make_float4(w[4], w[5], w[6], w[7]);
-    *reinterpret_cast<float4*>(p.m + e) = make_float4(mm[0], mm[1], mm[2], mm[3]);
-    *reinterpret_cast<float4*>(p.m + e + 4) = make_float4(mm[4], mm[5], mm[6], mm[7]);
-    *reinterpret_cast<float4*>(p.v + e) = make_float4(vv[0], vv[1], vv[2], vv[3]);
-    *reinterpret_cast<float4*>(p.v + e + 4) = make_float4(vv[4], vv[5], vv[6], vv[7]);
+    float w[8];
+    Rule::update8(p, s, e, g, inv_world, coef, decay, w);
     uint4 o;
     o.x = pack_bf16(w[0], w[1]); o.y = pack_bf16(w[2], w[3]);
     o.z = pack_bf16(w[4], w[5]); o.w = pack_bf16(w[6], w[7]);
@@ -120,62 +258,35 @@ __global__ void __launch_bounds__(256) reduce_adamw_kernel(const ReduceAdamWPara
 // memory, and the same shared-memory carve-out preference as the GEMM kernels (an SM is not re-partitioned while it
 // has resident CTAs).  Blocks are short-lived (8 vectors of 4 elements per thread) so they never hold an SM back from
 // a kernel that needs all of it (the attention kernels).  Same arithmetic, statement for statement, as
-// reduce_adamw_kernel with world == 1; the bias-corrected step size is computed once per step by adamw_prepare_kernel
-// (double pow, as the host would) instead of in every block.  The co-resident blocks are bound by the latency of their
-// own dependent load -> sqrt -> divide -> store chain, not by HBM queue depth.
+// reduce_update_kernel with world == 1; for AdamW the bias-corrected step size is computed once per step by
+// adamw_prepare_kernel (double pow, as the host would) instead of in every block.  The co-resident blocks are bound by
+// the latency of their own dependent load -> sqrt -> divide -> store chain, not by HBM queue depth.
+template <class Rule>
 struct SlimParams {
   const __nv_bfloat16* grads; __nv_bfloat16* shadow;
-  float* master; float* m; float* v;
+  float* master;
   const uint8_t* decay;
   long long begin, nvec4;
-  float beta1, beta2, one_minus_beta1, one_minus_beta2, eps, lr_wd;
   int has_wd;
-  const float* step_size;
   const float* clip_coef;   // optional (gradient clipping): gradients are multiplied by it
-  const double* lr_dev;     // optional device fp64 learning rate: lr_wd is computed from it (step_size already is)
-  double weight_decay;
+  const double* lr_dev;     // optional device fp64 learning rate
+  typename Rule::Args rule;
 };
 constexpr int kSlimThreads = 128, kSlimIters = 8;
-template <int DUMMY>
-__global__ void __launch_bounds__(DUMMY > 0 ? kSlimThreads : 0) __maxnreg__(DUMMY > 0 ? 32 : 24)
-adamw_slim_kernel(const SlimParams p) {
+template <class Rule>
+__global__ void __launch_bounds__(sizeof(Rule) > 0 ? kSlimThreads : 0) __maxnreg__(sizeof(Rule) > 0 ? 32 : 24)
+slim_update_kernel(const SlimParams<Rule> p) {
   pdl_wait();
   pdl_launch_dependents();
-  const float step_size = *p.step_size;
+  const typename Rule::Step s = Rule::slim_step(p.rule, p.lr_dev);
   const float coef = p.clip_coef != nullptr ? *p.clip_coef : 1.0f;   // x * 1.0f is exact
-  const float lr_wd = p.lr_dev != nullptr ? (float)(*p.lr_dev * p.weight_decay) : p.lr_wd;
   long long i = (long long)blockIdx.x * (kSlimThreads * kSlimIters) + threadIdx.x;
 #pragma unroll 1
   for (int it = 0; it < kSlimIters; ++it, i += kSlimThreads) {
     if (i >= p.nvec4) break;
     const long long e = p.begin + (i << 2);
     const uint2 q = *reinterpret_cast<const uint2*>(p.grads + e);
-    float4 mm = *reinterpret_cast<const float4*>(p.m + e);
-    float4 vv = *reinterpret_cast<const float4*>(p.v + e);
-    const float g0 = bf16_lo(q.x) * coef, g1 = bf16_hi(q.x) * coef, g2 = bf16_lo(q.y) * coef,
-                g3 = bf16_hi(q.y) * coef;
-    mm.x = mm.x * p.beta1 + g0 * p.one_minus_beta1; vv.x = vv.x * p.beta2 + g0 * g0 * p.one_minus_beta2;
-    mm.y = mm.y * p.beta1 + g1 * p.one_minus_beta1; vv.y = vv.y * p.beta2 + g1 * g1 * p.one_minus_beta2;
-    mm.z = mm.z * p.beta1 + g2 * p.one_minus_beta1; vv.z = vv.z * p.beta2 + g2 * g2 * p.one_minus_beta2;
-    mm.w = mm.w * p.beta1 + g3 * p.one_minus_beta1; vv.w = vv.w * p.beta2 + g3 * g3 * p.one_minus_beta2;
-    *reinterpret_cast<float4*>(p.m + e) = mm;
-    *reinterpret_cast<float4*>(p.v + e) = vv;
-    // the Adam direction first, then the master weights: fewer values live at once (no spills at 32 registers)
-    float4 u;
-    u.x = mm.x / (sqrtf(vv.x) + p.eps);
-    u.y = mm.y / (sqrtf(vv.y) + p.eps);
-    u.z = mm.z / (sqrtf(vv.z) + p.eps);
-    u.w = mm.w / (sqrtf(vv.w) + p.eps);
-    float4 w = *reinterpret_cast<const float4*>(p.master + e);
-    const bool decay = p.has_wd && p.decay[e >> 3];
-    w.x = w.x - step_size * u.x;
-    w.y = w.y - step_size * u.y;
-    w.z = w.z - step_size * u.z;
-    w.w = w.w - step_size * u.w;
-    if (decay) {
-      w.x = w.x - lr_wd * w.x; w.y = w.y - lr_wd * w.y; w.z = w.z - lr_wd * w.z; w.w = w.w - lr_wd * w.w;
-    }
-    *reinterpret_cast<float4*>(p.master + e) = w;
+    const float4 w = Rule::update4(p, s, e, q, coef);
     uint2 o;
     o.x = pack_bf16(w.x, w.y);
     o.y = pack_bf16(w.z, w.w);
@@ -186,7 +297,7 @@ adamw_slim_kernel(const SlimParams p) {
 // ---- gradient accumulation -----------------------------------------------------------------------------------------
 // One pass over [begin, end) of the bf16 gradient space and its fp32 accumulator (B2_ACCUM_* in the header).  It is
 // launched per bucket on the optimizer stream while the backward's GEMM CTAs hold the SMs, so it has the shape of
-// adamw_slim_kernel: 128 threads x <= 32 registers, no shared memory, the GEMMs' carve-out, short-lived blocks.  Each
+// slim_update_kernel: 128 threads x <= 32 registers, no shared memory, the GEMMs' carve-out, short-lived blocks.  Each
 // thread handles kAccIters vectors of 8 elements (16 bytes of bf16, 2 x float4 of fp32).  inf / nan pass through.
 constexpr int kAccThreads = 128, kAccIters = 8;
 template <int MODE>
@@ -275,7 +386,7 @@ __global__ void __maxnreg__(32) grad_reduce_sumsq_kernel(const SumsqParams p) {
       g[0] = bf16_lo(q.x); g[1] = bf16_hi(q.x); g[2] = bf16_lo(q.y); g[3] = bf16_hi(q.y);
       g[4] = bf16_lo(q.z); g[5] = bf16_hi(q.z); g[6] = bf16_lo(q.w); g[7] = bf16_hi(q.w);
     } else {
-      // the sum of reduce_adamw_kernel, from +0 in rank order: the stash holds exactly the gradient it would use
+      // the sum of reduce_update_kernel, from +0 in rank order: the stash holds exactly the gradient it would use
 #pragma unroll
       for (int k = 0; k < 8; ++k) g[k] = 0.f;
 #pragma unroll
@@ -420,48 +531,98 @@ extern "C" int32_t b2_accum_finish(float* src, void* dst, const int64_t* segment
   return 0;
 }
 
+// The launch both optimizers' reduce entry points share: checks, the gradient-path fields of the params (HP is
+// b2_adamw_hparams_t or b2_sgd_hparams_t, whose optional device fields have the same names), the grid.
+template <class Rule, class HP>
+static int32_t launch_reduce(const char* what, const void* const* peer_grads, void* const* peer_shadow, int32_t world,
+                             int32_t rank, float* master, const uint8_t* decay_flags, int64_t begin, int64_t end,
+                             const HP* hp, int has_wd, const typename Rule::Args& rule, void* stream_) {
+  B2_REQUIRE(world >= 1 && world <= MAX_WORLD && rank >= 0 && rank < world, "%s: world=%d rank=%d", what, world, rank);
+  B2_REQUIRE(begin >= 0 && end >= begin && begin % 8 == 0 && end % 8 == 0,
+             "%s: slice [%lld,%lld) must be 8-element aligned", what, (long long)begin, (long long)end);
+  if (end == begin) return 0;
+  ReduceParams<Rule> p;
+  for (int r = 0; r < MAX_WORLD; ++r) {
+    p.grads[r] = r < world ? (const __nv_bfloat16*)peer_grads[r] : nullptr;
+    p.shadow[r] = r < world ? (__nv_bfloat16*)peer_shadow[r] : nullptr;
+    // a NULL shadow entry = that peer's copy is delivered some other way (copy-engine all-gather)
+    if (r < world) B2_REQUIRE(p.grads[r] && (p.shadow[r] || r != rank), "%s: null peer pointer for rank %d", what, r);
+  }
+  p.world = world;
+  p.master = master; p.decay = decay_flags;
+  p.begin = begin; p.end = end;
+  p.has_wd = has_wd;
+  p.grad_scale = hp->grad_scale;
+  p.found_inf = hp->found_inf;
+  p.clip_coef = hp->clip_coef;
+  p.grad_f32 = hp->grad_f32;
+  p.lr_dev = hp->lr_dev;
+  p.rule = rule;
+  B2_REQUIRE((uintptr_t)p.grad_f32 % 16 == 0, "%s: grad_f32 must be 16-byte aligned", what);
+  const long long nvec = (end - begin) >> 3;
+  long long blocks = (nvec + 255) / 256;
+  const long long cap = 132 * 8;   // 8 blocks per SM of an H100
+  if (blocks > cap) blocks = cap;
+  B2_LAUNCH(reduce_update_kernel<Rule>, (unsigned)blocks, 256, 0, (cudaStream_t)stream_, p);
+  B2_CUDA(cudaGetLastError());
+  count_launches(1);
+  return 0;
+}
+
+template <class Rule, class HP>
+static int32_t launch_slim(const char* what, const void* grads, void* shadow, float* master,
+                           const uint8_t* decay_flags, int64_t begin, int64_t end, const HP* hp, int has_wd,
+                           const typename Rule::Args& rule, void* stream_) {
+  B2_REQUIRE(begin >= 0 && end >= begin && begin % 8 == 0 && end % 8 == 0,
+             "%s: slice [%lld,%lld) must be 8-element aligned", what, (long long)begin, (long long)end);
+  B2_REQUIRE(hp->grad_scale == nullptr && hp->found_inf == nullptr && hp->grad_f32 == nullptr,
+             "%s: GradScaler state and fp32 sources are handled by the bucket_reduce form", what);
+  if (end == begin) return 0;
+  static bool attr = false;
+  if (!attr) {   // same shared-memory carve-out as the GEMM CTAs it is meant to run beside
+    B2_CUDA(cudaFuncSetAttribute(slim_update_kernel<Rule>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 cudaSharedmemCarveoutMaxShared));
+    attr = true;
+  }
+  SlimParams<Rule> p;
+  p.grads = (const __nv_bfloat16*)grads; p.shadow = (__nv_bfloat16*)shadow;
+  p.master = master; p.decay = decay_flags;
+  p.begin = begin; p.nvec4 = (end - begin) >> 2;
+  p.has_wd = has_wd;
+  p.clip_coef = hp->clip_coef;
+  p.lr_dev = hp->lr_dev;
+  p.rule = rule;
+  const long long per_block = (long long)kSlimThreads * kSlimIters;
+  const long long blocks = (p.nvec4 + per_block - 1) / per_block;
+  B2_LAUNCH(slim_update_kernel<Rule>, (unsigned)blocks, kSlimThreads, 0, (cudaStream_t)stream_, p);
+  B2_CUDA(cudaGetLastError());
+  count_launches(1);
+  return 0;
+}
+
+static AdamWRule::Args adamw_args(const b2_adamw_hparams_t* hp, float* exp_avg, float* exp_avg_sq) {
+  AdamWRule::Args a;
+  a.m = exp_avg; a.v = exp_avg_sq;
+  a.lr_d = hp->lr; a.beta1_d = hp->beta1; a.beta2_d = hp->beta2; a.weight_decay_d = hp->weight_decay;
+  a.lr = (float)hp->lr; a.beta1 = (float)hp->beta1; a.beta2 = (float)hp->beta2;
+  a.one_minus_beta1 = (float)(1.0 - hp->beta1); a.one_minus_beta2 = (float)(1.0 - hp->beta2);
+  a.eps = (float)hp->eps; a.lr_wd = (float)(hp->lr * hp->weight_decay);
+  a.correct_bias = hp->correct_bias;
+  a.step_counter = nullptr;
+  a.step_size = nullptr;
+  return a;
+}
+
 extern "C" int32_t b2_bucket_reduce_adamw(const void* const* peer_grads, void* const* peer_shadow, int32_t world,
                                           int32_t rank, float* master, float* exp_avg, float* exp_avg_sq,
                                           const uint8_t* decay_flags, int64_t begin, int64_t end,
                                           const b2_adamw_hparams_t* hp, const int64_t* step_counter, void* stream_) {
   B2_REQUIRE(peer_grads && peer_shadow && master && exp_avg && exp_avg_sq && decay_flags && hp && step_counter,
              "bucket_reduce_adamw: null pointer");
-  B2_REQUIRE(world >= 1 && world <= MAX_WORLD && rank >= 0 && rank < world, "bucket_reduce_adamw: world=%d rank=%d",
-             world, rank);
-  B2_REQUIRE(begin >= 0 && end >= begin && begin % 8 == 0 && end % 8 == 0,
-             "bucket_reduce_adamw: slice [%lld,%lld) must be 8-element aligned", (long long)begin, (long long)end);
-  if (end == begin) return 0;
-  ReduceAdamWParams p;
-  for (int r = 0; r < MAX_WORLD; ++r) {
-    p.grads[r] = r < world ? (const __nv_bfloat16*)peer_grads[r] : nullptr;
-    p.shadow[r] = r < world ? (__nv_bfloat16*)peer_shadow[r] : nullptr;
-    // a NULL shadow entry = that peer's copy is delivered some other way (copy-engine all-gather)
-    if (r < world) B2_REQUIRE(p.grads[r] && (p.shadow[r] || r != rank), "bucket_reduce_adamw: null peer pointer for rank %d", r);
-  }
-  p.world = world;
-  p.master = master; p.m = exp_avg; p.v = exp_avg_sq; p.decay = decay_flags;
-  p.begin = begin; p.end = end;
-  p.lr_d = hp->lr; p.beta1_d = hp->beta1; p.beta2_d = hp->beta2;
-  p.lr = (float)hp->lr; p.beta1 = (float)hp->beta1; p.beta2 = (float)hp->beta2;
-  p.one_minus_beta1 = (float)(1.0 - hp->beta1); p.one_minus_beta2 = (float)(1.0 - hp->beta2);
-  p.eps = (float)hp->eps; p.lr_wd = (float)(hp->lr * hp->weight_decay);
-  p.correct_bias = hp->correct_bias; p.has_wd = hp->weight_decay > 0.0 ? 1 : 0;
-  p.step_counter = (const long long*)step_counter;
-  p.grad_scale = hp->grad_scale;
-  p.found_inf = hp->found_inf;
-  p.clip_coef = hp->clip_coef;
-  p.grad_f32 = hp->grad_f32;
-  p.lr_dev = hp->lr_dev;
-  p.weight_decay_d = hp->weight_decay;
-  B2_REQUIRE((uintptr_t)p.grad_f32 % 16 == 0, "bucket_reduce_adamw: grad_f32 must be 16-byte aligned");
-  const long long nvec = (end - begin) >> 3;
-  long long blocks = (nvec + 255) / 256;
-  const long long cap = 132 * 8;   // 8 blocks per SM of an H100
-  if (blocks > cap) blocks = cap;
-  B2_LAUNCH(reduce_adamw_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream_, p);
-  B2_CUDA(cudaGetLastError());
-  count_launches(1);
-  return 0;
+  AdamWRule::Args a = adamw_args(hp, exp_avg, exp_avg_sq);
+  a.step_counter = (const long long*)step_counter;
+  return launch_reduce<AdamWRule>("bucket_reduce_adamw", peer_grads, peer_shadow, world, rank, master, decay_flags,
+                                  begin, end, hp, hp->weight_decay > 0.0 ? 1 : 0, a, stream_);
 }
 
 extern "C" int32_t b2_adamw_prepare(const b2_adamw_hparams_t* hp, const int64_t* step_counter, float* step_size,
@@ -479,35 +640,52 @@ extern "C" int32_t b2_adamw_background(const void* grads, void* shadow, float* m
                                        const b2_adamw_hparams_t* hp, const float* step_size, void* stream_) {
   B2_REQUIRE(grads && shadow && master && exp_avg && exp_avg_sq && decay_flags && hp && step_size,
              "adamw_background: null pointer");
-  B2_REQUIRE(begin >= 0 && end >= begin && begin % 8 == 0 && end % 8 == 0,
-             "adamw_background: slice [%lld,%lld) must be 8-element aligned", (long long)begin, (long long)end);
-  B2_REQUIRE(hp->grad_scale == nullptr && hp->found_inf == nullptr && hp->grad_f32 == nullptr,
-             "adamw_background: GradScaler state and fp32 sources are handled by b2_bucket_reduce_adamw");
-  if (end == begin) return 0;
-  static bool attr = false;
-  if (!attr) {   // same shared-memory carve-out as the GEMM CTAs it is meant to run beside
-    B2_CUDA(cudaFuncSetAttribute(adamw_slim_kernel<1>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                 cudaSharedmemCarveoutMaxShared));
-    attr = true;
-  }
-  SlimParams p;
-  p.grads = (const __nv_bfloat16*)grads; p.shadow = (__nv_bfloat16*)shadow;
-  p.master = master; p.m = exp_avg; p.v = exp_avg_sq; p.decay = decay_flags;
-  p.begin = begin; p.nvec4 = (end - begin) >> 2;
-  p.beta1 = (float)hp->beta1; p.beta2 = (float)hp->beta2;
-  p.one_minus_beta1 = (float)(1.0 - hp->beta1); p.one_minus_beta2 = (float)(1.0 - hp->beta2);
-  p.eps = (float)hp->eps; p.lr_wd = (float)(hp->lr * hp->weight_decay);
-  p.has_wd = hp->weight_decay > 0.0 ? 1 : 0;
-  p.step_size = step_size;
-  p.clip_coef = hp->clip_coef;
-  p.lr_dev = hp->lr_dev;
-  p.weight_decay = hp->weight_decay;
-  const long long per_block = (long long)kSlimThreads * kSlimIters;
-  const long long blocks = (p.nvec4 + per_block - 1) / per_block;
-  B2_LAUNCH(adamw_slim_kernel<1>, (unsigned)blocks, kSlimThreads, 0, (cudaStream_t)stream_, p);
-  B2_CUDA(cudaGetLastError());
-  count_launches(1);
+  AdamWRule::Args a = adamw_args(hp, exp_avg, exp_avg_sq);
+  a.step_size = step_size;
+  return launch_slim<AdamWRule>("adamw_background", grads, shadow, master, decay_flags, begin, end, hp,
+                                hp->weight_decay > 0.0 ? 1 : 0, a, stream_);
+}
+
+// the buffer is there exactly when the update uses one; the step counter tells its first step
+static int32_t sgd_args(const char* what, const b2_sgd_hparams_t* hp, float* momentum_buffer,
+                        const int64_t* step_counter, SgdRule::Args* a) {
+  B2_REQUIRE((hp->momentum != 0.0) == (momentum_buffer != nullptr),
+             "%s: momentum_buffer must be given exactly when momentum != 0 (momentum=%g)", what, hp->momentum);
+  B2_REQUIRE(momentum_buffer == nullptr || step_counter != nullptr, "%s: step_counter is required with momentum", what);
+  B2_REQUIRE(!hp->nesterov || (hp->momentum > 0.0 && hp->dampening == 0.0),
+             "%s: Nesterov momentum requires a momentum and zero dampening", what);
+  a->buf = momentum_buffer;
+  a->step_counter = (const long long*)step_counter;
+  a->neg_lr = (float)(-hp->lr);
+  a->momentum = (float)hp->momentum;
+  a->one_minus_dampening = (float)(1.0 - hp->dampening);
+  a->weight_decay = (float)hp->weight_decay;
+  a->nesterov = hp->nesterov ? 1 : 0;
+  a->maximize = hp->maximize ? 1 : 0;
   return 0;
+}
+
+extern "C" int32_t b2_bucket_reduce_sgd(const void* const* peer_grads, void* const* peer_shadow, int32_t world,
+                                        int32_t rank, float* master, float* momentum_buffer,
+                                        const uint8_t* decay_flags, int64_t begin, int64_t end,
+                                        const b2_sgd_hparams_t* hp, const int64_t* step_counter, void* stream_) {
+  B2_REQUIRE(peer_grads && peer_shadow && master && decay_flags && hp, "bucket_reduce_sgd: null pointer");
+  SgdRule::Args a;
+  const int32_t st = sgd_args("bucket_reduce_sgd", hp, momentum_buffer, step_counter, &a);
+  if (st) return st;
+  return launch_reduce<SgdRule>("bucket_reduce_sgd", peer_grads, peer_shadow, world, rank, master, decay_flags, begin,
+                                end, hp, hp->weight_decay != 0.0 ? 1 : 0, a, stream_);
+}
+
+extern "C" int32_t b2_sgd_background(const void* grads, void* shadow, float* master, float* momentum_buffer,
+                                     const uint8_t* decay_flags, int64_t begin, int64_t end,
+                                     const b2_sgd_hparams_t* hp, const int64_t* step_counter, void* stream_) {
+  B2_REQUIRE(grads && shadow && master && decay_flags && hp, "sgd_background: null pointer");
+  SgdRule::Args a;
+  const int32_t st = sgd_args("sgd_background", hp, momentum_buffer, step_counter, &a);
+  if (st) return st;
+  return launch_slim<SgdRule>("sgd_background", grads, shadow, master, decay_flags, begin, end, hp,
+                              hp->weight_decay != 0.0 ? 1 : 0, a, stream_);
 }
 
 extern "C" int32_t b2_grad_accumulate(void* grads, float* accum, int64_t begin, int64_t end, int32_t mode,

@@ -1,10 +1,12 @@
-"""HF-semantics ``AdamW`` + the reference's ``build_optimizer`` on top of the fused CUDA update.
+"""HF-semantics ``AdamW``, torch-semantics ``SGD`` and the reference's ``build_optimizer`` on top of the fused CUDA
+update.
 
 Reference surface: ``build_optimizer(model, args)`` (multi-gpu-distributed-cls.py:100-111) returning an object with
 ``zero_grad()`` [:172] and ``step()`` [:174].  The arithmetic is transformers 4.28.1 ``optimization.py::AdamW.step``
 (eps added to sqrt(v) before the bias correction, weight decay applied after the Adam update with the updated
 weight, ``correct_bias=True``) — NOT ``torch.optim.AdamW``.  One kernel updates the whole flat parameter space
-(or, under DDP, this rank's slice of every bucket, fused with the gradient mean over peers).
+(or, under DDP, this rank's slice of every bucket, fused with the gradient mean over peers).  ``SGD`` is
+``torch.optim.SGD`` (fabric-cls.py's ``Args.optim = "sgd"`` branch) on the same kernels' gradient path.
 """
 import os
 
@@ -13,7 +15,10 @@ import torch
 from . import _lib as L
 
 
-class AdamW(torch.optim.Optimizer):
+class _FusedOptimizer(torch.optim.Optimizer):
+    """What every optimizer of a b200 model does around its update kernels: the device state, the GradScaler hooks,
+    gradient clipping, the per-bucket launches the backward and DDP make (update_range / prepare_background / advance)
+    and ``step()``.  A subclass supplies its hyperparameter struct, its state buffers and its two kernel forms."""
     # torch.cuda.amp.GradScaler contract for optimizers that unscale themselves (torch/amp/grad_scaler.py `step`):
     # the scaler sets `self.grad_scale` (device fp32 scalar) / `self.found_inf` around step() instead of walking
     # `.grad` tensors -- which do not exist here (gradients live in the bf16 bucket space).  This is what lets the
@@ -21,29 +26,21 @@ class AdamW(torch.optim.Optimizer):
     # scaler.step(optimizer), scaler.update()) run unchanged.  bf16 has fp32's exponent range, so no overflow check
     # is needed: found_inf stays 0 and the scale only has to be divided out (exactly: it is a power of two).
     _step_supports_amp_scaling = True
+    _shared_keys = ()     # the group hyperparameters besides lr that every group must share (one kernel, one value)
 
-    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.0, correct_bias=True,
-                 no_deprecation_warning=True):
-        if lr < 0.0:
-            raise ValueError(f"Invalid learning rate: {lr} - should be >= 0.0")
-        if not 0.0 <= betas[0] < 1.0:
-            raise ValueError(f"Invalid beta parameter: {betas[0]} - should be in [0.0, 1.0)")
-        if not 0.0 <= betas[1] < 1.0:
-            raise ValueError(f"Invalid beta parameter: {betas[1]} - should be in [0.0, 1.0)")
-        if not 0.0 <= eps:
-            raise ValueError(f"Invalid epsilon value: {eps} - should be >= 0.0")
-        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, correct_bias=correct_bias)
+    def __init__(self, params, defaults):
         super().__init__(params, defaults)
         owners = {id(getattr(p, "_b2_owner", None)) for g in self.param_groups for p in g["params"]}
         first = self.param_groups[0]["params"][0]
         self._model = getattr(first, "_b2_owner", None)
         if self._model is None or len(owners) != 1:
-            raise TypeError("this AdamW drives the fused CUDA update of ONE b200 BertForSequenceClassification; "
-                            "got parameters that do not belong to such a model")
+            raise TypeError("this %s drives the fused CUDA update of ONE b200 BertForSequenceClassification; "
+                            "got parameters that do not belong to such a model" % type(self).__name__)
         g0 = self.param_groups[0]
+        key = lambda g: (g["lr"],) + tuple(tuple(v) if isinstance(v, (list, tuple)) else v
+                                           for v in (g[k] for k in self._shared_keys))
         for g in self.param_groups[1:]:
-            if (g["lr"], tuple(g["betas"]), g["eps"], g["correct_bias"]) != \
-                    (g0["lr"], tuple(g0["betas"]), g0["eps"], g0["correct_bias"]):
+            if key(g) != key(g0):
                 raise ValueError("param groups may differ only in weight_decay (as the reference's two groups do)")
         wds = sorted({float(g["weight_decay"]) for g in self.param_groups if g["weight_decay"] > 0})
         if len(wds) > 1:
@@ -74,33 +71,31 @@ class AdamW(torch.optim.Optimizer):
         self._lr_dev_on = False
         self._model._optimizer = self
 
-    # -- device state (fp32 moments, step counter) ------------------------------------------------------------------
+    # -- device state (step counter, lr slot, decay flags, and the subclass's buffers) -------------------------------
     def _state(self):
         eng = self._model._engine
         if eng is None:
             raise RuntimeError("optimizer.step(): the model is not on CUDA")
         if self._dev_state is None or self._dev_state["dev"] != eng.dev:
-            n = self._model._layout.total
             self._dev_state = {
                 "dev": eng.dev,
-                "exp_avg": torch.zeros(n, dtype=torch.float32, device=eng.dev),
-                "exp_avg_sq": torch.zeros(n, dtype=torch.float32, device=eng.dev),
                 "step": torch.zeros(1, dtype=torch.int64, device=eng.dev),
-                "step_size": torch.zeros(1, dtype=torch.float32, device=eng.dev),   # see b2_adamw_prepare
                 "lr": torch.zeros(1, dtype=torch.float64, device=eng.dev),           # a captured step's lr
                 "decay": self._decay_flags_cpu.to(eng.dev),
             }
+            self._init_state(self._dev_state, self._model._layout.total)
             self._prepare(eng.stream())
         return self._dev_state
+
+    def _init_state(self, st, n):
+        """adds the optimizer's own device buffers to the fresh state `st` (n = elements of the flat space)"""
+
+    def _prepare(self, stream):
+        """per-step device values the background kernel reads, for the NEXT update"""
 
     def flush_pending(self):
         """No-op: every update is applied within the step that produced its gradients, so none is ever left pending.
         Kept for callers that flush before reading the weights."""
-
-    def _prepare(self, stream):
-        """bias-corrected step size of the NEXT update -> device float (read by the background kernel)"""
-        st = self._dev_state
-        L.call("b2_adamw_prepare", self.hparams(), L.ptr(st["step"]), L.ptr(st["step_size"]), stream)
 
     def current_lr(self):
         """The lr of the next update: param_groups' (a torch LR scheduler changes it between steps).  The update is
@@ -113,19 +108,8 @@ class AdamW(torch.optim.Optimizer):
                                  % ", ".join(repr(x["lr"]) for x in self.param_groups))
         return float(lr)
 
-    def captured_hparams(self):
-        """The hyperparameters a captured step bakes into its graph (all but the lr, which it reads at every replay)"""
-        return {"betas": tuple(tuple(float(b) for b in g["betas"]) for g in self.param_groups),
-                "eps": tuple(float(g["eps"]) for g in self.param_groups),
-                "weight_decay": tuple(float(g["weight_decay"]) for g in self.param_groups),
-                "correct_bias": tuple(bool(g["correct_bias"]) for g in self.param_groups)}
-
     def hparams(self):
-        g = self.param_groups[0]
-        hp = L.AdamWHParams()
-        hp.lr, hp.beta1, hp.beta2, hp.eps = float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"])
-        hp.weight_decay = float(self._wd)
-        hp.correct_bias = 1 if g["correct_bias"] else 0
+        hp = self._hparams()
         gs = getattr(self, "grad_scale", None)        # set by GradScaler.step() for the duration of step()
         hp.grad_scale = gs.data_ptr() if gs is not None else None
         if gs is not None and (gs.dtype != torch.float32 or not gs.is_cuda):
@@ -160,29 +144,22 @@ class AdamW(torch.optim.Optimizer):
         return None
 
     def update_range(self, begin, end, world, rank, peer_grads, peer_shadow, stream, background=False, grad_f32=None):
-        """Fused (mean over peers +) HF-AdamW on flat elements [begin, end).  background=True (one GPU, the update of
-        a bucket launched while the backward pass is still running): the form shaped to run beside the GEMM CTAs;
-        with nothing left to hide behind (the last bucket, or a plain optimizer.step()) the 256-thread kernel is the
-        faster one (5.2 vs 3.6 TB/s alone).  In a clipped step the gradient is multiplied by the clip coefficient;
+        """Fused (mean over peers +) update of flat elements [begin, end).  background=True (one GPU, the update of a
+        bucket launched while the backward pass is still running): the form shaped to run beside the GEMM CTAs; with
+        nothing left to hide behind (the last bucket, or a plain optimizer.step()) the 256-thread kernel is the faster
+        one (5.2 vs 3.6 TB/s alone for AdamW).  In a clipped step the gradient is multiplied by the clip coefficient;
         grad_f32: the fp32 mean gradient of the slice (the clip stash) to read instead of the peers' bf16 gradients."""
         if os.environ.get("B2_DEBUG_SKIP_ADAMW") == "1":
             return      # MEASUREMENT ONLY (how much of the optimizer is exposed in the step): weights are not updated
         st = self._state()
         hp = self.hparams()
         hp.grad_f32 = grad_f32
-        model = self._model
-        if background and world == 1 and hp.grad_scale is None and hp.found_inf is None and grad_f32 is None:
-            # one GPU: the form that fits beside the GEMM CTAs (csrc/optim.cu, adamw_slim_kernel)
-            L.call("b2_adamw_background", peer_grads[0], peer_shadow[0], L.ptr(model._flat), L.ptr(st["exp_avg"]),
-                   L.ptr(st["exp_avg_sq"]), L.ptr(st["decay"]), begin, end, hp, L.ptr(st["step_size"]), stream)
-            return
-        L.call("b2_bucket_reduce_adamw", L.ptr_array(peer_grads), L.ptr_array(peer_shadow), world, rank,
-               L.ptr(model._flat), L.ptr(st["exp_avg"]), L.ptr(st["exp_avg_sq"]), L.ptr(st["decay"]), begin, end,
-               hp, L.ptr(st["step"]), stream)
+        bg = background and world == 1 and hp.grad_scale is None and hp.found_inf is None and grad_f32 is None
+        self._launch(st, hp, begin, end, world, rank, peer_grads, peer_shadow, stream, bg)
 
     def prepare_background(self, stream):
-        """Before the first per-bucket background update of a step: the step size from the lr current now, not the
-        one of the previous step() (a scheduler has stepped since)"""
+        """Before the first per-bucket background update of a step: the per-step values from the lr current now, not
+        the one of the previous step() (a scheduler has stepped since)"""
         self._state()
         self._prepare(stream)
 
@@ -326,14 +303,147 @@ class AdamW(torch.optim.Optimizer):
         model._params_by_name["classifier.bias"].grad = None
         return loss
 
-    def moments(self):
-        """(exp_avg, exp_avg_sq) fp32 by HF parameter name — for tests/checkpoint tooling."""
-        st = self._state()
+    def _views(self, flat):
+        """`flat` (indexed like the flat parameter space) as views by HF parameter name"""
         out = {}
         for name, p in self._model._params_by_name.items():
             off, shape = self._model._layout.entries[name]
-            out[name] = (st["exp_avg"][off:off + p.numel()].view(shape), st["exp_avg_sq"][off:off + p.numel()].view(shape))
+            out[name] = flat[off:off + p.numel()].view(shape)
         return out
+
+
+class AdamW(_FusedOptimizer):
+    _shared_keys = ("betas", "eps", "correct_bias")
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.0, correct_bias=True,
+                 no_deprecation_warning=True):
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr} - should be >= 0.0")
+        if not 0.0 <= betas[0] < 1.0:
+            raise ValueError(f"Invalid beta parameter: {betas[0]} - should be in [0.0, 1.0)")
+        if not 0.0 <= betas[1] < 1.0:
+            raise ValueError(f"Invalid beta parameter: {betas[1]} - should be in [0.0, 1.0)")
+        if not 0.0 <= eps:
+            raise ValueError(f"Invalid epsilon value: {eps} - should be >= 0.0")
+        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, correct_bias=correct_bias)
+        super().__init__(params, defaults)
+
+    def _init_state(self, st, n):
+        st["exp_avg"] = torch.zeros(n, dtype=torch.float32, device=st["dev"])
+        st["exp_avg_sq"] = torch.zeros(n, dtype=torch.float32, device=st["dev"])
+        st["step_size"] = torch.zeros(1, dtype=torch.float32, device=st["dev"])   # see b2_adamw_prepare
+
+    def _prepare(self, stream):
+        """bias-corrected step size of the NEXT update -> device float (read by the background kernel)"""
+        st = self._dev_state
+        L.call("b2_adamw_prepare", self.hparams(), L.ptr(st["step"]), L.ptr(st["step_size"]), stream)
+
+    def captured_hparams(self):
+        """The hyperparameters a captured step bakes into its graph (all but the lr, which it reads at every replay)"""
+        return {"betas": tuple(tuple(float(b) for b in g["betas"]) for g in self.param_groups),
+                "eps": tuple(float(g["eps"]) for g in self.param_groups),
+                "weight_decay": tuple(float(g["weight_decay"]) for g in self.param_groups),
+                "correct_bias": tuple(bool(g["correct_bias"]) for g in self.param_groups)}
+
+    def _hparams(self):
+        g = self.param_groups[0]
+        hp = L.AdamWHParams()
+        hp.lr, hp.beta1, hp.beta2, hp.eps = float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"])
+        hp.weight_decay = float(self._wd)
+        hp.correct_bias = 1 if g["correct_bias"] else 0
+        return hp
+
+    def _launch(self, st, hp, begin, end, world, rank, peer_grads, peer_shadow, stream, background):
+        flat = self._model._flat
+        if background:
+            # one GPU: the form that fits beside the GEMM CTAs (csrc/optim.cu, slim_update_kernel)
+            L.call("b2_adamw_background", peer_grads[0], peer_shadow[0], L.ptr(flat), L.ptr(st["exp_avg"]),
+                   L.ptr(st["exp_avg_sq"]), L.ptr(st["decay"]), begin, end, hp, L.ptr(st["step_size"]), stream)
+            return
+        L.call("b2_bucket_reduce_adamw", L.ptr_array(peer_grads), L.ptr_array(peer_shadow), world, rank,
+               L.ptr(flat), L.ptr(st["exp_avg"]), L.ptr(st["exp_avg_sq"]), L.ptr(st["decay"]), begin, end,
+               hp, L.ptr(st["step"]), stream)
+
+    def moments(self):
+        """(exp_avg, exp_avg_sq) fp32 by HF parameter name — for tests/checkpoint tooling."""
+        st = self._state()
+        m, v = self._views(st["exp_avg"]), self._views(st["exp_avg_sq"])
+        return {name: (m[name], v[name]) for name in m}
+
+
+class SGD(_FusedOptimizer):
+    """``torch.optim.SGD`` (torch 2.11: momentum, dampening, coupled weight decay, Nesterov, maximize) as one fused
+    update over the flat parameter space, on every path AdamW runs: the eager loop, the captured steps and DDP.
+
+    The stock ``torch.optim.SGD`` cannot train a b200 model: its gradients live in the model's bf16 bucket space, not
+    in ``.grad``.  The momentum buffer is allocated when the first step with ``momentum != 0`` runs; as in torch, that
+    step sets it to the gradient.  ``foreach``, ``fused`` and ``differentiable=False`` are accepted and ignored."""
+    _shared_keys = ("momentum", "dampening", "nesterov", "maximize")
+
+    def __init__(self, params, lr=1e-3, momentum=0, dampening=0, weight_decay=0, nesterov=False, *, maximize=False,
+                 foreach=None, differentiable=False, fused=None):
+        if isinstance(lr, torch.Tensor) and lr.numel() != 1:
+            raise ValueError("Tensor lr must be 1-element")
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if momentum < 0.0:
+            raise ValueError(f"Invalid momentum value: {momentum}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        if differentiable:
+            raise ValueError("differentiable=True is not supported: the update is a fused kernel outside autograd")
+        defaults = dict(lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay, nesterov=nesterov,
+                        maximize=maximize, foreach=foreach, differentiable=differentiable, fused=fused)
+        if nesterov and (momentum <= 0 or dampening != 0):
+            raise ValueError("Nesterov momentum requires a momentum and zero dampening")
+        super().__init__(params, defaults)
+
+    def _init_state(self, st, n):
+        st["momentum_buffer"] = None     # allocated by the first step with momentum (torch: `momentum_buffer is None`)
+
+    def _buffer(self, st, stream):
+        """the momentum buffer, or None without momentum.  When it comes into use the step count restarts at 0 on
+        `stream`, the stream of the update about to read it: that update initialises the buffer from the gradient."""
+        if float(self.param_groups[0]["momentum"]) == 0.0:
+            return None
+        if st["momentum_buffer"] is None:
+            st["momentum_buffer"] = torch.empty(self._model._layout.total, dtype=torch.float32, device=st["dev"])
+            L.call("b2_zero", L.ptr(st["step"]), 8, stream)
+        return st["momentum_buffer"]
+
+    def captured_hparams(self):
+        """The hyperparameters a captured step bakes into its graph (all but the lr, which it reads at every replay)"""
+        return {"momentum": tuple(float(g["momentum"]) for g in self.param_groups),
+                "dampening": tuple(float(g["dampening"]) for g in self.param_groups),
+                "weight_decay": tuple(float(g["weight_decay"]) for g in self.param_groups),
+                "nesterov": tuple(bool(g["nesterov"]) for g in self.param_groups),
+                "maximize": tuple(bool(g["maximize"]) for g in self.param_groups)}
+
+    def _hparams(self):
+        g = self.param_groups[0]
+        if g["nesterov"] and (g["momentum"] <= 0 or g["dampening"] != 0):
+            raise ValueError("Nesterov momentum requires a momentum and zero dampening")
+        hp = L.SGDHParams()
+        hp.lr, hp.momentum, hp.dampening = float(g["lr"]), float(g["momentum"]), float(g["dampening"])
+        hp.weight_decay = float(self._wd)
+        hp.nesterov, hp.maximize = (1 if g["nesterov"] else 0), (1 if g["maximize"] else 0)
+        return hp
+
+    def _launch(self, st, hp, begin, end, world, rank, peer_grads, peer_shadow, stream, background):
+        flat = self._model._flat
+        buf = self._buffer(st, stream)
+        if background:
+            L.call("b2_sgd_background", peer_grads[0], peer_shadow[0], L.ptr(flat), L.ptr(buf), L.ptr(st["decay"]),
+                   begin, end, hp, L.ptr(st["step"]), stream)
+            return
+        L.call("b2_bucket_reduce_sgd", L.ptr_array(peer_grads), L.ptr_array(peer_shadow), world, rank, L.ptr(flat),
+               L.ptr(buf), L.ptr(st["decay"]), begin, end, hp, L.ptr(st["step"]), stream)
+
+    def momentum_buffers(self):
+        """fp32 momentum buffers by HF parameter name, or {} while there is none (momentum 0, or no step yet) — the
+        counterpart of AdamW.moments(), for tests and tooling."""
+        buf = self._state()["momentum_buffer"]
+        return {} if buf is None else self._views(buf)
 
 
 def clip_grad_norm_(parameters, max_norm, norm_type=2.0, error_if_nonfinite=False, foreach=None):
@@ -368,7 +478,7 @@ def clip_grad_norm_(parameters, max_norm, norm_type=2.0, error_if_nonfinite=Fals
         raise RuntimeError("clip_grad_norm_: the model is not on CUDA (there is no CPU path): call model.cuda() first")
     opt = model._optimizer
     if opt is None:
-        raise RuntimeError("clip_grad_norm_: the clip is applied by the model's AdamW inside optimizer.step(); build "
+        raise RuntimeError("clip_grad_norm_: the clip is applied by the model's optimizer inside optimizer.step(); build "
                            "the optimizer first")
     norm = opt.clip_now(max_norm)
     if error_if_nonfinite and not bool(torch.isfinite(norm)):
@@ -381,7 +491,15 @@ def clip_grad_norm_(parameters, max_norm, norm_type=2.0, error_if_nonfinite=Fals
 
 def build_optimizer(model, args):
     """Same grouping rule as the reference (multi-gpu-distributed-cls.py:100-111): no weight decay for names
-    containing 'bias' or 'LayerNorm.weight'; lr = args.learning_rate; HF AdamW defaults otherwise."""
+    containing 'bias' or 'LayerNorm.weight'; lr = args.learning_rate; HF AdamW defaults otherwise.
+
+    ``args.optim = "sgd"`` (fabric-cls.py's default, :281-285) gives that script's optimizer instead:
+    ``SGD(model.parameters(), lr=args.learning_rate)``, one group, no momentum and no weight decay."""
+    optim = getattr(args, "optim", "adamw")
+    if optim == "sgd":
+        return SGD(model.parameters(), lr=args.learning_rate)
+    if optim != "adamw":
+        raise ValueError("args.optim must be 'adamw' or 'sgd' (got %r)" % (optim,))
     no_decay = ['bias', 'LayerNorm.weight']
     optimizer_grouped_parameters = [
         {'params': [p for n, p in model.named_parameters() if not any(nd in n for nd in no_decay)],
