@@ -28,7 +28,7 @@ extern "C" {
 /* ------------------------------------------------------------------------------------------------------ */
 const char* b2_last_error(void);
 int32_t b2_abi_version(void);             /* bumped when a struct below changes */
-#define B2_ABI_VERSION 22
+#define B2_ABI_VERSION 23
 int64_t b2_launch_count(void);            /* kernels launched by this library so far (process-wide) */
 
 /* ------------------------------------------------------------------------------------------------------ */
@@ -362,6 +362,49 @@ int32_t b2_bucket_reduce_sgd(const void* const* peer_grads, void* const* peer_sh
 int32_t b2_sgd_background(const void* grads, void* shadow, float* master, float* momentum_buffer,
                           const uint8_t* decay_flags, int64_t begin, int64_t end, const b2_sgd_hparams_t* hp,
                           const int64_t* step_counter, void* stream);
+
+/* torch.optim.Adam / torch.optim.AdamW with fused=True (torch 2.11 ATen/native/cuda/fused_adam_utils.cuh, the
+ * default optimizer of HF transformers 5.5's Trainer) as the same two fused forms.  The optional device fields mean
+ * exactly what they mean in b2_adamw_hparams_t.  Everything is fp32: lr (or *lr_dev), betas, eps and weight_decay are
+ * the doubles cast to float, t = (float)(*step_counter + 1).  Per element, with g the gradient AdamW would use:
+ *   if maximize:     g = -g
+ *   if decay flag:   decoupled (AdamW): w = w - (lr * weight_decay) * w;  else (Adam): g = g + w * weight_decay
+ *   m = b1 * m + (g - b1 * g);  v = b2 * v + (g*g - b2 * g*g)        (torch's nested fmas)
+ *   if amsgrad:      vmax = max(vmax, v), used in place of v below
+ *   denom = sqrt(v) / sqrt(1 - b2^t) + eps;  w = w - (lr / (1 - b1^t)) * m / denom;  shadow = bf16_rne(w)
+ * Each `a * b + c` is one fma and every other operation is rounded on its own, as in torch's build, so the result is
+ * bitwise torch's fused kernel.  The one place that build varies is Adam's `g + w * weight_decay`: one fma with amsgrad
+ * or a grad_scale; otherwise a product and a sum when maximizing and in lane 0 of torch's loop, one fma in lanes 1-3.
+ * Lane 0 is an element whose index in its tensor is a multiple of 4; for a tensor whose size is not a multiple of 4
+ * the decay flags of its vectors say it: B2_ADAM_DECAY_UNALIGNED, plus B2_ADAM_DECAY_LANE0 where (index % 2048) < 512.
+ * `max_exp_avg_sq` (fp32, indexed like master) is given exactly when amsgrad is set.  A non-zero *found_inf leaves
+ * master, moments and shadow untouched (and b2_step_advance leaves the step count).
+ * bytes / parameter at world 1: 28 (2 gradient, 4 + 4 master, 8 + 8 moments, 2 shadow), 36 with amsgrad.       */
+#define B2_ADAM_DECAY_UNALIGNED 2   /* decay flag bits (with bit 0 set) read by the Adam entry points only */
+#define B2_ADAM_DECAY_LANE0 4
+typedef struct b2_adam_hparams {
+  double lr, beta1, beta2, eps, weight_decay; /* python doubles; the kernels cast them to float, as torch does */
+  int32_t amsgrad, maximize, decoupled;
+  const float* grad_scale;
+  const float* found_inf;
+  const float* clip_coef;
+  const float* grad_f32;
+  const double* lr_dev;
+} b2_adam_hparams_t;
+
+/* Any world: the form of b2_bucket_reduce_adamw.                                                                  */
+int32_t b2_bucket_reduce_adam(const void* const* peer_grads, void* const* peer_shadow, int32_t world, int32_t rank,
+                              float* master, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq,
+                              const uint8_t* decay_flags, int64_t begin, int64_t end, const b2_adam_hparams_t* hp,
+                              const int64_t* step_counter, void* stream);
+/* `prepared` = device float[2] {lr / (1 - b1^t), sqrt(1 - b2^t)} of the next update, written by b2_adam_prepare (t =
+ * *step_counter + 1, lr from *lr_dev when set); call it once per step, after b2_step_advance.  b2_adam_background is
+ * world 1 with no GradScaler state and no grad_f32: the form of b2_adamw_background (128 threads x <= 32 registers,
+ * no shared memory, with and without amsgrad), to run per bucket beside the backward's GEMM CTAs.               */
+int32_t b2_adam_prepare(const b2_adam_hparams_t* hp, const int64_t* step_counter, float* prepared, void* stream);
+int32_t b2_adam_background(const void* grads, void* shadow, float* master, float* exp_avg, float* exp_avg_sq,
+                           float* max_exp_avg_sq, const uint8_t* decay_flags, int64_t begin, int64_t end,
+                           const b2_adam_hparams_t* hp, const float* prepared, void* stream);
 
 /* Gradient accumulation over the slice [begin, end) (element indices, multiples of 8) of the bf16 gradient space
  * `grads` and its fp32 accumulator `accum` (both indexed from their base, 16-byte aligned).

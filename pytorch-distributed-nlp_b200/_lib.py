@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2ddpbert.so")
-ABI_VERSION = 22
+ABI_VERSION = 23
 
 MAJOR_K, MAJOR_MN = 0, 1
 EPI_NONE, EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_DROPOUT_RESIDUAL, EPI_RESIDUAL, EPI_GELU_BWD = 0, 1, 2, 3, 4, 5
@@ -16,6 +16,7 @@ EPI_RESIDUAL_F32 = 6
 EPI_ACCUM_F32 = 7
 ACCUM_STORE, ACCUM_ADD, ACCUM_FOLD, ACCUM_FLUSH = 0, 1, 2, 3     # b2_grad_accumulate modes
 LOSS_CE, LOSS_MSE, LOSS_BCE = 0, 1, 2                            # b2_loss_fwd_bwd modes
+ADAM_DECAY_UNALIGNED, ADAM_DECAY_LANE0 = 2, 4                    # decay-flag bits the Adam entry points read
 
 
 def sumsq_slots(n):
@@ -50,6 +51,12 @@ class AdamWHParams(C.Structure):
 class SGDHParams(C.Structure):
     _fields_ = [("lr", f64), ("momentum", f64), ("dampening", f64), ("weight_decay", f64),
                 ("nesterov", i32), ("maximize", i32), ("grad_scale", vp), ("found_inf", vp),
+                ("clip_coef", vp), ("grad_f32", vp), ("lr_dev", vp)]
+
+
+class AdamHParams(C.Structure):
+    _fields_ = [("lr", f64), ("beta1", f64), ("beta2", f64), ("eps", f64), ("weight_decay", f64),
+                ("amsgrad", i32), ("maximize", i32), ("decoupled", i32), ("grad_scale", vp), ("found_inf", vp),
                 ("clip_coef", vp), ("grad_f32", vp), ("lr_dev", vp)]
 
 
@@ -97,6 +104,10 @@ _SIGNATURES = {
     "b2_bucket_reduce_sgd": [C.POINTER(vp), C.POINTER(vp), i32, i32, vp, vp, vp, i64, i64, C.POINTER(SGDHParams), vp,
                              vp],
     "b2_sgd_background": [vp, vp, vp, vp, vp, i64, i64, C.POINTER(SGDHParams), vp, vp],
+    "b2_bucket_reduce_adam": [C.POINTER(vp), C.POINTER(vp), i32, i32, vp, vp, vp, vp, vp, i64, i64,
+                              C.POINTER(AdamHParams), vp, vp],
+    "b2_adam_prepare": [C.POINTER(AdamHParams), vp, vp, vp],
+    "b2_adam_background": [vp, vp, vp, vp, vp, vp, vp, i64, i64, C.POINTER(AdamHParams), vp, vp],
     "b2_grad_accumulate": [vp, vp, i64, i64, i32, vp],
     "b2_grad_reduce_sumsq": [C.POINTER(vp), i32, vp, i64, i64, vp, vp],
     "b2_grad_norm_finalize": [vp, i64, C.POINTER(vp), C.POINTER(vp), i32, i32, i32, vp, f32, vp, vp, vp, vp, vp, vp],

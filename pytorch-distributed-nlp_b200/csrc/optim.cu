@@ -190,6 +190,172 @@ struct SgdRule {
   }
 };
 
+// torch.optim.Adam / AdamW with fused=True (torch 2.11 ATen/native/cuda/fused_adam_utils.cuh, `adam_math`), per
+// element in fp32: the hyperparameters are the doubles cast to float, t is the float step count, and the two bias
+// corrections are formed in float (torch_adam_bias_correction).  AMSGRAD is a template flag, so the update without it
+// carries no max_exp_avg_sq traffic or registers; both slim instantiations fit in 32 registers with no spills.
+__device__ __forceinline__ void torch_adam_bias_correction(float lr, float beta1, float beta2, long long step,
+                                                           float* step_size, float* bc2_sqrt) {
+  const float t = (float)(step + 1);
+  *step_size = lr / (1.0f - powf(beta1, t));          // lr / bias_correction1
+  *bc2_sqrt = sqrtf(1.0f - powf(beta2, t));
+}
+
+template <bool AMSGRAD>
+struct TorchAdamRule {
+  struct Args {
+    float* m; float* v;
+    float* vmax;                     // max_exp_avg_sq (AMSGRAD only)
+    float lr, beta1, beta2, weight_decay, eps;   // static_cast<float> of the python doubles, as torch's opmath values
+    int maximize, decoupled;         // decoupled: AdamW's decay of the weight; else Adam's L2 term in the gradient
+    const long long* step_counter;   // reduce form: t = *step_counter + 1
+    const float* prepared;           // slim form: {lr / bias_correction1, sqrt(bias_correction2)} from the prepare kernel
+  };
+  struct Step { float step_size, bc2_sqrt, lr_wd; };
+
+  static __device__ __forceinline__ float lr_of(const Args& a, const double* lr_dev) {
+    return lr_dev != nullptr ? (float)*lr_dev : a.lr;   // torch: static_cast<opmath_t>(lr)
+  }
+  static __device__ __forceinline__ Step reduce_step(const Args& a, const double* lr_dev) {
+    Step s;
+    const float lr = lr_of(a, lr_dev);
+    torch_adam_bias_correction(lr, a.beta1, a.beta2, *a.step_counter, &s.step_size, &s.bc2_sqrt);
+    s.lr_wd = lr * a.weight_decay;
+    return s;
+  }
+  static __device__ __forceinline__ Step slim_step(const Args& a, const double* lr_dev) {
+    return {a.prepared[0], a.prepared[1], lr_of(a, lr_dev) * a.weight_decay};
+  }
+
+  // adam_math on one element in three parts, so the slim form can store the moments before it holds the weights.
+  // Each `a * b + c` is one fma and every other operation is rounded on its own, as in torch's build -- except Adam's
+  // L2 term `grad += param * weight_decay`, which torch's build (sm_90 SASS of FusedAdamMathFunctor) forms as one fma
+  // in the amsgrad kernel and whenever it unscales a GradScaler gradient, and otherwise as a product and a sum when
+  // maximizing and in the first of the four elements a thread holds (lane 0), one fma in the other three.  A thread's
+  // lanes are the elements 4i..4i+3 of a tensor whose size is a multiple of 4; a tensor of any other size goes through
+  // torch's unaligned loop, where element j is in lane (j % 2048) / 512: its decay flags carry that (B2_ADAM_DECAY_*).
+  static __device__ __forceinline__ bool l2_fma(const Args& a, bool scaled, bool lane0) {
+    return AMSGRAD || scaled || !(a.maximize || lane0);
+  }
+  static __device__ __forceinline__ bool lane0(uint8_t flags, int k) {
+    return (flags & B2_ADAM_DECAY_UNALIGNED) ? (flags & B2_ADAM_DECAY_LANE0) != 0 : (k & 3) == 0;
+  }
+  // grad: g the gradient of the shared path, w the master before the update
+  static __device__ __forceinline__ float grad(const Args& a, float g, float w, bool decay, bool fma_l2) {
+    if (a.maximize) g = -g;
+    if (decay && !a.decoupled)                                     // grad += param * weight_decay
+      g = fma_l2 ? fmaf(w, a.weight_decay, g) : __fadd_rn(g, __fmul_rn(w, a.weight_decay));
+    return g;
+  }
+  // moments: g from grad(); m, v and vm (AMSGRAD) are updated in place.  Returns the second moment the denominator uses.
+  static __device__ __forceinline__ float moments(const Args& a, float g, float& m, float& v, float& vm) {
+    m = fmaf(a.beta1, m, fmaf(-a.beta1, g, g));
+    const float g2 = __fmul_rn(g, g);
+    v = fmaf(a.beta2, v, fmaf(-a.beta2, g2, g2));
+    if (!AMSGRAD) return v;
+    vm = vm < v ? v : vm;                                          // std::max(max_exp_avg_sq, exp_avg_sq)
+    return vm;
+  }
+  // step_size * exp_avg / denom
+  static __device__ __forceinline__ float direction(const Args& a, const Step& s, float m, float d) {
+    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(d), s.bc2_sqrt), a.eps);
+    return __fdiv_rn(__fmul_rn(s.step_size, m), denom);
+  }
+  // the new master from the old one
+  static __device__ __forceinline__ float weight(const Args& a, const Step& s, float w, float u, bool decay) {
+    if (decay && a.decoupled) w = fmaf(-s.lr_wd, w, w);            // param -= lr * weight_decay * param
+    return __fsub_rn(w, u);                                        // param -= step_size * exp_avg / denom
+  }
+
+  template <class P>
+  static __device__ __forceinline__ void update8(const P& p, const Step& s, long long e, const float* g,
+                                                 float inv_world, float coef, bool decay, float* w) {
+    const Args& a = p.rule;
+    float4 w0 = *reinterpret_cast<const float4*>(p.master + e), w1 = *reinterpret_cast<const float4*>(p.master + e + 4);
+    float4 m0 = *reinterpret_cast<const float4*>(a.m + e), m1 = *reinterpret_cast<const float4*>(a.m + e + 4);
+    float4 v0 = *reinterpret_cast<const float4*>(a.v + e), v1 = *reinterpret_cast<const float4*>(a.v + e + 4);
+    w[0] = w0.x; w[1] = w0.y; w[2] = w0.z; w[3] = w0.w; w[4] = w1.x; w[5] = w1.y; w[6] = w1.z; w[7] = w1.w;
+    float mm[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
+    float vv[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+    float xx[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (AMSGRAD) {
+      const float4 x0 = *reinterpret_cast<const float4*>(a.vmax + e), x1 = *reinterpret_cast<const float4*>(a.vmax + e + 4);
+      xx[0] = x0.x; xx[1] = x0.y; xx[2] = x0.z; xx[3] = x0.w; xx[4] = x1.x; xx[5] = x1.y; xx[6] = x1.z; xx[7] = x1.w;
+    }
+    const uint8_t flags = decay ? p.decay[e >> 3] : 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const bool fma_l2 = l2_fma(a, p.grad_scale != nullptr, lane0(flags, k));
+      const float d = moments(a, grad(a, g[k] * inv_world * coef, w[k], decay, fma_l2), mm[k], vv[k], xx[k]);
+      w[k] = weight(a, s, w[k], direction(a, s, mm[k], d), decay);
+    }
+    *reinterpret_cast<float4*>(p.master + e) = make_float4(w[0], w[1], w[2], w[3]);
+    *reinterpret_cast<float4*>(p.master + e + 4) = make_float4(w[4], w[5], w[6], w[7]);
+    *reinterpret_cast<float4*>(a.m + e) = make_float4(mm[0], mm[1], mm[2], mm[3]);
+    *reinterpret_cast<float4*>(a.m + e + 4) = make_float4(mm[4], mm[5], mm[6], mm[7]);
+    *reinterpret_cast<float4*>(a.v + e) = make_float4(vv[0], vv[1], vv[2], vv[3]);
+    *reinterpret_cast<float4*>(a.v + e + 4) = make_float4(vv[4], vv[5], vv[6], vv[7]);
+    if (AMSGRAD) {
+      *reinterpret_cast<float4*>(a.vmax + e) = make_float4(xx[0], xx[1], xx[2], xx[3]);
+      *reinterpret_cast<float4*>(a.vmax + e + 4) = make_float4(xx[4], xx[5], xx[6], xx[7]);
+    }
+  }
+
+  template <class P>
+  static __device__ __forceinline__ float4 update4(const P& p, const Step& s, long long e, uint2 q, float coef) {
+    const Args& a = p.rule;
+    const uint8_t flags = p.has_wd ? p.decay[e >> 3] : 0;
+    const bool decay = flags != 0;
+    float4 mm, vv, d;
+    if constexpr (AMSGRAD) {
+      // the L2 term is always one fma here: the moments straight after the loads
+      mm = *reinterpret_cast<const float4*>(a.m + e);
+      vv = *reinterpret_cast<const float4*>(a.v + e);
+      const float4 w = *reinterpret_cast<const float4*>(p.master + e);   // the coupled decay reads it
+      float4 xx = *reinterpret_cast<const float4*>(a.vmax + e);
+      d.x = moments(a, grad(a, bf16_lo(q.x) * coef, w.x, decay, true), mm.x, vv.x, xx.x);
+      d.y = moments(a, grad(a, bf16_hi(q.x) * coef, w.y, decay, true), mm.y, vv.y, xx.y);
+      d.z = moments(a, grad(a, bf16_lo(q.y) * coef, w.z, decay, true), mm.z, vv.z, xx.z);
+      d.w = moments(a, grad(a, bf16_hi(q.y) * coef, w.w, decay, true), mm.w, vv.w, xx.w);
+      *reinterpret_cast<float4*>(a.vmax + e) = xx;
+    } else {
+      // the gradients first, while the master weights are live, then the moments: fewer values live at once.  e is a
+      // multiple of 4, so .x is the only element that can be in lane 0 of an aligned tensor (and this form has no
+      // GradScaler state)
+      float4 gg;
+      {
+        const float4 w = *reinterpret_cast<const float4*>(p.master + e);
+        gg.x = grad(a, bf16_lo(q.x) * coef, w.x, decay, l2_fma(a, false, lane0(flags, 0)));
+        gg.y = grad(a, bf16_hi(q.x) * coef, w.y, decay, l2_fma(a, false, lane0(flags, 1)));
+        gg.z = grad(a, bf16_lo(q.y) * coef, w.z, decay, l2_fma(a, false, lane0(flags, 2)));
+        gg.w = grad(a, bf16_hi(q.y) * coef, w.w, decay, l2_fma(a, false, lane0(flags, 3)));
+      }
+      mm = *reinterpret_cast<const float4*>(a.m + e);
+      vv = *reinterpret_cast<const float4*>(a.v + e);
+      float unused = 0.f;
+      d.x = moments(a, gg.x, mm.x, vv.x, unused);
+      d.y = moments(a, gg.y, mm.y, vv.y, unused);
+      d.z = moments(a, gg.z, mm.z, vv.z, unused);
+      d.w = moments(a, gg.w, mm.w, vv.w, unused);
+    }
+    *reinterpret_cast<float4*>(a.m + e) = mm;
+    *reinterpret_cast<float4*>(a.v + e) = vv;
+    // the directions first, then the master weights again (an L1 hit): fewer values live across the divisions
+    float4 u;
+    u.x = direction(a, s, mm.x, d.x);
+    u.y = direction(a, s, mm.y, d.y);
+    u.z = direction(a, s, mm.z, d.z);
+    u.w = direction(a, s, mm.w, d.w);
+    float4 w = *reinterpret_cast<const float4*>(p.master + e);
+    w.x = weight(a, s, w.x, u.x, decay);
+    w.y = weight(a, s, w.y, u.y, decay);
+    w.z = weight(a, s, w.z, u.z, decay);
+    w.w = weight(a, s, w.w, u.w, decay);
+    *reinterpret_cast<float4*>(p.master + e) = w;
+    return w;
+  }
+};
+
 // ---- reduce form: any world ----------------------------------------------------------------------------------------
 template <class Rule>
 struct ReduceParams {
@@ -467,6 +633,18 @@ __global__ void adamw_prepare_kernel(double lr_arg, const double* lr_dev, double
   }
 }
 
+// torch Adam's bias corrections for the NEXT update (t = *step + 1), read by the slim form: prepared[0] = lr / bc1,
+// prepared[1] = sqrt(bc2); lr is (float)*lr_dev when that is set
+__global__ void torch_adam_prepare_kernel(float lr_arg, const double* lr_dev, float beta1, float beta2,
+                                          const long long* step, float* prepared) {
+  pdl_wait();
+  pdl_launch_dependents();
+  if (threadIdx.x == 0 && blockIdx.x == 0) {
+    const float lr = lr_dev != nullptr ? (float)*lr_dev : lr_arg;
+    torch_adam_bias_correction(lr, beta1, beta2, *step, &prepared[0], &prepared[1]);
+  }
+}
+
 __global__ void step_advance_kernel(long long* step, unsigned long long* rng, const float* found_inf) {
   pdl_wait();               // PDL: predecessors complete + visible before any global access
   pdl_launch_dependents();  // let the next kernel in the stream begin launching
@@ -531,8 +709,8 @@ extern "C" int32_t b2_accum_finish(float* src, void* dst, const int64_t* segment
   return 0;
 }
 
-// The launch both optimizers' reduce entry points share: checks, the gradient-path fields of the params (HP is
-// b2_adamw_hparams_t or b2_sgd_hparams_t, whose optional device fields have the same names), the grid.
+// The launch every optimizer's reduce entry point shares: checks, the gradient-path fields of the params (HP is
+// b2_adamw_hparams_t, b2_sgd_hparams_t or b2_adam_hparams_t, whose optional device fields have the same names), the grid.
 template <class Rule, class HP>
 static int32_t launch_reduce(const char* what, const void* const* peer_grads, void* const* peer_shadow, int32_t world,
                              int32_t rank, float* master, const uint8_t* decay_flags, int64_t begin, int64_t end,
@@ -686,6 +864,80 @@ extern "C" int32_t b2_sgd_background(const void* grads, void* shadow, float* mas
   if (st) return st;
   return launch_slim<SgdRule>("sgd_background", grads, shadow, master, decay_flags, begin, end, hp,
                               hp->weight_decay != 0.0 ? 1 : 0, a, stream_);
+}
+
+// the max_exp_avg_sq buffer is there exactly when the update is amsgrad's
+template <bool AMSGRAD>
+static int32_t torch_adam_args(const char* what, const b2_adam_hparams_t* hp, float* exp_avg, float* exp_avg_sq,
+                               float* max_exp_avg_sq, typename TorchAdamRule<AMSGRAD>::Args* a) {
+  B2_REQUIRE(exp_avg && exp_avg_sq, "%s: null moment pointer", what);
+  B2_REQUIRE((hp->amsgrad != 0) == (max_exp_avg_sq != nullptr),
+             "%s: max_exp_avg_sq must be given exactly when amsgrad is set (amsgrad=%d)", what, (int)hp->amsgrad);
+  a->m = exp_avg; a->v = exp_avg_sq; a->vmax = max_exp_avg_sq;
+  a->lr = (float)hp->lr; a->beta1 = (float)hp->beta1; a->beta2 = (float)hp->beta2;
+  a->weight_decay = (float)hp->weight_decay; a->eps = (float)hp->eps;
+  a->maximize = hp->maximize ? 1 : 0;
+  a->decoupled = hp->decoupled ? 1 : 0;
+  a->step_counter = nullptr;
+  a->prepared = nullptr;
+  return 0;
+}
+
+template <bool AMSGRAD>
+static int32_t bucket_reduce_adam(const void* const* peer_grads, void* const* peer_shadow, int32_t world, int32_t rank,
+                                  float* master, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq,
+                                  const uint8_t* decay_flags, int64_t begin, int64_t end, const b2_adam_hparams_t* hp,
+                                  const int64_t* step_counter, void* stream_) {
+  typename TorchAdamRule<AMSGRAD>::Args a;
+  const int32_t st = torch_adam_args<AMSGRAD>("bucket_reduce_adam", hp, exp_avg, exp_avg_sq, max_exp_avg_sq, &a);
+  if (st) return st;
+  a.step_counter = (const long long*)step_counter;
+  return launch_reduce<TorchAdamRule<AMSGRAD>>("bucket_reduce_adam", peer_grads, peer_shadow, world, rank, master,
+                                               decay_flags, begin, end, hp, hp->weight_decay != 0.0 ? 1 : 0, a,
+                                               stream_);
+}
+
+extern "C" int32_t b2_bucket_reduce_adam(const void* const* peer_grads, void* const* peer_shadow, int32_t world,
+                                         int32_t rank, float* master, float* exp_avg, float* exp_avg_sq,
+                                         float* max_exp_avg_sq, const uint8_t* decay_flags, int64_t begin, int64_t end,
+                                         const b2_adam_hparams_t* hp, const int64_t* step_counter, void* stream_) {
+  B2_REQUIRE(peer_grads && peer_shadow && master && decay_flags && hp && step_counter,
+             "bucket_reduce_adam: null pointer");
+  return hp->amsgrad ? bucket_reduce_adam<true>(peer_grads, peer_shadow, world, rank, master, exp_avg, exp_avg_sq,
+                                                max_exp_avg_sq, decay_flags, begin, end, hp, step_counter, stream_)
+                     : bucket_reduce_adam<false>(peer_grads, peer_shadow, world, rank, master, exp_avg, exp_avg_sq,
+                                                 max_exp_avg_sq, decay_flags, begin, end, hp, step_counter, stream_);
+}
+
+extern "C" int32_t b2_adam_prepare(const b2_adam_hparams_t* hp, const int64_t* step_counter, float* prepared,
+                                   void* stream_) {
+  B2_REQUIRE(hp && step_counter && prepared, "adam_prepare: null pointer");
+  B2_LAUNCH(torch_adam_prepare_kernel, 1, 32, 0, (cudaStream_t)stream_, (float)hp->lr, hp->lr_dev, (float)hp->beta1,
+            (float)hp->beta2, (const long long*)step_counter, prepared);
+  B2_CUDA(cudaGetLastError());
+  count_launches(1);
+  return 0;
+}
+
+extern "C" int32_t b2_adam_background(const void* grads, void* shadow, float* master, float* exp_avg,
+                                      float* exp_avg_sq, float* max_exp_avg_sq, const uint8_t* decay_flags,
+                                      int64_t begin, int64_t end, const b2_adam_hparams_t* hp, const float* prepared,
+                                      void* stream_) {
+  B2_REQUIRE(grads && shadow && master && decay_flags && hp && prepared, "adam_background: null pointer");
+  if (hp->amsgrad) {
+    typename TorchAdamRule<true>::Args a;
+    const int32_t st = torch_adam_args<true>("adam_background", hp, exp_avg, exp_avg_sq, max_exp_avg_sq, &a);
+    if (st) return st;
+    a.prepared = prepared;
+    return launch_slim<TorchAdamRule<true>>("adam_background", grads, shadow, master, decay_flags, begin, end, hp,
+                                            hp->weight_decay != 0.0 ? 1 : 0, a, stream_);
+  }
+  typename TorchAdamRule<false>::Args a;
+  const int32_t st = torch_adam_args<false>("adam_background", hp, exp_avg, exp_avg_sq, max_exp_avg_sq, &a);
+  if (st) return st;
+  a.prepared = prepared;
+  return launch_slim<TorchAdamRule<false>>("adam_background", grads, shadow, master, decay_flags, begin, end, hp,
+                                           hp->weight_decay != 0.0 ? 1 : 0, a, stream_);
 }
 
 extern "C" int32_t b2_grad_accumulate(void* grads, float* accum, int64_t begin, int64_t end, int32_t mode,

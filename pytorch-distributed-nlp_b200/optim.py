@@ -1,12 +1,13 @@
-"""HF-semantics ``AdamW``, torch-semantics ``SGD`` and the reference's ``build_optimizer`` on top of the fused CUDA
-update.
+"""HF-semantics ``AdamW``, torch-semantics ``SGD``, ``Adam`` and ``TorchAdamW``, and the reference's
+``build_optimizer`` on top of the fused CUDA update.
 
 Reference surface: ``build_optimizer(model, args)`` (multi-gpu-distributed-cls.py:100-111) returning an object with
 ``zero_grad()`` [:172] and ``step()`` [:174].  The arithmetic is transformers 4.28.1 ``optimization.py::AdamW.step``
 (eps added to sqrt(v) before the bias correction, weight decay applied after the Adam update with the updated
 weight, ``correct_bias=True``) — NOT ``torch.optim.AdamW``.  One kernel updates the whole flat parameter space
 (or, under DDP, this rank's slice of every bucket, fused with the gradient mean over peers).  ``SGD`` is
-``torch.optim.SGD`` (fabric-cls.py's ``Args.optim = "sgd"`` branch) on the same kernels' gradient path.
+``torch.optim.SGD`` (fabric-cls.py's ``Args.optim = "sgd"`` branch) on the same kernels' gradient path, and ``Adam`` /
+``TorchAdamW`` are ``torch.optim.Adam`` / ``torch.optim.AdamW`` with ``fused=True`` (HF transformers 5.5's default).
 """
 import os
 
@@ -446,6 +447,141 @@ class SGD(_FusedOptimizer):
         return {} if buf is None else self._views(buf)
 
 
+class Adam(_FusedOptimizer):
+    """``torch.optim.Adam`` (torch 2.11: coupled or decoupled weight decay, amsgrad, maximize) as one fused update over
+    the flat parameter space, on every path AdamW runs: the eager loop, the captured steps and DDP.  The arithmetic is
+    that of ``fused=True`` (HF transformers 5.5's default ``"adamw_torch_fused"``), bit for bit on the same gradient.
+
+    The stock ``torch.optim.Adam`` / ``AdamW`` cannot train a b200 model: its gradients live in the model's bf16 bucket
+    space, not in ``.grad``.  ``foreach``, ``fused`` and ``capturable`` are accepted and ignored (the update is always
+    fused and capturable); ``differentiable=True`` raises.  The max_exp_avg_sq buffer is created by the first update
+    with ``amsgrad`` set; turning amsgrad on after an update has run raises at ``step()``."""
+    _shared_keys = ("betas", "eps", "amsgrad", "maximize", "decoupled_weight_decay")
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, *, foreach=None,
+                 maximize=False, capturable=False, differentiable=False, fused=None, decoupled_weight_decay=False):
+        # torch 2.11's checks, in its order, with its messages
+        if isinstance(lr, torch.Tensor):
+            if foreach and not capturable:
+                raise ValueError("lr as a Tensor is not supported for capturable=False and foreach=True")
+            if lr.numel() != 1:
+                raise ValueError("Tensor lr must be 1-element")
+        if not 0.0 <= lr:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if not 0.0 <= eps:
+            raise ValueError(f"Invalid epsilon value: {eps}")
+        if not 0.0 <= betas[0] < 1.0:
+            raise ValueError(f"Invalid beta parameter at index 0: {betas[0]}")
+        if not 0.0 <= betas[1] < 1.0:
+            raise ValueError(f"Invalid beta parameter at index 1: {betas[1]}")
+        if not 0.0 <= weight_decay:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        if not ((isinstance(betas[0], float) and isinstance(betas[1], float))
+                or (isinstance(betas[0], torch.Tensor) and isinstance(betas[1], torch.Tensor))):
+            raise ValueError("betas must be either both floats or both Tensors")
+        for i in (0, 1):
+            if isinstance(betas[i], torch.Tensor):
+                if not capturable and foreach:
+                    raise ValueError(f"betas[{i}] as a Tensor is not supported for capturable=False and foreach=True")
+                if betas[i].numel() != 1:
+                    raise ValueError(f"Tensor betas[{i}] must be 1-element")
+        if fused:
+            if differentiable:
+                raise RuntimeError("`fused` does not support `differentiable`")
+            if foreach:
+                raise RuntimeError("`fused` and `foreach` cannot be `True` together.")
+        if differentiable:
+            raise ValueError("differentiable=True is not supported: the update is a fused kernel outside autograd")
+        if isinstance(betas[0], torch.Tensor):
+            raise ValueError("Tensor betas are not supported: the fused update takes the betas by value")
+        defaults = dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, amsgrad=amsgrad,
+                        maximize=maximize, foreach=foreach, capturable=capturable, differentiable=differentiable,
+                        fused=fused, decoupled_weight_decay=decoupled_weight_decay)
+        super().__init__(params, defaults)
+        # torch's kernel forms the L2 term by the lane an element takes in its loop (see b2_adam_hparams_t): a tensor
+        # whose size is not a multiple of 4 goes through its unaligned loop, where element j is in lane (j % 2048) / 512
+        flags, lay = self._decay_flags_cpu, self._model._layout
+        for name, (off, shape) in lay.entries.items():
+            n = self._model._params_by_name[name].numel()
+            if n % 4:
+                j = torch.arange(0, n, 8)
+                bits = L.ADAM_DECAY_UNALIGNED + L.ADAM_DECAY_LANE0 * ((j % 2048) < 512).to(torch.uint8)
+                seg = flags[off // 8:off // 8 + len(j)]
+                seg |= seg * bits      # on decayed vectors only
+        self._updated = False    # an update has run on this state: amsgrad can no longer be turned on
+
+    def _init_state(self, st, n):
+        st["exp_avg"] = torch.zeros(n, dtype=torch.float32, device=st["dev"])
+        st["exp_avg_sq"] = torch.zeros(n, dtype=torch.float32, device=st["dev"])
+        st["max_exp_avg_sq"] = None             # created by the first update with amsgrad (see _hparams)
+        self._updated = False
+        st["prepared"] = torch.zeros(2, dtype=torch.float32, device=st["dev"])   # see b2_adam_prepare
+
+    def _prepare(self, stream):
+        """the bias corrections of the NEXT update -> device floats (read by the background kernel)"""
+        st = self._dev_state
+        L.call("b2_adam_prepare", self.hparams(), L.ptr(st["step"]), L.ptr(st["prepared"]), stream)
+
+    def captured_hparams(self):
+        """The hyperparameters a captured step bakes into its graph (all but the lr, which it reads at every replay)"""
+        return {"betas": tuple(tuple(float(b) for b in g["betas"]) for g in self.param_groups),
+                "eps": tuple(float(g["eps"]) for g in self.param_groups),
+                "weight_decay": tuple(float(g["weight_decay"]) for g in self.param_groups),
+                "amsgrad": tuple(bool(g["amsgrad"]) for g in self.param_groups),
+                "maximize": tuple(bool(g["maximize"]) for g in self.param_groups),
+                "decoupled_weight_decay": tuple(bool(g["decoupled_weight_decay"]) for g in self.param_groups)}
+
+    def _hparams(self):
+        g = self.param_groups[0]
+        st = self._dev_state
+        if g["amsgrad"] and st is not None and st["max_exp_avg_sq"] is None:
+            if self._updated:
+                # torch fails here too (a KeyError on the missing state entry)
+                raise ValueError("amsgrad was turned on after the first step: the max_exp_avg_sq buffer would start "
+                                 "from zero mid-run; build the optimizer with amsgrad=True")
+            # before any update (never inside a capture: the captured steps run eager passes first)
+            st["max_exp_avg_sq"] = torch.zeros(self._model._layout.total, dtype=torch.float32, device=st["dev"])
+            torch.cuda.current_stream(st["dev"]).synchronize()     # zeroed before another stream's update reads it
+        hp = L.AdamHParams()
+        hp.lr, hp.beta1, hp.beta2, hp.eps = float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"])
+        hp.weight_decay = float(self._wd)
+        hp.amsgrad, hp.maximize = (1 if g["amsgrad"] else 0), (1 if g["maximize"] else 0)
+        hp.decoupled = 1 if g["decoupled_weight_decay"] else 0
+        return hp
+
+    def _launch(self, st, hp, begin, end, world, rank, peer_grads, peer_shadow, stream, background):
+        flat = self._model._flat
+        vmax = st["max_exp_avg_sq"] if hp.amsgrad else None
+        self._updated = True
+        if background:
+            L.call("b2_adam_background", peer_grads[0], peer_shadow[0], L.ptr(flat), L.ptr(st["exp_avg"]),
+                   L.ptr(st["exp_avg_sq"]), L.ptr(vmax), L.ptr(st["decay"]), begin, end, hp, L.ptr(st["prepared"]),
+                   stream)
+            return
+        L.call("b2_bucket_reduce_adam", L.ptr_array(peer_grads), L.ptr_array(peer_shadow), world, rank, L.ptr(flat),
+               L.ptr(st["exp_avg"]), L.ptr(st["exp_avg_sq"]), L.ptr(vmax), L.ptr(st["decay"]), begin, end, hp,
+               L.ptr(st["step"]), stream)
+
+    moments = AdamW.moments
+
+    def max_exp_avg_sqs(self):
+        """amsgrad's fp32 max_exp_avg_sq by HF parameter name, or {} without amsgrad"""
+        buf = self._state()["max_exp_avg_sq"]
+        return {} if buf is None else self._views(buf)
+
+
+class TorchAdamW(Adam):
+    """``torch.optim.AdamW`` (torch 2.11: decoupled weight decay, default 0.01) on the fused update; see ``Adam``.
+    Exported under this name because the package's ``AdamW`` is the reference's HF AdamW, whose arithmetic differs
+    (eps before the bias correction, decay after the update)."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, amsgrad=False, *,
+                 maximize=False, foreach=None, capturable=False, differentiable=False, fused=None):
+        super().__init__(params, lr, betas, eps, weight_decay, amsgrad, foreach=foreach, maximize=maximize,
+                         capturable=capturable, differentiable=differentiable, fused=fused,
+                         decoupled_weight_decay=True)
+
+
 def clip_grad_norm_(parameters, max_norm, norm_type=2.0, error_if_nonfinite=False, foreach=None):
     """``torch.nn.utils.clip_grad_norm_`` for a b200 model: call it between ``backward()`` and ``optimizer.step()``.
 
@@ -494,12 +630,16 @@ def build_optimizer(model, args):
     containing 'bias' or 'LayerNorm.weight'; lr = args.learning_rate; HF AdamW defaults otherwise.
 
     ``args.optim = "sgd"`` (fabric-cls.py's default, :281-285) gives that script's optimizer instead:
-    ``SGD(model.parameters(), lr=args.learning_rate)``, one group, no momentum and no weight decay."""
+    ``SGD(model.parameters(), lr=args.learning_rate)``, one group, no momentum and no weight decay.
+
+    ``args.optim = "adamw_torch"`` or ``"adamw_torch_fused"`` (HF TrainingArguments' names; the second is transformers
+    5.5's default) gives ``TorchAdamW`` on the same two groups, torch's defaults otherwise (eps 1e-8)."""
     optim = getattr(args, "optim", "adamw")
     if optim == "sgd":
         return SGD(model.parameters(), lr=args.learning_rate)
-    if optim != "adamw":
-        raise ValueError("args.optim must be 'adamw' or 'sgd' (got %r)" % (optim,))
+    if optim not in ("adamw", "adamw_torch", "adamw_torch_fused"):
+        raise ValueError("args.optim must be 'adamw', 'adamw_torch', 'adamw_torch_fused' or 'sgd' (got %r)"
+                         % (optim,))
     no_decay = ['bias', 'LayerNorm.weight']
     optimizer_grouped_parameters = [
         {'params': [p for n, p in model.named_parameters() if not any(nd in n for nd in no_decay)],
@@ -507,5 +647,7 @@ def build_optimizer(model, args):
         {'params': [p for n, p in model.named_parameters() if any(nd in n for nd in no_decay)],
          'weight_decay': 0.0}
     ]
+    if optim != "adamw":
+        return TorchAdamW(optimizer_grouped_parameters, lr=args.learning_rate, weight_decay=args.weight_decay)
     optimizer = AdamW(optimizer_grouped_parameters, lr=args.learning_rate)
     return optimizer

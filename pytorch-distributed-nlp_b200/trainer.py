@@ -53,8 +53,9 @@ class Args:
                                # None: a constant lr (HF's default is "linear")
     warmup_steps = 0      # linear warmup from 0 over this many optimizer steps; when 0, ceil(warmup_ratio x total)
     warmup_ratio = 0.0
-    optim = "adamw"       # build_optimizer's optimizer: "adamw" (the reference's HF AdamW) or "sgd" (fabric-cls.py's
-                          # default: torch SGD, no momentum, no weight decay)
+    optim = "adamw"       # build_optimizer's optimizer: "adamw" (the reference's HF AdamW), "sgd" (fabric-cls.py's
+                          # default: torch SGD, no momentum, no weight decay), or "adamw_torch" / "adamw_torch_fused"
+                          # (HF's names: torch.optim.AdamW on the reference's two groups, eps 1e-8)
     log_every = 1         # the reference prints every step (forces a D2H sync per step)
     total_step = 0
 
