@@ -7,9 +7,11 @@ gradient mean over ranks during ``loss.backward()`` (Reducer, distributed.py:125
 
 Design (SURVEY.md §8e): every rank owns a contiguous 1/world slice of every bucket (embeddings | layer i | head).
 Gradients (bf16), shadow weights (bf16) and the fp32 master weights live in cudaMalloc'ed buffers that every peer maps
-through CUDA IPC; the exchange is ``b2_bucket_reduce_adamw``: read my slice from all peers over NVSwitch, mean in fp32,
-HF-AdamW on my fp32 master slice, store the new bf16 weights into every peer.  torch.distributed is used only for the
-one-time handle exchange and the initial broadcast.  ``state_dict()`` is ONE-SIDED: the calling rank pulls the fp32
+through CUDA IPC; the exchange is the optimizer's reduce-and-update kernel: read my slice from all peers over NVSwitch,
+mean in fp32, the optimizer's update on my fp32 master slice, store the new bf16 weights into every peer.  When which
+bucket is exchanged is the optimizer's step schedule (optim._FusedOptimizer); the wrapper is its transport for world > 1
+and answers what modeling._LocalTransport answers on one GPU.  torch.distributed is used only for the one-time handle
+exchange and the initial broadcast.  ``state_dict()`` is ONE-SIDED: the calling rank pulls the fp32
 slices it does not own out of their owners' HBM with copy-engine peer copies, so the reference's
 ``if local_rank == 0: torch.save(model.state_dict())`` (:190-197) works without the other ranks taking part.
 """
@@ -145,8 +147,7 @@ class DistributedDataParallel(nn.Module):
         self.dma = False
         self.comm = None
         self._master_stale = False
-        self._side = None
-        self._pending = None
+        self.side = None
         self._closed = False
         self._gather_calls = 0
         self._gather_cap = 0
@@ -169,10 +170,10 @@ class DistributedDataParallel(nn.Module):
             module._rebind_flat(self.comm.alloc("master", 4 * n).tensor(torch.float32, eng.dev))
             eng.refresh_shadow()
             self._slices = self._make_slices()
-            # staging for the DMA form of the exchange: my slice of every bucket as held by each peer
-            # transport form of the exchange: the fused peer-HBM kernel (default) or copy-engine DMA + local reduce.
-            # With the step body on a high-priority stream the exchange kernels do not hold SMs the GEMM chain is
-            # waiting for, which favours the kernel form; B2_DDP_DMA=1 selects the copy-engine form (A/B switch)
+            # form of the exchange: the fused peer-HBM kernel (default) or copy-engine DMA + local reduce.  With the
+            # step body on a high-priority stream the exchange kernels do not hold SMs the GEMM chain is waiting for,
+            # which favours the kernel form; B2_DDP_DMA=1 selects the copy-engine form (A/B switch).  _stage is the
+            # DMA form's staging: my slice of every bucket as held by each peer
             self.dma = os.environ.get("B2_DDP_DMA", "0") == "1"
             self._stage_off, off = [], 0
             for (sb, se) in self._slices:
@@ -183,7 +184,7 @@ class DistributedDataParallel(nn.Module):
                         off += (2 * (se - sb) + 255) // 256 * 256
                 self._stage_off.append(row)
             self._stage = torch.empty(max(off, 256), dtype=torch.uint8, device=eng.dev)
-            self._side = torch.cuda.Stream(device=eng.dev)
+            self.side = torch.cuda.Stream(device=eng.dev)      # runs the per-bucket work of an armed step
             self._grow_gather(_GATHER_SLOT_BYTES)
             torch.cuda.synchronize(eng.dev)
             dist.barrier(group=process_group)
@@ -266,41 +267,32 @@ class DistributedDataParallel(nn.Module):
         except Exception:
             pass
 
-    # ---- hooks called by the engine during backward (autograd thread) -----------------------------------------------
-    def _bucket_ready(self, idx, wg_event=None):
-        """Bucket `idx` holds this rank's final local gradients once the main stream reaches this point and `wg_event`
-        (the weight-gradient stream's marker for the layer) has fired.  With an optimizer attached and overlap on,
-        start its exchange + update on the side stream right away so it hides behind the rest of backward.  Only the
-        SIDE stream waits for the weight gradients: the main stream's dgrad chain never parks behind them."""
-        opt = self.module._optimizer
-        if self.world == 1 or not self.overlap or opt is None or not getattr(opt, "_armed", False):
-            return
-        eng = self.module._engine
-        main = torch.cuda.current_stream(eng.dev)
-        ev = torch.cuda.Event()
-        ev.record(main)
-        self._side.wait_event(ev)
-        if wg_event is not None:
-            self._side.wait_event(wg_event)
-        s = self._side.cuda_stream
-        op = eng._pass_op
-        if op is not None:
-            # gradient accumulation, on the local gradients of the whole bucket: an accumulating pass stops here (no
-            # barrier, no exchange); the final pass folds BEFORE the barrier, so peers read the window's sum
-            b, e, _label = self.module._layout.buckets[idx]
-            eng.accumulate_range(b, e, op, s)
-            if op != L.ACCUM_FOLD:
-                return
-        self.comm.barrier(_SLOT_BUCKET0 + idx, s)
-        if opt._clip is not None:
-            opt._clip_reduce(idx, self._grad_sources(idx, s), s)   # a clipped step: the update waits for the norm
-        else:
-            self._exchange_update(opt, idx, s)
-        if self._pending is None:
-            self._pending = set()
-        self._pending.add(idx)
+    # ---- what the optimizer's step schedule asks of its transport (modeling._LocalTransport is the one-GPU form); world,
+    # rank, overlap and side are set by the constructor --------------------------------------------------------------
+    background = False           # every update is the reduce form
+    # when backward updated every bucket, the closing barrier and the step counter follow on the side stream and step()
+    # joins once, after them; that join also covers the weight-gradient stream, which the side stream waited for
+    tail_on_side = True
+    side_carries_wgrad = True
 
-    def _grad_sources(self, idx, s):
+    def slice(self, idx):
+        return self._slices[idx]
+
+    def barrier(self, slot, stream):
+        self.comm.barrier(slot, stream)
+
+    def norm_exchange(self):
+        return (L.ptr_array(self.comm.peers["scalar_clip"]), L.ptr_array(self.comm.peers["flags"]), _SLOT_CLIP,
+                self.comm.epoch_ptr(_SLOT_CLIP))
+
+    def update(self, opt, buckets, stream, background=False):
+        for idx in buckets:
+            self._exchange_update(opt, idx, stream)
+
+    def stepped(self):
+        self._master_stale = True
+
+    def grad_sources(self, idx, s):
         """every rank's bf16 gradients of my slice of bucket `idx`, as the reduce kernels read them: the peers' mapped
         buffers (kernel form), or in the DMA form local staging copies filled by copy-engine transfers on `s`"""
         sb, se = self._slices[idx]
@@ -318,31 +310,28 @@ class DistributedDataParallel(nn.Module):
         return g_ptrs
 
     def _exchange_update(self, opt, idx, s):
-        """Mean over ranks + HF-AdamW on my slice of bucket `idx` + delivery of the new bf16 weights to every rank.
+        """Mean over ranks + the update of my slice of bucket `idx` + delivery of the new bf16 weights to every rank.
         Kernel form (default): the reduce kernel loads the peers' slices / stores the peers' shadows itself through the
         mapped pointers -- one launch per bucket does the one-shot peer-HBM reduction, the fp32 cast, the partitioned
-        AdamW and the delivery of the new weights.  DMA form (B2_DDP_DMA=1, every bucket but the last one produced):
+        update and the delivery of the new weights.  DMA form (B2_DDP_DMA=1, every bucket but the last one produced):
         the transfers are copy-engine copies over NVLink and the reduce kernel works on local memory only.  In a
         clipped step the mean is already in the clip stash (the reduce phase made it): no peer gradient is read."""
         sb, se = self._slices[idx]
         if se <= sb:
             return
         peers_g, peers_s = self.comm.peers["grads"], self.comm.peers["shadow"]
-        stash = opt._clip_stash_ptr(idx) if opt._clip is not None else None
+        stash = opt.clip_stash(idx)
         if not self.dma or idx == 0:
             opt.update_range(sb, se, self.world, self.rank, peers_g, peers_s, s, grad_f32=stash)
             return
         nbytes = 2 * (se - sb)
-        g_ptrs = list(peers_g) if stash is not None else self._grad_sources(idx, s)
+        g_ptrs = list(peers_g) if stash is not None else self.grad_sources(idx, s)
         s_ptrs = [peers_s[r] if r == self.rank else None for r in range(self.world)]
         opt.update_range(sb, se, self.world, self.rank, g_ptrs, s_ptrs, s, grad_f32=stash)
         mine = peers_s[self.rank] + 2 * sb
         for r in range(self.world):
             if r != self.rank:
                 L.call("b2_copy_async", peers_s[r] + 2 * sb, mine, nbytes, s)
-
-    def _on_backward_done(self):
-        pass
 
     def consensus_probe(self, probe):
         """GradScaler inf check under DDP (multi-gpu-distributed-mp-amp-cls.py:166-171): stock DDP all-reduces the
@@ -358,58 +347,6 @@ class DistributedDataParallel(nn.Module):
                L.ptr_array(self.comm.peers["flags"]), self.world, self.rank, _SLOT_INF,
                self.comm.epoch_ptr(_SLOT_INF), eng.stream())
         return torch.where(dst > 0, torch.full_like(probe, float("inf")), probe)
-
-    def _optimizer_step(self, opt):
-        """world > 1 body of ``optimizer.step()``."""
-        eng = self.module._engine
-        main = torch.cuda.current_stream(eng.dev)
-        nb = len(self.module._layout.buckets)
-        done = self._pending or set()
-        if opt._clip is not None:
-            # a clipped step: the hooks (or clip_grad_norm_) ran the reduce phase; the finalize and every update follow
-            if done:
-                ev = torch.cuda.Event()
-                ev.record(self._side)
-                main.wait_event(ev)
-            s = main.cuda_stream
-            opt._clip_before_update(s)
-            for idx in range(nb):
-                self._exchange_update(opt, idx, s)
-            self.comm.barrier(_SLOT_UPDATE_DONE, s)
-            opt.advance(s)
-        elif len(done) == nb:
-            # everything was launched from the backward hooks: just join
-            s = self._side.cuda_stream
-            self.comm.barrier(_SLOT_UPDATE_DONE, s)
-            opt.advance(s)
-            ev = torch.cuda.Event()
-            ev.record(self._side)
-            main.wait_event(ev)
-        else:
-            if done:
-                ev = torch.cuda.Event()
-                ev.record(self._side)
-                main.wait_event(ev)
-            s = main.cuda_stream
-            self.comm.barrier(_SLOT_GRADS_READY, s)
-            for idx in range(nb):
-                if idx in done:
-                    continue
-                self._exchange_update(opt, idx, s)
-            self.comm.barrier(_SLOT_UPDATE_DONE, s)
-            opt.advance(s)
-        self._pending = None
-        self._master_stale = True
-
-    def _clip_reduce_rest(self, opt, s):
-        """the reduce phase, on `s`, of every bucket no backward hook has reduced, behind the barrier that makes every
-        rank's gradients final"""
-        todo = [idx for idx in range(len(self.module._layout.buckets)) if idx not in opt._clip["reduced"]]
-        if not todo:
-            return
-        self.comm.barrier(_SLOT_GRADS_READY, s)
-        for idx in todo:
-            opt._clip_reduce(idx, self._grad_sources(idx, s), s)
 
     def _gather_master(self):
         """fp32 masters are updated slice-wise by their owner ranks.  Re-assemble them on THIS rank by pulling every

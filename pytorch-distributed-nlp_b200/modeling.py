@@ -224,7 +224,6 @@ class _StepFn(torch.autograd.Function):
         eng.start_pass(accumulate)
         eng.backward(d_logits, d_loss if ctx.has_loss else None)
         eng.end_pass()
-        model._notify_backward_done()
         # Gradients live in the engine's bf16 bucket space, not in `.grad`.  The anchor (classifier.bias) gets its
         # true gradient as a 6-float fp32 probe: it is the column sum of d_logits, so an inf/nan anywhere upstream
         # of the model shows up in it -- which is what torch.cuda.amp.GradScaler's inf check needs to see.  Autograd
@@ -451,10 +450,6 @@ class BertForSequenceClassification(nn.Module):
             self._pt_loss = (pt, problem_type_loss(pt, self.num_labels))
         return self._pt_loss[1]
 
-    def _notify_backward_done(self):
-        if self._ddp is not None:
-            self._ddp._on_backward_done()
-
     # ---- test / tooling helpers -----------------------------------------------------------------------------------------
     def grad_dict(self):
         """fp32 copies of what the next optimizer.step() would apply, keyed by HF parameter name: the (bf16) gradients of
@@ -467,6 +462,56 @@ class BertForSequenceClassification(nn.Module):
             off, shape = self._layout.entries[name]
             out[name] = g[off:off + p.numel()].view(shape).to(torch.float32, copy=True)
         return out
+
+
+class _LocalTransport:
+    """The facts the optimizer's step schedule (optim._FusedOptimizer: bucket_ready, step, the clip phases) needs about
+    where gradients and weights live, on one GPU.  DistributedDataParallel answers the same questions for a peer group
+    (world > 1).  A transport holds no policy: it never looks at accumulation, clipping or which buckets are done."""
+    world, rank = 1, 0
+    background = True            # an update launched under the backward takes the slim kernel form (and its prepare)
+    tail_on_side = False         # step() joins the side stream first; the step counter advances on the main stream
+    # the backward joins the weight-gradient stream itself at its end.  (It could leave that to the side stream, as
+    # the peer path does; that reorders the captured step and is a change to measure on its own.)
+    side_carries_wgrad = False
+
+    def __init__(self, eng):
+        self.eng = eng
+        self.side = torch.cuda.Stream(device=eng.dev)      # runs the per-bucket work of an armed step
+
+    @property
+    def overlap(self):
+        """may bucket_ready run during backward?  Not under a world-1 DistributedDataParallel wrapper: it keeps the
+        whole-range accumulate and update after backward.  (A missed optimisation, kept as it is: lifting it changes
+        that configuration's launch order and speed.)"""
+        return self.eng.model._ddp is None
+
+    def slice(self, idx):
+        """the elements of bucket `idx` this rank reduces and updates"""
+        b, e, _label = self.eng.lay.buckets[idx]
+        return b, e
+
+    def grad_sources(self, idx, stream):
+        """every rank's bf16 gradient buffer, as the reduce kernels index them"""
+        return [self.eng.grads.data_ptr()]
+
+    def barrier(self, slot, stream):
+        pass
+
+    def norm_exchange(self):
+        """(scratch, flags, slot, epoch) of the scalar exchange in the norm finalize"""
+        return None, None, 0, None
+
+    def update(self, opt, buckets, stream, background=False):
+        eng = self.eng
+        # the buckets tile the flat space: all of them are one launch
+        whole = len(buckets) == len(eng.lay.buckets)
+        for b, e in [(0, eng.lay.total)] if whole else [self.slice(idx) for idx in buckets]:
+            opt.update_range(b, e, 1, 0, [eng.grads.data_ptr()], [eng.shadow.data_ptr()], stream,
+                             background=background)
+
+    def stepped(self):
+        pass
 
 
 class _Engine:
@@ -495,7 +540,7 @@ class _Engine:
         self._ws = {}
         self._saved = None
         self.wgrad_stream = torch.cuda.Stream(device=self.dev)
-        self.opt_stream = torch.cuda.Stream(device=self.dev)
+        self._local = _LocalTransport(self)
         # gradient accumulation (no_sync(), Trainer gradient_accumulation_steps): fp32 accumulator over the flat space,
         # allocated on first use (local even under DDP); accum_in_use = some backward has accumulated into it;
         # accum_live = the accumulator holds gradients no fold / flush has consumed yet; _pass_op = the
@@ -541,6 +586,12 @@ class _Engine:
     # ---- plumbing ----
     def stream(self):
         return torch.cuda.current_stream(self.dev).cuda_stream
+
+    @property
+    def transport(self):
+        """whom the optimizer's step schedule asks about ranges, streams and peers"""
+        ddp = self.model._ddp
+        return ddp if ddp is not None and ddp.world > 1 else self._local
 
     def rebind(self, shadow, grads):
         """DDP moves the exchanged buffers into IPC-shared allocations."""
@@ -834,7 +885,6 @@ class _Engine:
         w, g = self.w, self.g
         KM, MN = L.MAJOR_K, L.MAJOR_MN
         scratch, scratch_bytes = self.partials.data_ptr(), self.partials.numel()
-        hooks = self.model._ddp
 
         # embedding-table gradients are scatter targets: clear the whole bucket (word rows not in the batch, unused
         # position rows and padding must read as zero for the dense DDP/AdamW pass, like the reference's dense grads)
@@ -864,45 +914,17 @@ class _Engine:
         ss = side.cuda_stream
         done = {}
 
-        opt = self.model._optimizer
-        overlap_opt = hooks is None and opt is not None and getattr(opt, "_armed", False)
-        # Under an armed DDP exchange the side stream takes the weight-gradient dependencies bucket by bucket
-        # (ddp._bucket_ready) and optimizer.step() joins it
-        ddp_overlap = (hooks is not None and hooks.world > 1 and hooks.overlap and opt is not None and
-                       getattr(opt, "_armed", False))
-        # an accumulating / folding backward: per bucket on the stream that runs the update (armed), else one
-        # whole-range launch in end_pass()
-        if self._pass_op is not None and (overlap_opt or ddp_overlap):
-            self._pass_stream = hooks._side if ddp_overlap else self.opt_stream
+        # An armed step (a captured train step owns backward + optimizer) runs each bucket's share of the optimizer
+        # step on the transport's side stream as soon as the bucket's gradients are final: opt.bucket_ready
+        opt, transport = self.model._optimizer, self.transport
+        per_bucket = opt is not None and opt._armed and transport.overlap
+        # an accumulating / folding backward: per bucket on that stream too, else one whole-range launch in end_pass()
+        if self._pass_op is not None and per_bucket:
+            self._pass_stream = transport.side
 
         def bucket_ready(idx, wg_event=None):
-            """bucket `idx` holds its final gradients once the main stream reaches this point (and `wg_event`,
-            the weight-gradient stream's marker for the layer, has fired)"""
-            if hooks is not None:
-                hooks._bucket_ready(idx, wg_event)
-            elif overlap_opt:
-                # single GPU: the HBM-bound AdamW of this bucket runs on its own stream under the rest of backward
-                ev = torch.cuda.Event()
-                ev.record(main)
-                self.opt_stream.wait_event(ev)
-                if wg_event is not None:
-                    self.opt_stream.wait_event(wg_event)
-                b0, e0, _lbl = self.lay.buckets[idx]
-                os_ = self.opt_stream.cuda_stream
-                if self._pass_op is not None:
-                    self.accumulate_range(b0, e0, self._pass_op, os_)
-                    if self._pass_op != L.ACCUM_FOLD:
-                        return      # an accumulating pass: no update
-                if opt._clip is not None:
-                    # a clipped step: only the reduce phase hides under the backward; no bucket may move before the
-                    # norm of the whole gradient is known (optimizer.step() finalizes and updates)
-                    opt._clip_reduce(idx, [self.grads.data_ptr()], os_)
-                else:
-                    if not opt._pending:
-                        opt.prepare_background(os_)      # the step size of this step's lr
-                    opt.update_range(b0, e0, 1, 0, [self.grads.data_ptr()], [self.shadow.data_ptr()], os_,
-                                     background=(idx != 0))
-                opt._pending.add(idx)
+            if per_bucket:
+                opt.bucket_ready(idx, wg_event)
 
         if not self.lay.head_in_last_layer:
             bucket_ready(len(self.lay.buckets) - 1)     # (a model without encoder layers: the head is its own bucket)
@@ -991,9 +1013,9 @@ class _Engine:
         else:
             L.call("b2_embed_bwd_packed", *emb_in, ws["pos32"].data_ptr(), *emb_tail)
         # Whoever consumes the gradients next on the main stream (optimizer.step, grad_dict) must see the weight-gradient
-        # stream's work.  Under an armed DDP exchange optimizer.step() (or end_pass) joins the side stream, which has
-        # taken those dependencies; in every other case join here.
-        if not ddp_overlap:
+        # stream's work.  Where the per-bucket side stream has taken those dependencies, optimizer.step() (or
+        # end_pass) joins it; in every other case join here.
+        if not (per_bucket and transport.side_carries_wgrad):
             for l in sorted(done)[:2]:       # the last two layers processed (0 and 1) may still be in flight
                 main.wait_event(done[l])
         bucket_ready(0)

@@ -14,12 +14,16 @@ import os
 import torch
 
 from . import _lib as L
+from .ddp import _SLOT_BUCKET0, _SLOT_GRADS_READY, _SLOT_UPDATE_DONE
 
 
 class _FusedOptimizer(torch.optim.Optimizer):
-    """What every optimizer of a b200 model does around its update kernels: the device state, the GradScaler hooks,
-    gradient clipping, the per-bucket launches the backward and DDP make (update_range / prepare_background / advance)
-    and ``step()``.  A subclass supplies its hyperparameter struct, its state buffers and its two kernel forms."""
+    """What every optimizer of a b200 model does around its update kernels: the device state, the GradScaler hooks and
+    the schedule of one optimizer step -- in which order, on which stream and over which element ranges accumulate,
+    clip-reduce, update, barrier and advance run (``bucket_ready`` during backward, ``step()`` after it, the clip
+    phases).  The schedule is written once; what differs between one GPU and a peer group it asks of the engine's
+    transport (see modeling._LocalTransport).  A subclass supplies its hyperparameter struct, its state buffers and its
+    two kernel forms."""
     # torch.cuda.amp.GradScaler contract for optimizers that unscale themselves (torch/amp/grad_scaler.py `step`):
     # the scaler sets `self.grad_scale` (device fp32 scalar) / `self.found_inf` around step() instead of walking
     # `.grad` tensors -- which do not exist here (gradients live in the bf16 bucket space).  This is what lets the
@@ -61,10 +65,12 @@ class _FusedOptimizer(torch.optim.Optimizer):
                              % (len(covered), len(lay.entries)))
         self._decay_flags_cpu = flags
         self._dev_state = None
-        self._armed = False      # set by FusedTrainStep: per-bucket updates may start during backward
-        self._pending = set()    # buckets already updated (on the engine's optimizer stream) in this step
-        # gradient clipping: _clip = the clipped step in progress (None: the next step does not clip), _clip_buf = its
-        # device buffers, kept across steps (captured graphs replay on them)
+        # the step schedule's state.  _armed: set by a captured train step, bucket_ready may run during backward;
+        # _pending: the buckets bucket_ready has already handled in this step (updated, or in a clipped step reduced)
+        # on the transport's side stream; _clip = the clipped step in progress (None: the next step does not clip),
+        # _clip_buf = its device buffers, kept across steps (captured graphs replay on them)
+        self._armed = False
+        self._pending = set()
         self._clip = None
         self._clip_buf = None
         # set by a captured train step for the duration of its body: the kernels read the lr from the device scalar
@@ -169,26 +175,87 @@ class _FusedOptimizer(torch.optim.Optimizer):
         L.call("b2_step_advance", L.ptr(st["step"]), L.ptr(self._model._engine.rng), self._found_inf_ptr(), stream)
         self._prepare(stream)
 
-    # -- gradient-norm clipping: reduce (+ partial sums of squares) per bucket, one norm, then the update -----------------
-    def _clip_ranges(self):
-        """(world, rank, [(begin, end)] per bucket): the bucket slices this rank reduces and updates"""
-        ddp = self._model._ddp
-        if ddp is not None and ddp.world > 1:
-            return ddp.world, ddp.rank, list(ddp._slices)
-        return 1, 0, [(b, e) for (b, e, _label) in self._model._layout.buckets]
+    # -- the schedule of one optimizer step ----------------------------------------------------------------------------
+    def _transport(self):
+        return self._model._engine.transport
 
+    def bucket_ready(self, idx, wg_event=None):
+        """Called by the backward of an armed step: bucket `idx` holds this rank's final local gradients once the main
+        stream reaches this point and `wg_event` (the weight-gradient stream's marker for the layer) has fired.  Its
+        share of the step starts on the transport's side stream right away, so it hides behind the rest of backward.
+        Only the SIDE stream waits for the weight gradients: the main stream's dgrad chain never parks behind them."""
+        eng, t = self._model._engine, self._transport()
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(eng.dev))
+        t.side.wait_event(ev)
+        if wg_event is not None:
+            t.side.wait_event(wg_event)
+        s = t.side.cuda_stream
+        op = eng._pass_op
+        if op is not None:
+            # gradient accumulation, on the local gradients of the whole bucket: an accumulating pass stops here (no
+            # barrier, no exchange, no update); the final pass folds BEFORE the barrier, so peers read the window's sum
+            b, e, _label = self._model._layout.buckets[idx]
+            eng.accumulate_range(b, e, op, s)
+            if op != L.ACCUM_FOLD:
+                return
+        t.barrier(_SLOT_BUCKET0 + idx, s)
+        if self._clip is not None:
+            # a clipped step: only the reduce phase hides under the backward; no bucket may move before the norm of
+            # the whole gradient is known (step() finalizes and updates)
+            self._clip_reduce(idx, s)
+        else:
+            if t.background and not self._pending:
+                self.prepare_background(s)      # the slim form reads the prepared values: those of this step's lr
+            # with nothing left to hide behind (bucket 0, the last one produced) the full-size kernel is the faster one
+            t.update(self, [idx], s, background=t.background and idx != 0)
+        self._pending.add(idx)
+
+    def _finish_step(self):
+        """What step() still has to do after the backward: the clip's remaining reduces and its norm, the update of
+        every bucket bucket_ready did not update, the step counter; with the side stream joined wherever it worked."""
+        eng, t = self._model._engine, self._transport()
+        main = torch.cuda.current_stream(eng.dev)
+        buckets = range(len(self._model._layout.buckets))
+        todo = [idx for idx in buckets if self._clip is not None or idx not in self._pending]
+        # nothing left but the closing barrier and the counter: they may stay behind the updates on the side stream
+        on_side = t.tail_on_side and not todo
+        if self._pending and not on_side:
+            main.wait_stream(t.side)
+        s = (t.side if on_side else main).cuda_stream
+        if self._clip is not None:
+            # the reduce phase of every bucket neither bucket_ready nor clip_grad_norm_ has reduced, then the finalize
+            # -- again when a GradScaler hands over its scale, since the norm clip_grad_norm_ returned was that of the
+            # scaled gradients
+            self._clip_reduce_rest(s)
+            if not self._clip["final"] or getattr(self, "grad_scale", None) is not None:
+                self._clip_finalize(s)
+        elif todo:
+            t.barrier(_SLOT_GRADS_READY, s)
+        if todo:
+            t.update(self, todo, s)
+        t.barrier(_SLOT_UPDATE_DONE, s)
+        self.advance(s)
+        if on_side:
+            main.wait_stream(t.side)
+        self._pending = set()
+        t.stepped()
+
+    # -- gradient-norm clipping: reduce (+ partial sums of squares) per bucket, one norm, then the update -----------------
     def _clip_arm(self, max_norm):
         """Starts a clipped step: from here until step() no bucket is updated before the norm of the whole gradient is
-        known.  The device buffers (and, under DDP, the fp32 stash of this rank's slices) are allocated on first use."""
+        known.  The device buffers (and, in a peer group, the fp32 stash of this rank's slices) are allocated on first
+        use."""
         if self._clip is not None:
             raise RuntimeError("clip_grad_norm_() called twice before optimizer.step(): the gradients of this step are "
                                "already clipped")
         max_norm = float(max_norm)
         if not max_norm > 0.0:
             raise ValueError("max_norm must be positive (got %r)" % max_norm)
-        world, rank, ranges = self._clip_ranges()
+        t = self._transport()
+        ranges = [t.slice(idx) for idx in range(len(self._model._layout.buckets))]
         dev = self._model._engine.dev
-        key = (world, rank, tuple(ranges), dev)
+        key = (t.world, t.rank, tuple(ranges), dev)
         if self._clip_buf is None or self._clip_buf["key"] != key:
             slot_off, stash_off, ns, nst = [], [], 0, 0
             for (b, e) in ranges:
@@ -200,70 +267,60 @@ class _FusedOptimizer(torch.optim.Optimizer):
             self._clip_buf = {
                 "key": key, "ranges": ranges, "slot_off": slot_off, "stash_off": stash_off, "nslots": ns,
                 "partials": torch.zeros(max(ns, 1), dtype=torch.float64, device=dev),
-                "stash": torch.empty(max(nst, 8), **f32) if world > 1 else None,   # 4 B x total / world
+                "stash": torch.empty(max(nst, 8), **f32) if t.world > 1 else None,   # 4 B x total / world
                 "norm": torch.zeros((), **f32), "coef": torch.ones((), **f32), "skip": torch.zeros((), **f32),
             }
         self._clip = {"max_norm": max_norm, "reduced": set(), "final": False}
 
-    def _clip_stash_ptr(self, idx):
+    def clip_stash(self, idx):
+        """in a clipped step of a peer group: the fp32 mean gradient of this rank's slice of bucket `idx`, which the
+        reduce phase left for the update to read; else None"""
         buf = self._clip_buf
-        return None if buf["stash"] is None else buf["stash"].data_ptr() + 4 * buf["stash_off"][idx]
+        if self._clip is None or buf["stash"] is None:
+            return None
+        return buf["stash"].data_ptr() + 4 * buf["stash_off"][idx]
 
-    def _clip_reduce(self, idx, peer_grads, stream):
-        """reduce phase of bucket `idx`: this rank's slice, read from `peer_grads` (one per rank)"""
+    def _clip_reduce(self, idx, stream):
+        """reduce phase of bucket `idx`: the mean over ranks of this rank's slice and its partial sums of squares"""
         buf = self._clip_buf
         b, e = buf["ranges"][idx]
         if e > b:
-            L.call("b2_grad_reduce_sumsq", L.ptr_array(peer_grads), len(peer_grads), self._clip_stash_ptr(idx), b, e,
+            sources = self._transport().grad_sources(idx, stream)
+            L.call("b2_grad_reduce_sumsq", L.ptr_array(sources), len(sources), self.clip_stash(idx), b, e,
                    buf["partials"].data_ptr() + 8 * buf["slot_off"][idx], stream)
         self._clip["reduced"].add(idx)
 
+    def _clip_reduce_rest(self, stream):
+        """the reduce phase of every bucket not reduced yet, behind the barrier that makes every rank's gradients final"""
+        todo = [idx for idx in range(len(self._clip_buf["ranges"])) if idx not in self._clip["reduced"]]
+        if todo:
+            self._transport().barrier(_SLOT_GRADS_READY, stream)
+        for idx in todo:
+            self._clip_reduce(idx, stream)
+
     def _clip_finalize(self, stream):
-        """the norm and the coefficient (collective under DDP).  Inside a GradScaler step it divides by the scale, so the
-        norm is that of the unscaled gradients, and a non-finite norm skips the step like GradScaler's inf check."""
-        buf, world, rank = self._clip_buf, 1, 0
-        scratch = flags = epoch = None
-        slot = 0
-        ddp = self._model._ddp
-        if ddp is not None and ddp.world > 1:
-            from .ddp import _SLOT_CLIP
-            world, rank, slot = ddp.world, ddp.rank, _SLOT_CLIP
-            scratch = L.ptr_array(ddp.comm.peers["scalar_clip"])
-            flags = L.ptr_array(ddp.comm.peers["flags"])
-            epoch = ddp.comm.epoch_ptr(_SLOT_CLIP)
+        """the norm and the coefficient (collective in a peer group).  Inside a GradScaler step it divides by the scale, so
+        the norm is that of the unscaled gradients, and a non-finite norm skips the step like GradScaler's inf check."""
+        buf, t = self._clip_buf, self._transport()
+        scratch, flags, slot, epoch = t.norm_exchange()
         gs = getattr(self, "grad_scale", None)
-        L.call("b2_grad_norm_finalize", buf["partials"].data_ptr(), buf["nslots"], scratch, flags, world, rank, slot,
+        L.call("b2_grad_norm_finalize", buf["partials"].data_ptr(), buf["nslots"], scratch, flags, t.world, t.rank, slot,
                epoch, self._clip["max_norm"], L.ptr(gs), self._scaler_found_inf_ptr(), buf["norm"].data_ptr(),
                buf["coef"].data_ptr(), buf["skip"].data_ptr(), stream)
         self._clip["final"] = True
 
-    def _clip_before_update(self, stream):
-        """in step(): the reduce phase of every bucket no backward hook has reduced, then the finalize -- again when a
-        GradScaler hands over its scale, since the norm clip_grad_norm_ returned was that of the scaled gradients"""
-        ddp = self._model._ddp
-        if ddp is not None and ddp.world > 1:
-            ddp._clip_reduce_rest(self, stream)
-        else:
-            eng = self._model._engine
-            for idx in range(len(self._model._layout.buckets)):
-                if idx not in self._clip["reduced"]:
-                    self._clip_reduce(idx, [eng.grads.data_ptr()], stream)
-        if not self._clip["final"] or getattr(self, "grad_scale", None) is not None:
-            self._clip_finalize(stream)
-
     def clip_now(self, max_norm):
         """The eager clip_grad_norm_: flush an open accumulation window, reduce every bucket, finalize; step() then runs
         the update with the coefficient.  Returns the device norm buffer."""
-        model = self._model
-        eng = model._engine
-        ddp = model._ddp
-        if self._pending or (ddp is not None and ddp._pending):
+        eng = self._model._engine
+        if self._pending:
             raise RuntimeError("clip_grad_norm_(): this step's update already ran during backward (the optimizer is "
                                "armed by a FusedTrainStep); clip through the captured step's max_grad_norm instead")
         s = torch.cuda.current_stream(eng.dev).cuda_stream
         eng.flush_accum(s)
         self._clip_arm(max_norm)
-        self._clip_before_update(s)
+        self._clip_reduce_rest(s)
+        self._clip_finalize(s)
         return self._clip_buf["norm"]
 
     @torch.no_grad()
@@ -276,27 +333,7 @@ class _FusedOptimizer(torch.optim.Optimizer):
             raise RuntimeError("optimizer.step(): the model is not on CUDA")
         # every pass of an accumulation window ran inside no_sync(): apply the accumulator (torch applies its .grad)
         eng.flush_accum(torch.cuda.current_stream(eng.dev).cuda_stream)
-        if model._ddp is not None and model._ddp.world > 1:
-            model._ddp._optimizer_step(self)
-        else:
-            main = torch.cuda.current_stream(eng.dev)
-            s = main.cuda_stream
-            if self._pending:
-                ev = torch.cuda.Event()
-                ev.record(eng.opt_stream)
-                main.wait_event(ev)
-            if self._clip is not None:
-                # the per-bucket launches of the backward were the reduce phase only
-                self._clip_before_update(s)
-                self.update_range(0, model._layout.total, 1, 0, [eng.grads.data_ptr()], [eng.shadow.data_ptr()], s)
-            elif len(self._pending) == 0:
-                self.update_range(0, model._layout.total, 1, 0, [eng.grads.data_ptr()], [eng.shadow.data_ptr()], s)
-            else:
-                for idx, (b0, e0, _lbl) in enumerate(model._layout.buckets):
-                    if idx not in self._pending:
-                        self.update_range(b0, e0, 1, 0, [eng.grads.data_ptr()], [eng.shadow.data_ptr()], s)
-            self._pending = set()
-            self.advance(s)
+        self._finish_step()
         self._clip = None
         model._grads_live = False
         # the inf-check probe has served its purpose (GradScaler reads it before calling step); the -amp scripts never

@@ -254,8 +254,8 @@ class _StagedGraphStep:
         # replays at the lr current when the step was built (or last staged)
         self._stage_lr()
         self._d_stage_all[-1:].copy_(self._h_stage_all[-1:])
-        # the fused step owns backward + optimizer: per-bucket AdamW (and, under DDP, the peer exchange) may start
-        # while backward is still running
+        # the fused step owns backward + optimizer: each bucket's update (in a peer group, its exchange) may start
+        # while backward is still running (optimizer.bucket_ready)
         optimizer._armed = True
 
     def _train_body(self, forward):
@@ -306,7 +306,6 @@ class FusedTrainStep(_StagedGraphStep):
                  criterion=None):
         super().__init__(model, batch_size, seq_len, use_graph, criterion)
         self._arm(optimizer, accum_steps, max_grad_norm)
-        self.kernel_launches = None
 
     # the step body, expressed only with stream-ordered work (capturable)
     def _body(self):
