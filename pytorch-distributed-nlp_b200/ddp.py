@@ -13,7 +13,8 @@ bucket is exchanged is the optimizer's step schedule (optim._FusedOptimizer); th
 and answers what modeling._LocalTransport answers on one GPU.  torch.distributed is used only for the one-time handle
 exchange and the initial broadcast.  ``state_dict()`` is ONE-SIDED: the calling rank pulls the fp32
 slices it does not own out of their owners' HBM with copy-engine peer copies, so the reference's
-``if local_rank == 0: torch.save(model.state_dict())`` (:190-197) works without the other ranks taking part.
+``if local_rank == 0: torch.save(model.state_dict())`` (:190-197) works without the other ranks taking part.  The
+optimizer's state buffers are peer-visible too, and its ``state_dict()`` is one-sided in the same way.
 """
 import os
 
@@ -169,6 +170,10 @@ class DistributedDataParallel(nn.Module):
             # fp32 masters move into a peer-visible buffer too: state_dict() pulls foreign slices one-sidedly
             module._rebind_flat(self.comm.alloc("master", 4 * n).tensor(torch.float32, eng.dev))
             eng.refresh_shadow()
+            # ... and so does the state of every existing optimizer (one built later allocates it so in its constructor);
+            # in creation order, which is the same on every rank, as each allocation is collective
+            for opt in sorted(module._optimizers, key=lambda o: o._uid):
+                opt._share_state()
             self._slices = self._make_slices()
             # form of the exchange: the fused peer-HBM kernel (default) or copy-engine DMA + local reduce.  With the
             # step body on a high-priority stream the exchange kernels do not hold SMs the GEMM chain is waiting for,
@@ -253,6 +258,8 @@ class DistributedDataParallel(nn.Module):
         eng = module._engine
         if eng is not None and self.comm is not None and "shadow" in self.comm.local:
             self._gather_master()
+            for opt in list(module._optimizers):
+                opt._unshare_state()
             module._rebind_flat(torch.empty_like(module._flat))
             eng.rebind(torch.empty_like(eng.shadow), torch.empty_like(eng.grads))
             torch.cuda.synchronize(eng.dev)
@@ -356,18 +363,21 @@ class DistributedDataParallel(nn.Module):
         barriers -- so between steps the peers' masters are quiescent."""
         if self.world == 1 or not self._master_stale or self.comm is None:
             return
-        eng = self.module._engine
-        s = eng.stream()
-        flat = self.module._flat
-        peers_m = self.comm.peers["master"]
+        self._pull_slices("master", self.module._flat)
+        self._master_stale = False
+
+    def _pull_slices(self, name, dst):
+        """copies every slice of the fp32 flat-space peer buffer `name` that another rank owns out of that owner's copy
+        into `dst` (this rank's copy), stream-ordered copy-engine copies; the masters and the optimizer state use it"""
+        s = self.module._engine.stream()
+        peers = self.comm.peers[name]
         for (b, e, _label) in self.module._layout.buckets:
             for r in range(self.world):
                 if r == self.rank:
                     continue
                 sb, se = self._bucket_slice(b, e, r, self.world)
                 if se > sb:
-                    L.call("b2_copy_async", flat.data_ptr() + 4 * sb, peers_m[r] + 4 * sb, 4 * (se - sb), s)
-        self._master_stale = False
+                    L.call("b2_copy_async", dst.data_ptr() + 4 * sb, peers[r] + 4 * sb, 4 * (se - sb), s)
 
     # ---- the two small collectives of the reference Trainer -------------------------------------------------------------
     def loss_reduce(self, loss):

@@ -13,6 +13,7 @@ the user sees.  There is no PyTorch fallback: without the CUDA library every cal
 """
 import contextlib
 import os
+import weakref
 from collections import OrderedDict
 
 import torch
@@ -257,7 +258,8 @@ class BertForSequenceClassification(nn.Module):
         self._build_skeleton()
         self._init_weights()
         self._engine = None
-        self._optimizer = None
+        self._optimizer = None       # the optimizer whose step schedule the backward drives (the last one built)
+        self._optimizers = weakref.WeakSet()   # every live optimizer of the model (their state moves with a wrapper)
         self._ddp = None
         self._grads_live = False     # an eager backward has produced gradients no optimizer.step() has consumed yet
         self._no_sync = False        # inside no_sync(): backwards accumulate
@@ -412,6 +414,36 @@ class BertForSequenceClassification(nn.Module):
         if self._ddp is not None:
             self._ddp._gather_master()
         return super().state_dict(*args, **kwargs)
+
+    def save_pretrained(self, save_directory):
+        """HF's layout: ``config.json`` (the config's attributes, problem_type included) and ``pytorch_model.bin``
+        (HF-keyed fp32 weights), which ``from_pretrained(save_directory)`` reads back exactly.  Under
+        DistributedDataParallel it is one-sided, as state_dict() is: call it on one rank."""
+        import json
+        os.makedirs(save_directory, exist_ok=True)
+        cfg = self.config.to_dict() if hasattr(self.config, "to_dict") else dict(vars(self.config))
+        with open(os.path.join(save_directory, "config.json"), "w") as f:
+            json.dump(cfg, f, indent=2, sort_keys=True)
+        sd = OrderedDict((k, v.detach().cpu().clone()) for k, v in self.state_dict().items())
+        torch.save(sd, os.path.join(save_directory, "pytorch_model.bin"))
+
+    # ---- dropout stream -------------------------------------------------------------------------------------------
+    def dropout_rng_state(self):
+        """the dropout streams' position: CPU int64 [seed, step].  Every optimizer step and every accumulating backward
+        moves `step` on; each rank has its own."""
+        if self._engine is None:
+            raise RuntimeError("the dropout state lives on the GPU: call model.cuda() first")
+        return self._engine.rng.cpu()
+
+    def set_dropout_rng_state(self, state):
+        """writes a dropout_rng_state() back, stream-ordered and in place (captured train steps keep replaying on it)"""
+        if self._engine is None:
+            raise RuntimeError("the dropout state lives on the GPU: call model.cuda() first")
+        t = torch.as_tensor(state).reshape(-1)
+        if t.numel() != 2 or t.is_floating_point():
+            raise ValueError("a dropout RNG state is an integer [seed, step] (got %s)" % (state,))
+        seed, step = (int(x) for x in t.tolist())
+        self._engine.seed_dropout(seed, step)
 
     # ---- forward ------------------------------------------------------------------------------------------------------
     def forward(self, input_ids=None, token_type_ids=None, attention_mask=None, labels=None, position_ids=None,

@@ -9,12 +9,16 @@ weight, ``correct_bias=True``) — NOT ``torch.optim.AdamW``.  One kernel update
 ``torch.optim.SGD`` (fabric-cls.py's ``Args.optim = "sgd"`` branch) on the same kernels' gradient path, and ``Adam`` /
 ``TorchAdamW`` are ``torch.optim.Adam`` / ``torch.optim.AdamW`` with ``fused=True`` (HF transformers 5.5's default).
 """
+import copy
+import itertools
 import os
 
 import torch
 
 from . import _lib as L
 from .ddp import _SLOT_BUCKET0, _SLOT_GRADS_READY, _SLOT_UPDATE_DONE
+
+_uids = itertools.count()
 
 
 class _FusedOptimizer(torch.optim.Optimizer):
@@ -32,6 +36,7 @@ class _FusedOptimizer(torch.optim.Optimizer):
     # is needed: found_inf stays 0 and the scale only has to be divided out (exactly: it is a power of two).
     _step_supports_amp_scaling = True
     _shared_keys = ()     # the group hyperparameters besides lr that every group must share (one kernel, one value)
+    _flat_keys = ()       # the subclass's state buffers over the flat space (peer-visible under DistributedDataParallel)
 
     def __init__(self, params, defaults):
         super().__init__(params, defaults)
@@ -41,29 +46,7 @@ class _FusedOptimizer(torch.optim.Optimizer):
         if self._model is None or len(owners) != 1:
             raise TypeError("this %s drives the fused CUDA update of ONE b200 BertForSequenceClassification; "
                             "got parameters that do not belong to such a model" % type(self).__name__)
-        g0 = self.param_groups[0]
-        key = lambda g: (g["lr"],) + tuple(tuple(v) if isinstance(v, (list, tuple)) else v
-                                           for v in (g[k] for k in self._shared_keys))
-        for g in self.param_groups[1:]:
-            if key(g) != key(g0):
-                raise ValueError("param groups may differ only in weight_decay (as the reference's two groups do)")
-        wds = sorted({float(g["weight_decay"]) for g in self.param_groups if g["weight_decay"] > 0})
-        if len(wds) > 1:
-            raise ValueError("at most one non-zero weight_decay value is supported")
-        self._wd = wds[0] if wds else 0.0
-        lay = self._model._layout
-        covered = set()
-        flags = torch.zeros(lay.total // 8, dtype=torch.uint8)
-        for g in self.param_groups:
-            for p in g["params"]:
-                off, _shape = lay.entries[p._b2_name]
-                covered.add(p._b2_name)
-                if g["weight_decay"] > 0:
-                    flags[off // 8:(off + (p.numel() + 7) // 8 * 8) // 8] = 1
-        if covered != set(lay.entries):
-            raise ValueError("the fused update steps every parameter of the model; %d of %d were passed"
-                             % (len(covered), len(lay.entries)))
-        self._decay_flags_cpu = flags
+        self._wd, self._decay_flags_cpu = self._group_rules(self.param_groups)
         self._dev_state = None
         # the step schedule's state.  _armed: set by a captured train step, bucket_ready may run during backward;
         # _pending: the buckets bucket_ready has already handled in this step (updated, or in a clipped step reduced)
@@ -76,9 +59,94 @@ class _FusedOptimizer(torch.optim.Optimizer):
         # set by a captured train step for the duration of its body: the kernels read the lr from the device scalar
         # the step refreshes before every replay (see hparams), not the value passed at launch / capture
         self._lr_dev_on = False
+        self._uid = next(_uids)
         self._model._optimizer = self
+        self._model._optimizers.add(self)    # every optimizer's state follows the model into and out of a peer group
+        if self._peer() is not None:
+            self._state()       # under a peer group the allocation is collective: every rank is here
+
+    def _group_rules(self, groups):
+        """What a grouping of the parameters must satisfy (one kernel: the groups may differ only in weight_decay, and
+        cover every parameter).  Returns (the one non-zero weight decay or 0, the decay flag of every 8 elements)."""
+        g0 = groups[0]
+        key = lambda g: (g["lr"],) + tuple(tuple(v) if isinstance(v, (list, tuple)) else v
+                                           for v in (g[k] for k in self._shared_keys))
+        for g in groups[1:]:
+            if key(g) != key(g0):
+                raise ValueError("param groups may differ only in weight_decay (as the reference's two groups do)")
+        wds = sorted({float(g["weight_decay"]) for g in groups if g["weight_decay"] > 0})
+        if len(wds) > 1:
+            raise ValueError("at most one non-zero weight_decay value is supported")
+        lay = self._model._layout
+        covered = set()
+        flags = torch.zeros(lay.total // 8, dtype=torch.uint8)
+        for g in groups:
+            for p in g["params"]:
+                off, _shape = lay.entries[p._b2_name]
+                covered.add(p._b2_name)
+                if g["weight_decay"] > 0:
+                    flags[off // 8:(off + (p.numel() + 7) // 8 * 8) // 8] = 1
+        if covered != set(lay.entries):
+            raise ValueError("the fused update steps every parameter of the model; %d of %d were passed"
+                             % (len(covered), len(lay.entries)))
+        return (wds[0] if wds else 0.0), flags
 
     # -- device state (step counter, lr slot, decay flags, and the subclass's buffers) -------------------------------
+    def _peer(self):
+        """the DistributedDataParallel wrapper (world > 1) whose peers map the state buffers, else None"""
+        ddp = self._model._ddp
+        return ddp if ddp is not None and ddp.world > 1 and ddp.comm is not None else None
+
+    def _new_flat(self, key, zero=True):
+        """an fp32 buffer over the flat space for the state `key`.  Under a peer group it is peer-visible memory, as the
+        masters are, so that state_dict() can pull the slices other ranks update; that allocation is collective, so it
+        happens only where every rank is: construction or wrap time, step() and its eager warm-ups, load_state_dict()."""
+        n, dev = self._model._layout.total, self._model._engine.dev
+        ddp = self._peer()
+        if ddp is None:
+            return (torch.zeros if zero else torch.empty)(n, dtype=torch.float32, device=dev)
+        t = ddp.comm.alloc(self._peer_name(key), 4 * n).tensor(torch.float32, dev)
+        return t.zero_() if zero else t
+
+    def _peer_name(self, key):
+        """this optimizer's name of the peer buffer of state `key`: every optimizer of a wrapped model has its own (the
+        buffers of one that is dropped stay mapped until the wrapper closes)"""
+        return "opt%d.%s" % (self._uid, key)
+
+    def _ensure_lazy(self, stream):
+        """creates the state buffers that come into use with an update (SGD's momentum, amsgrad's maximum); called
+        where every rank of a peer group is, before the updates of a step"""
+
+    def _share_state(self):
+        """DistributedDataParallel (world > 1) wrapping the model: the state buffers move into peer-visible memory"""
+        if self._dev_state is None or self._dev_state["dev"] != self._model._engine.dev:
+            self._state()
+            return
+        st = self._dev_state
+        for k in self._flat_keys:
+            if st.get(k) is not None:
+                st[k] = self._new_flat(k, zero=False).copy_(st[k])
+
+    def _gather_state(self):
+        """Under a peer group each rank updates only its slice of every bucket: pull the other slices of every state
+        buffer out of their owners' copies (DistributedDataParallel._pull_slices, one-sided and safe between steps
+        for the reason _gather_master gives)."""
+        ddp = self._peer()
+        if ddp is None or self._dev_state is None:
+            return
+        for k in self._flat_keys:
+            if self._dev_state.get(k) is not None:
+                ddp._pull_slices(self._peer_name(k), self._dev_state[k])
+
+    def _unshare_state(self):
+        """DistributedDataParallel.close(): private copies of the state buffers, every slice gathered, as the masters get"""
+        if self._dev_state is None or self._peer() is None:
+            return
+        self._gather_state()
+        for k in self._flat_keys:
+            if self._dev_state.get(k) is not None:
+                self._dev_state[k] = self._dev_state[k].clone()
+
     def _state(self):
         eng = self._model._engine
         if eng is None:
@@ -199,6 +267,8 @@ class _FusedOptimizer(torch.optim.Optimizer):
             eng.accumulate_range(b, e, op, s)
             if op != L.ACCUM_FOLD:
                 return
+        if not self._pending:
+            self._ensure_lazy(s)
         t.barrier(_SLOT_BUCKET0 + idx, s)
         if self._clip is not None:
             # a clipped step: only the reduce phase hides under the backward; no bucket may move before the norm of
@@ -233,6 +303,7 @@ class _FusedOptimizer(torch.optim.Optimizer):
         elif todo:
             t.barrier(_SLOT_GRADS_READY, s)
         if todo:
+            self._ensure_lazy(s)
             t.update(self, todo, s)
         t.barrier(_SLOT_UPDATE_DONE, s)
         self.advance(s)
@@ -349,9 +420,142 @@ class _FusedOptimizer(torch.optim.Optimizer):
             out[name] = flat[off:off + p.numel()].view(shape)
         return out
 
+    # -- checkpoint: torch's state_dict format over the flat device buffers ----------------------------------------------
+    def state_dict(self):
+        """torch's format: ``{"state": {i: {...}}, "param_groups": [{..., "params": [i, ...]}]}``, the parameters
+        numbered in param_groups order as torch numbers them.  The per-parameter tensors are views into the device
+        state buffers (torch also returns live references); ``Optimizer.state`` itself stays empty.  The state is empty
+        before the first update, as torch's is.  Under DistributedDataParallel with world > 1 the call is one-sided, as
+        ``model.state_dict()`` is: this rank pulls the slices other ranks update out of their memory."""
+        for pre_hook in self._optimizer_state_dict_pre_hooks.values():
+            pre_hook(self)
+        groups, idx = [], 0
+        for g in self.param_groups:        # torch's pack_group
+            packed = {k: v for k, v in g.items() if k != "params"}
+            packed["params"] = list(range(idx, idx + len(g["params"])))
+            idx += len(g["params"])
+            groups.append(packed)
+        sd = {"state": {}, "param_groups": groups}
+        if self._dev_state is not None:
+            self._gather_state()
+            entries = self._export(self._dev_state, int(self._dev_state["step"]))
+            if entries:
+                idx = 0
+                for g in self.param_groups:
+                    for p in g["params"]:
+                        sd["state"][idx] = entries(p._b2_name)
+                        idx += 1
+        for post_hook in self._optimizer_state_dict_post_hooks.values():
+            out = post_hook(self, sd)
+            if out is not None:
+                sd = out
+        return sd
+
+    def load_state_dict(self, state_dict):
+        """Loads a dict of ``state_dict()``'s format -- this class's, or the stock torch class's it restates.  torch's
+        checks first, then the group rules of the constructor; the tensors are copied into the existing device buffers
+        in place, so a captured train step replays on the loaded state.  Under DistributedDataParallel every rank must
+        call it (it may allocate a buffer the dict carries, collectively).  torch's load pre- and post-hooks run."""
+        state_dict = state_dict.copy()
+        for pre_hook in self._optimizer_load_state_dict_pre_hooks.values():
+            out = pre_hook(self, state_dict)
+            if out is not None:
+                state_dict = out
+        groups = self.param_groups
+        saved = copy.deepcopy(state_dict["param_groups"])
+        if len(groups) != len(saved):
+            raise ValueError("loaded state dict has a different number of parameter groups")
+        if any(len(g["params"]) != len(s["params"]) for g, s in zip(groups, saved)):
+            raise ValueError("loaded state dict contains a parameter group that doesn't match the size of optimizer's "
+                             "group")
+        names, new_groups = {}, []
+        for g, s in zip(groups, saved):
+            for p, i in zip(g["params"], s["params"]):
+                names[i] = p._b2_name
+            s["params"] = g["params"]
+            if "param_names" in g and "param_names" not in s:
+                s["param_names"] = g["param_names"]
+            for k, v in self.defaults.items():      # (as torch's subclasses' __setstate__ fill in newer keys)
+                s.setdefault(k, v)
+            new_groups.append(s)
+        wd, flags = self._group_rules(new_groups)
+        state = {names[i]: v for i, v in state_dict["state"].items() if i in names and v}
+        if state and len(state) != len(names):
+            raise ValueError("the loaded state covers %d of %d parameters: the fused update keeps one state for all of "
+                             "them" % (len(state), len(names)))
+        step = self._loaded_step(state)
+        self._check_loaded(state, step, new_groups[0])
+        shapes = {p._b2_name: tuple(p.shape) for g in groups for p in g["params"]}
+        for name, entry in state.items():
+            for key, v in entry.items():
+                if isinstance(v, torch.Tensor) and key != "step" and tuple(v.shape) != shapes[name]:
+                    raise ValueError("loaded state %r of %s has shape %s, the parameter %s"
+                                     % (key, name, tuple(v.shape), shapes[name]))
+        if state and self._model._engine is None:
+            raise RuntimeError("load_state_dict: the optimizer state lives on the GPU; call model.cuda() before "
+                               "loading a state with steps")
+        self.param_groups = new_groups
+        self._wd, self._decay_flags_cpu = wd, flags
+        if self._model._engine is None:
+            self._dev_state = None       # (created from the loaded groups' decay flags by the first step)
+        else:
+            st = self._state()
+            st["decay"].copy_(flags)
+            with torch.no_grad():
+                self._import(st, state, step)
+            self._prepare(self._model._engine.stream())
+        for post_hook in self._optimizer_load_state_dict_post_hooks.values():
+            post_hook(self)
+
+    def _loaded_step(self, state):
+        """the one step count of the loaded per-parameter states (int, float or tensor), 0 without state"""
+        steps = set()
+        for name, entry in state.items():
+            v = entry.get("step")
+            if v is None:
+                continue
+            x = float(v.item() if isinstance(v, torch.Tensor) else v)
+            if x != int(x) or x < 0:
+                raise ValueError("loaded state of %s has step %r; a step count is a non-negative integer" % (name, v))
+            steps.add(int(x))
+        if len(steps) > 1:
+            raise ValueError("the loaded parameters disagree on step (%s): the fused update keeps one step count"
+                             % sorted(steps))
+        return steps.pop() if steps else 0
+
+    def _check_loaded(self, state, step, group):
+        """raises before anything is changed when the loaded per-parameter states lack what this update needs"""
+        first = None
+        for name, entry in state.items():
+            for key in self._required:
+                if key not in entry:
+                    raise ValueError("loaded state of %s has no %r" % (name, key))
+            have = sorted(k for k in self._flat_keys if k in entry)
+            if first is None:
+                first = have
+            elif have != first:
+                raise ValueError("the loaded parameters disagree on which state they have (%s: %s, others: %s): the "
+                                 "fused update keeps one set of buffers" % (name, have, first))
+
+    def _load_flat(self, st, key, state):
+        """the loaded per-parameter `key` tensors into the flat buffer st[key] (created if the dict carries it and it
+        does not exist yet), in place, its 8-element padding zeroed; a buffer the dict does not carry is zeroed"""
+        if st.get(key) is None:
+            if not state or key not in next(iter(state.values())):
+                return
+            st[key] = self._new_flat(key, zero=False)
+        buf = st[key]
+        buf.zero_()
+        if state:
+            views = self._views(buf)
+            for name, entry in state.items():
+                views[name].copy_(entry[key])
+
 
 class AdamW(_FusedOptimizer):
     _shared_keys = ("betas", "eps", "correct_bias")
+    _flat_keys = ("exp_avg", "exp_avg_sq")
+    _required = ("step", "exp_avg", "exp_avg_sq")
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.0, correct_bias=True,
                  no_deprecation_warning=True):
@@ -367,9 +571,21 @@ class AdamW(_FusedOptimizer):
         super().__init__(params, defaults)
 
     def _init_state(self, st, n):
-        st["exp_avg"] = torch.zeros(n, dtype=torch.float32, device=st["dev"])
-        st["exp_avg_sq"] = torch.zeros(n, dtype=torch.float32, device=st["dev"])
+        st["exp_avg"] = self._new_flat("exp_avg")
+        st["exp_avg_sq"] = self._new_flat("exp_avg_sq")
         st["step_size"] = torch.zeros(1, dtype=torch.float32, device=st["dev"])   # see b2_adamw_prepare
+
+    def _export(self, st, step):
+        """transformers 4.28.1 AdamW.step's state of a parameter: step (a python int), exp_avg, exp_avg_sq"""
+        if step == 0:
+            return None
+        m, v = self._views(st["exp_avg"]), self._views(st["exp_avg_sq"])
+        return lambda name: {"step": step, "exp_avg": m[name], "exp_avg_sq": v[name]}
+
+    def _import(self, st, state, step):
+        for key in self._flat_keys:
+            self._load_flat(st, key, state)
+        st["step"].fill_(step)
 
     def _prepare(self, stream):
         """bias-corrected step size of the NEXT update -> device float (read by the background kernel)"""
@@ -403,8 +619,10 @@ class AdamW(_FusedOptimizer):
                hp, L.ptr(st["step"]), stream)
 
     def moments(self):
-        """(exp_avg, exp_avg_sq) fp32 by HF parameter name — for tests/checkpoint tooling."""
+        """(exp_avg, exp_avg_sq) fp32 by HF parameter name — for tests/checkpoint tooling (every slice gathered under
+        a peer group, as in state_dict())."""
         st = self._state()
+        self._gather_state()
         m, v = self._views(st["exp_avg"]), self._views(st["exp_avg_sq"])
         return {name: (m[name], v[name]) for name in m}
 
@@ -417,6 +635,8 @@ class SGD(_FusedOptimizer):
     in ``.grad``.  The momentum buffer is allocated when the first step with ``momentum != 0`` runs; as in torch, that
     step sets it to the gradient.  ``foreach``, ``fused`` and ``differentiable=False`` are accepted and ignored."""
     _shared_keys = ("momentum", "dampening", "nesterov", "maximize")
+    _flat_keys = ("momentum_buffer",)
+    _required = ()
 
     def __init__(self, params, lr=1e-3, momentum=0, dampening=0, weight_decay=0, nesterov=False, *, maximize=False,
                  foreach=None, differentiable=False, fused=None):
@@ -439,15 +659,34 @@ class SGD(_FusedOptimizer):
     def _init_state(self, st, n):
         st["momentum_buffer"] = None     # allocated by the first step with momentum (torch: `momentum_buffer is None`)
 
+    def _ensure_lazy(self, stream):
+        """When the momentum buffer comes into use the step count restarts at 0 on `stream`, the stream of the update
+        about to read it: that update initialises the buffer from the gradient."""
+        st = self._state()
+        if float(self.param_groups[0]["momentum"]) != 0.0 and st["momentum_buffer"] is None:
+            st["momentum_buffer"] = self._new_flat("momentum_buffer", zero=False)
+            L.call("b2_zero", L.ptr(st["step"]), 8, stream)
+
     def _buffer(self, st, stream):
-        """the momentum buffer, or None without momentum.  When it comes into use the step count restarts at 0 on
-        `stream`, the stream of the update about to read it: that update initialises the buffer from the gradient."""
+        """the momentum buffer, or None without momentum"""
         if float(self.param_groups[0]["momentum"]) == 0.0:
             return None
-        if st["momentum_buffer"] is None:
-            st["momentum_buffer"] = torch.empty(self._model._layout.total, dtype=torch.float32, device=st["dev"])
-            L.call("b2_zero", L.ptr(st["step"]), 8, stream)
+        self._ensure_lazy(stream)
         return st["momentum_buffer"]
+
+    def _export(self, st, step):
+        """torch.optim.SGD's state of a parameter: momentum_buffer once it exists (nothing without momentum)"""
+        if st["momentum_buffer"] is None or step == 0:
+            return None
+        views = self._views(st["momentum_buffer"])
+        return lambda name: {"momentum_buffer": views[name]}
+
+    def _import(self, st, state, step):
+        self._load_flat(st, "momentum_buffer", state)
+        # the device step only decides whether the next update initialises the buffer from the gradient (step 0):
+        # torch's `momentum_buffer is None`.  A loaded buffer is used; without one the next update starts it afresh.
+        carried = bool(state) and "momentum_buffer" in next(iter(state.values()))
+        st["step"].fill_(1 if carried else 0)
 
     def captured_hparams(self):
         """The hyperparameters a captured step bakes into its graph (all but the lr, which it reads at every replay)"""
@@ -481,6 +720,7 @@ class SGD(_FusedOptimizer):
         """fp32 momentum buffers by HF parameter name, or {} while there is none (momentum 0, or no step yet) — the
         counterpart of AdamW.moments(), for tests and tooling."""
         buf = self._state()["momentum_buffer"]
+        self._gather_state()
         return {} if buf is None else self._views(buf)
 
 
@@ -494,6 +734,8 @@ class Adam(_FusedOptimizer):
     fused and capturable); ``differentiable=True`` raises.  The max_exp_avg_sq buffer is created by the first update
     with ``amsgrad`` set; turning amsgrad on after an update has run raises at ``step()``."""
     _shared_keys = ("betas", "eps", "amsgrad", "maximize", "decoupled_weight_decay")
+    _flat_keys = ("exp_avg", "exp_avg_sq", "max_exp_avg_sq")
+    _required = ("step", "exp_avg", "exp_avg_sq")
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, *, foreach=None,
                  maximize=False, capturable=False, differentiable=False, fused=None, decoupled_weight_decay=False):
@@ -534,10 +776,14 @@ class Adam(_FusedOptimizer):
         defaults = dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, amsgrad=amsgrad,
                         maximize=maximize, foreach=foreach, capturable=capturable, differentiable=differentiable,
                         fused=fused, decoupled_weight_decay=decoupled_weight_decay)
+        self._updated = False    # an update has run on this state: amsgrad can no longer be turned on
         super().__init__(params, defaults)
+
+    def _group_rules(self, groups):
+        wd, flags = super()._group_rules(groups)
         # torch's kernel forms the L2 term by the lane an element takes in its loop (see b2_adam_hparams_t): a tensor
         # whose size is not a multiple of 4 goes through its unaligned loop, where element j is in lane (j % 2048) / 512
-        flags, lay = self._decay_flags_cpu, self._model._layout
+        lay = self._model._layout
         for name, (off, shape) in lay.entries.items():
             n = self._model._params_by_name[name].numel()
             if n % 4:
@@ -545,14 +791,50 @@ class Adam(_FusedOptimizer):
                 bits = L.ADAM_DECAY_UNALIGNED + L.ADAM_DECAY_LANE0 * ((j % 2048) < 512).to(torch.uint8)
                 seg = flags[off // 8:off // 8 + len(j)]
                 seg |= seg * bits      # on decayed vectors only
-        self._updated = False    # an update has run on this state: amsgrad can no longer be turned on
+        return wd, flags
 
     def _init_state(self, st, n):
-        st["exp_avg"] = torch.zeros(n, dtype=torch.float32, device=st["dev"])
-        st["exp_avg_sq"] = torch.zeros(n, dtype=torch.float32, device=st["dev"])
-        st["max_exp_avg_sq"] = None             # created by the first update with amsgrad (see _hparams)
+        st["exp_avg"] = self._new_flat("exp_avg")
+        st["exp_avg_sq"] = self._new_flat("exp_avg_sq")
+        # with amsgrad on from the start the buffer comes with the state; turned on later, with the first update that
+        # reads it (see _ensure_lazy)
+        st["max_exp_avg_sq"] = self._new_flat("max_exp_avg_sq") if self.param_groups[0]["amsgrad"] else None
         self._updated = False
         st["prepared"] = torch.zeros(2, dtype=torch.float32, device=st["dev"])   # see b2_adam_prepare
+
+    def _ensure_lazy(self, stream):
+        st = self._state()
+        if self.param_groups[0]["amsgrad"] and st["max_exp_avg_sq"] is None and not self._updated:
+            # before any update (never inside a capture: the captured steps run eager passes first).  After one,
+            # _hparams raises.
+            st["max_exp_avg_sq"] = self._new_flat("max_exp_avg_sq")
+            torch.cuda.current_stream(st["dev"]).synchronize()     # zeroed before another stream's update reads it
+
+    def _export(self, st, step):
+        """torch.optim.Adam / AdamW's state of a parameter: step (0-dim fp32), exp_avg, exp_avg_sq, and
+        max_exp_avg_sq once amsgrad has run"""
+        if step == 0:
+            return None
+        bufs = [(k, self._views(st[k])) for k in self._flat_keys if st.get(k) is not None]
+        return lambda name: dict([("step", torch.tensor(float(step), dtype=torch.float32))]
+                                 + [(k, v[name]) for k, v in bufs])
+
+    def _check_loaded(self, state, step, group):
+        super()._check_loaded(state, step, group)
+        if group["amsgrad"] and step > 0 and "max_exp_avg_sq" not in next(iter(state.values())):
+            raise ValueError("amsgrad is on but the loaded state has no max_exp_avg_sq after %d steps: the buffer would "
+                             "start from zero mid-run (as when amsgrad is turned on after the first step)" % step)
+
+    def _import(self, st, state, step):
+        self._load_flat(st, "exp_avg", state)
+        self._load_flat(st, "exp_avg_sq", state)
+        carried = bool(state) and "max_exp_avg_sq" in next(iter(state.values()))
+        if carried or self.param_groups[0]["amsgrad"]:
+            self._load_flat(st, "max_exp_avg_sq", state)
+        else:
+            st["max_exp_avg_sq"] = None         # as in torch: no amsgrad state without amsgrad having run
+        st["step"].fill_(step)
+        self._updated = step > 0
 
     def _prepare(self, stream):
         """the bias corrections of the NEXT update -> device floats (read by the background kernel)"""
@@ -571,14 +853,10 @@ class Adam(_FusedOptimizer):
     def _hparams(self):
         g = self.param_groups[0]
         st = self._dev_state
-        if g["amsgrad"] and st is not None and st["max_exp_avg_sq"] is None:
-            if self._updated:
-                # torch fails here too (a KeyError on the missing state entry)
-                raise ValueError("amsgrad was turned on after the first step: the max_exp_avg_sq buffer would start "
-                                 "from zero mid-run; build the optimizer with amsgrad=True")
-            # before any update (never inside a capture: the captured steps run eager passes first)
-            st["max_exp_avg_sq"] = torch.zeros(self._model._layout.total, dtype=torch.float32, device=st["dev"])
-            torch.cuda.current_stream(st["dev"]).synchronize()     # zeroed before another stream's update reads it
+        if g["amsgrad"] and st is not None and st["max_exp_avg_sq"] is None and self._updated:
+            # torch fails here too (a KeyError on the missing state entry)
+            raise ValueError("amsgrad was turned on after the first step: the max_exp_avg_sq buffer would start "
+                             "from zero mid-run; build the optimizer with amsgrad=True")
         hp = L.AdamHParams()
         hp.lr, hp.beta1, hp.beta2, hp.eps = float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"])
         hp.weight_decay = float(self._wd)
@@ -588,6 +866,8 @@ class Adam(_FusedOptimizer):
 
     def _launch(self, st, hp, begin, end, world, rank, peer_grads, peer_shadow, stream, background):
         flat = self._model._flat
+        if hp.amsgrad:
+            self._ensure_lazy(stream)
         vmax = st["max_exp_avg_sq"] if hp.amsgrad else None
         self._updated = True
         if background:
@@ -604,6 +884,7 @@ class Adam(_FusedOptimizer):
     def max_exp_avg_sqs(self):
         """amsgrad's fp32 max_exp_avg_sq by HF parameter name, or {} without amsgrad"""
         buf = self._state()["max_exp_avg_sq"]
+        self._gather_state()
         return {} if buf is None else self._views(buf)
 
 

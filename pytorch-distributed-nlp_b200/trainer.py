@@ -13,7 +13,12 @@ built from ``Args.lr_scheduler_type``), stepped once per optimizer step on every
 it sets at every replay.
 """
 import contextlib
+import json
 import math
+import os
+import random
+import re
+import shutil
 import time
 
 import numpy as np
@@ -58,10 +63,44 @@ class Args:
                           # (HF's names: torch.optim.AdamW on the reference's two groups, eps 1e-8)
     log_every = 1         # the reference prints every step (forces a D2H sync per step)
     total_step = 0
+    output_dir = None     # HF TrainingArguments' checkpoint names: train() writes output_dir/checkpoint-N every save_steps
+    save_steps = None     # optimizer steps (None: no checkpoints), keeping the newest save_total_limit of them (None:
+    save_total_limit = None   # all); train(resume_from_checkpoint=...) continues from one
 
 
 def _unwrap(model):
     return model.module if isinstance(model, DistributedDataParallel) else model
+
+
+CHECKPOINT_PREFIX = "checkpoint"     # HF Trainer's PREFIX_CHECKPOINT_DIR: output_dir/checkpoint-{optimizer step}
+
+
+def sorted_checkpoints(output_dir):
+    """the checkpoint-N directories under `output_dir`, oldest (smallest N) first"""
+    if output_dir is None or not os.path.isdir(output_dir):
+        return []
+    found = []
+    for name in os.listdir(output_dir):
+        m = re.fullmatch(CHECKPOINT_PREFIX + r"-(\d+)", name)
+        if m and os.path.isdir(os.path.join(output_dir, name)):
+            found.append((int(m.group(1)), os.path.join(output_dir, name)))
+    return [path for _n, path in sorted(found)]
+
+
+def latest_checkpoint(output_dir):
+    """HF's get_last_checkpoint: the checkpoint-N directory with the largest N, or None"""
+    found = sorted_checkpoints(output_dir)
+    return found[-1] if found else None
+
+
+def rotate_checkpoints(output_dir, save_total_limit):
+    """deletes the oldest checkpoint-N directories beyond the newest `save_total_limit` (None or <= 0: keeps all, as
+    HF does)"""
+    if save_total_limit is None or int(save_total_limit) <= 0:
+        return
+    found = sorted_checkpoints(output_dir)
+    for path in found[:max(0, len(found) - int(save_total_limit))]:
+        shutil.rmtree(path)
 
 
 def step_loss(model, criterion=None):
@@ -209,6 +248,10 @@ class _StagedGraphStep:
         self._run_device()
         if opt is not None:
             self.eng.accum_live = not final
+            if final:
+                # a replay runs no Python: tell the transport the weights moved (under a peer group the next
+                # state_dict() pulls the other ranks' slices again)
+                opt._transport().stepped()
 
     def _run_device(self):
         if not self.use_graph:
@@ -420,6 +463,11 @@ class Trainer:
         self.last_grad_norm = None   # device scalar: the pre-clip gradient norm of the last optimizer step (HF's
                                      # logged `grad_norm`); None when not clipping
         self.lr_scheduler = scheduler
+        self.global_step = 0  # optimizer steps taken (HF's global_step; checkpoint-N is named by it)
+        # where train() is, for trainer_state.json: batches done, the epoch and the batches of it consumed, best_acc
+        self._progress = {"batches": 0, "epoch": 1, "batches_in_epoch": 0, "best_acc": 0.0}
+        self._epoch_rng = None     # train(): the CPU RNG state the current epoch's loader iterator was created from
+        self._loaded_rng = None    # load_checkpoint(): the RNG states it restored (train() re-applies them after a skip)
 
     def num_training_steps(self, train_loader):
         """optimizer steps train() takes: epochs x ceil(batches / k).  HF Trainer floors batches / k; this Trainer
@@ -604,6 +652,7 @@ class Trainer:
                 self._scheduler_step()
         if final:
             self._note_grad_norm(clip)
+            self.global_step += 1
         return self.loss_reduce(loss.detach())
 
     def _scheduler_step(self):
@@ -653,18 +702,129 @@ class Trainer:
             self.optimizer.step()
             self._scheduler_step()
         self._note_grad_norm(clip)
+        self.global_step += 1
 
-    def train(self, train_loader, dev_loader=None, train_sampler=None):
+    # ---- checkpoints (HF Trainer's checkpoint-N layout) -------------------------------------------------------------------
+    def _rank(self):
+        return self.model.rank if isinstance(self.model, DistributedDataParallel) else 0
+
+    def save_checkpoint(self, output_dir):
+        """Writes HF Trainer's checkpoint layout into `output_dir`: ``pytorch_model.bin`` and ``config.json`` of the
+        unwrapped model (what ``from_pretrained`` reads), ``optimizer.pt``, ``scheduler.pt``, ``scaler.pt`` (when there
+        is a GradScaler), ``trainer_state.json``, and ``rng_state_{rank}.pth`` (python, numpy, torch CPU / CUDA and the
+        model's dropout stream, and inside train() the CPU RNG state the epoch's loader iterator was created from).
+        Rank 0 writes everything but the RNG files, which every rank writes for itself; under
+        DistributedDataParallel every rank must call it.  Only at an optimizer-step boundary."""
+        if self._micro != 0:
+            raise RuntimeError("save_checkpoint(): a gradient-accumulation window is open (%d of %d batches); "
+                               "checkpoints are taken between optimizer steps"
+                               % (self._micro, int(getattr(self.args, "gradient_accumulation_steps", 1))))
+        m, rank = _unwrap(self.model), self._rank()
+        os.makedirs(output_dir, exist_ok=True)
+        if rank == 0:
+            m.save_pretrained(output_dir)
+            torch.save(self.optimizer.state_dict(), os.path.join(output_dir, "optimizer.pt"))
+            if self.lr_scheduler is not None:
+                torch.save(self.lr_scheduler.state_dict(), os.path.join(output_dir, "scheduler.pt"))
+            if self._scaler is not None:
+                torch.save(self._scaler.state_dict(), os.path.join(output_dir, "scaler.pt"))
+            progress = dict(self._progress, global_step=self.global_step)
+            with open(os.path.join(output_dir, "trainer_state.json"), "w") as f:
+                json.dump(progress, f, indent=2)
+        rng = {"python": random.getstate(), "numpy": np.random.get_state(), "cpu": torch.random.get_rng_state(),
+               "cuda": torch.cuda.get_rng_state(m._engine.dev), "dropout": m.dropout_rng_state(),
+               "cpu_epoch_start": self._epoch_rng}
+        torch.save(rng, os.path.join(output_dir, "rng_state_%d.pth" % rank))
+
+    def load_checkpoint(self, checkpoint_dir, restore_dropout=True):
+        """Restores what save_checkpoint wrote, on every rank (each rank its own RNG file): the weights, the optimizer,
+        the scheduler and the GradScaler, the random states and the optimizer-step count.  Returns the trainer state
+        (trainer_state.json).  restore_dropout=False leaves the model's dropout stream where it is."""
+        m, rank = _unwrap(self.model), self._rank()
+        f = lambda name: os.path.join(checkpoint_dir, name)
+        self._loaded_rng = None
+        sd = torch.load(f("pytorch_model.bin"), map_location="cpu")
+        if isinstance(self.model, DistributedDataParallel):
+            self.model.load_state_dict({"module." + k: v for k, v in sd.items()})
+        else:
+            m.load_state_dict(sd)
+        self.optimizer.load_state_dict(torch.load(f("optimizer.pt"), map_location="cpu"))
+        if self.lr_scheduler is not None and os.path.exists(f("scheduler.pt")):
+            self.lr_scheduler.load_state_dict(torch.load(f("scheduler.pt"), weights_only=False))
+        if os.path.exists(f("scaler.pt")):
+            if self._scaler is None:
+                self._scaler = torch.amp.GradScaler("cuda")
+            self._scaler.load_state_dict(torch.load(f("scaler.pt")))
+        if os.path.exists(f("rng_state_%d.pth" % rank)):
+            rng = torch.load(f("rng_state_%d.pth" % rank), weights_only=False)
+            self._restore_host_rng(rng)
+            self._loaded_rng = rng
+            if restore_dropout:
+                m.set_dropout_rng_state(rng["dropout"])
+        with open(f("trainer_state.json")) as fp:
+            progress = json.load(fp)
+        self.global_step = int(progress["global_step"])
+        self._micro = 0
+        return progress
+
+    def _restore_host_rng(self, rng):
+        random.setstate(rng["python"])
+        np.random.set_state(rng["numpy"])
+        torch.random.set_rng_state(rng["cpu"])
+        torch.cuda.set_rng_state(rng["cuda"], _unwrap(self.model)._engine.dev)
+
+    def _maybe_save(self):
+        """train(): checkpoint-{optimizer step} under args.output_dir every args.save_steps optimizer steps, keeping
+        the newest args.save_total_limit"""
+        every = getattr(self.args, "save_steps", None)
+        if not every or self._micro != 0 or self.global_step % int(every) != 0:
+            return
+        out = getattr(self.args, "output_dir", None)
+        if out is None:
+            raise ValueError("args.save_steps is set but args.output_dir is None")
+        self.save_checkpoint(os.path.join(out, "%s-%d" % (CHECKPOINT_PREFIX, self.global_step)))
+        if self._rank() == 0:
+            rotate_checkpoints(out, getattr(self.args, "save_total_limit", None))
+
+    def train(self, train_loader, dev_loader=None, train_sampler=None, resume_from_checkpoint=None):
+        """resume_from_checkpoint: a checkpoint directory, or True for the newest checkpoint-N under args.output_dir.
+        The run continues from it: every state save_checkpoint wrote, and the batches the checkpoint's run consumed in
+        its epoch are skipped (the loader is iterated past them, as HF Trainer does).  A shuffling loader gives the
+        resumed epoch the order the interrupted one had: its iterator is created from the CPU RNG state that epoch's was,
+        and every RNG is set back to the checkpoint's once the consumed batches are skipped."""
         gloabl_step = 1
         best_acc = 0.
         if self.args.local_rank == 0:
             start = time.time()
         if self.lr_scheduler is None and getattr(self.args, "lr_scheduler_type", None) is not None:
             self.create_scheduler(self.num_training_steps(train_loader))
-        for epoch in range(1, self.args.epochs + 1):
+        first_epoch, skip, resume_rng = 1, 0, None
+        if resume_from_checkpoint:
+            path = resume_from_checkpoint
+            if path is True:
+                path = latest_checkpoint(getattr(self.args, "output_dir", None))
+                if path is None:
+                    raise ValueError("resume_from_checkpoint=True: no %s-N directory under args.output_dir (%r)"
+                                     % (CHECKPOINT_PREFIX, getattr(self.args, "output_dir", None)))
+            progress = self.load_checkpoint(path)
+            gloabl_step, best_acc = int(progress["batches"]) + 1, float(progress["best_acc"])
+            first_epoch, skip = int(progress["epoch"]), int(progress["batches_in_epoch"])
+            resume_rng = self._loaded_rng
+        for epoch in range(first_epoch, self.args.epochs + 1):
             if train_sampler is not None:
                 train_sampler.set_epoch(epoch)
+            if resume_rng is not None and resume_rng.get("cpu_epoch_start") is not None:
+                # a DataLoader draws its shuffling seed from the CPU RNG when its iterator starts: the resumed epoch's
+                # order is the interrupted epoch's only from the state that epoch started with
+                torch.random.set_rng_state(resume_rng["cpu_epoch_start"])
+            self._epoch_rng = torch.random.get_rng_state()
             for step, batch_data in enumerate(train_loader):
+                if skip:
+                    skip -= 1
+                    continue
+                if resume_rng is not None:
+                    self._restore_host_rng(resume_rng)     # past the consumed batches: the checkpoint's RNG states
+                    resume_rng = None
                 loss = self.train_step(batch_data)
                 if self.args.local_rank == 0 and gloabl_step % max(1, getattr(self.args, "log_every", 1)) == 0:
                     print("【train】 epoch：{}/{} step：{}/{} loss：{:.6f}".format(
@@ -684,7 +844,17 @@ class Trainer:
                                 # rank 0 alone, as in the reference [:190-192]: under DDP state_dict() pulls the fp32
                                 # slices other ranks own out of their HBM one-sidedly (ddp.py::_gather_master)
                                 torch.save(self.model.state_dict(), self.args.ckpt_path)
+                self._progress = {"batches": gloabl_step - 1, "epoch": epoch, "batches_in_epoch": step + 1,
+                                  "best_acc": float(best_acc)}
+                self._maybe_save()
+            if resume_rng is not None:       # the checkpoint's run had consumed the whole epoch
+                self._restore_host_rng(resume_rng)
+                resume_rng = None
+            skip = 0
+            stepped = self._micro != 0
             self.close_window()
+            if stepped:
+                self._maybe_save()
         if self.args.local_rank == 0:
             end = time.time()
             print("耗时：{}分钟".format((end - start) / 60))
