@@ -62,21 +62,27 @@ typedef struct b2_gemm_args {
   void* D;                /* bf16 [M, ldd]                                                                   */
   int64_t ldd;
   int32_t epilogue;
-  const void* bias;       /* bf16 [N] or NULL                                                                */
-  const void* aux_in;     /* bf16 [M, ld_aux_in]: residual (3,4) or saved pre-activation (5)                 */
+  const void* bias;       /* bf16 [N], 16-byte aligned: required by (1,2,3), must be NULL otherwise           */
+  const void* aux_in;     /* bf16 [M, ld_aux_in]: residual (3,4) or saved pre-activation (5); fp32 for (6);
+                             16-byte aligned; required by (3,4,5,6)                                          */
   int64_t ld_aux_in;
-  void* aux_out;          /* bf16 [M, ld_aux_out]: pre-activation saved by (2)                               */
+  void* aux_out;          /* bf16 [M, ld_aux_out], 16-byte aligned: pre-activation saved by (2); required by (2),
+                             must be NULL otherwise                                                          */
   int64_t ld_aux_out;
-  float dropout_p;        /* (3) only                                                                        */
-  const void* rng_state;  /* device uint64[2] = {seed, step}; see b2_rng_*                                   */
+  float dropout_p;        /* [0, 1) for (3); must be 0 otherwise                                             */
+  const void* rng_state;  /* device uint64[2] = {seed, step}; see b2_rng_*.  Required by (3) with p > 0; may be
+                             set (and is not read) otherwise                                                 */
   uint32_t rng_site;      /* distinct per dropout site                                                       */
-  void* workspace;        /* fp32 scratch for split-K (may be NULL -> never split)                           */
+  void* workspace;        /* fp32 scratch for split-K of (0) (may be NULL -> never split; may be set on
+                             problems that do not split)                                                     */
   int64_t workspace_bytes;
   int32_t force_bn;       /* 0 = auto, else 128 / 256 (tests, tuning)                                        */
-  int32_t force_splits;   /* 0 = auto, else >= 1                                                             */
+  int32_t force_splits;   /* 0 = auto, else >= 1; > 1 needs (7), or (0) with a workspace of force_splits*M*N*4
+                             bytes and no colsum_out                                                         */
   int32_t force_kernel;   /* kernel choice (tests, tuning); the H100 build has one GEMM kernel and ignores it       */
-  void* debug_timing;     /* unused (NULL)                                                                        */
-  float* colsum_out;      /* NULL, or fp32 [N]: += column sums of the (bf16-rounded) output D, by atomic add        */
+  void* debug_timing;     /* unused (may be set, is not read)                                                     */
+  float* colsum_out;      /* NULL, or fp32 [N]: += column sums of the (bf16-rounded) output D, by atomic add.  Only
+                             with the bf16-output epilogues (0-5); a problem with it is never split               */
 } b2_gemm_args_t;
 
 int32_t b2_gemm_bf16(const b2_gemm_args_t* args, void* stream);

@@ -322,7 +322,9 @@ static Choice choose_config(const b2_gemm_args_t& a) {
   const int sms = num_sms();
   const int kblocks = (int)((a.K + BK - 1) / BK);
   const bool accum = a.epilogue == B2_EPI_ACCUM_F32;   // split-K slices add in place: no workspace, any split count
-  const bool can_split = accum || ((a.epilogue == B2_EPI_NONE) && a.workspace != nullptr && a.bias == nullptr);
+  // the split-K partials path has no column sums: a problem with colsum_out runs whole tiles
+  const bool can_split = accum || ((a.epilogue == B2_EPI_NONE) && a.workspace != nullptr && a.bias == nullptr &&
+                                   a.colsum_out == nullptr);
   double best = 1e30;
   Choice c{128, 1};
   const double l2_bytes_per_cycle = 3000.0;   // L2 -> SM bandwidth shared by the busy SMs, bytes per SM clock
@@ -355,8 +357,9 @@ static Choice choose_config(const b2_gemm_args_t& a) {
 
 using namespace b2;
 
-extern "C" int32_t b2_gemm_bf16(const b2_gemm_args_t* a, void* stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
+// Every argument check of b2_gemm_bf16, host-only (no device access), so that the grouped entry point can reject a
+// table before it launches any of it.  An argument an epilogue would not read is an error, not a silent no-op.
+static int32_t check_args(const b2_gemm_args_t* a) {
   B2_REQUIRE(a != nullptr, "b2_gemm_bf16: null args");
   B2_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0, "b2_gemm_bf16: empty problem M=%lld N=%lld K=%lld",
              (long long)a->M, (long long)a->N, (long long)a->K);
@@ -366,36 +369,50 @@ extern "C" int32_t b2_gemm_bf16(const b2_gemm_args_t* a, void* stream_) {
              "b2_gemm_bf16: K and leading dimensions must be multiples of 8 elements (16 B)");
   B2_REQUIRE(((uintptr_t)a->A % 16 == 0) && ((uintptr_t)a->B % 16 == 0) && ((uintptr_t)a->D % 16 == 0),
              "b2_gemm_bf16: operands must be 16-byte aligned");
-  B2_REQUIRE(a->epilogue >= B2_EPI_NONE && a->epilogue <= B2_EPI_ACCUM_F32, "b2_gemm_bf16: bad epilogue %d",
-             a->epilogue);
-  if (a->epilogue == B2_EPI_BIAS || a->epilogue == B2_EPI_BIAS_GELU || a->epilogue == B2_EPI_BIAS_DROPOUT_RESIDUAL)
-    B2_REQUIRE(a->bias != nullptr, "b2_gemm_bf16: epilogue %d needs a bias", a->epilogue);
-  if (a->epilogue == B2_EPI_BIAS_DROPOUT_RESIDUAL || a->epilogue == B2_EPI_RESIDUAL ||
-      a->epilogue == B2_EPI_GELU_BWD || a->epilogue == B2_EPI_RESIDUAL_F32)
-    B2_REQUIRE(a->aux_in != nullptr && a->ld_aux_in % 8 == 0, "b2_gemm_bf16: epilogue %d needs aux_in",
-               a->epilogue);
-  if (a->epilogue == B2_EPI_BIAS_GELU)
+  const int e = a->epilogue;
+  B2_REQUIRE(e >= B2_EPI_NONE && e <= B2_EPI_ACCUM_F32, "b2_gemm_bf16: bad epilogue %d", e);
+  const bool with_bias = e == B2_EPI_BIAS || e == B2_EPI_BIAS_GELU || e == B2_EPI_BIAS_DROPOUT_RESIDUAL;
+  const bool f32_out = e == B2_EPI_RESIDUAL_F32 || e == B2_EPI_ACCUM_F32;
+  if (with_bias) B2_REQUIRE(a->bias != nullptr, "b2_gemm_bf16: epilogue %d needs a bias", e);
+  else           B2_REQUIRE(a->bias == nullptr, "b2_gemm_bf16: epilogue %d adds no bias: bias must be NULL", e);
+  if (e == B2_EPI_BIAS_DROPOUT_RESIDUAL || e == B2_EPI_RESIDUAL || e == B2_EPI_GELU_BWD || e == B2_EPI_RESIDUAL_F32)
+    B2_REQUIRE(a->aux_in != nullptr && a->ld_aux_in % 8 == 0, "b2_gemm_bf16: epilogue %d needs aux_in", e);
+  if (e == B2_EPI_BIAS_GELU)
     B2_REQUIRE(a->aux_out != nullptr && a->ld_aux_out % 8 == 0, "b2_gemm_bf16: BIAS_GELU needs aux_out");
-  if (a->epilogue == B2_EPI_BIAS_DROPOUT_RESIDUAL && a->dropout_p > 0.f)
-    B2_REQUIRE(a->rng_state != nullptr, "b2_gemm_bf16: dropout needs rng_state");
+  else
+    B2_REQUIRE(a->aux_out == nullptr, "b2_gemm_bf16: only BIAS_GELU writes aux_out: aux_out must be NULL");
+  // bias, aux_in and aux_out move in 16-byte vectors (ldg16, cp.async, uint4 stores)
+  B2_REQUIRE((uintptr_t)a->bias % 16 == 0, "b2_gemm_bf16: bias must be 16-byte aligned");
+  B2_REQUIRE((uintptr_t)a->aux_in % 16 == 0, "b2_gemm_bf16: aux_in must be 16-byte aligned");
+  B2_REQUIRE((uintptr_t)a->aux_out % 16 == 0, "b2_gemm_bf16: aux_out must be 16-byte aligned");
   B2_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, "b2_gemm_bf16: dropout_p out of range");
-
-  Choice c = choose_config(*a);
-  // force_kernel (1 / 2) selects between kernels on other builds; this one has a single GEMM kernel
-  if (a->force_bn == 128 || a->force_bn == 256) {
+  if (e == B2_EPI_BIAS_DROPOUT_RESIDUAL && a->dropout_p > 0.f)
+    B2_REQUIRE(a->rng_state != nullptr, "b2_gemm_bf16: dropout needs rng_state");
+  if (e != B2_EPI_BIAS_DROPOUT_RESIDUAL)
+    B2_REQUIRE(a->dropout_p == 0.f, "b2_gemm_bf16: epilogue %d applies no dropout: dropout_p must be 0", e);
+  // column sums are taken in the bf16 epilogue of a whole (unsplit) tile
+  B2_REQUIRE(a->colsum_out == nullptr || !f32_out, "b2_gemm_bf16: epilogue %d has no bf16 output: colsum_out must be "
+             "NULL", e);
+  B2_REQUIRE(a->colsum_out == nullptr || a->force_splits <= 1, "b2_gemm_bf16: colsum_out needs force_splits <= 1");
+  if (a->force_bn == 128 || a->force_bn == 256)
     B2_REQUIRE(a->N % a->force_bn == 0 || a->force_bn == 128, "b2_gemm_bf16: force_bn does not divide N");
-    c.bn = a->force_bn;
-  }
-  if (a->force_splits >= 1) {
-    B2_REQUIRE(a->force_splits == 1 ||
-                   a->epilogue == B2_EPI_ACCUM_F32 ||
-                   (a->epilogue == B2_EPI_NONE && a->workspace &&
+  if (a->force_splits > 1)
+    B2_REQUIRE(e == B2_EPI_ACCUM_F32 ||
+                   (e == B2_EPI_NONE && a->workspace &&
                     (size_t)a->force_splits * a->M * a->N * 4 <= (size_t)a->workspace_bytes),
                "b2_gemm_bf16: split-K needs EPI_ACCUM_F32, or EPI_NONE and a large enough workspace");
-    c.splits = a->force_splits;
-  }
+  B2_REQUIRE(!(a->a_major == B2_MAJOR_MN && a->b_major != B2_MAJOR_MN),
+             "b2_gemm_bf16: layout TT (A MN-major, B K-major) is not on the path");
+  return 0;
+}
+
+// one problem that has passed check_args: pick the configuration and launch
+static int32_t launch_checked(const b2_gemm_args_t* a, cudaStream_t stream) {
+  Choice c = choose_config(*a);
+  // force_kernel (1 / 2) selects between kernels on other builds; this one has a single GEMM kernel
+  if (a->force_bn == 128 || a->force_bn == 256) c.bn = a->force_bn;
+  if (a->force_splits >= 1) c.splits = a->force_splits;
   const bool a_mn = a->a_major == B2_MAJOR_MN, b_mn = a->b_major == B2_MAJOR_MN;
-  B2_REQUIRE(!(a_mn && !b_mn), "b2_gemm_bf16: layout TT (A MN-major, B K-major) is not on the path");
 
 #define B2_DISPATCH(BN_)                                                          \
   if (c.bn == BN_) {                                                              \
@@ -410,24 +427,32 @@ extern "C" int32_t b2_gemm_bf16(const b2_gemm_args_t* a, void* stream_) {
   return -2;
 }
 
+extern "C" int32_t b2_gemm_bf16(const b2_gemm_args_t* a, void* stream_) {
+  const int32_t st = check_args(a);
+  if (st) return st;
+  return launch_checked(a, (cudaStream_t)stream_);
+}
+
 extern "C" int32_t b2_gemm_bf16_grouped(const b2_gemm_args_t* args, int32_t count, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   B2_REQUIRE(args != nullptr && count >= 1, "b2_gemm_bf16_grouped: no problems");
+  for (int i = 0; i < count; ++i) {   // reject the whole table before any of it runs
+    const int32_t st = check_args(&args[i]);
+    if (st) return st;
+  }
   // the one-launch path covers what the weight-gradient step needs: TN layouts, plain bf16 output, 256-wide tiles,
-  // one contraction length; anything else is issued problem by problem (same results, more launches)
+  // one contraction length; anything else is issued problem by problem (same results, more launches).  Every
+  // problem has passed check_args, so only the tiling conditions are left to test here.
   bool groupable = count <= kMaxGroup;
   for (int i = 0; i < count && groupable; ++i) {
     const b2_gemm_args_t& a = args[i];
     groupable = a.a_major == B2_MAJOR_MN && a.b_major == B2_MAJOR_MN && a.epilogue == B2_EPI_NONE &&
-                a.bias == nullptr && a.colsum_out == nullptr && a.N % 256 == 0 && a.K == args[0].K && a.M > 0 &&
-                a.K > 0 && a.A && a.B && a.D && a.K % 8 == 0 && a.lda % 8 == 0 && a.ldb % 8 == 0 &&
-                a.ldd % 8 == 0 && ((uintptr_t)a.A % 16 == 0) && ((uintptr_t)a.B % 16 == 0) &&
-                ((uintptr_t)a.D % 16 == 0) && a.force_splits <= 1 &&
+                a.colsum_out == nullptr && a.N % 256 == 0 && a.K == args[0].K && a.force_splits <= 1 &&
                 (a.force_bn == 0 || a.force_bn == 256);
   }
   if (!groupable) {
     for (int i = 0; i < count; ++i) {
-      const int32_t st = b2_gemm_bf16(&args[i], stream_);
+      const int32_t st = launch_checked(&args[i], stream);
       if (st) return st;
     }
     return 0;
