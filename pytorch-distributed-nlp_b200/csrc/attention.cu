@@ -14,7 +14,12 @@
 // one product and as an MN-major operand for another (e.g. dO is A of dP = dO V^T and B of dV = P^T dO), so nothing
 // is ever transposed in memory.  Results leave the same way: the context tile, dQ, dK and dV are written into
 // operand tiles the last products have released and stored with TMA.  Kernels: attention_fwd128_kernel (seq 128),
-// attention_fwd_kernel (any seq <= 512, online softmax), attention_bwd_kernel<kOneQ>.
+// attention_fwd_kernel (any seq <= 512, online softmax), attention_bwd128_kernel (seq 128), attention_bwd_kernel.
+// The seq-128 backward is persistent: a CTA walks (batch, head) items and loads the next item's tiles under this
+// one's compute.
+#include <algorithm>
+#include <cstdlib>
+
 #include "common.cuh"
 #include "../../include/b2_ddp_bert.h"
 
@@ -403,29 +408,69 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attention_fwd128_kernel(const 
   }
 }
 
+// the key-padding mask of batch row b as four 32-key words (bit set: masked), in every warp
+__device__ __forceinline__ void mask_words128(const long long* mask, int b, int lane, uint32_t (&mw)[4]) {
+#pragma unroll
+  for (int w = 0; w < 4; ++w)
+    mw[w] = __ballot_sync(0xffffffffu, mask != nullptr && mask[(size_t)b * 128 + 32 * w + lane] == 0);
+}
+// the dropout decisions of one 128-key row (quad_keep16) as two 64-bit words, keys 0-63 and 64-127: bit c % 64 set
+// when key c is kept -- the keep_bits layout
+__device__ __forceinline__ void quad_keep128(const DropCtx& d, unsigned long long base, int lane,
+                                             unsigned long long (&kept)[2]) {
+  uint32_t keep[16];
+  quad_keep16(d, base, lane, keep);
+  kept[0] = kept[1] = 0ull;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    kept[0] |= (unsigned long long)(keep[j] & 0xffu) << (8 * j);
+    kept[1] |= (unsigned long long)(keep[j + 8] & 0xffu) << (8 * j);
+  }
+}
+
+// A thread's 32 columns of one accumulator row (Frag::col: 8 j + 2 t + e) as the bits 2 j + e of one word, so that
+// the per-element loops test a bit at a constant position: frag_bit(i) is that bit for accumulator index i.
+__device__ __forceinline__ constexpr int frag_bit(int i) { return 2 * (i >> 2) + (i & 1); }
+template <bool kSeg>   // key_masked for this thread's columns
+__device__ __forceinline__ uint32_t frag_masked_bits(const uint32_t (&mw)[4], int seg_word, int t) {
+  uint32_t m = 0;
+#pragma unroll
+  for (int i = 0; i < 32; ++i) m |= (uint32_t)key_masked<kSeg>(mw, seg_word, 8 * (i >> 1) + 2 * t + (i & 1)) << i;
+  return m;
+}
+// keep decisions of this thread's columns, from a row's two keep_bits words
+__device__ __forceinline__ uint32_t frag_keep_bits(const unsigned long long (&kept)[2], int t) {
+  const unsigned long long k0 = kept[0] >> (2 * t), k1 = kept[1] >> (2 * t);
+  uint32_t m = 0;
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    const int j = i >> 1, e = i & 1;
+    m |= (uint32_t)(((j < 8 ? k0 : k1) >> (8 * (j & 7) + e)) & 1ull) << i;
+  }
+  return m;
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // backward: grid (seq/128 kv blocks, heads, batch); loops over query blocks
 // ------------------------------------------------------------------------------------------------------------
 //
-// kOneQ (seq == 128, the benchmark shape): shared memory 7 tiles instead of 8 -- V is dead once dP = dO V^T has
-// completed, so the first 64-key half of P lives in V's tile.  O comes in with Q and dO (into P's second half, free
-// until the dS pass) so delta = rowsum(dO * O) reads two swizzled smem rows while S and dP are being multiplied; dQ /
-// dK / dV leave through the operand tiles that the last products have released, as TMA tile stores.
-template <bool kOneQ, bool kSeg = false>   // kSeg (with kOneQ): packed bins, per-row segment mask (p.seg)
+// seq > 128 (attention_bwd128_kernel takes seq == 128).  O comes in with Q and dO (into P's second half, free until
+// the dS pass) so delta = rowsum(dO * O) reads two swizzled smem rows while S and dP are being multiplied; dK / dV
+// leave through the operand tiles that the last products have released, as TMA tile stores.
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
                      const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_dqkv,
                      const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align_1024(smem_raw);
-  constexpr int kTiles = kOneQ ? 7 : 8;
+  constexpr int kTiles = 8;
   uint8_t* sK = smem;
   uint8_t* sV = smem + TILE_BYTES;
   uint8_t* sQ = smem + 2 * TILE_BYTES;
   uint8_t* sdO = smem + 3 * TILE_BYTES;
-  uint8_t* sP0 = kOneQ ? sV : smem + 4 * TILE_BYTES;                       // keys 0-63 of P
-  uint8_t* sP1 = kOneQ ? smem + 4 * TILE_BYTES : smem + 5 * TILE_BYTES;    // keys 64-127 of P; holds O before that
-  uint8_t* sdS = smem + (kOneQ ? 5 : 6) * TILE_BYTES;                      // 2 tiles
+  uint8_t* sP0 = smem + 4 * TILE_BYTES;   // keys 0-63 of P
+  uint8_t* sP1 = smem + 5 * TILE_BYTES;   // keys 64-127 of P; holds O before that
+  uint8_t* sdS = smem + 6 * TILE_BYTES;   // 2 tiles
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kTiles * TILE_BYTES);
   uint64_t* bar_kv = &bars[0];
   uint64_t* bar_q = &bars[1];
@@ -455,11 +500,6 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
   }
   __syncthreads();
   const uint32_t mw[4] = {s_mbits[0], s_mbits[1], s_mbits[2], s_mbits[3]};
-  int seg[2] = {0, 0};
-  if (kOneQ && kSeg) {               // packed bins (seq == 128): fr.r is a query row of the only block
-    seg[0] = p.seg[(size_t)b * 128 + fr.r];
-    seg[1] = p.seg[(size_t)b * 128 + fr.r + 8];
-  }
 
   const int row0 = b * p.seq;
   const int col_q = h * 64, col_k = p.hidden + h * 64, col_v = 2 * p.hidden + h * 64;
@@ -507,19 +547,12 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
       s_delta[tid] = delta;
     }
     float lse2[2], xm[2], delta[2];
-    unsigned long long kept[2][2];
-    const bool have_bits = kOneQ && p.keep_bits != nullptr;
     uint32_t keep[2][16];
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
       const int q_row = i * 128 + fr.r + 8 * u;   // this thread's query rows in the sequence
       lse2[u] = p.lse[bh * p.seq + q_row] * kLog2e;
-      if (have_bits) {
-        kept[u][0] = p.keep_bits[(bh * 128 + q_row) * 2];
-        kept[u][1] = p.keep_bits[(bh * 128 + q_row) * 2 + 1];
-      } else {
-        quad_keep16(drop, ((bh * p.seq + q_row) * p.seq) + jb * 128, lane, keep[u]);
-      }
+      quad_keep16(drop, ((bh * p.seq + q_row) * p.seq) + jb * 128, lane, keep[u]);
     }
     wgmma_wait<0>();
     wgmma_fence_regs(s);
@@ -538,9 +571,9 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
       for (int e = 0; e < 2; ++e) {
         const int cc = c + e;
         float x = fmaf(s[ii + e], c2, -lse2[u]);
-        if (key_masked<kOneQ && kSeg>(mw, seg[u], cc)) x = xm[u];   // what score*c2 + (-3.4e38) rounds to (row_masked_x)
+        if (key_masked<false>(mw, 0, cc)) x = xm[u];   // what score*c2 + (-3.4e38) rounds to (row_masked_x)
         const float pr = ex2_approx(x);
-        const bool kp = have_bits ? ((kept[u][cc >> 6] >> (cc & 63)) & 1ull) : ((keep[u][cc >> 3] >> (cc & 7)) & 1u);
+        const bool kp = (keep[u][cc >> 3] >> (cc & 7)) & 1u;
         pd[e] = kp ? pr * drop.scale : 0.f;
         const float dpv = kp ? dp[ii + e] * drop.scale : 0.f;
         ds[e] = pr * (dpv - delta[u]) * p.scale;
@@ -591,11 +624,11 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
       for (int e = 0; e < 32; ++e)
         atomicAdd(p.dq_accum + (size_t)(row0 + i * 128 + fr.r + 8 * Frag::hi(e)) * p.hidden + h * 64 + fr.col(e), dq[e]);
     }
-    if (!kOneQ) __syncthreads();   // the next query block reuses the tiles
+    __syncthreads();   // the next query block reuses the tiles
   }
 
   // dK, dV of this block's keys -> K's and V's tiles -> TMA stores
-  __syncthreads();   // every product has read K and V (kOneQ: P in V's tile)
+  __syncthreads();   // every product has read K and V
 #pragma unroll
   for (int e = 0; e < 32; e += 2) {
     const int r = fr.r + 8 * Frag::hi(e), c = fr.col(e);
@@ -618,6 +651,198 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// backward, seq == 128 (the benchmark shape): one query block and one key block per (batch, head) item.  Persistent:
+// CTA c takes the items c, c + gridDim.x, ... through two operand buffers of five tiles (K, V, Q, dO, O), the next item's loaded into the
+// other buffer once this item's have landed.  Within a buffer, V is dead once dP = dO V^T has completed, so the first
+// 64-key half of P lives in V's tile, and the second in O's, which the delta = rowsum(dO * O) pass has read by then
+// (two swizzled smem rows per query row, while S and dP are being multiplied).  dQ / dK / dV leave through the Q, K
+// and V tiles once the last products have released them, as TMA tile stores that must have read the buffer out
+// before it is refilled.  The dS scratch (2 tiles) is shared by the items.
+// ------------------------------------------------------------------------------------------------------------
+template <bool kSeg>   // kSeg: packed bins (per-row segment mask, p.seg) instead of the key-padding mask
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attention_bwd128_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
+                        const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_dqkv,
+                        const AttnParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_align_1024(smem_raw);   // buffer u: tiles [5 u, 5 u + 5) = K, V, Q, dO, O
+  uint8_t* sdS = smem + 10 * TILE_BYTES;       // 2 tiles
+  uint64_t* bar_load = reinterpret_cast<uint64_t*>(smem + 12 * TILE_BYTES);   // [2], one per buffer
+  float* s_delta = reinterpret_cast<float*>(smem + 12 * TILE_BYTES + 64);      // [128]
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const Frag fr(warp, lane);
+  const int items = p.batch * p.heads;   // item = b * heads + h; the grid never exceeds it
+  const int col_q = 0, col_k = p.hidden, col_v = 2 * p.hidden;   // + h * 64
+
+  if (tid == 0) {
+    tma_prefetch_desc(&tmap_qkv);
+    tma_prefetch_desc(&tmap_do);
+    tma_prefetch_desc(&tmap_o);
+    tma_prefetch_desc(&tmap_dqkv);
+    mbar_init(&bar_load[0], 1);
+    mbar_init(&bar_load[1], 1);
+    fence_mbar_init();
+  }
+  pdl_wait();               // PDL: setup above overlapped the predecessor's tail; global reads start below
+  pdl_launch_dependents();
+  __syncthreads();          // barriers initialised
+  // K, V, Q, dO, O of an item -> buffer u
+  auto load = [&](int u, int it) {
+    uint8_t* t = smem + u * 5 * TILE_BYTES;
+    const int h = it % p.heads, row = (it / p.heads) * 128;
+    mbar_expect_tx(&bar_load[u], 5 * TILE_BYTES);
+    tma_load_2d(t, &tmap_qkv, &bar_load[u], col_k + h * 64, row);
+    tma_load_2d(t + TILE_BYTES, &tmap_qkv, &bar_load[u], col_v + h * 64, row);
+    tma_load_2d(t + 2 * TILE_BYTES, &tmap_qkv, &bar_load[u], col_q + h * 64, row);
+    tma_load_2d(t + 3 * TILE_BYTES, &tmap_do, &bar_load[u], h * 64, row);
+    tma_load_2d(t + 4 * TILE_BYTES, &tmap_o, &bar_load[u], h * 64, row);
+  };
+  if (tid == 0) load(0, blockIdx.x);
+  const float c2 = p.scale * kLog2e;
+  // the n-th item of this CTA uses buffer n % 2, whose mbarrier then completes its (n / 2)-th phase
+  for (int item = blockIdx.x, n = 0; item < items; item += gridDim.x, ++n) {
+    const int buf = n & 1;
+    const int b = item / p.heads, h = item % p.heads;
+    const size_t bh = (size_t)item;
+    // read per item: the Philox key would otherwise hold registers through the products
+    const DropCtx drop = make_drop_ctx(p.rng, p.rng_site, p.dropout_p);
+    uint8_t* sK = smem + buf * 5 * TILE_BYTES;
+    uint8_t* sV = sK + TILE_BYTES;          // later: keys 0-63 of P, then dV on its way out
+    uint8_t* sQ = sK + 2 * TILE_BYTES;
+    uint8_t* sdO = sK + 3 * TILE_BYTES;
+    uint8_t* sO = sK + 4 * TILE_BYTES;      // later: keys 64-127 of P
+    // mask, segments, log-sum-exp and dropout decisions: read while the operands are in flight
+    uint32_t mw[4], masked[2], keep[2];
+    mask_words128(p.mask, b, lane, mw);
+    float lse2[2];
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const size_t row = bh * 128 + fr.r + 8 * u;
+      masked[u] = frag_masked_bits<kSeg>(mw, kSeg ? p.seg[(size_t)b * 128 + fr.r + 8 * u] : 0, fr.t);
+      lse2[u] = p.lse[row] * kLog2e;
+      unsigned long long kept[2];
+      if (p.keep_bits != nullptr) {
+        kept[0] = p.keep_bits[row * 2];
+        kept[1] = p.keep_bits[row * 2 + 1];
+      } else {
+        quad_keep128(drop, row * 128, lane, kept);
+      }
+      keep[u] = frag_keep_bits(kept, fr.t);
+    }
+
+    mbar_wait(&bar_load[buf], (n >> 1) & 1);
+    float s[64], dp[64];
+    wgmma_fence();
+    mma_nt_128(s, sQ, sK, wg);
+    mma_nt_128(dp, sdO, sV, wg);
+    wgmma_commit();
+    const int next = item + gridDim.x;
+    if (tid == 0 && next < items) {
+      // the other buffer last held item - gridDim.x: every thread is past its products (barriers since), and its
+      // dQ / dK / dV tiles must have been read out by the TMA stores before the loads overwrite them
+      tma_store_wait_read();
+      load(buf ^ 1, next);
+    }
+    // delta = rowsum(dO * O) from the two smem tiles while the products run
+    if (tid < 128) {
+      float delta = 0.f;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        const int off = tid * 128 + ((c ^ (tid & 7)) << 4);
+        const uint4 a = *reinterpret_cast<const uint4*>(sO + off);
+        const uint4 g = *reinterpret_cast<const uint4*>(sdO + off);
+        delta += bf16_lo(a.x) * bf16_lo(g.x) + bf16_hi(a.x) * bf16_hi(g.x) + bf16_lo(a.y) * bf16_lo(g.y) +
+                 bf16_hi(a.y) * bf16_hi(g.y) + bf16_lo(a.z) * bf16_lo(g.z) + bf16_hi(a.z) * bf16_hi(g.z) +
+                 bf16_lo(a.w) * bf16_lo(g.w) + bf16_hi(a.w) * bf16_hi(g.w);
+      }
+      s_delta[tid] = delta;
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    wgmma_fence_regs(dp);
+    __syncthreads();   // delta is in; O has been read and every product has read V: P may overwrite both
+    float xm[2], delta[2];
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      delta[u] = s_delta[fr.r + 8 * u];
+      xm[u] = row_masked_x(lse2[u], p.neg_log2_seq);
+    }
+#pragma unroll
+    for (int ii = 0; ii < 64; ii += 2) {
+      const int u = Frag::hi(ii), c = fr.col(ii);
+      float pd[2], ds[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float x = fmaf(s[ii + e], c2, -lse2[u]);
+        if ((masked[u] >> frag_bit(ii + e)) & 1u) x = xm[u];   // what score*c2 + (-3.4e38) rounds to (row_masked_x)
+        const float pr = ex2_approx(x);
+        const bool kp = (keep[u] >> frag_bit(ii + e)) & 1u;
+        pd[e] = kp ? pr * drop.scale : 0.f;
+        const float dpv = kp ? dp[ii + e] * drop.scale : 0.f;
+        ds[e] = pr * (dpv - delta[u]) * p.scale;
+      }
+      st_pair(sV, sO, fr.r + 8 * u, c, pd[0], pd[1]);
+      st_pair(sdS, sdS + TILE_BYTES, fr.r + 8 * u, c, ds[0], ds[1]);
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    float dv[32], dk[32], dq[32];
+    wgmma_fence();
+    {
+      // dV[key, d] = sum_q P[q, key] dO[q, d]      (A = P as MN-major: rows = q = K index; this warpgroup's 64 keys
+      // are one sub-tile)
+      const uint32_t ap = smem_u32(wg ? sO : sV), ado = smem_u32(sdO);
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        wgmma_bf16<64, 1, 1>(dv, make_smem_desc(ap + k * 2048, 8192, 1024), make_smem_desc(ado + k * 2048, 8192, 1024),
+                             k > 0 ? 1u : 0u);
+      // dK[key, d] = sum_q dS[q, key] Q[q, d]
+      const uint32_t ads = smem_u32(sdS), aq = smem_u32(sQ), ak = smem_u32(sK);
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        wgmma_bf16<64, 1, 1>(dk, make_smem_desc(ads + wg * TILE_BYTES + k * 2048, 8192, 1024),
+                             make_smem_desc(aq + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
+      // dQ[q, d] = sum_key dS[q, key] K[key, d]     (A = dS as K-major)
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        wgmma_bf16<64, 0, 1>(dq, make_smem_desc(ads + (k >> 2) * TILE_BYTES + wg * 8192 + (k & 3) * 32, 16, 1024),
+                             make_smem_desc(ak + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(dv);
+    wgmma_fence_regs(dk);
+    wgmma_fence_regs(dq);
+    __syncthreads();   // every product has read Q, K and V (P): dQ, dK, dV may overwrite them
+#pragma unroll
+    for (int e = 0; e < 32; e += 2) {
+      const int r = fr.r + 8 * Frag::hi(e), c = fr.col(e);
+      (void)pack_bf16_round(dq[e], dq[e + 1]);   // bf16-rounded values (what the GEMMs will read) for the sums
+      (void)pack_bf16_round(dk[e], dk[e + 1]);
+      (void)pack_bf16_round(dv[e], dv[e + 1]);
+      st_pair(sQ, sQ, r, c, dq[e], dq[e + 1]);
+      st_pair(sK, sK, r, c, dk[e], dk[e + 1]);
+      st_pair(sV, sV, r, c, dv[e], dv[e + 1]);
+    }
+    if (p.dbias != nullptr) {
+      frag_colsum64(dq, lane, p.dbias + col_q + h * 64);
+      frag_colsum64(dk, lane, p.dbias + col_k + h * 64);
+      frag_colsum64(dv, lane, p.dbias + col_v + h * 64);
+    }
+    fence_proxy_async_smem();   // generic-proxy tile writes above -> visible to the TMA engine
+    __syncthreads();
+    if (tid == 0) {
+      tma_store_2d(&tmap_dqkv, sQ, col_q + h * 64, b * 128);
+      tma_store_2d(&tmap_dqkv, sK, col_k + h * 64, b * 128);
+      tma_store_2d(&tmap_dqkv, sV, col_v + h * 64, b * 128);
+      tma_store_commit();
+    }
+  }
+  if (tid == 0) tma_store_wait();
+}
+
 // fp32 dQ accumulator [tokens, hidden] -> the Q column block of d_qkv (bf16 [tokens, 3*hidden])
 __global__ void dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict__ d_qkv, long long tokens,
                                   int hidden) {
@@ -637,8 +862,29 @@ __global__ void dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* 
 constexpr int kFwdSmem = 5 * TILE_BYTES + 128 + 1024;
 constexpr int kFwd128Smem = 3 * TILE_BYTES + 64 + 1024;
 constexpr int kBwdSmem = 8 * TILE_BYTES + 64 + 512 + 1024;
+constexpr int kBwd128Smem = 12 * TILE_BYTES + 64 + 512 + 1024;    // two buffers of K, V, Q, dO, O + dS
 
-constexpr int kBwdSmemOneQ = 7 * TILE_BYTES + 64 + 512 + 1024;
+// Grid of the persistent seq-128 backward: one CTA per resident slot (`per_sm` x the SM count), at most one per (batch,
+// head) item.  B2_DEBUG_ATTN_CTAS=n caps it, so that tests can check that results do not depend on how the items are
+// spread over the CTAs.
+static int32_t persistent_grid(int per_sm, int64_t items, unsigned* grid) {
+  B2_REQUIRE(per_sm > 0, "attention: the seq-128 kernel does not fit on an SM");
+  B2_REQUIRE(items < (int64_t)1 << 31, "attention: batch * heads = %lld exceeds int", (long long)items);
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0;
+    B2_CUDA(cudaGetDevice(&dev));
+    B2_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  }
+  int64_t n = std::min<int64_t>(items, (int64_t)per_sm * sms);
+  if (const char* cap = getenv("B2_DEBUG_ATTN_CTAS")) {
+    const long long c = atoll(cap);
+    B2_REQUIRE(c > 0, "B2_DEBUG_ATTN_CTAS=%s: expected a positive CTA count", cap);
+    n = std::min<int64_t>(n, c);
+  }
+  *grid = (unsigned)n;
+  return 0;
+}
 
 static int32_t check_attn_shapes(const char* who, int64_t batch, int64_t seq, int64_t heads, int64_t head_dim) {
   B2_REQUIRE(batch > 0 && seq > 0 && heads > 0, "%s: empty problem (batch=%lld seq=%lld heads=%lld)", who,
@@ -771,27 +1017,33 @@ static int32_t attention_bwd_impl(const void* qkv, const int64_t* attention_mask
   p.dbias = dbias_accum;
   p.keep_bits = (seq == 128 && dropout_p > 0.f) ? (unsigned long long*)keep_bits : nullptr;
   if (p.dq_accum) B2_CUDA(cudaMemsetAsync(p.dq_accum, 0, (size_t)tokens * hidden * 4, stream));
-  static bool attr = false;
-  if (!attr) {
-    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmem));
-    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 kBwdSmemOneQ));
-    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
+  static int per_sm = 0;   // resident CTAs per SM of attention_bwd128_kernel (1)
+  if (per_sm == 0) {
+    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmem));
+    B2_CUDA(cudaFuncSetAttribute(attention_bwd128_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 kBwd128Smem));
+    B2_CUDA(cudaFuncSetAttribute(attention_bwd128_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                  cudaSharedmemCarveoutMaxShared));
-    B2_CUDA((cudaFuncSetAttribute(attention_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  kBwdSmemOneQ)));
-    B2_CUDA((cudaFuncSetAttribute(attention_bwd_kernel<true, true>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                  cudaSharedmemCarveoutMaxShared)));
-    attr = true;
+    B2_CUDA(cudaFuncSetAttribute(attention_bwd128_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 kBwd128Smem));
+    B2_CUDA(cudaFuncSetAttribute(attention_bwd128_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 cudaSharedmemCarveoutMaxShared));
+    B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, attention_bwd128_kernel<false>, ATT_THREADS,
+                                                          kBwd128Smem));
   }
-  dim3 grid((unsigned)(seq / 128), (unsigned)heads, (unsigned)batch);
-  if (seq == 128 && segments != nullptr) {
-    B2_LAUNCH((attention_bwd_kernel<true, true>), grid, ATT_THREADS, kBwdSmemOneQ, stream, tm_qkv, tm_do, tm_o, tm_dqkv,
-              p);
-  } else if (seq == 128) {
-    B2_LAUNCH(attention_bwd_kernel<true>, grid, ATT_THREADS, kBwdSmemOneQ, stream, tm_qkv, tm_do, tm_o, tm_dqkv, p);
+  if (seq == 128) {
+    unsigned grid = 0;
+    st = persistent_grid(per_sm, batch * heads, &grid);
+    if (st) return st;
+    if (segments != nullptr) {
+      B2_LAUNCH(attention_bwd128_kernel<true>, grid, ATT_THREADS, kBwd128Smem, stream, tm_qkv, tm_do, tm_o, tm_dqkv, p);
+    } else {
+      B2_LAUNCH(attention_bwd128_kernel<false>, grid, ATT_THREADS, kBwd128Smem, stream, tm_qkv, tm_do, tm_o, tm_dqkv,
+                p);
+    }
   } else {
-    B2_LAUNCH(attention_bwd_kernel<false>, grid, ATT_THREADS, kBwdSmem, stream, tm_qkv, tm_do, tm_o, tm_dqkv, p);
+    dim3 grid((unsigned)(seq / 128), (unsigned)heads, (unsigned)batch);
+    B2_LAUNCH(attention_bwd_kernel, grid, ATT_THREADS, kBwdSmem, stream, tm_qkv, tm_do, tm_o, tm_dqkv, p);
   }
   B2_CUDA(cudaGetLastError());
   count_launches(1);

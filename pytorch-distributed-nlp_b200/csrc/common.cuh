@@ -268,6 +268,12 @@ __device__ __forceinline__ void tma_store_commit_and_wait() {
   asm volatile("cp.async.bulk.commit_group;" ::: "memory");
   asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
+// the same in steps, for a CTA that goes on working while its stores drain: close the bulk group; wait until every
+// store issued by this thread has read its smem source (the tile may then be overwritten); wait until they have
+// completed (before the CTA exits)
+__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void tma_store_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
 // clusters and distributed shared memory
