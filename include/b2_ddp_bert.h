@@ -59,6 +59,8 @@ typedef struct b2_gemm_args {
   const void* B;          /* bf16. b_major K : B[n*ldb + k];  MN : B[k*ldb + n]                              */
   int64_t ldb;
   int32_t b_major;
+  /* Every leading dimension covers the row it describes: lda >= K (a_major K) or >= M (MN); ldb >= K (K) or
+     >= N (MN); ldd >= N; ld_aux_in / ld_aux_out >= N where the epilogue reads / writes them (not read otherwise). */
   void* D;                /* bf16 [M, ldd]                                                                   */
   int64_t ldd;
   int32_t epilogue;
@@ -100,7 +102,10 @@ int32_t b2_gemm_bf16_grouped(const b2_gemm_args_t* args, int32_t count, void* st
  * rounded to bf16 (kept for the backward), y the normalised output as bf16 (the next GEMM's operand), y_f32 (optional)
  * the same as fp32 (the next block's residual), mean / rstd (fp32 [M]) the row statistics -- computed from the
  * UNROUNDED fp32 sum.  A row's N columns are spread over a cluster of N / 256 CTAs; the row statistics travel
- * through distributed shared memory.
+ * through distributed shared memory.  Leading dimensions as for b2_gemm_bf16 (lda, ldb >= K; ldd, ld_aux_in >= N),
+ * and ldy >= N, ldyf >= N when y_f32 is set.  Rejected, because the kernel would not honour them: colsum_out,
+ * aux_out, force_splits > 1, force_bn other than 0 / 256, a workspace.  force_kernel and debug_timing are accepted
+ * and not read.
  * b2_gemm_ln_max_clusters(hidden): how many such clusters the device can hold at once (0 = shape / device not
  * supported: issue b2_gemm_bf16 + b2_layernorm_fwd instead).                                                    */
 int32_t b2_gemm_ln_fwd(const b2_gemm_args_t* args, const void* gamma, const void* beta, float eps, void* y,

@@ -369,17 +369,30 @@ static int32_t check_args(const b2_gemm_args_t* a) {
              "b2_gemm_bf16: K and leading dimensions must be multiples of 8 elements (16 B)");
   B2_REQUIRE(((uintptr_t)a->A % 16 == 0) && ((uintptr_t)a->B % 16 == 0) && ((uintptr_t)a->D % 16 == 0),
              "b2_gemm_bf16: operands must be 16-byte aligned");
+  // a leading dimension shorter than its row would make rows overlap: stores race, loads read the wrong elements
+  const int64_t a_row = a->a_major == B2_MAJOR_MN ? a->M : a->K, b_row = a->b_major == B2_MAJOR_MN ? a->N : a->K;
+  B2_REQUIRE(a->lda >= a_row, "b2_gemm_bf16: lda=%lld is below the row it describes (%lld)", (long long)a->lda,
+             (long long)a_row);
+  B2_REQUIRE(a->ldb >= b_row, "b2_gemm_bf16: ldb=%lld is below the row it describes (%lld)", (long long)a->ldb,
+             (long long)b_row);
+  B2_REQUIRE(a->ldd >= a->N, "b2_gemm_bf16: ldd=%lld is below N=%lld", (long long)a->ldd, (long long)a->N);
   const int e = a->epilogue;
   B2_REQUIRE(e >= B2_EPI_NONE && e <= B2_EPI_ACCUM_F32, "b2_gemm_bf16: bad epilogue %d", e);
   const bool with_bias = e == B2_EPI_BIAS || e == B2_EPI_BIAS_GELU || e == B2_EPI_BIAS_DROPOUT_RESIDUAL;
   const bool f32_out = e == B2_EPI_RESIDUAL_F32 || e == B2_EPI_ACCUM_F32;
   if (with_bias) B2_REQUIRE(a->bias != nullptr, "b2_gemm_bf16: epilogue %d needs a bias", e);
   else           B2_REQUIRE(a->bias == nullptr, "b2_gemm_bf16: epilogue %d adds no bias: bias must be NULL", e);
-  if (e == B2_EPI_BIAS_DROPOUT_RESIDUAL || e == B2_EPI_RESIDUAL || e == B2_EPI_GELU_BWD || e == B2_EPI_RESIDUAL_F32)
+  // the epilogues that read aux_in / write aux_out need a full row of it; elsewhere its ld is not read (0 is fine)
+  if (e == B2_EPI_BIAS_DROPOUT_RESIDUAL || e == B2_EPI_RESIDUAL || e == B2_EPI_GELU_BWD || e == B2_EPI_RESIDUAL_F32) {
     B2_REQUIRE(a->aux_in != nullptr && a->ld_aux_in % 8 == 0, "b2_gemm_bf16: epilogue %d needs aux_in", e);
-  if (e == B2_EPI_BIAS_GELU)
+    B2_REQUIRE(a->ld_aux_in >= a->N, "b2_gemm_bf16: ld_aux_in=%lld is below N=%lld", (long long)a->ld_aux_in,
+               (long long)a->N);
+  }
+  if (e == B2_EPI_BIAS_GELU) {
     B2_REQUIRE(a->aux_out != nullptr && a->ld_aux_out % 8 == 0, "b2_gemm_bf16: BIAS_GELU needs aux_out");
-  else
+    B2_REQUIRE(a->ld_aux_out >= a->N, "b2_gemm_bf16: ld_aux_out=%lld is below N=%lld", (long long)a->ld_aux_out,
+               (long long)a->N);
+  } else
     B2_REQUIRE(a->aux_out == nullptr, "b2_gemm_bf16: only BIAS_GELU writes aux_out: aux_out must be NULL");
   // bias, aux_in and aux_out move in 16-byte vectors (ldg16, cp.async, uint4 stores)
   B2_REQUIRE((uintptr_t)a->bias % 16 == 0, "b2_gemm_bf16: bias must be 16-byte aligned");

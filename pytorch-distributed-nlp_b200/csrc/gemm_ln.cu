@@ -322,6 +322,23 @@ extern "C" int32_t b2_gemm_ln_fwd(const b2_gemm_args_t* a, const void* gamma, co
   B2_REQUIRE(a->epilogue == B2_EPI_BIAS_DROPOUT_RESIDUAL, "b2_gemm_ln_fwd: epilogue must be BIAS_DROPOUT_RESIDUAL");
   B2_REQUIRE(a->A && a->B && a->D && a->bias && a->aux_in && gamma && beta && y && mean && rstd,
              "b2_gemm_ln_fwd: null pointer");
+  // arguments of b2_gemm_bf16 this kernel has no use for: an error rather than a silent no-op
+  B2_REQUIRE(a->colsum_out == nullptr, "b2_gemm_ln_fwd: the fused kernel takes no column sums: colsum_out must be NULL");
+  B2_REQUIRE(a->aux_out == nullptr, "b2_gemm_ln_fwd: the fused kernel writes no aux_out: aux_out must be NULL");
+  B2_REQUIRE(a->force_splits <= 1, "b2_gemm_ln_fwd: force_splits=%d: the fused kernel does not split K",
+             (int)a->force_splits);
+  B2_REQUIRE(a->force_bn == 0 || a->force_bn == 256, "b2_gemm_ln_fwd: force_bn=%d: the fused kernel's tiles are 256 "
+             "wide", (int)a->force_bn);
+  B2_REQUIRE(a->workspace == nullptr, "b2_gemm_ln_fwd: the fused kernel needs no workspace: workspace must be NULL");
+  // a leading dimension shorter than its row would make rows overlap
+  B2_REQUIRE(a->lda >= a->K, "b2_gemm_ln_fwd: lda=%lld is below K=%lld", (long long)a->lda, (long long)a->K);
+  B2_REQUIRE(a->ldb >= a->K, "b2_gemm_ln_fwd: ldb=%lld is below K=%lld", (long long)a->ldb, (long long)a->K);
+  B2_REQUIRE(a->ldd >= a->N, "b2_gemm_ln_fwd: ldd=%lld is below N=%lld", (long long)a->ldd, (long long)a->N);
+  B2_REQUIRE(a->ld_aux_in >= a->N, "b2_gemm_ln_fwd: ld_aux_in=%lld is below N=%lld", (long long)a->ld_aux_in,
+             (long long)a->N);
+  B2_REQUIRE(ldy >= a->N, "b2_gemm_ln_fwd: ldy=%lld is below N=%lld", (long long)ldy, (long long)a->N);
+  B2_REQUIRE(y_f32 == nullptr || ldyf >= a->N, "b2_gemm_ln_fwd: ldyf=%lld is below N=%lld", (long long)ldyf,
+             (long long)a->N);
   B2_REQUIRE(a->K % 8 == 0 && a->lda % 8 == 0 && a->ldb % 8 == 0 && a->ldd % 8 == 0 && a->ld_aux_in % 4 == 0 &&
                  ldy % 8 == 0 && (y_f32 == nullptr || ldyf % 4 == 0),
              "b2_gemm_ln_fwd: K and leading dimensions must be multiples of 16 bytes");

@@ -238,65 +238,3 @@ def test_grouped_weight_gradients(cuda_dev, shapes):
         assert launches == 1
     for (_a, A, B, D) in probs:
         _check(D, A.float().t() @ B.float())
-
-
-@pytest.mark.parametrize("shape", [(4096, 768, 768), (4096, 768, 3072), (2048, 1024, 1024), (2048, 1024, 4096),
-                                   (1000, 768, 768), (200, 1024, 136), (8192, 768, 768)])
-@pytest.mark.parametrize("p", [0.0, 0.1])
-def test_gemm_layernorm_cluster_kernel(cuda_dev, shape, p):
-    """b2_gemm_ln_fwd: dense + bias + dropout + fp32 residual + LayerNorm over a cluster of N / 256 CTAs (row
-    statistics through distributed shared memory) vs torch fp32 on the same operands and the same Philox mask:
-      D     == bf16 of the fp32 sum z (what the backward reads)               -- to one bf16 rounding
-      y_f32 == LayerNorm(z) computed from the UNROUNDED z                     -- to fp32 summation-order accuracy
-      y     == bf16(y_f32) exactly;  mean / rstd of the unrounded z
-    Covers both cluster shapes (N = 768 -> 3 CTAs, N = 1024 -> 4 CTAs), K = 768..4096, a ragged last row block, a K
-    tail, and more row blocks than clusters fit at once (M = 8192)."""
-    M, N, K = shape
-    dev = cuda_dev
-    if L.load().b2_gemm_ln_max_clusters(N) <= 0:
-        pytest.skip("device cannot co-schedule such a cluster")
-    torch.manual_seed(11)
-    A, B, bias = _rand((M, K), dev), _rand((N, K), dev, 0.05), _rand((N,), dev)
-    X = torch.randn(M, N, device=dev)                                          # fp32 residual
-    gamma, beta = (1 + 0.1 * torch.randn(N, device=dev)).to(torch.bfloat16), _rand((N,), dev, 0.1)
-    rng = _rng_state(dev)
-    s = torch.cuda.current_stream().cuda_stream
-    a = L.GemmArgs()
-    a.M, a.N, a.K = M, N, K
-    a.A, a.lda, a.a_major = A.data_ptr(), K, L.MAJOR_K
-    a.B, a.ldb, a.b_major = B.data_ptr(), K, L.MAJOR_K
-    Z = torch.full((M + 2, N), 7.0, dtype=torch.bfloat16, device=dev)      # guard rows: nothing beyond M is written
-    Y = torch.full((M + 2, N), 7.0, dtype=torch.bfloat16, device=dev)
-    Yf = torch.full((M + 2, N), 7.0, dtype=torch.float32, device=dev)
-    a.D, a.ldd, a.epilogue = Z.data_ptr(), N, L.EPI_BIAS_DROPOUT_RESIDUAL
-    a.bias, a.aux_in, a.ld_aux_in = bias.data_ptr(), X.data_ptr(), N
-    a.dropout_p, a.rng_state, a.rng_site = p, rng.data_ptr(), 5
-    mean, rstd = torch.zeros(M, device=dev), torch.zeros(M, device=dev)
-    L.call("b2_gemm_ln_fwd", a, gamma.data_ptr(), beta.data_ptr(), 1e-12, Y.data_ptr(), N, Yf.data_ptr(), N,
-           mean.data_ptr(), rstd.data_ptr(), s)
-    torch.cuda.synchronize()
-    assert float(Z[M:].float().min()) == 7.0 and float(Y[M:].float().min()) == 7.0 and float(Yf[M:].min()) == 7.0
-    lin = A.float() @ B.float().t() + bias.float()
-    if p > 0:
-        keep = torch.from_numpy(philox_keep_mask(M * N, 77, 3, 5, p).reshape(M, N)).to(dev)
-        lin = lin * keep / (1 - p)
-    z = lin + X
-    # D: bf16(z) up to the accumulation-order noise of the fp32 GEMM: within one bf16 rounding (2^-8 relative) everywhere,
-    # and identical to torch's rounding of its own fp32 z almost everywhere
-    dz = (Z[:M].float() - z).abs()
-    assert bool((dz <= 2.0 ** -7 * (1.0 + z.abs())).all())
-    assert float((Z[:M] != z.to(torch.bfloat16)).float().mean()) < 2e-2
-    mu = z.mean(1)
-    var = z.var(1, unbiased=False)
-    assert float((mean - mu).abs().max()) <= 2e-5 * (1 + float(mu.abs().max()))
-    assert float(((rstd - torch.rsqrt(var + 1e-12)) * torch.sqrt(var)).abs().max()) <= 2e-5
-    ref = torch.nn.functional.layer_norm(z, (N,), gamma.float(), beta.float(), 1e-12)
-    assert float((Yf[:M] - ref).abs().max()) <= 2e-4 * (1 + float(ref.abs().max()))
-    assert torch.equal(Y[:M], Yf[:M].to(torch.bfloat16))
-    # without the fp32 output
-    Y2 = torch.zeros(M, N, dtype=torch.bfloat16, device=dev)
-    a.D = Z.data_ptr()
-    L.call("b2_gemm_ln_fwd", a, gamma.data_ptr(), beta.data_ptr(), 1e-12, Y2.data_ptr(), N, None, 0,
-           mean.data_ptr(), rstd.data_ptr(), s)
-    torch.cuda.synchronize()
-    assert torch.equal(Y2, Y[:M])

@@ -118,13 +118,13 @@ def drop_scale(p):
     return float(np.float32(1.0) / (np.float32(1.0) - np.float32(p))) if p > 0 else 1.0
 
 
-def within(got, ref, bound, family, what):
-    """element-wise |got - ref| <= bound; the worst ratio goes to the parity report.  Anything that is not <= 1 fails,
-    so a NaN (or inf) in the output fails too."""
+def within(got, ref, bound, family, what, tag="gemm_reference"):
+    """element-wise |got - ref| <= bound; the worst ratio goes to the parity report under `tag`.  Anything that is not
+    <= 1 fails, so a NaN (or inf) in the output fails too."""
     err = (got.double() - ref).abs()
     ratio = err / bound.clamp_min(1e-300)
     worst = float(ratio.max()) if err.numel() else 0.0      # NaN if any element is NaN
-    report("gemm_reference", {"family": family, "check": what, "err_over_bound": worst})
+    report(tag, {"family": family, "check": what, "err_over_bound": worst})
     bad = ~(ratio <= 1.0)
     if bool(bad.any()):
         nan = torch.isnan(ratio)
@@ -134,11 +134,11 @@ def within(got, ref, bound, family, what):
             what, worst, idx, float(got[idx]), float(ref[idx]), int(bad.sum()), int(nan.sum())))
 
 
-def same(got, ref, family, what):
+def same(got, ref, family, what, tag="gemm_reference"):
     """bitwise, up to the sign of zero"""
     bad = got != ref
     n = int(bad.sum())
-    report("gemm_reference", {"family": family, "check": what, "mismatches": n})
+    report(tag, {"family": family, "check": what, "mismatches": n})
     if n:
         idx = tuple(bad.nonzero()[0].tolist())
         raise AssertionError("%s: %d elements differ, first at %s (got %r, ref %r)" % (

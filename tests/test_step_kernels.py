@@ -87,32 +87,42 @@ def bf_bound(ref, E):
 
 
 # ---- float64 references -------------------------------------------------------------------------------------------
-def ln_fwd_check(v, mean, rstd, y, g, b, what, keep=None, y_f32=None):
+def ln_fwd_check(v, mean, rstd, y, g, b, what, keep=None, y_f32=None, stats_bound=None, ev=None, check=within):
     """v: the fp32 row values the kernel normalised (as fp64); mean / rstd / y: the kernel's outputs.
-    Statistics against fp64 two-pass statistics; y against fp64 LayerNorm from the kernel's own statistics."""
+    Statistics against fp64 two-pass statistics; y against fp64 LayerNorm from the kernel's own statistics.
+    stats_bound: (e_mu, e_rel) of a kernel whose statistics take another path (default: this file's one-warp row,
+    H/32 + 6 deep chains, two-pass variance around the fp32 mean); ev: how far the kernel's own row values may lie
+    from v (default: they are v); check: the within(got, ref, bound, what) that asserts and reports."""
     H = v.shape[1]
-    depth = H / 32 + 6                      # per-lane sequential sum + 5 shuffle levels
     mu64 = v.mean(1)
     var64 = ((v - mu64[:, None]) ** 2).mean(1)
-    e_mu = depth * U * v.abs().mean(1)
-    within(mean, mu64, e_mu, what + " mean")
-    # two-pass variance around the fp32 mean: the mean's error enters squared; rsqrtf is within 2 ulp
+    if stats_bound is None:
+        depth = H / 32 + 6                  # per-lane sequential sum + 5 shuffle levels
+        e_mu = depth * U * v.abs().mean(1)
+        # two-pass variance around the fp32 mean: the mean's error enters squared; rsqrtf is within 2 ulp
+        e_rel = depth * U + 4 * U + (e_mu ** 2) / (2 * (var64 + EPS))
+    else:
+        e_mu, e_rel = stats_bound
+    check(mean, mu64, e_mu, what + " mean")
     rs64 = 1.0 / torch.sqrt(var64 + EPS)
-    e_rel = depth * U + 4 * U + (e_mu ** 2) / (2 * (var64 + EPS))
-    within(rstd, rs64, e_rel * rs64, what + " rstd")
+    check(rstd, rs64, e_rel * rs64, what + " rstd")
     mu, rs = mean.double()[:, None], rstd.double()[:, None]
     ref = (v - mu) * rs * g.double() + b.double()
     E = 4 * U * (((v - mu) * rs * g.double()).abs() + b.double().abs())
+    if ev is not None:
+        E = E + ev * rs * g.double().abs()
     if keep is not None:
         ref, E = ref * keep, (E * keep + U * (ref * keep).abs())
-    within(y, ref, bf_bound(ref, E), what + " y")
+    check(y, ref, bf_bound(ref, E), what + " y")
     if y_f32 is not None:
-        within(y_f32, ref, E, what + " y_f32")
+        check(y_f32, ref, E, what + " y_f32")
 
 
-def ln_bwd_ref(dy, x, mean, rstd, g):
+def ln_bwd_ref(dy, x, mean, rstd, g, ex_extra=0.0):
     """fp64 LayerNorm backward from the kernel's own fp32 statistics and bf16 input.  Returns dx, the bound of the
-    kernel's fp32 dx, and xhat.  Row sums are chains of H/32 + 8 additions in either kernel form."""
+    kernel's fp32 dx, and xhat.  Row sums are chains of H/32 + 8 additions in either kernel form.
+    ex_extra: a further bound on how far the kernel's xhat lies from (x - mean) * rstd, where x, mean and rstd are
+    not exactly what the kernel reads."""
     H = x.shape[1]
     depth = H / 32 + 8
     dy, x, g = dy.double(), x.double(), g.double()
@@ -122,7 +132,7 @@ def ln_bwd_ref(dy, x, mean, rstd, g):
     s1 = dxh.mean(1, keepdim=True)
     s2 = (dxh * xh).mean(1, keepdim=True)
     dx = rs * (dxh - s1 - xh * s2)
-    ex = 2 * U * (x.abs() + mu.abs()) * rs                     # the kernel's xhat
+    ex = 2 * U * (x.abs() + mu.abs()) * rs + ex_extra          # the kernel's xhat
     e_s1 = depth * U * dxh.abs().mean(1, keepdim=True)
     e_s2 = depth * U * (dxh * xh).abs().mean(1, keepdim=True) + (dxh.abs() * ex).mean(1, keepdim=True)
     E = rs * (6 * U * (dxh.abs() + s1.abs() + (xh * s2).abs()) + e_s1 + (xh.abs() + ex) * e_s2 + ex * s2.abs())
