@@ -910,6 +910,8 @@ static int32_t attention_fwd_impl(const void* qkv, const int64_t* attention_mask
              "attention_fwd: packed bins are 128 tokens long (seq=%lld)", (long long)seq);
   int32_t st = check_attn_shapes("attention_fwd", batch, seq, heads, head_dim);
   if (st) return st;
+  // also rejects NaN, which would otherwise run without dropout
+  B2_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "attention_fwd: dropout_p out of range");
   B2_REQUIRE(!(dropout_p > 0.f) || rng_state, "attention_fwd: dropout needs rng_state");
   const int64_t hidden = heads * 64, tokens = batch * seq;
   CUtensorMap tm;
@@ -988,6 +990,7 @@ static int32_t attention_bwd_impl(const void* qkv, const int64_t* attention_mask
              (long long)seq);
   int32_t st = check_attn_shapes("attention_bwd", batch, seq, heads, head_dim);
   if (st) return st;
+  B2_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "attention_bwd: dropout_p out of range");
   B2_REQUIRE(!(dropout_p > 0.f) || rng_state, "attention_bwd: dropout needs rng_state");
   B2_REQUIRE(seq == 128 || dq_accum != nullptr, "attention_bwd: seq > 128 needs the fp32 dq_accum buffer");
   const int64_t hidden = heads * 64, tokens = batch * seq;

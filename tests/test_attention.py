@@ -204,21 +204,31 @@ def check_against_reference(qkv, dctx, vis, ids, B, S, nh, p, out, scale):
     # Where dS = P (dP - delta) cancels -- nearly one-hot rows at scores of std ~16, one-token segments under dropout
     # -- the true dQ / dK are ~0 and what any bf16 implementation returns is the residue of rounding O (inside delta),
     # P and dS: the float64 emulation below, which rounds exactly where the kernels do, misses the reference by up to
-    # ~12x the block norm there (H100 runs), while it stays within 1.1e-2 wherever the gradient does not cancel.  So
-    # a block's bound is max(GRAD_TOL, 3x the emulation's error): GRAD_TOL wherever bf16 can meet it, and in the
-    # cancelling blocks a bound on the size of the rounding residue (kernel and emulation residues are not correlated
-    # element for element: fp32 vs float64 sums flip bf16 roundings of O and dS).
+    # ~12x the block norm there (H100 runs), while it stays within 1.1e-2 wherever the gradient does not cancel.
+    # Every element is held to the running-error bound of test_attention_reference, and a block to GRAD_TOL wherever
+    # that bound's own rel-L2 is within GRAD_TOL (which the element-wise bound then implies; the block rule stays as
+    # the statement that bf16 meets GRAD_TOL there).  The cancelling blocks get the element-wise bound alone: kernel and
+    # emulation residues are not correlated element for element (in a one-token row under dropout, ctx = bf16(1.109375
+    # v) is an exact bf16 tie for about 1 element in 64, which float64 rounds to even and the kernel by the last bit of
+    # its 1 / l), so no multiple of the emulation's block error bounds the kernel's.
+    from test_attention_reference import check_outputs   # imports this module
+    bounds = torch.empty(B * S, 3 * H, dtype=torch.float64, device=qkv.device)
+    elementwise = check_outputs("test_attention B=%d S=%d heads=%d p=%g x%d" % (B, S, nh, p, scale), qkv, dctx, vis,
+                                B, S, nh, p, keep, ctx, lse, dqkv, grad_bounds=bounds)
+    bad += elementwise.bad
     _, emu = emulate(qkv, vis, B, nh, keep, p, dctx)
     stats = []
     for i, nm in enumerate("qkv"):
         cols = slice(i * H, (i + 1) * H)
-        err = grad_block_err(dqkv[:, cols], qr.grad[:, cols], ids, nh)
-        e_emu = grad_block_err(emu[:, cols], qr.grad[:, cols], ids, nh)
+        ref = qr.grad[:, cols]
+        err = grad_block_err(dqkv[:, cols], ref, ids, nh)
+        e_emu = grad_block_err(emu[:, cols], ref, ids, nh)
         e_ke = grad_block_err(dqkv[:, cols], emu[:, cols], ids, nh)
-        tol = torch.clamp_min(3.0 * e_emu, GRAD_TOL)
-        stats.append("d%s %.3g/%.3g/%.3g" % (nm, float(err.max()), float(e_emu.max()), float(e_ke.max())))
-        if not bool((err <= tol).all()):
-            bad.append(("d" + nm, torch.nonzero(err > tol)[:8].tolist(), float(err.max())))
+        plain = grad_block_err(ref + bounds[:, cols], ref, ids, nh) <= GRAD_TOL
+        stats.append("d%s %.3g/%.3g/%.3g (%d of %d blocks cancel)" % (
+            nm, float(err.max()), float(e_emu.max()), float(e_ke.max()), int((~plain).sum()), plain.numel()))
+        if not bool((err[plain] <= GRAD_TOL).all()):
+            bad.append(("d" + nm, torch.nonzero(plain & (err > GRAD_TOL))[:8].tolist(), float(err[plain].max())))
     print("attention B=%d S=%d heads=%d p=%g x%d  ctx %.3g  worst block rel-L2 kernel-ref/emulation-ref/kernel-emulation"
           " %s" % (B, S, nh, p, scale, worst, "  ".join(stats)))
     assert not bad, bad
@@ -244,10 +254,7 @@ def test_padded_matches_reference(cuda_dev, S, nh, B_min, p, scale):
         check_dbias(out[3], out[2])
 
 
-# Not covered: x4 with dropout.  There the dQ / dK rows of one-token segments (exactly 0 in the reference) come out
-# up to ~50x larger than the emulated algorithm's rounding residue, though still below 1e-3 of the largest block
-# norm; the cause is not yet understood, so the case is left out rather than given a bound that merely fits it.
-@pytest.mark.parametrize("p,scale", [(0.0, 1), (0.1, 1), (0.0, 4)])
+@pytest.mark.parametrize("p,scale", [(0.0, 1), (0.1, 1), (0.0, 4), (0.1, 4)])
 def test_packed_matches_reference(cuda_dev, p, scale):
     """the Trainer's bins, one-token segments, a full bin, segments straddling the 32-key words and 64-key halves,
     a segment ending at row 128 -- per (segment, head), with the keep-bit cache and the fused QKV-bias sums"""
