@@ -264,6 +264,19 @@ int32_t b2_attention_bwd_packed(const void* qkv, const int32_t* segments, const 
                                 const float* lse, int64_t bins, int64_t heads, int64_t head_dim, float dropout_p,
                                 const void* rng_state, uint32_t rng_site, void* d_qkv, float* dbias_accum,
                                 const uint64_t* keep_bits, void* stream);
+/* Bins of `seq` tokens (a multiple of 128, at most 512); segments int32 [bins * seq].  The segments of a bin must be  */
+/* contiguous with every row inside its own (pack_batch builds them so): above 128 the kernels visit only the 128-row */
+/* blocks a segment reaches; other segment words give wrong results for their bin, never an access outside it.      */
+/* At seq == 128 these are b2_attention_{fwd,bwd}_packed.  Above 128 the backward takes                              */
+/* the fp32 dq_accum [bins * seq, heads * 64] as b2_attention_bwd does, dbias_accum must be null (b2_colsum), and     */
+/* keep_bits is not used (the backward regenerates the dropout decisions).                                           */
+int32_t b2_attention_fwd_packed_seq(const void* qkv, const int32_t* segments, int64_t bins, int64_t seq, int64_t heads,
+                                    int64_t head_dim, float dropout_p, const void* rng_state, uint32_t rng_site,
+                                    void* ctx, float* lse, uint64_t* keep_bits, void* stream);
+int32_t b2_attention_bwd_packed_seq(const void* qkv, const int32_t* segments, const void* ctx, const void* d_ctx,
+                                    const float* lse, int64_t bins, int64_t seq, int64_t heads, int64_t head_dim,
+                                    float dropout_p, const void* rng_state, uint32_t rng_site, void* d_qkv,
+                                    float* dq_accum, float* dbias_accum, const uint64_t* keep_bits, void* stream);
 int32_t b2_head_fwd_packed(const void* hidden_states, const int64_t* cls_rows, int64_t batch, int64_t hidden,
                            const void* pool_w, const void* pool_b, const void* cls_w, const void* cls_b,
                            int64_t num_labels, float dropout_p, const void* rng_state, uint32_t rng_site,

@@ -93,6 +93,8 @@ _SIGNATURES = {
                             vp, vp, vp, vp, i64, vp, vp],
     "b2_attention_fwd_packed": [vp, vp, i64, i64, i64, f32, vp, u32, vp, vp, vp, vp],
     "b2_attention_bwd_packed": [vp, vp, vp, vp, vp, i64, i64, i64, f32, vp, u32, vp, vp, vp, vp],
+    "b2_attention_fwd_packed_seq": [vp, vp, i64, i64, i64, i64, f32, vp, u32, vp, vp, vp, vp],
+    "b2_attention_bwd_packed_seq": [vp, vp, vp, vp, vp, i64, i64, i64, i64, f32, vp, u32, vp, vp, vp, vp, vp],
     "b2_head_fwd_packed": [vp, vp, i64, i64, vp, vp, vp, vp, i64, f32, vp, u32, vp, vp, vp],
     "b2_head_bwd_packed": [vp, vp, vp, vp, i64, i64, i64, vp, vp, i64, f32, vp, u32, vp, vp, vp, vp, vp, i32, vp, vp],
     "b2_head_bwd_split": [vp, vp, vp, vp, i64, i64, i64, i64, vp, vp, i64, f32, vp, u32, vp, vp, vp, vp, vp, i32, vp, vp,

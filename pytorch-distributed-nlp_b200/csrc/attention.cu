@@ -16,7 +16,8 @@
 // operand tiles the last products have released and stored with TMA.  Kernels: attention_fwd128_kernel (seq 128),
 // attention_fwd_kernel (any seq <= 512, online softmax), attention_bwd128_kernel (seq 128), attention_bwd_kernel.
 // The seq-128 backward is persistent: a CTA walks (batch, head) items and loads the next item's tiles under this
-// one's compute.
+// one's compute.  Each kernel has a packed-bin form (kSeg) that masks with per-row segments; the long forms visit
+// only the 128-key (fwd) or 128-query (bwd) blocks that some row of the CTA's block can see.
 #include <algorithm>
 #include <cstdlib>
 
@@ -55,8 +56,10 @@ struct AttnParams {
   // optional (seq == 128, dropout on): the forward's dropout decisions, one 64-bit word per (b, h, query row, key
   // half) -- written by the forward, read by the backward instead of regenerating Philox
   unsigned long long* keep_bits;
-  // optional (seq == 128): packed bins -- row r of bin b may attend to keys [lo, hi) of the same bin only,
-  // seg[b * 128 + r] = lo | hi << 16 (pytorch-distributed-nlp_b200/packing.py); replaces the key-padding mask
+  // optional: packed bins -- row r of bin b may attend to keys [lo, hi) of the same bin only,
+  // seg[b * seq + r] = lo | hi << 16 (pytorch-distributed-nlp_b200/packing.py); replaces the key-padding mask.  The
+  // segments of a bin are contiguous and every row lies in its own (lo <= r < hi), which the long kernels' block
+  // skipping relies on.
   const int* seg;
 };
 
@@ -94,6 +97,12 @@ template <bool kSeg>
 __device__ __forceinline__ bool key_masked(const uint32_t (&mw)[4], int seg_word, int col) {
   if (kSeg) return col < (seg_word & 0xffff) || col >= (seg_word >> 16);
   return (mw[col >> 5] >> (col & 31)) & 1u;
+}
+// a row's segment word lo | hi << 16 (bin coordinates) relative to the 128-key block that starts at key k0, both ends
+// clamped to [0, 128]: key_masked<true> then tests the block's columns 0..127
+__device__ __forceinline__ int seg_in_block(int seg_word, int k0) {
+  const int lo = min(max((seg_word & 0xffff) - k0, 0), 128), hi = min(max((seg_word >> 16) - k0, 0), 128);
+  return lo | hi << 16;
 }
 // Backward: the log2-domain exponent of a masked key of a query row whose log2 LSE is lse2.  A row with no visible key
 // (an all-zero attention_mask row) has all scores equal to finfo.min in HF, so its softmax is uniform.  The forward
@@ -139,6 +148,11 @@ __device__ __forceinline__ void mma_pv(float (&o)[32], const uint8_t* p_lo, cons
 // ------------------------------------------------------------------------------------------------------------
 // forward: grid (seq/128, heads, batch)
 // ------------------------------------------------------------------------------------------------------------
+// kSeg: packed bins.  The CTA's 128 query rows see keys in [min lo, max hi) of their segments only, so it visits just
+// the key blocks that range meets.  A skipped block would add exactly 0 (every key masked: p = exp2(kMaskBias - m) =
+// 0, alpha = 1), and a visited block before a row's first visible key is cancelled exactly by the next block's
+// alpha = exp2(kMaskBias - m) = 0, so per sequence the arithmetic is that of the padded kernel.
+template <bool kSeg>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv,
                                                                       const __grid_constant__ CUtensorMap tmap_ctx,
                                                                       const AttnParams p) {
@@ -149,7 +163,8 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_fwd_kernel(const __g
   uint8_t* sV = smem + 2 * TILE_BYTES;
   uint8_t* sP = smem + 3 * TILE_BYTES;  // 2 tiles
   uint64_t* bar_load = reinterpret_cast<uint64_t*>(smem + 5 * TILE_BYTES);
-  uint32_t* s_mbits = reinterpret_cast<uint32_t*>(smem + 5 * TILE_BYTES + 64);  // [seq / 32 <= 16] masked-key bits
+  // [seq / 32 <= 16] masked-key bits; kSeg: [0, 4) each warp's smallest lo, [4, 8) its largest hi
+  uint32_t* s_mbits = reinterpret_cast<uint32_t*>(smem + 5 * TILE_BYTES + 64);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const Frag fr(warp, lane);
@@ -164,12 +179,36 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_fwd_kernel(const __g
   }
   pdl_wait();               // PDL: setup above overlapped the predecessor's tail; global reads start below
   pdl_launch_dependents();
-  for (int c = tid; c < p.seq; c += ATT_THREADS) {   // seq % 128 == 0: whole warps take part in every round
-    const bool masked = p.mask != nullptr && p.mask[(size_t)b * p.seq + c] == 0;
-    const unsigned bits = __ballot_sync(0xffffffffu, masked);
-    if (lane == 0) s_mbits[c >> 5] = bits;
+  int seg[2] = {0, 0};      // kSeg: this thread's two rows' segment words
+  if (kSeg) {
+    seg[0] = p.seg[(size_t)b * p.seq + qb * 128 + fr.r];
+    seg[1] = p.seg[(size_t)b * p.seq + qb * 128 + fr.r + 8];
+    if (tid < 128) {
+      const int w = p.seg[(size_t)b * p.seq + qb * 128 + tid];
+      const unsigned lo = __reduce_min_sync(0xffffffffu, (unsigned)(w & 0xffff));
+      const unsigned hi = __reduce_max_sync(0xffffffffu, (unsigned)w >> 16);
+      if (lane == 0) {
+        s_mbits[warp] = lo;
+        s_mbits[4 + warp] = hi;
+      }
+    }
+  } else {
+    for (int c = tid; c < p.seq; c += ATT_THREADS) {   // seq % 128 == 0: whole warps take part in every round
+      const bool masked = p.mask != nullptr && p.mask[(size_t)b * p.seq + c] == 0;
+      const unsigned bits = __ballot_sync(0xffffffffu, masked);
+      if (lane == 0) s_mbits[c >> 5] = bits;
+    }
   }
   __syncthreads();
+  int j0 = 0, j1 = nkv;     // the key blocks this CTA visits
+  if (kSeg) {
+    const unsigned lo = min(min(s_mbits[0], s_mbits[1]), min(s_mbits[2], s_mbits[3]));
+    const unsigned hi = max(max(s_mbits[4], s_mbits[5]), max(s_mbits[6], s_mbits[7]));
+    // kept inside the bin and around the block's own keys (which every valid segment of its rows contains), so that
+    // malformed segments cannot take the loads past the bin or leave the loop empty
+    j0 = min((int)(lo >> 7), qb);
+    j1 = min(max((int)((hi + 127) >> 7), qb + 1), nkv);
+  }
 
   const int row0 = b * p.seq;           // first token row of this sequence
   const int col_q = h * 64, col_k = p.hidden + h * 64, col_v = 2 * p.hidden + h * 64;
@@ -182,10 +221,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_fwd_kernel(const __g
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // l_run: this lane's share of the row sum
   uint32_t ph_load = 0;
 
-  for (int j = 0; j < nkv; ++j) {
+  for (int j = j0; j < j1; ++j) {
     if (tid == 0) {
-      mbar_expect_tx(bar_load, (j == 0 ? 3 : 2) * TILE_BYTES);
-      if (j == 0) tma_load_2d(sQ, &tmap_qkv, bar_load, col_q, row0 + qb * 128);
+      mbar_expect_tx(bar_load, (j == j0 ? 3 : 2) * TILE_BYTES);
+      if (j == j0) tma_load_2d(sQ, &tmap_qkv, bar_load, col_q, row0 + qb * 128);
       tma_load_2d(sK, &tmap_qkv, bar_load, col_k, row0 + j * 128);
       tma_load_2d(sV, &tmap_qkv, bar_load, col_v, row0 + j * 128);
     }
@@ -199,12 +238,13 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_fwd_kernel(const __g
     wgmma_fence_regs(s);
 
     const uint32_t mw[4] = {s_mbits[j * 4], s_mbits[j * 4 + 1], s_mbits[j * 4 + 2], s_mbits[j * 4 + 3]};
+    const int sw[2] = {kSeg ? seg_in_block(seg[0], j * 128) : 0, kSeg ? seg_in_block(seg[1], j * 128) : 0};
     // maximum of the row's scaled + masked scores (log2 domain); a masked key counts as score*c2 + (-3.4e38),
     // which is -3.4e38 in fp32
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int i = 0; i < 64; ++i)
-      if (!key_masked<false>(mw, 0, fr.col(i))) mx[Frag::hi(i)] = fmaxf(mx[Frag::hi(i)], s[i]);
+      if (!key_masked<kSeg>(mw, sw[Frag::hi(i)], fr.col(i))) mx[Frag::hi(i)] = fmaxf(mx[Frag::hi(i)], s[i]);
     float m_new[2], alpha[2];
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
@@ -227,7 +267,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_fwd_kernel(const __g
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         float x = fmaf(s[i + e], c2, -m_new[u]);
-        if (key_masked<false>(mw, 0, c + e)) x = kMaskBias - m_new[u];
+        if (key_masked<kSeg>(mw, sw[u], c + e)) x = kMaskBias - m_new[u];
         const float pr = ex2_approx(x);
         l_blk[u] += pr;
         q2[e] = ((keep[u][c >> 3] >> ((c + e) & 7)) & 1u) ? pr * drop.scale : 0.f;
@@ -457,6 +497,10 @@ __device__ __forceinline__ uint32_t frag_keep_bits(const unsigned long long (&ke
 // seq > 128 (attention_bwd128_kernel takes seq == 128).  O comes in with Q and dO (into P's second half, free until
 // the dS pass) so delta = rowsum(dO * O) reads two swizzled smem rows while S and dP are being multiplied; dK / dV
 // leave through the operand tiles that the last products have released, as TMA tile stores.
+// kSeg: packed bins.  Segments are contiguous and symmetric, so the rows that see a key of this block are those of
+// the segments of its first and last keys, [lo(first), hi(last)): only the query blocks they fall in are visited.  A
+// skipped query block would add exactly 0 to dK, dV (P = 0) and to its rows' dQ.
+template <bool kSeg>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
                      const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_dqkv,
@@ -493,17 +537,25 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
   }
   pdl_wait();               // PDL: setup above overlapped the predecessor's tail; global reads start below
   pdl_launch_dependents();
-  if (tid < 128) {
+  if (!kSeg && tid < 128) {
     const bool masked = p.mask != nullptr && p.mask[(size_t)b * p.seq + jb * 128 + tid] == 0;
     const unsigned bits = __ballot_sync(0xffffffffu, masked);
     if (lane == 0) s_mbits[warp] = bits;
   }
   __syncthreads();
   const uint32_t mw[4] = {s_mbits[0], s_mbits[1], s_mbits[2], s_mbits[3]};
+  int i0 = 0, i1 = nq;      // the query blocks this CTA visits
+  if (kSeg) {
+    const int* sg = p.seg + (size_t)b * p.seq + jb * 128;
+    // kept inside the bin and around the block's own rows (which every valid segment of its keys contains), so that
+    // malformed segments cannot take the lse / segment reads and dQ atomics past the bin, or skip the K / V wait
+    i0 = min((int)(((unsigned)sg[0] & 0xffffu) >> 7), jb);
+    i1 = min(max((int)((((unsigned)sg[127] >> 16) + 127) >> 7), jb + 1), nq);
+  }
 
   const int row0 = b * p.seq;
   const int col_q = h * 64, col_k = p.hidden + h * 64, col_v = 2 * p.hidden + h * 64;
-  const DropCtx drop = make_drop_ctx(p.rng, p.rng_site, p.dropout_p);
+  const DropCtx drop0 = make_drop_ctx(p.rng, p.rng_site, p.dropout_p);
   const float c2 = p.scale * kLog2e;
   const size_t bh = (size_t)b * p.heads + h;
 
@@ -517,14 +569,16 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
   for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
   uint32_t ph_q = 0;
 
-  for (int i = 0; i < nq; ++i) {
+  for (int i = i0; i < i1; ++i) {
+    // kSeg: read per query block, so that the Philox key does not hold registers through the products
+    const DropCtx drop = kSeg ? make_drop_ctx(p.rng, p.rng_site, p.dropout_p) : drop0;
     if (tid == 0) {
       mbar_expect_tx(bar_q, 3 * TILE_BYTES);
       tma_load_2d(sQ, &tmap_qkv, bar_q, col_q, row0 + i * 128);
       tma_load_2d(sdO, &tmap_do, bar_q, h * 64, row0 + i * 128);
       tma_load_2d(sP1, &tmap_o, bar_q, h * 64, row0 + i * 128);   // O, consumed by the delta pass below
     }
-    if (i == 0) mbar_wait(bar_kv, 0);
+    if (i == i0) mbar_wait(bar_kv, 0);
     mbar_wait(bar_q, ph_q);
     ph_q ^= 1;
     float s[64], dp[64];
@@ -552,12 +606,26 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
     for (int u = 0; u < 2; ++u) {
       const int q_row = i * 128 + fr.r + 8 * u;   // this thread's query rows in the sequence
       lse2[u] = p.lse[bh * p.seq + q_row] * kLog2e;
-      quad_keep16(drop, ((bh * p.seq + q_row) * p.seq) + jb * 128, lane, keep[u]);
+      if (!kSeg) quad_keep16(drop, ((bh * p.seq + q_row) * p.seq) + jb * 128, lane, keep[u]);
     }
     wgmma_wait<0>();
     wgmma_fence_regs(s);
     wgmma_fence_regs(dp);
     __syncthreads();   // delta is in; O has been read and every product has read V: P may overwrite both
+    if (kSeg) {
+      // keys outside the row's segment: score -inf, so P = ex2(-inf) = 0 -- what the masked exponent gives every
+      // row with a visible key (each packed row sees itself).  The mask is a pass of its own, and the dropout
+      // decisions are drawn after it rather than under the products: testing the segment inside the loop below, or
+      // holding keep through the products next to the segment words, spills.
+      const int sw[2] = {seg_in_block(p.seg[(size_t)row0 + i * 128 + fr.r], jb * 128),
+                         seg_in_block(p.seg[(size_t)row0 + i * 128 + fr.r + 8], jb * 128)};
+#pragma unroll
+      for (int ii = 0; ii < 64; ++ii)
+        if (key_masked<true>(mw, sw[Frag::hi(ii)], fr.col(ii))) s[ii] = -INFINITY;
+#pragma unroll
+      for (int u = 0; u < 2; ++u)
+        quad_keep16(drop, ((bh * p.seq + i * 128 + fr.r + 8 * u) * p.seq) + jb * 128, lane, keep[u]);
+    }
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
       delta[u] = s_delta[fr.r + 8 * u];
@@ -571,7 +639,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
       for (int e = 0; e < 2; ++e) {
         const int cc = c + e;
         float x = fmaf(s[ii + e], c2, -lse2[u]);
-        if (key_masked<false>(mw, 0, cc)) x = xm[u];   // what score*c2 + (-3.4e38) rounds to (row_masked_x)
+        if (!kSeg && key_masked<false>(mw, 0, cc)) x = xm[u];   // what score*c2 + (-3.4e38) rounds to (row_masked_x)
         const float pr = ex2_approx(x);
         const bool kp = (keep[u][cc >> 3] >> (cc & 7)) & 1u;
         pd[e] = kp ? pr * drop.scale : 0.f;
@@ -592,13 +660,13 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
 #pragma unroll
       for (int k = 0; k < 8; ++k)
         wgmma_bf16<64, 1, 1>(dv, make_smem_desc(ap + k * 2048, 8192, 1024), make_smem_desc(ado + k * 2048, 8192, 1024),
-                             (i > 0 || k > 0) ? 1u : 0u);
+                             (i > i0 || k > 0) ? 1u : 0u);
       // dK[key, d] += sum_q dS[q, key] Q[q, d]
       const uint32_t ads = smem_u32(sdS), aq = smem_u32(sQ), ak = smem_u32(sK);
 #pragma unroll
       for (int k = 0; k < 8; ++k)
         wgmma_bf16<64, 1, 1>(dk, make_smem_desc(ads + wg * TILE_BYTES + k * 2048, 8192, 1024),
-                             make_smem_desc(aq + k * 2048, 8192, 1024), (i > 0 || k > 0) ? 1u : 0u);
+                             make_smem_desc(aq + k * 2048, 8192, 1024), (i > i0 || k > 0) ? 1u : 0u);
       // dQ[q, d] = sum_key dS[q, key] K[key, d]     (A = dS as K-major)
 #pragma unroll
       for (int k = 0; k < 8; ++k)
@@ -906,8 +974,6 @@ static int32_t attention_fwd_impl(const void* qkv, const int64_t* attention_mask
                                   uint64_t* keep_bits, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   B2_REQUIRE(qkv && ctx, "attention_fwd: null pointer");
-  B2_REQUIRE(segments == nullptr || seq == 128,
-             "attention_fwd: packed bins are 128 tokens long (seq=%lld)", (long long)seq);
   int32_t st = check_attn_shapes("attention_fwd", batch, seq, heads, head_dim);
   if (st) return st;
   // also rejects NaN, which would otherwise run without dropout
@@ -928,7 +994,8 @@ static int32_t attention_fwd_impl(const void* qkv, const int64_t* attention_mask
   p.keep_bits = (seq == 128 && dropout_p > 0.f) ? (unsigned long long*)keep_bits : nullptr;
   static bool attr = false;
   if (!attr) {
-    B2_CUDA(cudaFuncSetAttribute(attention_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmem));
+    B2_CUDA(cudaFuncSetAttribute(attention_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmem));
+    B2_CUDA(cudaFuncSetAttribute(attention_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmem));
     attr = true;
   }
   CUtensorMap tm_ctx;
@@ -957,7 +1024,11 @@ static int32_t attention_fwd_impl(const void* qkv, const int64_t* attention_mask
     count_launches(1);
     return 0;
   }
-  B2_LAUNCH(attention_fwd_kernel, grid, ATT_THREADS, kFwdSmem, stream, tm, tm_ctx, p);
+  if (segments != nullptr) {
+    B2_LAUNCH(attention_fwd_kernel<true>, grid, ATT_THREADS, kFwdSmem, stream, tm, tm_ctx, p);
+  } else {
+    B2_LAUNCH(attention_fwd_kernel<false>, grid, ATT_THREADS, kFwdSmem, stream, tm, tm_ctx, p);
+  }
   B2_CUDA(cudaGetLastError());
   count_launches(1);
   return 0;
@@ -979,6 +1050,15 @@ extern "C" int32_t b2_attention_fwd_packed(const void* qkv, const int32_t* segme
                             lse, keep_bits, stream_);
 }
 
+extern "C" int32_t b2_attention_fwd_packed_seq(const void* qkv, const int32_t* segments, int64_t bins, int64_t seq,
+                                               int64_t heads, int64_t head_dim, float dropout_p, const void* rng_state,
+                                               uint32_t rng_site, void* ctx, float* lse, uint64_t* keep_bits,
+                                               void* stream_) {
+  B2_REQUIRE(segments != nullptr, "attention_fwd_packed_seq: null segments");
+  return attention_fwd_impl(qkv, nullptr, segments, bins, seq, heads, head_dim, dropout_p, rng_state, rng_site, ctx,
+                            lse, keep_bits, stream_);
+}
+
 static int32_t attention_bwd_impl(const void* qkv, const int64_t* attention_mask, const int32_t* segments,
                                   const void* ctx, const void* d_ctx, const float* lse, int64_t batch, int64_t seq,
                                   int64_t heads, int64_t head_dim, float dropout_p, const void* rng_state,
@@ -986,13 +1066,13 @@ static int32_t attention_bwd_impl(const void* qkv, const int64_t* attention_mask
                                   const uint64_t* keep_bits, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   B2_REQUIRE(qkv && ctx && d_ctx && lse && d_qkv, "attention_bwd: null pointer");
-  B2_REQUIRE(segments == nullptr || seq == 128, "attention_bwd: packed bins are 128 tokens long (seq=%lld)",
-             (long long)seq);
   int32_t st = check_attn_shapes("attention_bwd", batch, seq, heads, head_dim);
   if (st) return st;
   B2_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "attention_bwd: dropout_p out of range");
   B2_REQUIRE(!(dropout_p > 0.f) || rng_state, "attention_bwd: dropout needs rng_state");
   B2_REQUIRE(seq == 128 || dq_accum != nullptr, "attention_bwd: seq > 128 needs the fp32 dq_accum buffer");
+  B2_REQUIRE(dbias_accum == nullptr || seq == 128,
+             "attention_bwd: the fused QKV bias gradient covers seq == 128 (longer sequences: use b2_colsum)");
   const int64_t hidden = heads * 64, tokens = batch * seq;
   CUtensorMap tm_qkv, tm_do;
   st = get_tensor_map_2d(&tm_qkv, qkv, (uint64_t)tokens, (uint64_t)(3 * hidden), (uint64_t)(3 * hidden * 2), 128, 64);
@@ -1015,14 +1095,13 @@ static int32_t attention_bwd_impl(const void* qkv, const int64_t* attention_mask
   p.ctx_in = (const __nv_bfloat16*)ctx; p.d_ctx = (const __nv_bfloat16*)d_ctx;
   p.d_qkv = (__nv_bfloat16*)d_qkv;
   p.dq_accum = seq > 128 ? dq_accum : nullptr;
-  B2_REQUIRE(dbias_accum == nullptr || seq == 128,
-             "attention_bwd: the fused QKV bias gradient covers seq == 128 (longer sequences: use b2_colsum)");
   p.dbias = dbias_accum;
   p.keep_bits = (seq == 128 && dropout_p > 0.f) ? (unsigned long long*)keep_bits : nullptr;
   if (p.dq_accum) B2_CUDA(cudaMemsetAsync(p.dq_accum, 0, (size_t)tokens * hidden * 4, stream));
   static int per_sm = 0;   // resident CTAs per SM of attention_bwd128_kernel (1)
   if (per_sm == 0) {
-    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmem));
+    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmem));
+    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmem));
     B2_CUDA(cudaFuncSetAttribute(attention_bwd128_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  kBwd128Smem));
     B2_CUDA(cudaFuncSetAttribute(attention_bwd128_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
@@ -1046,7 +1125,11 @@ static int32_t attention_bwd_impl(const void* qkv, const int64_t* attention_mask
     }
   } else {
     dim3 grid((unsigned)(seq / 128), (unsigned)heads, (unsigned)batch);
-    B2_LAUNCH(attention_bwd_kernel, grid, ATT_THREADS, kBwdSmem, stream, tm_qkv, tm_do, tm_o, tm_dqkv, p);
+    if (segments != nullptr) {
+      B2_LAUNCH(attention_bwd_kernel<true>, grid, ATT_THREADS, kBwdSmem, stream, tm_qkv, tm_do, tm_o, tm_dqkv, p);
+    } else {
+      B2_LAUNCH(attention_bwd_kernel<false>, grid, ATT_THREADS, kBwdSmem, stream, tm_qkv, tm_do, tm_o, tm_dqkv, p);
+    }
   }
   B2_CUDA(cudaGetLastError());
   count_launches(1);
@@ -1075,4 +1158,14 @@ extern "C" int32_t b2_attention_bwd_packed(const void* qkv, const int32_t* segme
   B2_REQUIRE(segments != nullptr, "attention_bwd_packed: null segments");
   return attention_bwd_impl(qkv, nullptr, segments, ctx, d_ctx, lse, bins, 128, heads, head_dim, dropout_p, rng_state,
                             rng_site, d_qkv, nullptr, dbias_accum, keep_bits, stream_);
+}
+
+extern "C" int32_t b2_attention_bwd_packed_seq(const void* qkv, const int32_t* segments, const void* ctx,
+                                               const void* d_ctx, const float* lse, int64_t bins, int64_t seq,
+                                               int64_t heads, int64_t head_dim, float dropout_p,
+                                               const void* rng_state, uint32_t rng_site, void* d_qkv, float* dq_accum,
+                                               float* dbias_accum, const uint64_t* keep_bits, void* stream_) {
+  B2_REQUIRE(segments != nullptr, "attention_bwd_packed_seq: null segments");
+  return attention_bwd_impl(qkv, nullptr, segments, ctx, d_ctx, lse, bins, seq, heads, head_dim, dropout_p, rng_state,
+                            rng_site, d_qkv, dq_accum, dbias_accum, keep_bits, stream_);
 }

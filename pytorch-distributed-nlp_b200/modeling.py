@@ -449,7 +449,8 @@ class BertForSequenceClassification(nn.Module):
     def forward(self, input_ids=None, token_type_ids=None, attention_mask=None, labels=None, position_ids=None,
                 segments=None, cls_index=None, **unused):
         """`position_ids` / `segments` / `cls_index` (all three or none): the batch is PACKED -- the rows of
-        `input_ids` are the 128-token bins of `packing.pack_batch`, logits come back one row per original sequence."""
+        `input_ids` are the bins of `packing.pack_batch` (128, 256, 384 or 512 tokens), logits come back one row per
+        original sequence."""
         if self._engine is None:
             raise RuntimeError("BertForSequenceClassification (b200) only runs on CUDA: call model.cuda() first; "
                                "there is no CPU path.")
@@ -784,8 +785,9 @@ class _Engine:
     # ---- forward --------------------------------------------------------------------------------------------------------
     def forward(self, input_ids, token_type_ids, attention_mask, labels, training, need_backward, packed=None,
                 loss_fn=None):
-        """packed: None, or (position_ids int64 [bins, 128], segments int32 [bins, 128], cls_index int64 [batch]) --
-        the rows of `input_ids` are then 128-token bins produced by packing.pack_batch, not sequences.
+        """packed: None, or (position_ids int64 [bins, S], segments int32 [bins, S], cls_index int64 [batch]) -- the
+        rows of `input_ids` are then S-token bins produced by packing.pack_batch (S a multiple of 128, at most 512),
+        not sequences.
         loss_fn: the losses.Loss of `labels` (None: the model's problem-type loss, HF's in-model loss)."""
         cfg, H, I = self.cfg, self.H, self.I
         if input_ids.dim() != 2:
@@ -794,8 +796,6 @@ class _Engine:
         Bo = B
         if packed is not None:
             pos_ids, segs, cls_rows = packed
-            if S != 128:
-                raise ValueError("packed bins are 128 tokens long (got %d)" % S)
             if attention_mask is not None:
                 raise ValueError("packed bins carry their own (block-diagonal) mask: pass attention_mask=None")
             for t, nm, dt, shape in ((pos_ids, "position_ids", torch.int64, (B, S)), (segs, "segments", torch.int32, (B, S)),
@@ -855,10 +855,13 @@ class _Engine:
             if packed is None:
                 L.call("b2_attention_fwd", a["qkv"].data_ptr(), L.ptr(mask), B, S, self.heads, 64, p_a, rng, 1 + 3 * l,
                        a["ctx"].data_ptr(), a["lse"].data_ptr(), L.ptr(a["keep"]) if need_backward else None, s)
-            else:
+            elif S == 128:
                 L.call("b2_attention_fwd_packed", a["qkv"].data_ptr(), segs.data_ptr(), B, self.heads, 64, p_a, rng,
                        1 + 3 * l, a["ctx"].data_ptr(), a["lse"].data_ptr(),
                        L.ptr(a["keep"]) if need_backward else None, s)
+            else:
+                L.call("b2_attention_fwd_packed_seq", a["qkv"].data_ptr(), segs.data_ptr(), B, S, self.heads, 64, p_a,
+                       rng, 1 + 3 * l, a["ctx"].data_ptr(), a["lse"].data_ptr(), None, s)
             self.dense_dropout_residual_layernorm(
                 M, H, a["ctx"].data_ptr(), w(pre + "attention.output.dense.weight"),
                 w(pre + "attention.output.dense.bias"), x.data_ptr(), L.ptr(xf), p_h, 2 + 3 * l,
@@ -1002,11 +1005,15 @@ class _Engine:
                 L.call("b2_attention_bwd", a["qkv"].data_ptr(), L.ptr(mask), a["ctx"].data_ptr(),
                        ws["dctx"].data_ptr(), a["lse"].data_ptr(), B, S, self.heads, 64, p_a, rng, 1 + 3 * l,
                        dqkv.data_ptr(), L.ptr(ws["dq_accum"]), acc_l if S == 128 else None, L.ptr(a["keep"]), s)
-            else:
+            elif S == 128:
                 L.call("b2_attention_bwd_packed", a["qkv"].data_ptr(), packed[0].data_ptr(), a["ctx"].data_ptr(),
                        ws["dctx"].data_ptr(), a["lse"].data_ptr(), B, self.heads, 64, p_a, rng, 1 + 3 * l,
                        dqkv.data_ptr(), acc_l, L.ptr(a["keep"]), s)
-            if S != 128:   # long-sequence parity configs: separate column-sum pass into the same accumulator slot
+            else:
+                L.call("b2_attention_bwd_packed_seq", a["qkv"].data_ptr(), packed[0].data_ptr(), a["ctx"].data_ptr(),
+                       ws["dctx"].data_ptr(), a["lse"].data_ptr(), B, S, self.heads, 64, p_a, rng, 1 + 3 * l,
+                       dqkv.data_ptr(), ws["dq_accum"].data_ptr(), None, None, s)
+            if S != 128:   # longer sequences or bins: separate column-sum pass into the same accumulator slot
                 L.call("b2_colsum", dqkv.data_ptr(), M, 3 * H, 3 * H, g(pre + "attention.self.query.bias"),
                        scratch, scratch_bytes, s)
             self.gemm(3 * H, H, M, dqkv.data_ptr(), 3 * H, MN, x_in.data_ptr(), H, MN,

@@ -2,18 +2,28 @@
 
 The reference tokenises with ``padding="max_length", max_length=128`` (multi-gpu-distributed-cls.py:76) while the rows
 of data/train.json average 18 characters: ~85 % of every [batch, 128] input is padding that the step still pays full
-price for.  `pack_batch` re-arranges such a batch into fewer 128-token BINS: the valid prefixes of several sequences
-share one bin (first-fit, longest first), every token keeps the position id it had in its own sequence, and every bin
-row carries the [lo, hi) range of its own sequence inside the bin.  The attention kernels then mask with that range
+price for.  `pack_batch` re-arranges such a batch into fewer BINS of 128, 256, 384 or 512 tokens (`bin_length`: the
+shortest that holds the batch's longest sequence): the valid prefixes of several sequences share one bin (first-fit,
+longest first), every token keeps the position id it had in its own sequence, and every bin row carries the [lo, hi)
+range of its own sequence inside the bin.  The attention kernels then mask with that range
 (a block-diagonal mask per bin) instead of the key-padding mask, every other kernel is token-wise and simply sees
 fewer rows, and the pooler reads each sequence's first token through `cls_index`.  Per sequence the arithmetic is
 exactly that of the padded batch (a padded key contributes exp(-3.4e38 - m) = 0 to its softmax row, like a key of
-another sequence here).
+another sequence here).  In bins longer than 128 tokens the attention kernels visit only the 128-token blocks a
+sequence reaches, so a bin of short sequences costs little more than their tokens.
 """
 import numpy as np
 import torch
 
 BIN = 128
+MAX_BIN = 512      # the attention kernels' longest sequence
+
+
+def bin_length(attention_mask, seq_len):
+    """the bin length pack_batch should use for a [B, seq_len] batch: the smallest multiple of BIN that holds its
+    longest valid sequence (attention_mask None: every token is valid)"""
+    longest = int(attention_mask.ne(0).sum(1).max()) if attention_mask is not None else seq_len
+    return BIN * max(1, -(-longest // BIN))
 
 
 def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN):

@@ -27,6 +27,7 @@ import torch
 from .ddp import DistributedDataParallel
 from .losses import criterion_key, infer_problem_type, loss_from_criterion, problem_type_loss
 from .optim import clip_grad_norm_
+from .packing import MAX_BIN, bin_length, pack_batch
 from .schedules import get_scheduler, warmup_steps
 
 
@@ -48,8 +49,9 @@ class Args:
     dev = False
     use_amp = False       # the -amp scripts' flag (multi-gpu-distributed-mp-amp-cls.py:160): GradScaler loop on the eager path
     fused = True          # capture fwd + bwd + exchange + AdamW in one CUDA graph
-    pack = False          # pack the valid prefixes of the padded [B, 128] batches into 128-token bins (packing.py): the
-                          # reference pads every row to max_seq_len although real rows average 18 tokens [:76]
+    pack = False          # pack the valid prefixes of padded [B, S <= 512] batches into bins of the shortest multiple of
+                          # 128 that holds the batch's longest row (packing.py): the reference pads every row to
+                          # max_seq_len although real rows average 18 tokens [:76]
     gradient_accumulation_steps = 1   # k > 1: one optimizer step per k batches, each batch's loss scaled by 1/k (the
                                       # HF Trainer / DeepSpeed name; fabric-cls.py's grad_accumulation)
     max_grad_norm = None  # clip the gradient's 2-norm to this before every optimizer step (HF TrainingArguments'
@@ -366,37 +368,38 @@ class FusedTrainStep(_StagedGraphStep):
 
 
 class PackedTrainStep(_StagedGraphStep):
-    """FusedTrainStep for PACKED batches (packing.pack_batch): `bins` 128-token bins carrying `batch` sequences.  One
-    instance (staging buffers + CUDA graph) per bin count; the Trainer keeps a small cache of them, since the number of
-    bins a batch packs into varies with its lengths."""
+    """FusedTrainStep for PACKED batches (packing.pack_batch): `bins` bins of `bin_len` tokens carrying `batch`
+    sequences.  One instance (staging buffers + CUDA graph) per bin count and length; the Trainer keeps a small cache of
+    them, since the bins a batch packs into vary with its lengths."""
 
     def __init__(self, model, optimizer, bins, batch, use_graph=True, accum_steps=1, max_grad_norm=None,
-                 criterion=None):
-        super().__init__(model, bins, 128, use_graph, criterion)
+                 criterion=None, bin_len=128):
+        super().__init__(model, bins, bin_len, use_graph, criterion)
         dev = self.eng.dev
-        self.bins, self.batch = bins, batch
-        n = bins * 128
+        self.bins, self.batch, self.bin_len = bins, batch, bin_len
+        n = bins * bin_len
         # pinned staging: ids | token types | positions | segments (as int64) | cls rows | labels
         self.d_lab, lab_slots = self._label_buffer(batch)
         self._alloc_stage(4 * n + batch + lab_slots)
         z = lambda *sh: torch.zeros(*sh, dtype=torch.int64, device=dev)
-        self.d_pos, self.d_cls = z(bins, 128), z(batch)
-        self.d_seg = torch.zeros(bins, 128, dtype=torch.int32, device=dev)
+        self.d_pos, self.d_cls = z(bins, bin_len), z(batch)
+        self.d_seg = torch.zeros(bins, bin_len, dtype=torch.int32, device=dev)
         self._arm(optimizer, accum_steps, max_grad_norm)
 
     def _unstage(self):
-        n, st = self.bins * 128, self.d_stage
-        self.d_ids.copy_(st[0:n].view(self.bins, 128))
-        self.d_tt.copy_(st[n:2 * n].view(self.bins, 128))
-        self.d_pos.copy_(st[2 * n:3 * n].view(self.bins, 128))
-        self.d_seg.copy_(st[3 * n:4 * n].view(self.bins, 128))          # int64 -> int32
+        n, st, S = self.bins * self.bin_len, self.d_stage, self.bin_len
+        self.d_ids.copy_(st[0:n].view(self.bins, S))
+        self.d_tt.copy_(st[n:2 * n].view(self.bins, S))
+        self.d_pos.copy_(st[2 * n:3 * n].view(self.bins, S))
+        self.d_seg.copy_(st[3 * n:4 * n].view(self.bins, S))            # int64 -> int32
         self.d_cls.copy_(st[4 * n:4 * n + self.batch])
         self._unstage_labels(st[4 * n + self.batch:])
 
     def stage(self, packed, label):
-        n, hs = self.bins * 128, self.h_stage
-        if packed["bins"] != self.bins or label.shape[0] != self.batch:
-            raise ValueError("PackedTrainStep was built for %d bins / %d sequences" % (self.bins, self.batch))
+        n, hs = self.bins * self.bin_len, self.h_stage
+        if packed["bins"] != self.bins or packed["input_ids"].shape[1] != self.bin_len or label.shape[0] != self.batch:
+            raise ValueError("PackedTrainStep was built for %d bins of %d tokens / %d sequences"
+                             % (self.bins, self.bin_len, self.batch))
         if self._h2d_done is not None:
             self._h2d_done.synchronize()
         hs[0:n].copy_(packed["input_ids"].reshape(-1))
@@ -455,7 +458,7 @@ class Trainer:
         self.criterion = criterion
         self.optimizer = optimizer
         self._fused = None
-        self._packed = {}     # bins -> PackedTrainStep
+        self._packed = {}     # (bins, batch, bin length) -> PackedTrainStep
         self._scaler = None
         self._fused_eval = {}
         self._pin = {}
@@ -599,17 +602,18 @@ class Trainer:
         first, final = self._micro == 0, self._micro >= k - 1
         self._micro = 0 if final else self._micro + 1
         if getattr(self.args, "fused", True) and getattr(self.args, "pack", False) and \
-                batch_data["input_ids"].shape[1] == 128 and not batch_data["input_ids"].is_cuda:
-            from .packing import pack_batch
-            packed = pack_batch(batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"])
-            key = (packed["bins"], batch_data["input_ids"].shape[0])
+                batch_data["input_ids"].shape[1] <= MAX_BIN and not batch_data["input_ids"].is_cuda:
+            bin_len = bin_length(batch_data["attention_mask"], batch_data["input_ids"].shape[1])
+            packed = pack_batch(batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"],
+                                bin_len)
+            key = (packed["bins"], batch_data["input_ids"].shape[0], bin_len)
             lkey = self._captured_loss_key(batch_data["label"])
             if key not in self._packed or (self._packed[key].accum_steps, self._packed[key].max_grad_norm,
                                            self._packed[key].loss_key) != (k, clip, lkey):
                 if len(self._packed) >= 16:           # bound the graph cache: drop the oldest entry
                     self._packed.pop(next(iter(self._packed)))
                 self._packed[key] = PackedTrainStep(self.model, self.optimizer, key[0], key[1], accum_steps=k,
-                                                    max_grad_norm=clip, criterion=self.criterion)
+                                                    max_grad_norm=clip, criterion=self.criterion, bin_len=bin_len)
                 self._packed[key].loss_key = lkey
             self.model.train()
             loss = self._packed[key](packed, batch_data["label"], final)
