@@ -129,14 +129,25 @@ int32_t b2_embed_fwd(const int64_t* input_ids, const int64_t* token_type_ids, in
 /* arms the owner table used by b2_embed_bwd (int32[vocab] = INT_MAX); call once after allocation */
 int32_t b2_embed_owner_init(int32_t* owner, int64_t vocab, void* stream);
 
-/* backward of the above: LN backward, then the three scatter-adds (deterministic: one owner CTA per touched
- * vocabulary row sums its duplicates in token order).  d_word must be zeroed by the caller (b2_zero).  The row
- * `pad_token_id` gets no gradient (nn.Embedding padding_idx semantics, modeling_bert.py:58).                 */
+/* backward of the above: LN backward, then the three scatter-adds.  Word rows are keyed by an owner token per
+ * touched vocabulary row; when the scratch holds [tokens + seq * type_vocab][hidden] fp32 (and type_vocab <= 3) every
+ * token adds its row into the owner's fp32 accumulator with L2 reductions, so the summation order of a row that
+ * occurs more than once varies from run to run.  Otherwise one owner CTA sums the duplicates in token order.
+ * d_word must be zeroed by the caller (b2_zero).  The row `pad_token_id` gets no gradient (nn.Embedding padding_idx
+ * semantics, modeling_bert.py:58).  b2_embed_bwd_ordered: the same, with the word rows always summed by the owner
+ * CTA in token order: bitwise reproducible (torch.use_deterministic_algorithms).  Its fused position / token-type pass
+ * needs seq * type_vocab * hidden fp32 of scratch.                                                        */
 int32_t b2_embed_bwd(const void* dy /* bf16, or fp32 when dy_fp32 */, int32_t dy_fp32, const void* pre_ln, const float* mean, const float* rstd, const void* gamma,
                      const int32_t* ids32, const int32_t* tt32, int64_t batch, int64_t seq, int64_t hidden,
                      int64_t vocab, int64_t type_vocab, int64_t pad_token_id /* -1: none */, float dropout_p,
                      const void* rng_state, uint32_t rng_site, void* d_word, void* d_pos, void* d_type, void* d_gamma, void* d_beta, void* scratch_dx,
                      float* scratch_partials, int64_t scratch_partials_bytes, int32_t* owner, void* stream);
+int32_t b2_embed_bwd_ordered(const void* dy, int32_t dy_fp32, const void* pre_ln, const float* mean, const float* rstd,
+                             const void* gamma, const int32_t* ids32, const int32_t* tt32, int64_t batch, int64_t seq,
+                             int64_t hidden, int64_t vocab, int64_t type_vocab, int64_t pad_token_id, float dropout_p,
+                             const void* rng_state, uint32_t rng_site, void* d_word, void* d_pos, void* d_type,
+                             void* d_gamma, void* d_beta, void* scratch_dx, float* scratch_partials,
+                             int64_t scratch_partials_bytes, int32_t* owner, void* stream);
 
 /* LayerNorm over the last dim (BertSelfOutput / BertOutput LayerNorm, modeling_bert.py:297,355).
  * x is the already-summed (dropout(dense)+residual) input produced by the GEMM epilogue.                   */
@@ -277,6 +288,29 @@ int32_t b2_attention_bwd_packed_seq(const void* qkv, const int32_t* segments, co
                                     const float* lse, int64_t bins, int64_t seq, int64_t heads, int64_t head_dim,
                                     float dropout_p, const void* rng_state, uint32_t rng_site, void* d_qkv,
                                     float* dq_accum, float* dbias_accum, const uint64_t* keep_bits, void* stream);
+/* The ordered dQ of the seq > 128 backward (torch.use_deterministic_algorithms): instead of adding every key block's
+ * dQ contribution into dq_accum with atomics, the CTA of key block jb stores it into slice jb of
+ *   dq_partials  fp32 [seq / 128][bins * seq, heads * 64]   (4 slices x 25.2 MB at 16 x 512 tokens, hidden 768)
+ * and a second kernel sums the slices in ascending jb into d_qkv's Q columns: dQ is bitwise the same on every run.
+ * dK and dV are those of the atomic form, bit for bit.  A slice a CTA never visits (packed bins skip blocks) is never
+ * read, so the buffer needs no clearing.  Rejected: seq <= 128 (whose backward has no cross-CTA dQ sum) and a null
+ * dq_partials.  No fused bias sums (b2_colsum) and no keep_bits, as for the atomic form above 128.              */
+int32_t b2_attention_bwd_ordered(const void* qkv, const int64_t* attention_mask, const void* ctx, const void* d_ctx,
+                                 const float* lse, int64_t batch, int64_t seq, int64_t heads, int64_t head_dim,
+                                 float dropout_p, const void* rng_state, uint32_t rng_site, void* d_qkv,
+                                 float* dq_partials, void* stream);
+int32_t b2_attention_bwd_packed_seq_ordered(const void* qkv, const int32_t* segments, const void* ctx,
+                                            const void* d_ctx, const float* lse, int64_t bins, int64_t seq,
+                                            int64_t heads, int64_t head_dim, float dropout_p, const void* rng_state,
+                                            uint32_t rng_site, void* d_qkv, float* dq_partials, void* stream);
+/* b2_embed_bwd_ordered for packed bins (type_vocab <= 3)                                                          */
+int32_t b2_embed_bwd_packed_ordered(const void* dy, int32_t dy_fp32, const void* pre_ln, const float* mean,
+                                    const float* rstd, const void* gamma, const int32_t* ids32, const int32_t* tt32,
+                                    const int32_t* pos32, int64_t bins, int64_t seq, int64_t hidden, int64_t vocab,
+                                    int64_t type_vocab, int64_t pad_token_id, float dropout_p, const void* rng_state,
+                                    uint32_t rng_site, void* d_word, void* d_pos, void* d_type, void* d_gamma,
+                                    void* d_beta, void* scratch_dx, float* scratch_partials,
+                                    int64_t scratch_partials_bytes, int32_t* owner, void* stream);
 int32_t b2_head_fwd_packed(const void* hidden_states, const int64_t* cls_rows, int64_t batch, int64_t hidden,
                            const void* pool_w, const void* pool_b, const void* cls_w, const void* cls_b,
                            int64_t num_labels, float dropout_p, const void* rng_state, uint32_t rng_site,

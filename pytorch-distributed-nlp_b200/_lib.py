@@ -95,6 +95,13 @@ _SIGNATURES = {
     "b2_attention_bwd_packed": [vp, vp, vp, vp, vp, i64, i64, i64, f32, vp, u32, vp, vp, vp, vp],
     "b2_attention_fwd_packed_seq": [vp, vp, i64, i64, i64, i64, f32, vp, u32, vp, vp, vp, vp],
     "b2_attention_bwd_packed_seq": [vp, vp, vp, vp, vp, i64, i64, i64, i64, f32, vp, u32, vp, vp, vp, vp, vp],
+    # fixed-order forms (torch.use_deterministic_algorithms)
+    "b2_attention_bwd_ordered": [vp, vp, vp, vp, vp, i64, i64, i64, i64, f32, vp, u32, vp, vp, vp],
+    "b2_attention_bwd_packed_seq_ordered": [vp, vp, vp, vp, vp, i64, i64, i64, i64, f32, vp, u32, vp, vp, vp],
+    "b2_embed_bwd_ordered": [vp, i32, vp, vp, vp, vp, vp, vp, i64, i64, i64, i64, i64, i64, f32, vp, u32, vp, vp, vp, vp,
+                             vp, vp, vp, i64, vp, vp],
+    "b2_embed_bwd_packed_ordered": [vp, i32, vp, vp, vp, vp, vp, vp, vp, i64, i64, i64, i64, i64, i64, f32, vp, u32, vp,
+                                    vp, vp, vp, vp, vp, vp, i64, vp, vp],
     "b2_head_fwd_packed": [vp, vp, i64, i64, vp, vp, vp, vp, i64, f32, vp, u32, vp, vp, vp],
     "b2_head_bwd_packed": [vp, vp, vp, vp, i64, i64, i64, vp, vp, i64, f32, vp, u32, vp, vp, vp, vp, vp, i32, vp, vp],
     "b2_head_bwd_split": [vp, vp, vp, vp, i64, i64, i64, i64, vp, vp, i64, f32, vp, u32, vp, vp, vp, vp, vp, i32, vp, vp,

@@ -490,6 +490,23 @@ __device__ __forceinline__ uint32_t frag_keep_bits(const unsigned long long (&ke
   return m;
 }
 
+// The query blocks [i0, i1) the backward CTA of key block jb of bin / sequence b visits.  kSeg: segments are
+// contiguous and symmetric, so the rows that see a key of this block are those of the segments of its first and last
+// keys, [lo(first), hi(last)).  The range is kept inside the bin and around the block's own rows (which every valid
+// segment of its keys contains), so that malformed segments cannot take the lse / segment reads and the dQ writes past
+// the bin, or skip the K / V wait.  The ordered dQ reduction asks the same question to know which slices exist.
+template <bool kSeg>
+__device__ __forceinline__ void bwd_query_blocks(const int* seg, int seq, int b, int jb, int& i0, int& i1) {
+  const int nq = seq / 128;
+  i0 = 0;
+  i1 = nq;
+  if (kSeg) {
+    const int* sg = seg + (size_t)b * seq + jb * 128;
+    i0 = min((int)(((unsigned)sg[0] & 0xffffu) >> 7), jb);
+    i1 = min(max((int)((((unsigned)sg[127] >> 16) + 127) >> 7), jb + 1), nq);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // backward: grid (seq/128 kv blocks, heads, batch); loops over query blocks
 // ------------------------------------------------------------------------------------------------------------
@@ -497,10 +514,12 @@ __device__ __forceinline__ uint32_t frag_keep_bits(const unsigned long long (&ke
 // seq > 128 (attention_bwd128_kernel takes seq == 128).  O comes in with Q and dO (into P's second half, free until
 // the dS pass) so delta = rowsum(dO * O) reads two swizzled smem rows while S and dP are being multiplied; dK / dV
 // leave through the operand tiles that the last products have released, as TMA tile stores.
-// kSeg: packed bins.  Segments are contiguous and symmetric, so the rows that see a key of this block are those of
-// the segments of its first and last keys, [lo(first), hi(last)): only the query blocks they fall in are visited.  A
-// skipped query block would add exactly 0 to dK, dV (P = 0) and to its rows' dQ.
-template <bool kSeg>
+// kSeg: packed bins: only the query blocks of bwd_query_blocks are visited.  A skipped query block would add exactly
+// 0 to dK, dV (P = 0) and to its rows' dQ.
+// kOrderedDq: the dQ contribution of this key block to query block i is stored (plain fp32 stores) into slice jb of
+// p.dq_accum = [seq / 128][tokens][hidden] instead of being added atomically into [tokens][hidden];
+// dq_reduce_ordered_kernel sums the slices in key-block order, so dQ does not depend on which CTA finishes first.
+template <bool kSeg, bool kOrderedDq>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
                      const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_dqkv,
@@ -544,14 +563,8 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
   }
   __syncthreads();
   const uint32_t mw[4] = {s_mbits[0], s_mbits[1], s_mbits[2], s_mbits[3]};
-  int i0 = 0, i1 = nq;      // the query blocks this CTA visits
-  if (kSeg) {
-    const int* sg = p.seg + (size_t)b * p.seq + jb * 128;
-    // kept inside the bin and around the block's own rows (which every valid segment of its keys contains), so that
-    // malformed segments cannot take the lse / segment reads and dQ atomics past the bin, or skip the K / V wait
-    i0 = min((int)(((unsigned)sg[0] & 0xffffu) >> 7), jb);
-    i1 = min(max((int)((((unsigned)sg[127] >> 16) + 127) >> 7), jb + 1), nq);
-  }
+  int i0, i1;      // the query blocks this CTA visits
+  bwd_query_blocks<kSeg>(p.seg, p.seq, b, jb, i0, i1);
 
   const int row0 = b * p.seq;
   const int col_q = h * 64, col_k = p.hidden + h * 64, col_v = 2 * p.hidden + h * 64;
@@ -687,6 +700,13 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_
         st_pair(sQ, sQ, fr.r + 8 * Frag::hi(e), fr.col(e), dq[e], dq[e + 1]);
       }
       if (p.dbias != nullptr) frag_colsum64(dq, lane, p.dbias + col_q);
+    } else if (kOrderedDq) {
+      // (the slice row in int, like the atomic form's row: the byte offset is formed once, in 64 bits, per store)
+      const int srow = (jb * p.batch + b) * p.seq + i * 128;
+#pragma unroll
+      for (int e = 0; e < 32; e += 2)
+        *reinterpret_cast<float2*>(p.dq_accum + (size_t)(srow + fr.r + 8 * Frag::hi(e)) * p.hidden + h * 64 +
+                                   fr.col(e)) = make_float2(dq[e], dq[e + 1]);
     } else {
 #pragma unroll
       for (int e = 0; e < 32; ++e)
@@ -927,6 +947,38 @@ __global__ void dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* 
   *reinterpret_cast<uint2*>(d_qkv + t * 3 * hidden + c) = o;
 }
 
+// The ordered form of dq_convert_kernel: dQ of a row = the sum of the slices jb = 0, 1, ... of `parts`
+// ([seq / 128][tokens, hidden] fp32, written by attention_bwd_kernel<kSeg, true>) in that order, then bf16.  Only the
+// slices whose key block visited the row's query block (bwd_query_blocks) exist: the others count as zero and are
+// never read, so the buffer needs no clearing.
+template <bool kSeg>
+__global__ void dq_reduce_ordered_kernel(const float* __restrict__ parts, const int* __restrict__ seg,
+                                         __nv_bfloat16* __restrict__ d_qkv, int batch, int seq, int hidden) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const long long tokens = (long long)batch * seq;
+  const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  if (i >= tokens * hidden) return;
+  const long long t = i / hidden;
+  const int c = (int)(i % hidden);
+  const int b = (int)(t / seq), qb = (int)(t % seq) >> 7;
+  float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int jb = 0; jb < seq / 128; ++jb) {
+    int i0, i1;
+    bwd_query_blocks<kSeg>(seg, seq, b, jb, i0, i1);
+    if (qb < i0 || qb >= i1) continue;
+    const float4 v = *reinterpret_cast<const float4*>(parts + (size_t)jb * tokens * hidden + i);
+    s.x += v.x;
+    s.y += v.y;
+    s.z += v.z;
+    s.w += v.w;
+  }
+  uint2 o;
+  o.x = pack_bf16(s.x, s.y);
+  o.y = pack_bf16(s.z, s.w);
+  *reinterpret_cast<uint2*>(d_qkv + t * 3 * hidden + c) = o;
+}
+
 constexpr int kFwdSmem = 5 * TILE_BYTES + 128 + 1024;
 constexpr int kFwd128Smem = 3 * TILE_BYTES + 64 + 1024;
 constexpr int kBwdSmem = 8 * TILE_BYTES + 64 + 512 + 1024;
@@ -1063,7 +1115,7 @@ static int32_t attention_bwd_impl(const void* qkv, const int64_t* attention_mask
                                   const void* ctx, const void* d_ctx, const float* lse, int64_t batch, int64_t seq,
                                   int64_t heads, int64_t head_dim, float dropout_p, const void* rng_state,
                                   uint32_t rng_site, void* d_qkv, float* dq_accum, float* dbias_accum,
-                                  const uint64_t* keep_bits, void* stream_) {
+                                  const uint64_t* keep_bits, void* stream_, bool ordered_dq = false) {
   cudaStream_t stream = (cudaStream_t)stream_;
   B2_REQUIRE(qkv && ctx && d_ctx && lse && d_qkv, "attention_bwd: null pointer");
   int32_t st = check_attn_shapes("attention_bwd", batch, seq, heads, head_dim);
@@ -1097,11 +1149,17 @@ static int32_t attention_bwd_impl(const void* qkv, const int64_t* attention_mask
   p.dq_accum = seq > 128 ? dq_accum : nullptr;
   p.dbias = dbias_accum;
   p.keep_bits = (seq == 128 && dropout_p > 0.f) ? (unsigned long long*)keep_bits : nullptr;
-  if (p.dq_accum) B2_CUDA(cudaMemsetAsync(p.dq_accum, 0, (size_t)tokens * hidden * 4, stream));
+  if (p.dq_accum && !ordered_dq) B2_CUDA(cudaMemsetAsync(p.dq_accum, 0, (size_t)tokens * hidden * 4, stream));
   static int per_sm = 0;   // resident CTAs per SM of attention_bwd128_kernel (1)
   if (per_sm == 0) {
-    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmem));
-    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmem));
+    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 kBwdSmem));
+    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 kBwdSmem));
+    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 kBwdSmem));
+    B2_CUDA(cudaFuncSetAttribute(attention_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 kBwdSmem));
     B2_CUDA(cudaFuncSetAttribute(attention_bwd128_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  kBwd128Smem));
     B2_CUDA(cudaFuncSetAttribute(attention_bwd128_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
@@ -1125,15 +1183,34 @@ static int32_t attention_bwd_impl(const void* qkv, const int64_t* attention_mask
     }
   } else {
     dim3 grid((unsigned)(seq / 128), (unsigned)heads, (unsigned)batch);
-    if (segments != nullptr) {
-      B2_LAUNCH(attention_bwd_kernel<true>, grid, ATT_THREADS, kBwdSmem, stream, tm_qkv, tm_do, tm_o, tm_dqkv, p);
+    if (segments != nullptr && ordered_dq) {
+      B2_LAUNCH((attention_bwd_kernel<true, true>), grid, ATT_THREADS, kBwdSmem, stream, tm_qkv, tm_do, tm_o, tm_dqkv,
+                p);
+    } else if (ordered_dq) {
+      B2_LAUNCH((attention_bwd_kernel<false, true>), grid, ATT_THREADS, kBwdSmem, stream, tm_qkv, tm_do, tm_o, tm_dqkv,
+                p);
+    } else if (segments != nullptr) {
+      B2_LAUNCH((attention_bwd_kernel<true, false>), grid, ATT_THREADS, kBwdSmem, stream, tm_qkv, tm_do, tm_o, tm_dqkv,
+                p);
     } else {
-      B2_LAUNCH(attention_bwd_kernel<false>, grid, ATT_THREADS, kBwdSmem, stream, tm_qkv, tm_do, tm_o, tm_dqkv, p);
+      B2_LAUNCH((attention_bwd_kernel<false, false>), grid, ATT_THREADS, kBwdSmem, stream, tm_qkv, tm_do, tm_o,
+                tm_dqkv, p);
     }
   }
   B2_CUDA(cudaGetLastError());
   count_launches(1);
-  if (p.dq_accum) {
+  if (ordered_dq) {
+    const long long n4 = tokens * hidden / 4;
+    if (segments != nullptr) {
+      B2_LAUNCH(dq_reduce_ordered_kernel<true>, (unsigned)((n4 + 255) / 256), 256, 0, stream, p.dq_accum, segments,
+                (__nv_bfloat16*)d_qkv, (int)batch, (int)seq, (int)hidden);
+    } else {
+      B2_LAUNCH(dq_reduce_ordered_kernel<false>, (unsigned)((n4 + 255) / 256), 256, 0, stream, p.dq_accum, segments,
+                (__nv_bfloat16*)d_qkv, (int)batch, (int)seq, (int)hidden);
+    }
+    B2_CUDA(cudaGetLastError());
+    count_launches(1);
+  } else if (p.dq_accum) {
     const long long n4 = tokens * hidden / 4;
     B2_LAUNCH(dq_convert_kernel, (unsigned)((n4 + 255) / 256), 256, 0, stream, p.dq_accum, (__nv_bfloat16*)d_qkv,
               tokens, (int)hidden);
@@ -1168,4 +1245,29 @@ extern "C" int32_t b2_attention_bwd_packed_seq(const void* qkv, const int32_t* s
   B2_REQUIRE(segments != nullptr, "attention_bwd_packed_seq: null segments");
   return attention_bwd_impl(qkv, nullptr, segments, ctx, d_ctx, lse, bins, seq, heads, head_dim, dropout_p, rng_state,
                             rng_site, d_qkv, dq_accum, dbias_accum, keep_bits, stream_);
+}
+
+// Ordered dQ (include/b2_ddp_bert.h): seq > 128 only; dq_partials is fp32 [seq / 128][tokens, heads * 64].
+extern "C" int32_t b2_attention_bwd_ordered(const void* qkv, const int64_t* attention_mask, const void* ctx,
+                                            const void* d_ctx, const float* lse, int64_t batch, int64_t seq,
+                                            int64_t heads, int64_t head_dim, float dropout_p, const void* rng_state,
+                                            uint32_t rng_site, void* d_qkv, float* dq_partials, void* stream_) {
+  B2_REQUIRE(seq > 128, "attention_bwd_ordered: seq=%lld (the ordered dQ covers seq > 128; seq 128 has no dQ sum "
+             "across CTAs)", (long long)seq);
+  B2_REQUIRE(dq_partials != nullptr, "attention_bwd_ordered: null dq_partials");
+  return attention_bwd_impl(qkv, attention_mask, nullptr, ctx, d_ctx, lse, batch, seq, heads, head_dim, dropout_p,
+                            rng_state, rng_site, d_qkv, dq_partials, nullptr, nullptr, stream_, true);
+}
+
+extern "C" int32_t b2_attention_bwd_packed_seq_ordered(const void* qkv, const int32_t* segments, const void* ctx,
+                                                       const void* d_ctx, const float* lse, int64_t bins, int64_t seq,
+                                                       int64_t heads, int64_t head_dim, float dropout_p,
+                                                       const void* rng_state, uint32_t rng_site, void* d_qkv,
+                                                       float* dq_partials, void* stream_) {
+  B2_REQUIRE(segments != nullptr, "attention_bwd_packed_seq_ordered: null segments");
+  B2_REQUIRE(seq > 128, "attention_bwd_packed_seq_ordered: seq=%lld (the ordered dQ covers seq > 128)",
+             (long long)seq);
+  B2_REQUIRE(dq_partials != nullptr, "attention_bwd_packed_seq_ordered: null dq_partials");
+  return attention_bwd_impl(qkv, nullptr, segments, ctx, d_ctx, lse, bins, seq, heads, head_dim, dropout_p, rng_state,
+                            rng_site, d_qkv, dq_partials, nullptr, nullptr, stream_, true);
 }

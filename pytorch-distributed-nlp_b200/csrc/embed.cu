@@ -2,9 +2,9 @@
 // forward : word + position + token-type gather, add, LayerNorm, dropout, one warp per token, one pass over HBM.
 // backward: LayerNorm backward, then deterministic scatter-adds:
 //   word rows      keyed by the "owner" token of each touched vocabulary row (lowest token index wins an atomicMin):
-//                  fast path = every token adds its row into fp32 acc[owner] (vector reductions at L2), the owner
-//                  converts; fallback (scratch too small) = the owner CTA scans the later tokens in order
-//                  (no float atomics, bit-reproducible);
+//                  fast path = every token adds its row into fp32 acc[owner] (vector reductions at L2: the order of a
+//                  duplicated row's adds varies), the owner converts; ordered entry points and fallback (scratch too
+//                  small) = the owner CTA scans the later tokens in order (no float atomics, bit-reproducible);
 //   position rows  row s = sum over the batch of dx[b, s, :]  } one pass (embed_pos_type_kernel) on the fast path,
 //   type rows      filtered column sums                        } separate kernels on the fallback.
 #include "common.cuh"
@@ -311,7 +311,8 @@ static int32_t embed_bwd_impl(const void* dy, int32_t dy_fp32, const void* pre_l
                                 float dropout_p, const void* rng_state, uint32_t rng_site, void* d_word, void* d_pos,
                                 void* d_type,
                                 void* d_gamma, void* d_beta, void* scratch_dx, float* scratch_partials,
-                                int64_t scratch_partials_bytes, int32_t* owner, void* stream_) {
+                                int64_t scratch_partials_bytes, int32_t* owner, void* stream_,
+                                bool ordered = false) {
   cudaStream_t stream = (cudaStream_t)stream_;
   B2_REQUIRE(dy && pre_ln && mean && rstd && gamma && ids32 && tt32 && d_word && d_pos && d_type && d_gamma &&
                  d_beta && scratch_dx && scratch_partials && owner,
@@ -328,20 +329,29 @@ static int32_t embed_bwd_impl(const void* dy, int32_t dy_fp32, const void* pre_l
   B2_LAUNCH(embed_owner_kernel, (tokens + 255) / 256, 256, 0, stream, ids32, tokens, (int)pad_token_id, owner);
   B2_CUDA(cudaGetLastError());
   count_launches(1);
-  // fast path: fp32 owner-row accumulation + fused position/type pass (needs scratch for [tokens + seq*T][H] fp32)
-  const int64_t fast_bytes = 4 * hidden * ((int64_t)tokens + seq * type_vocab);
+  // fast path: fp32 owner-row accumulation + fused position/type pass (needs scratch for [tokens + seq*T][H] fp32);
+  // ordered: the in-order owner scan for the word rows + the same position/type pass (scratch for [seq*T][H] fp32)
+  const int64_t acc_rows = ordered ? 0 : (int64_t)tokens;
+  const int64_t fast_bytes = 4 * hidden * (acc_rows + seq * type_vocab);
   if (type_vocab <= kMaxTypeFast && scratch_partials_bytes >= fast_bytes) {
     float* acc = scratch_partials;
-    float* type_part = scratch_partials + (size_t)tokens * hidden;
-    B2_CUDA(cudaMemsetAsync(acc, 0, (size_t)tokens * hidden * 4, stream));
-    B2_LAUNCH(embed_word_accum_kernel, tokens, (unsigned)(hidden / 8), 0, stream, (const __nv_bfloat16*)scratch_dx, ids32,
-              (int)hidden, (int)pad_token_id, owner, acc);
-    B2_CUDA(cudaGetLastError());
-    count_launches(1);
-    B2_LAUNCH(embed_word_finish_kernel, tokens, (unsigned)(hidden / 8), 0, stream, acc, ids32, (int)hidden,
-              (int)pad_token_id, owner, (__nv_bfloat16*)d_word);
-    B2_CUDA(cudaGetLastError());
-    count_launches(1);
+    float* type_part = scratch_partials + (size_t)acc_rows * hidden;
+    if (ordered) {
+      B2_LAUNCH(embed_word_scatter_kernel, tokens, 128, 0, stream, (const __nv_bfloat16*)scratch_dx, ids32, tokens,
+                (int)hidden, (int)pad_token_id, owner, (__nv_bfloat16*)d_word);
+      B2_CUDA(cudaGetLastError());
+      count_launches(1);
+    } else {
+      B2_CUDA(cudaMemsetAsync(acc, 0, (size_t)tokens * hidden * 4, stream));
+      B2_LAUNCH(embed_word_accum_kernel, tokens, (unsigned)(hidden / 8), 0, stream, (const __nv_bfloat16*)scratch_dx,
+                ids32, (int)hidden, (int)pad_token_id, owner, acc);
+      B2_CUDA(cudaGetLastError());
+      count_launches(1);
+      B2_LAUNCH(embed_word_finish_kernel, tokens, (unsigned)(hidden / 8), 0, stream, acc, ids32, (int)hidden,
+                (int)pad_token_id, owner, (__nv_bfloat16*)d_word);
+      B2_CUDA(cudaGetLastError());
+      count_launches(1);
+    }
     B2_LAUNCH(embed_pos_type_kernel, (unsigned)seq, (unsigned)(hidden / 8), 0, stream, (const __nv_bfloat16*)scratch_dx,
               tt32, pos32, (int)batch, (int)seq, (int)hidden, (int)type_vocab, (__nv_bfloat16*)d_pos, type_part);
     B2_CUDA(cudaGetLastError());
@@ -395,6 +405,34 @@ extern "C" int32_t b2_embed_bwd_packed(const void* dy, int32_t dy_fp32, const vo
   return embed_bwd_impl(dy, dy_fp32, pre_ln, mean, rstd, gamma, ids32, tt32, pos32, bins, seq, hidden, vocab,
                         type_vocab, pad_token_id, dropout_p, rng_state, rng_site, d_word, d_pos, d_type, d_gamma,
                         d_beta, scratch_dx, scratch_partials, scratch_partials_bytes, owner, stream_);
+}
+
+// The ordered forms: word rows always by the in-order owner scan (embed_word_scatter_kernel), never by the fp32
+// owner-row reductions, so a row's duplicates are summed in token order and the result is the same on every run.
+extern "C" int32_t b2_embed_bwd_ordered(const void* dy, int32_t dy_fp32, const void* pre_ln, const float* mean,
+                                        const float* rstd, const void* gamma, const int32_t* ids32, const int32_t* tt32,
+                                        int64_t batch, int64_t seq, int64_t hidden, int64_t vocab, int64_t type_vocab,
+                                        int64_t pad_token_id, float dropout_p, const void* rng_state, uint32_t rng_site,
+                                        void* d_word, void* d_pos, void* d_type, void* d_gamma, void* d_beta,
+                                        void* scratch_dx, float* scratch_partials, int64_t scratch_partials_bytes,
+                                        int32_t* owner, void* stream_) {
+  return embed_bwd_impl(dy, dy_fp32, pre_ln, mean, rstd, gamma, ids32, tt32, nullptr, batch, seq, hidden, vocab,
+                        type_vocab, pad_token_id, dropout_p, rng_state, rng_site, d_word, d_pos, d_type, d_gamma,
+                        d_beta, scratch_dx, scratch_partials, scratch_partials_bytes, owner, stream_, true);
+}
+
+extern "C" int32_t b2_embed_bwd_packed_ordered(const void* dy, int32_t dy_fp32, const void* pre_ln, const float* mean,
+                                               const float* rstd, const void* gamma, const int32_t* ids32,
+                                               const int32_t* tt32, const int32_t* pos32, int64_t bins, int64_t seq,
+                                               int64_t hidden, int64_t vocab, int64_t type_vocab, int64_t pad_token_id,
+                                               float dropout_p, const void* rng_state, uint32_t rng_site, void* d_word,
+                                               void* d_pos, void* d_type, void* d_gamma, void* d_beta, void* scratch_dx,
+                                               float* scratch_partials, int64_t scratch_partials_bytes, int32_t* owner,
+                                               void* stream_) {
+  B2_REQUIRE(pos32 != nullptr, "embed_bwd_packed_ordered: null pos32");
+  return embed_bwd_impl(dy, dy_fp32, pre_ln, mean, rstd, gamma, ids32, tt32, pos32, bins, seq, hidden, vocab,
+                        type_vocab, pad_token_id, dropout_p, rng_state, rng_site, d_word, d_pos, d_type, d_gamma,
+                        d_beta, scratch_dx, scratch_partials, scratch_partials_bytes, owner, stream_, true);
 }
 
 // arms the owner table (INT_MAX) once; the scatter kernel re-arms what it touched

@@ -12,6 +12,7 @@ The arithmetic follows HF ``BertForSequenceClassification`` (SP/transformers/mod
 the user sees.  There is no PyTorch fallback: without the CUDA library every call raises.
 """
 import contextlib
+import ctypes
 import os
 import weakref
 from collections import OrderedDict
@@ -611,6 +612,10 @@ class _Engine:
             segs.append([b1_ + 2 * H_, o(pre + "attention.output.dense.bias"), H_])
         self.segs_per_layer = 8
         self.bias_segs = torch.tensor(segs if segs else [[0, 0, 0]], dtype=torch.int64, device=self.dev)
+        # fixed-order backward (torch.use_deterministic_algorithms): scratch of its own for the weight-gradient stream's
+        # column sums, and the per-block partials of the two LayerNorm backwards of a layer, double-buffered by layer
+        # parity like dzd / dU (layer l - 2 reuses a set only after done[l]); allocated on the first such backward
+        self._det_bufs = None
         s = self.stream()
         L.call("b2_embed_owner_init", L.ptr(self.owner), cfg.vocab_size, s)
         L.call("b2_rng_seed", L.ptr(self.rng), int(torch.initial_seed()) & ((1 << 63) - 1), 0, s)
@@ -729,6 +734,18 @@ class _Engine:
         self._ws[key] = ws
         return ws
 
+    def det_buffers(self):
+        """(weight-gradient-stream column-sum scratch, LayerNorm-backward partials [parity][LN2, LN1]) of the
+        fixed-order backward.  A partials buffer holds one [3][hidden] fp32 row per block of the LayerNorm backward's
+        single wave (one block per SM), as many as the accumulating form launches."""
+        if self._det_bufs is None:
+            sms = torch.cuda.get_device_properties(self.dev).multi_processor_count
+            u8 = dict(dtype=torch.uint8, device=self.dev)
+            ln_bytes = sms * 3 * self.H * 4
+            side = torch.empty(32 * 4 * max(3 * self.H, self.I), **u8)    # b2_colsum's at most 32 partial rows
+            self._det_bufs = (side, [[torch.empty(ln_bytes, **u8) for _ in range(2)] for _ in range(2)])
+        return self._det_bufs
+
     def gemm_grouped(self, problems, stream):
         """independent GEMMs behind one launch where the library can group them (the layer's weight gradients)"""
         arr = (L.GemmArgs * len(problems))(*problems)
@@ -736,8 +753,9 @@ class _Engine:
 
     def gemm(self, M, N, K, A, lda, a_major, Bm, ldb, b_major, D, ldd, epi=L.EPI_NONE, bias=None, aux_in=None,
              ld_aux_in=0, aux_out=None, ld_aux_out=0, p=0.0, site=0, split=False, stream=None, colsum=None,
-             defer=None):
-        """defer: a list -> the problem is appended to it instead of being launched (see gemm_grouped)"""
+             defer=None, splits=0):
+        """defer: a list -> the problem is appended to it instead of being launched (see gemm_grouped);
+        splits: force_splits (0: the cost model's choice)"""
         a = L.GemmArgs()
         a.M, a.N, a.K = M, N, K
         a.A, a.lda, a.a_major = A, lda, a_major
@@ -749,7 +767,8 @@ class _Engine:
             a.workspace, a.workspace_bytes = self.split_ws.data_ptr(), self.split_ws.numel()
         else:
             a.workspace, a.workspace_bytes = None, 0
-        a.force_bn = a.force_splits = a.force_kernel = 0
+        a.force_bn = a.force_kernel = 0
+        a.force_splits = splits
         a.debug_timing = None
         a.colsum_out = colsum
         if defer is not None:
@@ -920,6 +939,15 @@ class _Engine:
         w, g = self.w, self.g
         KM, MN = L.MAJOR_K, L.MAJOR_MN
         scratch, scratch_bytes = self.partials.data_ptr(), self.partials.numel()
+        # torch.use_deterministic_algorithms: every sum of the backward in a fixed order.  The bias and LayerNorm
+        # column sums leave the atomic epilogues / accumulators for column-sum passes on the weight-gradient stream,
+        # the N = hidden dgrads run unsplit (one add onto what the LayerNorm backward left), dQ above 128 tokens
+        # goes through per-key-block slices, and the word-embedding rows through the in-order owner scan.
+        det = torch.are_deterministic_algorithms_enabled()
+        if det:
+            side_scratch, ln_parts = self.det_buffers()
+            if S > 128 and ws.get("dq_parts") is None:
+                ws["dq_parts"] = torch.empty(S // 128, M, H, dtype=torch.float32, device=self.dev)
 
         # embedding-table gradients are scatter targets: clear the whole bucket (word rows not in the batch, unused
         # position rows and padding must read as zero for the dense DDP/AdamW pass, like the reference's dense grads)
@@ -973,47 +1001,71 @@ class _Engine:
                 main.wait_event(done[l + 2])
             # --- BertOutput: LN2 backward (+ dropout mask, bias grad), FFN2 wgrad/dgrad(+GELU')
             acc_l = self.bias_acc.data_ptr() + 4 * l * self.acc_per_layer
-            # column sums (d_gamma, d_beta, d_bias) are added into this layer's fp32 accumulators by the kernel itself
-            L.call("b2_layernorm_bwd_accum", dx.data_ptr(), a["z2"].data_ptr(), a["mean2"].data_ptr(),
-                   a["rstd2"].data_ptr(), w(pre + "output.LayerNorm.weight"), M, H, p_h, rng, 3 + 3 * l,
-                   dx_other.data_ptr(), dzd.data_ptr(), acc_l + 4 * (3 * H + I), s)
+            ln_out = (g(pre + "output.LayerNorm.weight"), g(pre + "output.LayerNorm.bias"), g(pre + "output.dense.bias"))
+            ln_att = (g(pre + "attention.output.LayerNorm.weight"), g(pre + "attention.output.LayerNorm.bias"),
+                      g(pre + "attention.output.dense.bias"))
+            if det:
+                # per-block partials; b2_colsum_finish on the weight-gradient stream turns them into the gradients
+                n2 = ctypes.c_int32()
+                L.call("b2_layernorm_bwd", dx.data_ptr(), None, a["z2"].data_ptr(), a["mean2"].data_ptr(),
+                       a["rstd2"].data_ptr(), w(pre + "output.LayerNorm.weight"), M, H, p_h, rng, 3 + 3 * l, 1,
+                       dx_other.data_ptr(), dzd.data_ptr(), *ln_out, ln_parts[st][0].data_ptr(),
+                       ln_parts[st][0].numel(), ctypes.addressof(n2), s)
+            else:
+                # column sums (d_gamma, d_beta, d_bias) are added into this layer's fp32 accumulators by the kernel
+                L.call("b2_layernorm_bwd_accum", dx.data_ptr(), a["z2"].data_ptr(), a["mean2"].data_ptr(),
+                       a["rstd2"].data_ptr(), w(pre + "output.LayerNorm.weight"), M, H, p_h, rng, 3 + 3 * l,
+                       dx_other.data_ptr(), dzd.data_ptr(), acc_l + 4 * (3 * H + I), s)
             # the layer's four weight gradients: collected here and issued as ONE launch on the side stream once the
             # last operand (dqkv) exists
             wgrads = []
             self.gemm(H, I, M, dzd.data_ptr(), H, MN, a["h"].data_ptr(), I, MN, g(pre + "output.dense.weight"), I,
                       split=True, defer=wgrads)
             # dU = (dY2 W2) * gelu'(u); its column sums (= intermediate bias gradient) accumulate in the same epilogue
+            # (det: a b2_colsum of dU on the weight-gradient stream)
             self.gemm(M, I, H, dzd.data_ptr(), H, KM, w(pre + "output.dense.weight"), I, MN, dU.data_ptr(), I,
-                      L.EPI_GELU_BWD, aux_in=a["u"].data_ptr(), ld_aux_in=I, colsum=acc_l + 4 * 3 * H)
+                      L.EPI_GELU_BWD, aux_in=a["u"].data_ptr(), ld_aux_in=I,
+                      colsum=None if det else acc_l + 4 * 3 * H)
             # --- BertIntermediate
             self.gemm(I, H, M, dU.data_ptr(), I, MN, a["x1"].data_ptr(), H, MN,
                       g(pre + "intermediate.dense.weight"), H, split=True, defer=wgrads)
             # dX1 = dZ2 + dU W1: LayerNorm backward left dZ2 (fp32) in dx_other and the GEMM adds into it (split-K
             # slices reduce in place at L2)
             self.gemm(M, H, I, dU.data_ptr(), I, KM, w(pre + "intermediate.dense.weight"), H, MN,
-                      dx_other.data_ptr(), H, L.EPI_ACCUM_F32)
+                      dx_other.data_ptr(), H, L.EPI_ACCUM_F32, splits=1 if det else 0)
             # --- BertSelfOutput
-            L.call("b2_layernorm_bwd_accum", dx_other.data_ptr(), a["z1"].data_ptr(), a["mean1"].data_ptr(),
-                   a["rstd1"].data_ptr(), w(pre + "attention.output.LayerNorm.weight"), M, H, p_h, rng, 2 + 3 * l,
-                   dx.data_ptr(), dz1d.data_ptr(), acc_l + 4 * (6 * H + I), s)
+            if det:
+                n1 = ctypes.c_int32()
+                L.call("b2_layernorm_bwd", dx_other.data_ptr(), None, a["z1"].data_ptr(), a["mean1"].data_ptr(),
+                       a["rstd1"].data_ptr(), w(pre + "attention.output.LayerNorm.weight"), M, H, p_h, rng,
+                       2 + 3 * l, 1, dx.data_ptr(), dz1d.data_ptr(), *ln_att, ln_parts[st][1].data_ptr(),
+                       ln_parts[st][1].numel(), ctypes.addressof(n1), s)
+            else:
+                L.call("b2_layernorm_bwd_accum", dx_other.data_ptr(), a["z1"].data_ptr(), a["mean1"].data_ptr(),
+                       a["rstd1"].data_ptr(), w(pre + "attention.output.LayerNorm.weight"), M, H, p_h, rng,
+                       2 + 3 * l, dx.data_ptr(), dz1d.data_ptr(), acc_l + 4 * (6 * H + I), s)
             self.gemm(H, H, M, dz1d.data_ptr(), H, MN, a["ctx"].data_ptr(), H, MN,
                       g(pre + "attention.output.dense.weight"), H, split=True, defer=wgrads)
             self.gemm(M, H, H, dz1d.data_ptr(), H, KM, w(pre + "attention.output.dense.weight"), H, MN,
                       ws["dctx"].data_ptr(), H)
             # --- BertSelfAttention
-            if packed is None:
-                L.call("b2_attention_bwd", a["qkv"].data_ptr(), L.ptr(mask), a["ctx"].data_ptr(),
-                       ws["dctx"].data_ptr(), a["lse"].data_ptr(), B, S, self.heads, 64, p_a, rng, 1 + 3 * l,
-                       dqkv.data_ptr(), L.ptr(ws["dq_accum"]), acc_l if S == 128 else None, L.ptr(a["keep"]), s)
+            att_in = (a["qkv"].data_ptr(), L.ptr(mask) if packed is None else packed[0].data_ptr(),
+                      a["ctx"].data_ptr(), ws["dctx"].data_ptr(), a["lse"].data_ptr())
+            qkv_acc = None if det else acc_l     # det: the QKV bias gradient is a b2_colsum of dqkv
+            if det and S > 128:
+                L.call("b2_attention_bwd_ordered" if packed is None else "b2_attention_bwd_packed_seq_ordered",
+                       *att_in, B, S, self.heads, 64, p_a, rng, 1 + 3 * l, dqkv.data_ptr(),
+                       ws["dq_parts"].data_ptr(), s)
+            elif packed is None:
+                L.call("b2_attention_bwd", *att_in, B, S, self.heads, 64, p_a, rng, 1 + 3 * l,
+                       dqkv.data_ptr(), L.ptr(ws["dq_accum"]), qkv_acc if S == 128 else None, L.ptr(a["keep"]), s)
             elif S == 128:
-                L.call("b2_attention_bwd_packed", a["qkv"].data_ptr(), packed[0].data_ptr(), a["ctx"].data_ptr(),
-                       ws["dctx"].data_ptr(), a["lse"].data_ptr(), B, self.heads, 64, p_a, rng, 1 + 3 * l,
-                       dqkv.data_ptr(), acc_l, L.ptr(a["keep"]), s)
+                L.call("b2_attention_bwd_packed", *att_in, B, self.heads, 64, p_a, rng, 1 + 3 * l,
+                       dqkv.data_ptr(), qkv_acc, L.ptr(a["keep"]), s)
             else:
-                L.call("b2_attention_bwd_packed_seq", a["qkv"].data_ptr(), packed[0].data_ptr(), a["ctx"].data_ptr(),
-                       ws["dctx"].data_ptr(), a["lse"].data_ptr(), B, S, self.heads, 64, p_a, rng, 1 + 3 * l,
+                L.call("b2_attention_bwd_packed_seq", *att_in, B, S, self.heads, 64, p_a, rng, 1 + 3 * l,
                        dqkv.data_ptr(), ws["dq_accum"].data_ptr(), None, None, s)
-            if S != 128:   # longer sequences or bins: separate column-sum pass into the same accumulator slot
+            if S != 128 and not det:   # longer sequences or bins: separate column-sum pass into the same accumulator slot
                 L.call("b2_colsum", dqkv.data_ptr(), M, 3 * H, 3 * H, g(pre + "attention.self.query.bias"),
                        scratch, scratch_bytes, s)
             self.gemm(3 * H, H, M, dqkv.data_ptr(), 3 * H, MN, x_in.data_ptr(), H, MN,
@@ -1026,18 +1078,29 @@ class _Engine:
             # their reduce kernels; largest problems first
             wgrads.sort(key=lambda t: -(t.M * t.N))
             self.gemm_grouped(wgrads, ss)
-            # fp32 accumulators -> bf16 bias gradients of this layer (and re-arm them); for S != 128 the QKV segment's
-            # accumulator is unused (zero) and must not overwrite the colsum result: finish only the intermediate one.
-            # Every kernel that adds into this layer's accumulators is behind the fork above, and only the optimizer /
-            # exchange reads the result: the launch rides the weight-gradient stream, off the critical path.
-            spl = self.segs_per_layer
-            seg0 = spl * l if S == 128 else spl * l + 1
-            L.call("b2_accum_finish", self.bias_acc.data_ptr(), self.grads.data_ptr(),
-                   self.bias_segs.data_ptr() + 24 * seg0, spl * (l + 1) - seg0, max(3 * H, I), ss)
+            if det:
+                # the layer's bias and LayerNorm gradients in a fixed order, off the critical path; the accumulators
+                # stay untouched (zero), so there is nothing for b2_accum_finish to finish
+                sb, sn = side_scratch.data_ptr(), side_scratch.numel()
+                L.call("b2_colsum", dU.data_ptr(), M, I, I, g(pre + "intermediate.dense.bias"), sb, sn, ss)
+                L.call("b2_colsum", dqkv.data_ptr(), M, 3 * H, 3 * H, g(pre + "attention.self.query.bias"), sb, sn,
+                       ss)
+                L.call("b2_colsum_finish", ln_parts[st][0].data_ptr(), n2.value, 3, H, *ln_out, ss)
+                L.call("b2_colsum_finish", ln_parts[st][1].data_ptr(), n1.value, 3, H, *ln_att, ss)
+            else:
+                # fp32 accumulators -> bf16 bias gradients of this layer (and re-arm them); for S != 128 the QKV
+                # segment's accumulator is unused (zero) and must not overwrite the colsum result: finish only the
+                # intermediate one.  Every kernel that adds into this layer's accumulators is behind the fork above,
+                # and only the optimizer / exchange reads the result: the launch rides the weight-gradient stream,
+                # off the critical path.
+                spl = self.segs_per_layer
+                seg0 = spl * l if S == 128 else spl * l + 1
+                L.call("b2_accum_finish", self.bias_acc.data_ptr(), self.grads.data_ptr(),
+                       self.bias_segs.data_ptr() + 24 * seg0, spl * (l + 1) - seg0, max(3 * H, I), ss)
             done[l] = torch.cuda.Event()
             done[l].record(side)
             self.gemm(M, H, 3 * H, dqkv.data_ptr(), 3 * H, KM, w(pre + "attention.self.query.weight"), H, MN,
-                      dx.data_ptr(), H, L.EPI_ACCUM_F32)
+                      dx.data_ptr(), H, L.EPI_ACCUM_F32, splits=1 if det else 0)
             bucket_ready(1 + l, done[l])   # complete only with this layer's weight gradients
         emb_in = (dx.data_ptr(), 1, ws["emb_pre"].data_ptr(), ws["emb_mean"].data_ptr(), ws["emb_rstd"].data_ptr(),
                   w("bert.embeddings.LayerNorm.weight"), ws["ids32"].data_ptr(), ws["tt32"].data_ptr())
@@ -1047,10 +1110,13 @@ class _Engine:
                     g("bert.embeddings.token_type_embeddings.weight"), g("bert.embeddings.LayerNorm.weight"),
                     g("bert.embeddings.LayerNorm.bias"), ws["emb_dx"].data_ptr(), scratch, scratch_bytes,
                     self.owner.data_ptr(), s)
+        emb_fn = "b2_embed_bwd" if packed is None else "b2_embed_bwd_packed"
+        if det:
+            emb_fn += "_ordered"
         if packed is None:
-            L.call("b2_embed_bwd", *emb_in, *emb_tail)
+            L.call(emb_fn, *emb_in, *emb_tail)
         else:
-            L.call("b2_embed_bwd_packed", *emb_in, ws["pos32"].data_ptr(), *emb_tail)
+            L.call(emb_fn, *emb_in, ws["pos32"].data_ptr(), *emb_tail)
         # Whoever consumes the gradients next on the main stream (optimizer.step, grad_dict) must see the weight-gradient
         # stream's work.  Where the per-bucket side stream has taken those dependencies, optimizer.step() (or
         # end_pass) joins it; in every other case join here.

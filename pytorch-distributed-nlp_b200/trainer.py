@@ -68,6 +68,8 @@ class Args:
     output_dir = None     # HF TrainingArguments' checkpoint names: train() writes output_dir/checkpoint-N every save_steps
     save_steps = None     # optimizer steps (None: no checkpoints), keeping the newest save_total_limit of them (None:
     save_total_limit = None   # all); train(resume_from_checkpoint=...) continues from one
+    full_determinism = False  # HF TrainingArguments' name: Trainer() calls torch.use_deterministic_algorithms(True), and
+                              # every training path then runs its fixed-order backward (bitwise reproducible runs)
 
 
 def _unwrap(model):
@@ -244,6 +246,11 @@ class _StagedGraphStep:
         """The step with inputs already staged on the device (bench `value` path).  final=False: a micro-batch of a
         gradient-accumulation window (forward, backward, accumulate; no optimizer step)."""
         opt = getattr(self, "opt", None)
+        if opt is not None and torch.are_deterministic_algorithms_enabled() != self.deterministic:
+            raise RuntimeError("%s was built with torch.use_deterministic_algorithms(%s) and is called with it %s; its "
+                               "captured backward keeps the summation order it was built with, so build a new %s in "
+                               "this mode" % (type(self).__name__, self.deterministic,
+                                              "on" if not self.deterministic else "off", type(self).__name__))
         # the body's accumulation mode (STORE / ADD / FOLD / none) follows from these two, and a graph replay runs no
         # Python: one graph per combination, and the host-side flags are kept current here
         self._role = (final, opt is not None and self.eng.accum_live)
@@ -291,6 +298,8 @@ class _StagedGraphStep:
 
     def _arm(self, optimizer, accum_steps, max_grad_norm=None):
         self.opt = optimizer
+        # the backward's summation order is baked into the graph: fixed-order under use_deterministic_algorithms
+        self.deterministic = torch.are_deterministic_algorithms_enabled()
         self.accum_steps = accum_steps
         self.max_grad_norm = float(max_grad_norm) if max_grad_norm else None
         if accum_steps > 1:
@@ -452,13 +461,15 @@ class Trainer:
         step; it takes precedence over args.lr_scheduler_type"""
         if scheduler is not None and getattr(scheduler, "optimizer", None) is not optimizer:
             raise ValueError("the scheduler must belong to the Trainer's optimizer")
+        if getattr(args, "full_determinism", False):
+            torch.use_deterministic_algorithms(True)      # as HF's enable_full_determinism does
         self.args = args
         self.config = config          # (the reference's `self.config = config,` stores a 1-tuple by accident, :121)
         self.model = model
         self.criterion = criterion
         self.optimizer = optimizer
         self._fused = None
-        self._packed = {}     # (bins, batch, bin length) -> PackedTrainStep
+        self._packed = {}     # (bins, batch, bin length, deterministic mode) -> PackedTrainStep
         self._scaler = None
         self._fused_eval = {}
         self._pin = {}
@@ -606,7 +617,8 @@ class Trainer:
             bin_len = bin_length(batch_data["attention_mask"], batch_data["input_ids"].shape[1])
             packed = pack_batch(batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"],
                                 bin_len)
-            key = (packed["bins"], batch_data["input_ids"].shape[0], bin_len)
+            key = (packed["bins"], batch_data["input_ids"].shape[0], bin_len,
+                   torch.are_deterministic_algorithms_enabled())
             lkey = self._captured_loss_key(batch_data["label"])
             if key not in self._packed or (self._packed[key].accum_steps, self._packed[key].max_grad_norm,
                                            self._packed[key].loss_key) != (k, clip, lkey):
@@ -622,8 +634,9 @@ class Trainer:
         elif getattr(self.args, "fused", True):
             B, S = batch_data["input_ids"].shape
             lkey = self._captured_loss_key(batch_data["label"])
-            if self._fused is None or (self._fused.B, self._fused.S, self._fused.accum_steps,
-                                       self._fused.max_grad_norm, self._fused.loss_key) != (B, S, k, clip, lkey):
+            det = torch.are_deterministic_algorithms_enabled()
+            if self._fused is None or (self._fused.B, self._fused.S, self._fused.accum_steps, self._fused.max_grad_norm,
+                                       self._fused.loss_key, self._fused.deterministic) != (B, S, k, clip, lkey, det):
                 self._fused = FusedTrainStep(self.model, self.optimizer, B, S, accum_steps=k, max_grad_norm=clip,
                                              criterion=self.criterion)
                 self._fused.loss_key = lkey
