@@ -332,6 +332,26 @@ int32_t b2_head_bwd_split(const float* dlogits, const void* hidden_states, const
                           void* d_cls_b, void* d_hidden, int32_t d_hidden_fp32, float* scratch, void* stream,
                           void* weight_stream);
 
+/* token-classification head (HF BertForTokenClassification: no pooler; dropout + Linear on every token), over the
+ * `tokens` rows of the last hidden state (batch x seq, or bins x bin_len when packed); 256 <= hidden <= 1024 a
+ * multiple of 256, 1 <= num_labels <= 64, tokens <= 131072.  Dropout: Philox key (seed, step, rng_site,
+ * (m * hidden + h) / 8), regenerated by the backward.
+ *   logits[m, c] = cls_b[c] + sum_h drop(x[m, h]) cls_w[c, h]      (fp32 [tokens, num_labels])                   */
+int32_t b2_token_head_fwd(const void* hidden_states, int64_t tokens, int64_t hidden, const void* cls_w,
+                          const void* cls_b, int64_t num_labels, float dropout_p, const void* rng_state,
+                          uint32_t rng_site, float* logits, void* stream);
+/* backward: d_hidden[m, h] = keep(m, h) / (1 - p) sum_c dlogits[m, c] cls_w[c, h] (fp32, every row) on `stream`;
+ * d_cls_w = sum_m dlogits[m]^T drop(x[m]) and d_cls_b = sum_m dlogits[m] (bf16) on `weight_stream` (ordered behind
+ * `stream` by an event; `stream` when NULL), summed as fp32 partials per row block added in ascending block order:
+ * bitwise repeatable, no atomics.  scratch: fp32, at least b2_token_head_scratch_floats(tokens, hidden, num_labels)
+ * floats.  Whatever reads d_cls_w / d_cls_b must be ordered behind `weight_stream`.                              */
+int32_t b2_token_head_bwd_split(const float* dlogits, const void* hidden_states, int64_t tokens, int64_t hidden,
+                                const void* cls_w, int64_t num_labels, float dropout_p, const void* rng_state,
+                                uint32_t rng_site, void* d_cls_w, void* d_cls_b, float* d_hidden, float* scratch,
+                                int64_t scratch_floats, void* stream, void* weight_stream);
+/* the fp32 scratch b2_token_head_bwd_split needs (a count, not a status)                                         */
+int64_t b2_token_head_scratch_floats(int64_t tokens, int64_t hidden, int64_t num_labels);
+
 /* ------------------------------------------------------------------------------------------------------ */
 /* optimizer + gradient exchange                                                                          */
 /*   replaces: HF AdamW.step (transformers 4.28.1 optimization.py, built at multi-gpu-distributed-cls.py    */

@@ -106,6 +106,9 @@ _SIGNATURES = {
     "b2_head_bwd_packed": [vp, vp, vp, vp, i64, i64, i64, vp, vp, i64, f32, vp, u32, vp, vp, vp, vp, vp, i32, vp, vp],
     "b2_head_bwd_split": [vp, vp, vp, vp, i64, i64, i64, i64, vp, vp, i64, f32, vp, u32, vp, vp, vp, vp, vp, i32, vp, vp,
                           vp],
+    # token-classification head (csrc/token_head.cu)
+    "b2_token_head_fwd": [vp, i64, i64, vp, vp, i64, f32, vp, u32, vp, vp],
+    "b2_token_head_bwd_split": [vp, vp, i64, i64, vp, i64, f32, vp, u32, vp, vp, vp, vp, i64, vp, vp],
     "b2_bucket_reduce_adamw": [C.POINTER(vp), C.POINTER(vp), i32, i32, vp, vp, vp, vp, i64, i64,
                                C.POINTER(AdamWHParams), vp, vp],
     "b2_adamw_prepare": [C.POINTER(AdamWHParams), vp, vp, vp],
@@ -136,7 +139,7 @@ _SIGNATURES = {
     "b2_scalar_allreduce_mean": [vp, vp, C.POINTER(vp), C.POINTER(vp), i32, i32, i32, vp, vp],
 }
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + ["b2_last_error", "b2_abi_version", "b2_launch_count",
-                                              "b2_gemm_ln_max_clusters"])
+                                              "b2_gemm_ln_max_clusters", "b2_token_head_scratch_floats"])
 
 _lib = None
 
@@ -159,6 +162,8 @@ def load():
     lib.b2_launch_count.argtypes = []
     lib.b2_gemm_ln_max_clusters.restype = i32     # a count, not a status
     lib.b2_gemm_ln_max_clusters.argtypes = [i64]
+    lib.b2_token_head_scratch_floats.restype = i64     # a count, not a status
+    lib.b2_token_head_scratch_floats.argtypes = [i64, i64, i64]
     if lib.b2_abi_version() != ABI_VERSION:
         raise RuntimeError("libb2ddpbert.so ABI %d != expected %d: rebuild" % (lib.b2_abi_version(), ABI_VERSION))
     for name, argtypes in _SIGNATURES.items():

@@ -141,6 +141,16 @@ def loss_from_criterion(criterion, num_labels, device):
     return Loss(L.LOSS_MSE, num_labels, device)
 
 
+def check_token_criterion(criterion):
+    """A token-classification model's loss is a cross-entropy over every token's C logits (HF's CrossEntropyLoss over
+    logits.view(-1, C)); MSELoss / BCEWithLogitsLoss would need float per-token targets, which the tagging path does
+    not carry.  Raises ValueError for those two."""
+    if isinstance(criterion, (nn.MSELoss, nn.BCEWithLogitsLoss)):
+        raise ValueError("%s does not apply to a token-classification model: its labels are one int64 class index per "
+                         "token (-100 on ignored ones) and its loss is CrossEntropyLoss over logits.view(-1, C), as HF's "
+                         "BertForTokenClassification computes it" % type(criterion).__name__)
+
+
 def _tensor_key(t):
     return None if t is None else (id(t), t._version)
 

@@ -21,7 +21,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib as L
-from .losses import PROBLEM_TYPES, infer_problem_type, problem_type_loss
+from .losses import PROBLEM_TYPES, Loss, infer_problem_type, problem_type_loss
 
 
 class BertConfig:
@@ -105,6 +105,10 @@ def _round8(n):
     return (n + 7) // 8 * 8
 
 
+HEAD_KINDS = ("sequence", "token")     # BertForSequenceClassification's pooler + classifier, or a classifier per token
+TOKEN_HEAD_MAX_LABELS = 64             # b2_token_head_fwd's bound
+
+
 class _Holder(nn.Module):
     """Name-only container so that ``named_parameters()`` reproduces the HF module paths."""
 
@@ -114,9 +118,12 @@ class _Layout:
     Buckets (DDP exchange / AdamW launch units) = embeddings | encoder layer 0..L-2 | last layer + head.  The head
     (pooler + classifier, 0.6 M parameters) rides with the last encoder layer -- they are adjacent in the flat space and
     final within microseconds of each other at the start of backward -- instead of paying a barrier, an exchange and
-    a kernel launch of its own."""
+    a kernel launch of its own.  head "token" (BertForTokenClassification): the tail is the classifier alone."""
 
-    def __init__(self, cfg):
+    def __init__(self, cfg, head="sequence"):
+        if head not in HEAD_KINDS:
+            raise ValueError("head=%r: expected one of %s" % (head, HEAD_KINDS))
+        self.head = head
         H, I, L_ = cfg.hidden_size, cfg.intermediate_size, cfg.num_hidden_layers
         self.entries = OrderedDict()  # hf name -> (offset, shape)
         self.buckets = []             # (begin, end, label)
@@ -159,8 +166,9 @@ class _Layout:
             add(p + "output.LayerNorm.bias", (H,))
             self.buckets.append((b0, off, "layer%d" % l))
         b0 = off
-        add("bert.pooler.dense.weight", (H, H))
-        add("bert.pooler.dense.bias", (H,))
+        if head == "sequence":
+            add("bert.pooler.dense.weight", (H, H))
+            add("bert.pooler.dense.bias", (H,))
         add("classifier.weight", (cfg.num_labels, H))
         add("classifier.bias", (cfg.num_labels,))
         if L_ > 0:
@@ -175,8 +183,9 @@ class _Layout:
         return self.entries[name][0]
 
 
-# HF named_parameters() order (201 tensors for 12 layers); differs from the flat order only inside attention.self
-def _hf_order(cfg):
+# HF named_parameters() order (201 tensors for 12 layers, 199 without the pooler); differs from the flat order only
+# inside attention.self
+def _hf_order(cfg, head="sequence"):
     names = ["bert.embeddings.word_embeddings.weight", "bert.embeddings.position_embeddings.weight",
              "bert.embeddings.token_type_embeddings.weight", "bert.embeddings.LayerNorm.weight",
              "bert.embeddings.LayerNorm.bias"]
@@ -185,7 +194,9 @@ def _hf_order(cfg):
         for m in ("attention.self.query", "attention.self.key", "attention.self.value", "attention.output.dense",
                   "attention.output.LayerNorm", "intermediate.dense", "output.dense", "output.LayerNorm"):
             names += [p + m + ".weight", p + m + ".bias"]
-    names += ["bert.pooler.dense.weight", "bert.pooler.dense.bias", "classifier.weight", "classifier.bias"]
+    if head == "sequence":
+        names += ["bert.pooler.dense.weight", "bert.pooler.dense.bias"]
+    names += ["classifier.weight", "classifier.bias"]
     return names
 
 
@@ -241,7 +252,12 @@ class _StepFn(torch.autograd.Function):
         return probe, None, None, None, None, None, None
 
 
-class BertForSequenceClassification(nn.Module):
+class _BertClassifier(nn.Module):
+    """What the classification models share: the HF parameter skeleton over one flat fp32 space, construction,
+    device movement, state dicts, the dropout stream and no_sync().  The subclass names its head kind (_Layout)."""
+    _head = None
+    _config_extra = {}       # written into save_pretrained's config.json over the config's attributes
+
     def __init__(self, config):
         super().__init__()
         self.config = config
@@ -252,7 +268,7 @@ class BertForSequenceClassification(nn.Module):
         if getattr(cfg, "hidden_act", "gelu") != "gelu":
             raise ValueError("only the erf GELU of the reference config is on the path")
         self.num_labels = cfg.num_labels
-        self._layout = _Layout(cfg)
+        self._layout = _Layout(cfg, self._head)
         lay = self._layout
         # fp32 master weights: ONE flat tensor, every nn.Parameter is a view into it
         self._flat = torch.zeros(lay.total, dtype=torch.float32)
@@ -298,11 +314,12 @@ class BertForSequenceClassification(nn.Module):
                 cur = getattr(cur, part)
             return cur
 
-        # registration order fixes named_parameters() order: embeddings, encoder, pooler, classifier (as HF)
+        # registration order fixes named_parameters() order: embeddings, encoder, pooler (sequence head), classifier
+        # (as HF)
         holder(root, ["bert", "embeddings"])
         enc = holder(root, ["bert", "encoder"])
         enc.layer = nn.ModuleList([_Holder() for _ in range(cfg.num_hidden_layers)])
-        for name in _hf_order(cfg):
+        for name in _hf_order(cfg, self._head):
             off, shape = self._layout.entries[name]
             n = 1
             for s in shape:
@@ -423,6 +440,7 @@ class BertForSequenceClassification(nn.Module):
         import json
         os.makedirs(save_directory, exist_ok=True)
         cfg = self.config.to_dict() if hasattr(self.config, "to_dict") else dict(vars(self.config))
+        cfg.update(self._config_extra)
         with open(os.path.join(save_directory, "config.json"), "w") as f:
             json.dump(cfg, f, indent=2, sort_keys=True)
         sd = OrderedDict((k, v.detach().cpu().clone()) for k, v in self.state_dict().items())
@@ -445,6 +463,25 @@ class BertForSequenceClassification(nn.Module):
             raise ValueError("a dropout RNG state is an integer [seed, step] (got %s)" % (state,))
         seed, step = (int(x) for x in t.tolist())
         self._engine.seed_dropout(seed, step)
+
+    # ---- test / tooling helpers -----------------------------------------------------------------------------------------
+    def grad_dict(self):
+        """fp32 copies of what the next optimizer.step() would apply, keyed by HF parameter name: the (bf16) gradients of
+        the last backward, or inside an open accumulation window the fp32 accumulator."""
+        if self._engine is None:
+            raise RuntimeError("no engine (model not on CUDA)")
+        out = OrderedDict()
+        g = self._engine.accum if self._engine.accum_live else self._engine.grads
+        for name, p in self._params_by_name.items():
+            off, shape = self._layout.entries[name]
+            out[name] = g[off:off + p.numel()].view(shape).to(torch.float32, copy=True)
+        return out
+
+
+class BertForSequenceClassification(_BertClassifier):
+    """HF's BertForSequenceClassification: the pooler's tanh(dense) of each sequence's first token, dropout and a
+    linear classifier; the loss follows config.problem_type."""
+    _head = "sequence"
 
     # ---- forward ------------------------------------------------------------------------------------------------------
     def forward(self, input_ids=None, token_type_ids=None, attention_mask=None, labels=None, position_ids=None,
@@ -484,18 +521,52 @@ class BertForSequenceClassification(nn.Module):
             self._pt_loss = (pt, problem_type_loss(pt, self.num_labels))
         return self._pt_loss[1]
 
-    # ---- test / tooling helpers -----------------------------------------------------------------------------------------
-    def grad_dict(self):
-        """fp32 copies of what the next optimizer.step() would apply, keyed by HF parameter name: the (bf16) gradients of
-        the last backward, or inside an open accumulation window the fp32 accumulator."""
+
+class BertForTokenClassification(_BertClassifier):
+    """HF's BertForTokenClassification: BertModel without the pooler, dropout (config.classifier_dropout, else
+    hidden_dropout_prob) and a linear classifier on every token (csrc/token_head.cu), and with labels HF's
+    ``CrossEntropyLoss()`` over ``logits.view(-1, C)`` / ``labels.view(-1)`` (-100 ignored; config.problem_type is not
+    read).  Padding positions must carry -100, as HF's tagging collators put there.  Logits are fp32 [batch, seq, C],
+    or [bins, bin_len, C] for a packed batch."""
+    _head = "token"
+    _config_extra = {"architectures": ["BertForTokenClassification"]}
+
+    def __init__(self, config):
+        if not 1 <= int(config.num_labels) <= TOKEN_HEAD_MAX_LABELS:
+            raise ValueError("BertForTokenClassification: num_labels=%d, the token head supports 1 to %d labels"
+                             % (int(config.num_labels), TOKEN_HEAD_MAX_LABELS))
+        super().__init__(config)
+        self._ce = None
+
+    def forward(self, input_ids=None, token_type_ids=None, attention_mask=None, labels=None, position_ids=None,
+                segments=None, **unused):
+        """`position_ids` / `segments` (both or neither): the rows of `input_ids` are the bins of
+        `packing.pack_batch`, and `labels` its packed "labels" (unused bin rows hold -100)."""
         if self._engine is None:
-            raise RuntimeError("no engine (model not on CUDA)")
-        out = OrderedDict()
-        g = self._engine.accum if self._engine.accum_live else self._engine.grads
-        for name, p in self._params_by_name.items():
-            off, shape = self._layout.entries[name]
-            out[name] = g[off:off + p.numel()].view(shape).to(torch.float32, copy=True)
-        return out
+            raise RuntimeError("BertForTokenClassification (b200) only runs on CUDA: call model.cuda() first; "
+                               "there is no CPU path.")
+        if input_ids is None:
+            raise ValueError("input_ids is required")
+        packed = None
+        if segments is not None or position_ids is not None:
+            if position_ids is None or segments is None:
+                raise ValueError("a packed batch needs position_ids and segments together")
+            packed = (position_ids, segments, None)
+        if labels is not None and labels.is_floating_point():
+            raise TypeError("token labels are int64 class indices (CrossEntropyLoss), got %s" % labels.dtype)
+        if torch.is_grad_enabled() and self.training:
+            anchor = self._params_by_name["classifier.bias"]
+            logits, loss = _StepFn.apply(anchor, self, input_ids, token_type_ids, attention_mask, labels, packed)
+            return SequenceClassifierOutput(loss=loss if labels is not None else None, logits=logits)
+        logits, loss = self._engine.forward(input_ids, token_type_ids, attention_mask, labels,
+                                            training=self.training, need_backward=False, packed=packed)
+        return SequenceClassifierOutput(loss=None if loss is None else loss.clone(), logits=logits.clone())
+
+    def _problem_type_loss(self, labels):
+        """HF's in-model loss of the token model: CrossEntropyLoss() whatever config.problem_type says"""
+        if self._ce is None:
+            self._ce = Loss(L.LOSS_CE, self.num_labels)
+        return self._ce
 
 
 class _LocalTransport:
@@ -563,6 +634,7 @@ class _Engine:
         self.p_attn = float(cfg.attention_probs_dropout_prob)
         cd = getattr(cfg, "classifier_dropout", None)
         self.p_cls = float(cd if cd is not None else cfg.hidden_dropout_prob)
+        self.token_head = self.lay.head == "token"     # a classifier on every token row instead of pooler + classifier
         n = self.lay.total
         self.shadow = torch.empty(n, dtype=torch.bfloat16, device=self.dev)   # bf16 copy the GEMMs read
         self.grads = torch.zeros(n, dtype=torch.bfloat16, device=self.dev)    # bf16 gradient bucket space
@@ -684,6 +756,12 @@ class _Engine:
     def seed_dropout(self, seed, step=0):
         L.call("b2_rng_seed", L.ptr(self.rng), int(seed), int(step), self.stream())
 
+    def head_rows(self, B, S, packed):
+        """rows of the head's logits: every token (token head), else one per sequence (packed: its cls rows)"""
+        if self.token_head:
+            return B * S
+        return B if packed is None else packed[1].numel()
+
     def w(self, name):
         return self.shadow.data_ptr() + 2 * self.lay.off(name)
 
@@ -719,12 +797,16 @@ class _Engine:
                  "x1f": e(M, H, dtype=f32) if self.fused_ln else None,
                  "x2f": e(M, H, dtype=f32) if (self.fused_ln and li < nl - 1) else None}
                 for li in range(nl)],
-            "pooled": e(Bo, H), "logits": e(Bo, self.C, dtype=f32), "loss": e((), dtype=f32),
+            "pooled": None if self.token_head else e(Bo, H), "logits": e(Bo, self.C, dtype=f32),
+            "loss": e((), dtype=f32),
             "dlogits": e(Bo, self.C, dtype=f32), "dloss_logits": e(Bo, self.C, dtype=f32),
             # gradient of the residual stream: fp32 (12 layers of residual adds would otherwise each round it to bf16);
             # dzd / dz1d are the bf16 (dropout-masked) copies the tensor cores consume
             "dxA": e(M, H, dtype=f32), "dxB": e(M, H, dtype=f32),
-            "emb_dx": e(M, H), "dctx": e(M, H), "head_scratch": e(2 * Bo, H, dtype=f32),
+            "emb_dx": e(M, H), "dctx": e(M, H),
+            # the token head's fp32 parameter-gradient partials, the sequence head's two [batch, H] planes
+            "head_scratch": e(int(L.load().b2_token_head_scratch_floats(M, H, self.C)), dtype=f32) if self.token_head
+            else e(2 * Bo, H, dtype=f32),
             # operands of the weight-gradient GEMMs, double-buffered by layer parity (see _backward_from_dlogits)
             "dzd": [e(M, H), e(M, H)], "dz1d": [e(M, H), e(M, H)], "dU": [e(M, I), e(M, I)],
             "dqkv": [e(M, 3 * H), e(M, 3 * H)],
@@ -819,11 +901,17 @@ class _Engine:
                 raise ValueError("packed bins carry their own (block-diagonal) mask: pass attention_mask=None")
             for t, nm, dt, shape in ((pos_ids, "position_ids", torch.int64, (B, S)), (segs, "segments", torch.int32, (B, S)),
                                      (cls_rows, "cls_index", torch.int64, None)):
+                if t is None and self.token_head and nm == "cls_index":
+                    continue      # the token head reads every bin row
                 if t.device != self.dev or t.dtype != dt or (shape is not None and tuple(t.shape) != shape):
                     raise TypeError("%s must be a %s tensor%s on %s" % (nm, dt, "" if shape is None else " of shape %s"
                                                                         % (shape,), self.dev))
-            pos_ids, segs, cls_rows = pos_ids.contiguous(), segs.contiguous(), cls_rows.contiguous().view(-1)
-            Bo = cls_rows.numel()
+            pos_ids, segs = pos_ids.contiguous(), segs.contiguous()
+            if not self.token_head:
+                cls_rows = cls_rows.contiguous().view(-1)
+                Bo = cls_rows.numel()
+        if self.token_head:
+            Bo = B * S
         if B == 0 or S == 0:
             raise ValueError("empty batch")
         if S % 128 != 0 or S > 512 or S > cfg.max_position_embeddings:
@@ -895,12 +983,17 @@ class _Engine:
                 w(pre + "output.LayerNorm.bias"), a["z2"].data_ptr(), a["x2"].data_ptr(), L.ptr(a["x2f"]),
                 a["mean2"].data_ptr(), a["rstd2"].data_ptr())
             x, xf = a["x2"], a["x2f"]
-        head_w = (w("bert.pooler.dense.weight"), w("bert.pooler.dense.bias"), w("classifier.weight"),
-                  w("classifier.bias"))
-        if packed is None:
+        if self.token_head:
+            L.call("b2_token_head_fwd", x.data_ptr(), M, H, w("classifier.weight"), w("classifier.bias"), self.C, p_c,
+                   rng, 1 + 3 * self.nl, ws["logits"].data_ptr(), s)
+        elif packed is None:
+            head_w = (w("bert.pooler.dense.weight"), w("bert.pooler.dense.bias"), w("classifier.weight"),
+                      w("classifier.bias"))
             L.call("b2_head_fwd", x.data_ptr(), B, S, H, *head_w, self.C, p_c, rng, 1 + 3 * self.nl,
                    ws["pooled"].data_ptr(), ws["logits"].data_ptr(), s)
         else:
+            head_w = (w("bert.pooler.dense.weight"), w("bert.pooler.dense.bias"), w("classifier.weight"),
+                      w("classifier.bias"))
             L.call("b2_head_fwd_packed", x.data_ptr(), cls_rows.data_ptr(), Bo, H, *head_w, self.C, p_c, rng,
                    1 + 3 * self.nl, ws["pooled"].data_ptr(), ws["logits"].data_ptr(), s)
         loss = None
@@ -910,6 +1003,8 @@ class _Engine:
             loss = ws["loss"]
         if need_backward:
             self._saved = (B, S, mask, p_h, p_a, p_c, None if packed is None else (segs, cls_rows))
+        if self.token_head:
+            return ws["logits"].view(B, S, self.C), loss
         return ws["logits"], loss
 
     # ---- backward ---------------------------------------------------------------------------------------------------------
@@ -919,7 +1014,7 @@ class _Engine:
             raise RuntimeError("backward called without a training forward")
         B, S, mask, p_h, p_a, p_c, packed = self._saved
         self._saved = None
-        Bo = B if packed is None else packed[1].numel()
+        Bo = self.head_rows(B, S, packed)
         ws = self.workspace(B, S, Bo)
         dl = ws["dlogits"]
         if d_logits is not None:
@@ -932,7 +1027,7 @@ class _Engine:
 
     def _backward_from_dlogits(self, dl, B, S, mask, p_h, p_a, p_c, packed=None):
         cfg, H, I, M = self.cfg, self.H, self.I, B * S
-        Bo = B if packed is None else packed[1].numel()
+        Bo = self.head_rows(B, S, packed)
         ws = self.workspace(B, S, Bo)
         s = self.stream()
         rng = self.rng.data_ptr()
@@ -955,8 +1050,6 @@ class _Engine:
         L.call("b2_zero", self.grads.data_ptr() + 2 * eb, 2 * (ee - eb), s)
 
         x_last = ws["layers"][-1]["x2"] if self.nl > 0 else ws["emb_out"]
-        head_g = (g("bert.pooler.dense.weight"), g("bert.pooler.dense.bias"), g("classifier.weight"),
-                  g("classifier.bias"))
         # data gradient (d_hidden) on the main stream; the four head parameter gradients on the weight-gradient stream
         # (they belong to the last layer's bucket, whose readiness waits for that stream's marker of the layer anyway).
         # A model without encoder layers announces its head bucket right away: keep everything on one stream there.
@@ -965,10 +1058,19 @@ class _Engine:
         if self.nl > 0:
             # the side stream may still be busy with the previous step's tail; it must also not overtake this step
             side.wait_stream(main)
-        L.call("b2_head_bwd_split", dl.data_ptr(), x_last.data_ptr(), ws["pooled"].data_ptr(),
-               None if packed is None else packed[1].data_ptr(), M, Bo, S, H, w("bert.pooler.dense.weight"),
-               w("classifier.weight"), self.C, p_c, rng, 1 + 3 * self.nl, *head_g, ws["dxA"].data_ptr(), 1,
-               ws["head_scratch"].data_ptr(), s, side.cuda_stream if self.nl > 0 else None)
+        if self.token_head:
+            # every row of d_hidden is written: no memset
+            L.call("b2_token_head_bwd_split", dl.data_ptr(), x_last.data_ptr(), M, H, w("classifier.weight"), self.C,
+                   p_c, rng, 1 + 3 * self.nl, g("classifier.weight"), g("classifier.bias"), ws["dxA"].data_ptr(),
+                   ws["head_scratch"].data_ptr(), ws["head_scratch"].numel(), s,
+                   side.cuda_stream if self.nl > 0 else None)
+        else:
+            head_g = (g("bert.pooler.dense.weight"), g("bert.pooler.dense.bias"), g("classifier.weight"),
+                      g("classifier.bias"))
+            L.call("b2_head_bwd_split", dl.data_ptr(), x_last.data_ptr(), ws["pooled"].data_ptr(),
+                   None if packed is None else packed[1].data_ptr(), M, Bo, S, H, w("bert.pooler.dense.weight"),
+                   w("classifier.weight"), self.C, p_c, rng, 1 + 3 * self.nl, *head_g, ws["dxA"].data_ptr(), 1,
+                   ws["head_scratch"].data_ptr(), s, side.cuda_stream if self.nl > 0 else None)
         dx, dx_other = ws["dxA"], ws["dxB"]
         # Weight gradients are off the critical path (only the optimizer consumes them): they run on a second stream,
         # overlapping the dgrad / LayerNorm / attention chain of the main stream.  Their A operands (dzd, dU, dz1d,

@@ -26,7 +26,7 @@ def bin_length(attention_mask, seq_len):
     return BIN * max(1, -(-longest // BIN))
 
 
-def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN):
+def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN, labels=None, ignore_index=-100):
     """input_ids / token_type_ids / attention_mask: int64 [B, S] host tensors as the reference's Collate yields them
     (valid tokens first: the tokenizer pads on the right).  Returns a dict of host tensors:
       input_ids, token_type_ids, position_ids   int64 [NB, bin_len]   (unused bin rows: pad id 0, position 0)
@@ -35,6 +35,8 @@ def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN):
       cls_index                                  int64 [B]             flat row (bin * bin_len + lo) of sequence b's
                                                                        first token, in the ORIGINAL batch order
       lengths                                    int64 [B]
+      labels (when `labels`, int64 [B, S] token labels are given)
+                                                 int64 [NB, bin_len]   unused bin rows: ignore_index
     NB <= B; a sequence longer than bin_len is not supported (the reference truncates to max_seq_len = 128)."""
     if input_ids.dim() != 2:
         raise ValueError("input_ids must be [batch, seq]")
@@ -47,6 +49,14 @@ def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN):
         raise ValueError("pack_batch: attention_mask is not a right-padded prefix mask")
     if int(lens.min()) < 1:
         raise ValueError("pack_batch: empty sequence (no valid token)")
+    if labels is not None:
+        if labels.is_floating_point() or tuple(labels.shape) != (B, S):
+            raise ValueError("pack_batch: labels must be int64 [%d, %d] token labels" % (B, S))
+        lab_np = labels.numpy()
+        # packing drops masked positions: a label there would vanish, where HF's loss would count it
+        if bool((lab_np[~mask_np] != ignore_index).any()):
+            raise ValueError("pack_batch: a masked position carries a label other than ignore_index=%d; packing drops "
+                             "masked positions, so their labels must be ignored" % ignore_index)
     if int(lens.max()) > bin_len:
         raise ValueError("pack_batch: a sequence has %d valid tokens, more than the %d-token bin"
                          % (int(lens.max()), bin_len))
@@ -85,6 +95,11 @@ def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN):
     pos[dst] = within
     seg[dst] = (lo[seq_of_tok] | ((lo[seq_of_tok] + lens[seq_of_tok]) << 16)).astype(np.int32)
     t = torch.from_numpy
-    return {"input_ids": t(ids).view(NB, bin_len), "token_type_ids": t(tts).view(NB, bin_len),
-            "position_ids": t(pos).view(NB, bin_len), "segments": t(seg).view(NB, bin_len), "cls_index": t(first),
-            "lengths": t(lens), "bins": NB}
+    out = {"input_ids": t(ids).view(NB, bin_len), "token_type_ids": t(tts).view(NB, bin_len),
+           "position_ids": t(pos).view(NB, bin_len), "segments": t(seg).view(NB, bin_len), "cls_index": t(first),
+           "lengths": t(lens), "bins": NB}
+    if labels is not None:
+        lab = np.full(NB * bin_len, ignore_index, dtype=np.int64)
+        lab[dst] = lab_np.reshape(-1)[src]
+        out["labels"] = t(lab).view(NB, bin_len)
+    return out

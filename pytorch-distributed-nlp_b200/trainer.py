@@ -25,7 +25,9 @@ import numpy as np
 import torch
 
 from .ddp import DistributedDataParallel
-from .losses import criterion_key, infer_problem_type, loss_from_criterion, problem_type_loss
+from . import _lib as L
+from .losses import Loss, check_token_criterion, criterion_key, infer_problem_type, loss_from_criterion, \
+    problem_type_loss
 from .optim import clip_grad_norm_
 from .packing import MAX_BIN, bin_length, pack_batch
 from .schedules import get_scheduler, warmup_steps
@@ -76,6 +78,14 @@ def _unwrap(model):
     return model.module if isinstance(model, DistributedDataParallel) else model
 
 
+def _is_token(model):
+    """a BertForTokenClassification (or a wrapper of one): logits and labels per token"""
+    return _unwrap(model)._layout.head == "token"
+
+
+TOKEN_PROBLEM_TYPE = "token_classification"     # what Trainer.problem_type reports for a token model (not stored)
+
+
 CHECKPOINT_PREFIX = "checkpoint"     # HF Trainer's PREFIX_CHECKPOINT_DIR: output_dir/checkpoint-{optimizer step}
 
 
@@ -112,6 +122,10 @@ def step_loss(model, criterion=None):
     ValueError), and with no criterion the model's problem-type loss -- single-label cross-entropy when the config has
     no problem_type and more than one label (the step then stages int64 labels, as the reference's Collate yields)."""
     m = _unwrap(model)
+    if _is_token(m):
+        check_token_criterion(criterion)
+        if criterion is None:
+            return Loss(L.LOSS_CE, m.num_labels)      # HF's in-model loss of the token model
     if criterion is not None:
         return loss_from_criterion(criterion, m.num_labels, m._engine.dev if m._engine is not None else None)
     pt = getattr(m.config, "problem_type", None)
@@ -134,9 +148,10 @@ class _StagedGraphStep:
         self.B, self.S = batch_size, seq_len
         self.loss_fn = step_loss(self.model, criterion)
         self.criterion_key = criterion_key(criterion)
+        self.token = _is_token(self.model)     # labels per token row: B * S int64 slots
         z = lambda *s: torch.zeros(*s, dtype=torch.int64, device=dev)
         self.d_ids, self.d_tt, self.d_mask = z(batch_size, seq_len), z(batch_size, seq_len), z(batch_size, seq_len)
-        self.d_lab, lab_slots = self._label_buffer(batch_size)
+        self.d_lab, lab_slots = self._label_buffer(batch_size * seq_len if self.token else batch_size)
         self._alloc_stage(3 * batch_size * seq_len + lab_slots)
         self.loss_out = torch.zeros((), dtype=torch.float32, device=dev)
         self.h_loss = torch.zeros((), dtype=torch.float32).pin_memory()
@@ -167,6 +182,8 @@ class _StagedGraphStep:
     def _stage_labels(self, hs, lab):
         """host labels -> the label slots `hs` of the pinned staging buffer (fp32 labels bit for bit)"""
         fn = self.loss_fn
+        if self.token:
+            self._check_token_labels(lab)
         if not fn.float_labels:
             if lab.is_floating_point():
                 raise TypeError("%s was built for int64 class labels, got %s: pass a criterion (or config.problem_type)"
@@ -179,6 +196,20 @@ class _StagedGraphStep:
             raise type(e)("%s was built for %s labels of shape %s: %s"
                           % (type(self).__name__, "fp32", list(self.d_lab.shape), e)) from None
         hs.view(torch.float32)[:self.d_lab.numel()].copy_(lab.reshape(-1))
+
+    def _check_token_labels(self, lab):
+        """host token labels: int64, one per staged row, each a class index or the loss's ignore_index (the loss
+        kernel traps on anything else; padding must carry the ignore index, as HF's tagging collators put there)"""
+        if lab.is_floating_point():
+            raise TypeError("token labels are int64 class indices (CrossEntropyLoss), got %s" % lab.dtype)
+        if lab.numel() != self.d_lab.numel():
+            raise ValueError("%s was built for %d token labels, got %s" % (type(self).__name__, self.d_lab.numel(),
+                                                                           list(lab.shape)))
+        fn = self.loss_fn
+        bad = (lab != fn.ignore_index) & ((lab < 0) | (lab >= fn.C))
+        if bool(bad.any()):
+            raise ValueError("token label %d is outside [0, %d) and is not the ignore_index %d (padding positions must "
+                             "carry the ignore_index)" % (int(lab[bad].flatten()[0]), fn.C, fn.ignore_index))
 
     def _unstage_labels(self, st):
         if self.loss_fn.float_labels:
@@ -329,7 +360,7 @@ class _StagedGraphStep:
         logits, loss = forward()
         B, S, mask, p_h, p_a, p_c, packed = eng._saved
         eng._saved = None
-        Bo = B if packed is None else packed[1].numel()
+        Bo = eng.head_rows(B, S, packed)
         ws = eng.workspace(B, S, Bo)
         if self.accum_steps > 1:
             ws["dloss_logits"].mul_(1.0 / self.accum_steps)     # what an eager loop does with loss / k
@@ -387,8 +418,9 @@ class PackedTrainStep(_StagedGraphStep):
         dev = self.eng.dev
         self.bins, self.batch, self.bin_len = bins, batch, bin_len
         n = bins * bin_len
-        # pinned staging: ids | token types | positions | segments (as int64) | cls rows | labels
-        self.d_lab, lab_slots = self._label_buffer(batch)
+        # pinned staging: ids | token types | positions | segments (as int64) | cls rows | labels (per sequence, or
+        # per bin row for a token model: pack_batch's "labels")
+        self.d_lab, lab_slots = self._label_buffer(n if self.token else batch)
         self._alloc_stage(4 * n + batch + lab_slots)
         z = lambda *sh: torch.zeros(*sh, dtype=torch.int64, device=dev)
         self.d_pos, self.d_cls = z(bins, bin_len), z(batch)
@@ -406,7 +438,9 @@ class PackedTrainStep(_StagedGraphStep):
 
     def stage(self, packed, label):
         n, hs = self.bins * self.bin_len, self.h_stage
-        if packed["bins"] != self.bins or packed["input_ids"].shape[1] != self.bin_len or label.shape[0] != self.batch:
+        want = (self.bins, self.bin_len) if self.token else (self.batch,)
+        if packed["bins"] != self.bins or packed["input_ids"].shape[1] != self.bin_len or \
+                tuple(label.shape[:len(want)]) != want:
             raise ValueError("PackedTrainStep was built for %d bins of %d tokens / %d sequences"
                              % (self.bins, self.bin_len, self.batch))
         if self._h2d_done is not None:
@@ -422,11 +456,12 @@ class PackedTrainStep(_StagedGraphStep):
 
     def _body(self):
         self._unstage()
-        packed = (self.d_pos, self.d_seg, self.d_cls)
+        packed = (self.d_pos, self.d_seg, None if self.token else self.d_cls)
         self._train_body(lambda: self.eng.forward(self.d_ids, self.d_tt, None, self.d_lab, training=True,
                                                   need_backward=True, packed=packed, loss_fn=self.loss_fn))
 
     def __call__(self, packed, label, final=True):
+        """label: per sequence [batch], or for a token model pack_batch's "labels" [bins, bin_len]"""
         self.stage(packed, label)
         self.run_device(final)
         return self.loss_out
@@ -440,7 +475,8 @@ class FusedEvalStep(_StagedGraphStep):
 
     def __init__(self, model, batch_size, seq_len, use_graph=True, criterion=None):
         super().__init__(model, batch_size, seq_len, use_graph, criterion)
-        self.logits_out = torch.zeros(batch_size, self.model.num_labels, dtype=torch.float32, device=self.eng.dev)
+        shape = (batch_size, seq_len) if self.token else (batch_size,)
+        self.logits_out = torch.zeros(*shape, self.model.num_labels, dtype=torch.float32, device=self.eng.dev)
 
     def _body(self):
         self._unstage()
@@ -452,7 +488,7 @@ class FusedEvalStep(_StagedGraphStep):
     def __call__(self, batch_data):
         self.stage(batch_data)
         self.run_device()
-        return self.logits_out, self.d_lab, self.loss_out
+        return self.logits_out, self.d_lab.view(self.B, self.S) if self.token else self.d_lab, self.loss_out
 
 
 class Trainer:
@@ -526,18 +562,23 @@ class Trainer:
         """on_step's model call: (output, device label)"""
         d = self._to_device(batch_data)
         label = d["label"]
+        # a token model with a criterion leaves the loss to it: its in-model CrossEntropyLoss() would not know the
+        # criterion's ignore_index
+        model_labels = None if self.criterion is not None and _is_token(self.model) else label
         output = self.model(input_ids=d["input_ids"], token_type_ids=d["token_type_ids"],
-                            attention_mask=d["attention_mask"], labels=label)
+                            attention_mask=d["attention_mask"], labels=model_labels)
         return output, label
 
     def on_step(self, batch_data):
         output, label = self._forward(batch_data)
-        logits = output[1]
+        logits = output.logits
         return logits, label
 
     def problem_type(self, label):
         """the model's config.problem_type; when None, HF's rule applied to `label` (stored on the config, as the
         model's first labelled forward does)"""
+        if _is_token(self.model):
+            return TOKEN_PROBLEM_TYPE      # HF's token model never reads or sets config.problem_type
         cfg = _unwrap(self.model).config
         if getattr(cfg, "problem_type", None) is None:
             cfg.problem_type = infer_problem_type(_unwrap(self.model).num_labels, label)
@@ -550,6 +591,10 @@ class Trainer:
             if model_loss is None:
                 raise ValueError("Trainer has no criterion and the model returned no loss")
             return model_loss
+        if _is_token(self.model):
+            check_token_criterion(self.criterion)
+            C = _unwrap(self.model).num_labels
+            return self.criterion(logits.reshape(-1, C), label.reshape(-1))
         if _unwrap(self.model).num_labels == 1 and label.is_floating_point():
             return self.criterion(logits.reshape(-1), label.reshape(-1))
         return self.criterion(logits, label)
@@ -567,13 +612,15 @@ class Trainer:
         replay per batch instead of ~100 eager launches), else the eager call"""
         if not getattr(self.args, "fused", True) or batch_data["input_ids"].is_cuda:
             output, label = self._forward(batch_data)
-            return output[1], label, output[0]
+            return output.logits, label, output.loss
         self.problem_type(batch_data["label"])
         B, S = batch_data["input_ids"].shape
         m = _unwrap(self.model)
-        key = (id(m), B, S, m.config.problem_type)     # `test` may swap the model [:222-224]
+        # a token model's staged labels are checked against its loss's ignore_index: the criterion's
+        crit = self.criterion if _is_token(m) else None
+        key = (id(m), B, S, m.config.problem_type, criterion_key(crit))     # `test` may swap the model [:222-224]
         if key not in self._fused_eval:
-            self._fused_eval[key] = FusedEvalStep(self.model, B, S)
+            self._fused_eval[key] = FusedEvalStep(self.model, B, S, criterion=crit)
         return self._fused_eval[key](batch_data)
 
     def eval_step(self, batch_data):
@@ -615,8 +662,10 @@ class Trainer:
         if getattr(self.args, "fused", True) and getattr(self.args, "pack", False) and \
                 batch_data["input_ids"].shape[1] <= MAX_BIN and not batch_data["input_ids"].is_cuda:
             bin_len = bin_length(batch_data["attention_mask"], batch_data["input_ids"].shape[1])
+            token = _is_token(self.model)
             packed = pack_batch(batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"],
-                                bin_len)
+                                bin_len, labels=batch_data["label"] if token else None,
+                                ignore_index=self._ignore_index())
             key = (packed["bins"], batch_data["input_ids"].shape[0], bin_len,
                    torch.are_deterministic_algorithms_enabled())
             lkey = self._captured_loss_key(batch_data["label"])
@@ -628,7 +677,7 @@ class Trainer:
                                                     max_grad_norm=clip, criterion=self.criterion, bin_len=bin_len)
                 self._packed[key].loss_key = lkey
             self.model.train()
-            loss = self._packed[key](packed, batch_data["label"], final)
+            loss = self._packed[key](packed, packed["labels"] if token else batch_data["label"], final)
             if final:
                 self._scheduler_step()      # after the replay: the next stage() reads the new lr
         elif getattr(self.args, "fused", True):
@@ -671,6 +720,10 @@ class Trainer:
             self._note_grad_norm(clip)
             self.global_step += 1
         return self.loss_reduce(loss.detach())
+
+    def _ignore_index(self):
+        """the token labels' ignore index: the criterion's, else CrossEntropyLoss()'s -100"""
+        return int(getattr(self.criterion, "ignore_index", -100))
 
     def _scheduler_step(self):
         if self.lr_scheduler is not None:
@@ -881,7 +934,7 @@ class Trainer:
 
     def dev(self, dev_loader):
         """(summed rank-mean loss, metric) over the gathered rows.  The metric, higher is better: accuracy
-        (single-label), subset accuracy -- every column of (logits > 0) equal to (labels >= 0.5) -- (multi-label), or
+        (single-label; a token model's over the tokens whose label is not the ignore index), subset accuracy -- every column of (logits > 0) equal to (labels >= 0.5) -- (multi-label), or
         the Pearson correlation of predictions and labels (regression)."""
         self.model.eval()
         correct_total = 0
@@ -898,6 +951,13 @@ class Trainer:
                 loss_total += loss
                 logits, label = self.output_reduce(logits, label)
                 logits = logits.detach().cpu().numpy()
+                if problem_type == TOKEN_PROBLEM_TYPE:
+                    label = label.reshape(-1).detach().cpu().numpy()
+                    keep = label != self._ignore_index()
+                    preds = np.argmax(logits.reshape(label.shape[0], -1), axis=1)
+                    num_total += int(keep.sum())
+                    correct_total += int((preds[keep] == label[keep]).sum())
+                    continue
                 if problem_type == "regression":
                     reg_preds.append(logits.reshape(-1))
                     reg_trues.append(label.reshape(-1).detach().cpu().numpy())
@@ -917,7 +977,8 @@ class Trainer:
         return loss_total, correct_total / num_total
 
     def test(self, model, test_loader, labels):
-        """sklearn's classification_report over the gathered rows: of the argmax class (single-label) or of the
+        """sklearn's classification_report over the gathered rows: of the argmax class (single-label; a token model's
+        over the tokens whose label is not the ignore index) or of the
         indicator arrays (logits > 0) against (labels >= 0.5) (multi-label).  Regression raises ValueError."""
         self.model = model
         self.model.eval()
@@ -932,6 +993,12 @@ class Trainer:
                                      "use dev() for the Pearson correlation")
                 logits, label = self.output_reduce(logits, label)
                 logits = logits.detach().cpu().numpy()
+                if problem_type == TOKEN_PROBLEM_TYPE:
+                    label = label.reshape(-1).detach().cpu().numpy()
+                    keep = label != self._ignore_index()
+                    trues.extend(label[keep].tolist())
+                    preds.extend(np.argmax(logits.reshape(label.shape[0], -1), axis=1)[keep].tolist())
+                    continue
                 if problem_type == "multi_label_classification":
                     trues.append(label.detach().cpu().numpy() >= 0.5)
                     preds.append(logits > 0)
