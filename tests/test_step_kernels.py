@@ -338,14 +338,16 @@ def index_sums(idx, vals, n):
     return ref, mag, cnt
 
 
-def check_embed_grads(g, fw, dy, keep, gam, S, H, T, pad, scratch_bytes, what):
+def check_embed_grads(g, fw, dy, keep, gam, S, H, T, pad, scratch_bytes, what, vocab=VOCAB, max_pos=MAX_POS,
+                      unused=SENT, check=within):
     """stage 1: scratch_dx against fp64 LayerNorm backward (mask on the output); stage 2: the table gradients against
-    fp64 sums of the kernel's own scratch_dx"""
+    fp64 sums of the kernel's own scratch_dx.  Rows outside the batch must hold `unused` (what was there before the
+    backward); check: the within(got, ref, bound, what) that asserts and reports."""
     dev = dy.device
     M = dy.shape[0]
     dym = dy.double() * keep
     ref, E, xh, ex = ln_bwd_ref(dym, fw["pre"], fw["mean"], fw["rstd"], gam)
-    within(g["sdx"], ref, bf_bound(ref, E), what + " scratch_dx")
+    check(g["sdx"], ref, bf_bound(ref, E), what + " scratch_dx")
     sdx = g["sdx"].double()
     ids, tt = fw["ids32"].long(), fw["tt32"].long()
     posi = fw["pos32"].long() if fw.get("packed") else torch.arange(M, device=dev) % S
@@ -353,30 +355,31 @@ def check_embed_grads(g, fw, dy, keep, gam, S, H, T, pad, scratch_bytes, what):
     valid = ids != pad
     uniq, inv = torch.unique(ids[valid], return_inverse=True)
     ref, mag, cnt = index_sums(inv, sdx[valid], uniq.numel())
-    within(g["word"][uniq], ref, bf_bound(ref, cnt * U * mag), what + " d_word")
-    untouched = torch.ones(VOCAB, dtype=torch.bool, device=dev)
+    check(g["word"][uniq], ref, bf_bound(ref, cnt * U * mag), what + " d_word")
+    untouched = torch.ones(vocab, dtype=torch.bool, device=dev)
     untouched[uniq] = False
-    assert (g["word"][untouched] == SENT).all(), what + ": a row outside the batch was written"
+    assert (g["word"][untouched] == unused).all(), what + ": a row outside the batch was written"
     if pad >= 0:
-        assert (g["word"][pad] == SENT).all(), what + ": the pad row was written"
+        assert (g["word"][pad] == unused).all(), what + ": the pad row was written"
     # position rows
-    ref, mag, cnt = index_sums(posi, sdx, MAX_POS)
-    within(g["pos"][:S], ref[:S], bf_bound(ref[:S], cnt[:S] * U * mag[:S]), what + " d_pos")
-    assert (g["pos"][S:] == SENT).all(), what + ": d_pos rows >= seq were written"
+    ref, mag, cnt = index_sums(posi, sdx, max_pos)
+    check(g["pos"][:S], ref[:S], bf_bound(ref[:S], cnt[:S] * U * mag[:S]), what + " d_pos")
+    assert (g["pos"][S:] == unused).all(), what + ": d_pos rows >= seq were written"
     # type rows: per-position chains then the partial reduction (fast path) or the filtered column sums (fallback)
     ref, mag, _ = index_sums(tt, sdx, T)
     depth = int(cnt.max()) + S + M // 8 + 48
-    within(g["type"][:T], ref, bf_bound(ref, depth * U * mag), what + " d_type")
-    assert (g["type"][T] == SENT).all()
+    check(g["type"][:T], ref, bf_bound(ref, depth * U * mag), what + " d_type")
+    if g["type"].shape[0] > T:
+        assert (g["type"][T] == unused).all()
     # LayerNorm parameters (the generic backward's partial rows + colsum_finish)
     nb = min(296, scratch_bytes // (12 * H), (M + 7) // 8)
     depth = -(-M // (8 * nb)) + 8 + nb // 8 + 9
     t_g, t_b = dym * xh, dym
     ref = t_g.sum(0)
     E = (depth + 3) * U * t_g.abs().sum(0) + (dym.abs() * ex).sum(0)
-    within(g["gamma"], ref, bf_bound(ref, E), what + " d_gamma")
+    check(g["gamma"], ref, bf_bound(ref, E), what + " d_gamma")
     ref = t_b.sum(0)
-    within(g["beta"], ref, bf_bound(ref, depth * U * t_b.abs().sum(0)), what + " d_beta")
+    check(g["beta"], ref, bf_bound(ref, depth * U * t_b.abs().sum(0)), what + " d_beta")
 
 
 EMBED_CASES = [  # H, packed, type_vocab, pad_token_id, p, fp32 dy
@@ -481,7 +484,9 @@ def head_fwd(hs, cls, B, S, H, params, C, p, dev):
     return pooled, logits
 
 
-def check_head_fwd(hs, rows, pooled, logits, params, p, what):
+def check_head_fwd(hs, rows, pooled, logits, params, p, what, keep=None, check=within):
+    """pooled and logits of the sequence head from the kernel's own bf16 pooled; keep: the scaled fp64 [B, H] mask of
+    the classifier dropout (None: this file's key at HEAD_SITE)"""
     Wp, bp, Wc, bc = (t.double() for t in params)
     B, H = pooled.shape
     h0 = hs[rows].double()
@@ -489,11 +494,13 @@ def check_head_fwd(hs, rows, pooled, logits, params, p, what):
     pre = h0 @ Wp.t() + bp
     ref = torch.tanh(pre)
     E = (1 - ref ** 2) * (depth * U * (h0.abs() @ Wp.abs().t() + bp.abs())) + 4 * U * ref.abs() + U
-    within(pooled, ref, bf_bound(ref, E), what + " pooled")
-    x = pooled.double() * keep_mask(B, H, HEAD_SITE, p, hs.device) if p > 0 else pooled.double()
+    check(pooled, ref, bf_bound(ref, E), what + " pooled")
+    if keep is None and p > 0:
+        keep = keep_mask(B, H, HEAD_SITE, p, hs.device)
+    x = pooled.double() * keep if keep is not None else pooled.double()
     ref = x @ Wc.t() + bc
     E = (depth + 2) * U * (x.abs() @ Wc.abs().t() + bc.abs())
-    within(logits, ref, E, what + " logits")
+    check(logits, ref, E, what + " logits")
 
 
 @pytest.mark.parametrize("B,H,C,p", HEAD_FWD_CASES)
@@ -555,32 +562,37 @@ def test_head_bwd_split(cuda_dev, packed, f32):
     g2, dh2 = head_bwd(dl, hs, pooled, cls, tokens, B, S, H, params, C, p, f32, side, dev)
     for a, b in zip(g1 + [dh1], g2 + [dh2]):
         assert torch.equal(a, b), "the weight-gradient stream changed a result"
-    other = torch.ones(tokens, dtype=torch.bool, device=dev)
+    what = "head_bwd packed=%d f32=%d" % (packed, f32)
+    check_head_bwd(dl, hs, rows, pooled, params, g1, dh1, f32, keep_mask(B, H, HEAD_SITE, p, dev), what)
+    if not packed:
+        with pytest.raises(RuntimeError, match="tokens / seq mismatch"):
+            head_bwd(dl, hs, pooled, None, tokens - 1, B, S, H, params, C, p, f32, None, dev)
+
+
+def check_head_bwd(dl, hs, rows, pooled, params, grads, dh, f32, m, what, check=within):
+    """the four head parameter gradients and d_hidden (rows: the cls rows; every other row must be 0), in fp64 from
+    the kernel's own pooled (the same statements autograd runs); m: the scaled fp64 [B, H] keep mask"""
+    B, C, H = dl.shape[0], dl.shape[1], pooled.shape[1]
+    other = torch.ones(dh.shape[0], dtype=torch.bool, device=dh.device)
     other[rows] = False
-    assert bool((dh1[other] == 0).all()), "non-CLS rows of d_hidden are not zero"
-    # fp64 reference from the kernel's own pooled (the same statements autograd runs)
+    assert bool((dh[other] == 0).all()), what + ": non-CLS rows of d_hidden are not zero"
     Wp, _, Wc, _ = (t.double() for t in params)
     P = pooled.double()
-    m = keep_mask(B, H, HEAD_SITE, p, dev)
     h0, dl64 = hs[rows].double(), dl.double()
     dpd, apd = dl64 @ Wc, dl64.abs() @ Wc.abs()
     d_pre = dpd * m * (1 - P ** 2)
     e_pre = apd * m * ((C + 3) * U * (1 - P ** 2).abs() + 2 * U * (1 + P ** 2))
     a_pre = apd * m * (1 - P ** 2).abs()
     pm = P * m
-    what = "head_bwd packed=%d f32=%d" % (packed, f32)
     refs = [(d_pre.t() @ h0, (B + 2) * U * (a_pre.t() @ h0.abs()) + e_pre.t() @ h0.abs()),
             (d_pre.sum(0), B * U * a_pre.sum(0) + e_pre.sum(0)),
             (dl64.t() @ pm, (B + 2) * U * (dl64.abs().t() @ pm.abs())),
             (dl64.sum(0), B * U * dl64.abs().sum(0))]
     for k, (ref, E) in enumerate(refs):
-        within(g1[k], ref, bf_bound(ref, E), "%s grad %d" % (what, k))
+        check(grads[k], ref, bf_bound(ref, E), "%s grad %d" % (what, k))
     ref = d_pre @ Wp
     E = (H / 8 + 9) * U * (a_pre @ Wp.abs()) + e_pre @ Wp.abs()
-    within(dh1[rows], ref, E if f32 else bf_bound(ref, E), what + " d_hidden")
-    if not packed:
-        with pytest.raises(RuntimeError, match="tokens / seq mismatch"):
-            head_bwd(dl, hs, pooled, None, tokens - 1, B, S, H, params, C, p, f32, None, dev)
+    check(dh[rows], ref, E if f32 else bf_bound(ref, E), what + " d_hidden")
 
 
 @pytest.mark.parametrize("B,C", [(1, 1), (1, 100), (300, 7), (1000, 100), (1000, 2)])
@@ -597,6 +609,12 @@ def test_ce_fwd_bwd(cuda_dev, B, C, with_grad):
     dlog = torch.full((B, C), float("nan"), device=dev) if with_grad else None
     L.call("b2_ce_fwd_bwd", z.data_ptr(), labels.data_ptr(), B, C, loss.data_ptr(), L.ptr(dlog), stream())
     torch.cuda.synchronize()
+    check_ce(z, labels, loss, dlog, "ce B=%d C=%d" % (B, C))
+
+
+def check_ce(z, labels, loss, dlog, what, check=within):
+    """the mean cross-entropy and (dlog not None) its logits gradient against float64 from the kernel's logits"""
+    B, C = z.shape
     zz = z.double().requires_grad_(True)
     ref = F.cross_entropy(zz, labels)
     ref.backward()
@@ -609,13 +627,13 @@ def test_ce_fwd_bwd(cuda_dev, B, C, with_grad):
     e_lse = (C + 3) * U + U * (z64 - z64.max(1).values[:, None]).abs().max(1).values + 2 * U * lse.abs()
     lb = (lse - zy)
     e_loss = ((e_lse + U * zy.abs() + U * lb.abs())[valid].sum() + (-(-B // 256) + 9) * U * lb[valid].abs().sum()) / n
-    within(loss.view(1), ref.detach().view(1), (e_loss + 2 * U * ref.detach().abs()).view(1), "ce B=%d C=%d loss" % (B, C))
-    if with_grad:
+    check(loss.view(1), ref.detach().view(1), (e_loss + 2 * U * ref.detach().abs()).view(1), what + " loss")
+    if dlog is not None:
         sm = torch.softmax(z64, 1)
         # expf underflows below 2^-126 (gradual, to 2^-149): an absolute floor of 2^-126 / n
         E = (sm * (U * (z64 - lse[:, None]).abs() + e_lse[:, None] + 2 * U) + 2.0 ** -126) / n + 4 * U * zz.grad.abs()
-        within(dlog, zz.grad, E, "ce B=%d C=%d dlogits" % (B, C))
-        assert bool((dlog[~valid] == 0).all())
+        check(dlog, zz.grad, E, what + " dlogits")
+        assert bool((dlog[~valid] == 0).all()), what + ": ignored rows have a nonzero gradient"
 
 
 # ======================================================================================================================

@@ -88,28 +88,36 @@ def test_token_head_kernels_against_float64(cuda_dev, M, H, C, p):
     seed, step, site = 987654321, 5, 37
     logits, dh, dW, db = _run_kernels(x.to(cuda_dev), W.to(cuda_dev), bvec.to(cuda_dev), dl.to(cuda_dev), p, seed,
                                       step, site)
-    keep = torch.from_numpy(philox_keep_mask(M * H, seed, step, site, p).reshape(M, H)).double()
-    sc = _scale(p)
-    xd = x.double() * keep * sc
-    Wd, dld = W.double(), dl.double()
-    # forward
+    keep = torch.from_numpy(philox_keep_mask(M * H, seed, step, site, p).reshape(M, H)).double() * _scale(p)
+    check_token_head_fwd(x, W, bvec, keep, logits.cpu(), "token head")
+    check_token_head_bwd(x, W, dl, keep, dh.cpu(), dW.cpu(), db.cpu(), "token head")
+    assert not torch.isnan(dh).any() and not torch.isnan(logits).any()
+
+
+def check_token_head_fwd(x, W, bvec, keep, logits, what, check=_within):
+    """logits of b2_token_head_fwd at the module docstring's bound; keep: the scaled fp64 [M, H] dropout mask"""
+    H = x.shape[1]
+    xd, Wd = x.double() * keep, W.double()
     z = xd @ Wd.t() + bvec.double()
     zabs = (xd.abs() @ Wd.abs().t()) + bvec.double().abs()
-    _within(logits.cpu(), z, (H / 32 + 8) * U32 * zabs + 1e-30, "logits")
-    # data gradient
-    dref = (dld @ Wd) * keep * sc
-    dabs = (dld.abs() @ Wd.abs()) * keep * sc
-    _within(dh.cpu(), dref, (C + 3) * U32 * dabs + 1e-30, "d_hidden")
-    # parameter gradients
+    check(logits, z, (H / 32 + 8) * U32 * zabs + 1e-30, what + " logits")
+
+
+def check_token_head_bwd(x, W, dl, keep, dh, dW, db, what, check=_within):
+    """d_hidden, d_W and d_b of b2_token_head_bwd_split at the module docstring's bounds"""
+    M, C = dl.shape
+    xd, Wd, dld = x.double() * keep, W.double(), dl.double()
+    dref = (dld @ Wd) * keep
+    dabs = (dld.abs() @ Wd.abs()) * keep
+    check(dh, dref, (C + 3) * U32 * dabs + 1e-30, what + " d_hidden")
     rpb, nblk = _row_blocks(M)
     n = rpb + nblk + 3
     wref, wabs = dld.t() @ xd, dld.abs().t() @ xd.abs()
     e32 = n * U32 * wabs
-    _within(dW.cpu(), wref, 2.0 ** -8 * (wref.abs() + e32) + e32 + 1e-30, "dW")
+    check(dW, wref, 2.0 ** -8 * (wref.abs() + e32) + e32 + 1e-30, what + " dW")
     bref, babs = dld.sum(0), dld.abs().sum(0)
     e32 = n * U32 * babs
-    _within(db.cpu(), bref, 2.0 ** -8 * (bref.abs() + e32) + e32 + 1e-30, "db")
-    assert not torch.isnan(dh).any() and not torch.isnan(logits).any()
+    check(db, bref, 2.0 ** -8 * (bref.abs() + e32) + e32 + 1e-30, what + " db")
 
 
 @gpu
