@@ -353,6 +353,39 @@ int32_t b2_token_head_bwd_split(const float* dlogits, const void* hidden_states,
 int64_t b2_token_head_scratch_floats(int64_t tokens, int64_t hidden, int64_t num_labels);
 
 /* ------------------------------------------------------------------------------------------------------ */
+/* masked-language-model head (csrc/mlm_head.cu, HF BertForMaskedLM's cls.predictions)                     */
+/* ------------------------------------------------------------------------------------------------------ */
+/* The head runs on the labelled rows only, listed into `capacity` rows (capacity <= tokens).  b2_mlm_compact:
+ * rows[i] = the i-th token (in token order) whose label is not ignore_index, slot_labels[i] its label, slot[m] = the
+ * row of token m or -1, *count the number of them; the capacity rows past *count get row 0 and label -1.  A label
+ * outside [0, vocab) that is not ignore_index, or more labelled tokens than the capacity, traps.               */
+int32_t b2_mlm_compact(const int64_t* labels, int64_t tokens, int64_t ignore_index, int64_t vocab, int64_t capacity,
+                       int32_t* rows, int32_t* slot, int32_t* slot_labels, int32_t* count, void* stream);
+/* out[i] = x[rows[i]] (bf16 [capacity, hidden]) for i < *count, zero rows after it                              */
+int32_t b2_mlm_gather_rows(const void* x, const int32_t* rows, const int32_t* count, int64_t capacity, int64_t hidden,
+                           void* out, void* stream);
+/* dx[m] = src[slot[m]] (fp32) for slot[m] >= 0, a zero row otherwise: every row of dx [tokens, hidden] is written  */
+int32_t b2_mlm_scatter_rows(const float* src, const int32_t* slot, int64_t tokens, int64_t hidden, float* dx,
+                            void* stream);
+/* du = bf16(dg * gelu'(u)) elementwise, n a multiple of 8 (dg fp32, u bf16: the transform's pre-activation)      */
+int32_t b2_mlm_gelu_bwd(const float* dg, const void* u, int64_t n, void* du, void* stream);
+/* logits[r, c] = bias[c] (fp32 [rows, vocab_pad]), vocab_pad a multiple of 64: EPI_ACCUM_F32 then adds x W^T    */
+int32_t b2_mlm_bias_fill(const void* bias, int64_t rows, int64_t vocab_pad, float* logits, void* stream);
+/* Vocabulary cross-entropy over fp32 logits [rows, vocab_pad], one block per row.  labels int32 [rows] (NULL: all
+ * -1), -1 = no loss term; rows at or past *n_rows (NULL: none) are capacity padding.  For each row:
+ *   row_loss[r] = logsumexp(x[r, :vocab]) - x[r, y]   (0 without a label),   pred[r] = argmax (-1 without a label)
+ *   d_logits[r, c] = bf16(d_extra[r, c] + (softmax - onehot) * (*d_loss) / (*n_labelled)) for c < vocab, 0 above
+ * (d_loss NULL: 1; d_extra NULL: 0; pred / d_logits NULL: not written; padding rows get zero rows).  loss (NULL: not
+ * written) = sum of row_loss / *n_labelled, summed in a fixed order: nan when *n_labelled is 0.  A label outside
+ * [-1, vocab) traps.                                                                                           */
+int32_t b2_mlm_ce(const float* logits, int64_t rows, int64_t vocab, int64_t vocab_pad, const int32_t* labels,
+                  const int32_t* n_rows, const int32_t* n_labelled, const float* d_loss, const float* d_extra,
+                  int64_t ld_extra, float* row_loss, int32_t* pred, void* d_logits, float* loss, void* stream);
+/* grad = bf16(grad + dec) over n elements (a multiple of 8): the tied decoder's fp32 part of the word-embedding
+ * gradient added onto the embedding backward's rows                                                           */
+int32_t b2_mlm_tied_add(const float* dec, void* grad, int64_t n, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------ */
 /* optimizer + gradient exchange                                                                          */
 /*   replaces: HF AdamW.step (transformers 4.28.1 optimization.py, built at multi-gpu-distributed-cls.py    */
 /*   :100-111, stepped :174), optimizer.zero_grad (:172), and the DDP Reducer's bucket all-reduce            */

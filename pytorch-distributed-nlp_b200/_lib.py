@@ -109,6 +109,14 @@ _SIGNATURES = {
     # token-classification head (csrc/token_head.cu)
     "b2_token_head_fwd": [vp, i64, i64, vp, vp, i64, f32, vp, u32, vp, vp],
     "b2_token_head_bwd_split": [vp, vp, i64, i64, vp, i64, f32, vp, u32, vp, vp, vp, vp, i64, vp, vp],
+    # masked-language-model head (csrc/mlm_head.cu)
+    "b2_mlm_compact": [vp, i64, i64, i64, i64, vp, vp, vp, vp, vp],
+    "b2_mlm_gather_rows": [vp, vp, vp, i64, i64, vp, vp],
+    "b2_mlm_scatter_rows": [vp, vp, i64, i64, vp, vp],
+    "b2_mlm_gelu_bwd": [vp, vp, i64, vp, vp],
+    "b2_mlm_bias_fill": [vp, i64, i64, vp, vp],
+    "b2_mlm_ce": [vp, i64, i64, i64, vp, vp, vp, vp, vp, i64, vp, vp, vp, vp, vp],
+    "b2_mlm_tied_add": [vp, vp, i64, vp],
     "b2_bucket_reduce_adamw": [C.POINTER(vp), C.POINTER(vp), i32, i32, vp, vp, vp, vp, i64, i64,
                                C.POINTER(AdamWHParams), vp, vp],
     "b2_adamw_prepare": [C.POINTER(AdamWHParams), vp, vp, vp],

@@ -105,7 +105,15 @@ def _round8(n):
     return (n + 7) // 8 * 8
 
 
-HEAD_KINDS = ("sequence", "token")     # BertForSequenceClassification's pooler + classifier, or a classifier per token
+def vocab_pad(vocab_size):
+    """the masked-LM model's vocabulary rows in the flat space: vocab_size rounded up to 64, the GEMM's N granule"""
+    return (vocab_size + 63) // 64 * 64
+
+
+HEAD_KINDS = ("sequence", "token", "mlm")   # BertForSequenceClassification's pooler + classifier, a classifier per
+                                            # token, or BertForMaskedLM's cls.predictions
+MLM_TIED = {"cls.predictions.decoder.weight": "bert.embeddings.word_embeddings.weight",
+            "cls.predictions.decoder.bias": "cls.predictions.bias"}    # HF's tied state-dict keys of the MLM head
 TOKEN_HEAD_MAX_LABELS = 64             # b2_token_head_fwd's bound
 
 
@@ -118,7 +126,10 @@ class _Layout:
     Buckets (DDP exchange / AdamW launch units) = embeddings | encoder layer 0..L-2 | last layer + head.  The head
     (pooler + classifier, 0.6 M parameters) rides with the last encoder layer -- they are adjacent in the flat space and
     final within microseconds of each other at the start of backward -- instead of paying a barrier, an exchange and
-    a kernel launch of its own.  head "token" (BertForTokenClassification): the tail is the classifier alone."""
+    a kernel launch of its own.  head "token" (BertForTokenClassification): the tail is the classifier alone.  head
+    "mlm" (BertForMaskedLM): the tail is cls.predictions (its decoder is the word-embedding table), and the word table
+    and cls.predictions.bias reserve vocab_pad(V) rows / entries, so the vocabulary projection is one GEMM with a
+    multiple of 64 columns; the extra rows stay zero and lie outside every parameter view."""
 
     def __init__(self, cfg, head="sequence"):
         if head not in HEAD_KINDS:
@@ -129,16 +140,18 @@ class _Layout:
         self.buckets = []             # (begin, end, label)
         off = 0
 
-        def add(name, shape):
+        def add(name, shape, reserve=None):
             nonlocal off
             n = 1
             for s in shape:
                 n *= s
             self.entries[name] = (off, tuple(shape))
-            off += _round8(n)
+            off += _round8(n if reserve is None else reserve)
 
+        mlm = head == "mlm"
+        self.vocab_pad = vocab_pad(cfg.vocab_size) if mlm else cfg.vocab_size
         b0 = off
-        add("bert.embeddings.word_embeddings.weight", (cfg.vocab_size, H))
+        add("bert.embeddings.word_embeddings.weight", (cfg.vocab_size, H), self.vocab_pad * H if mlm else None)
         add("bert.embeddings.position_embeddings.weight", (cfg.max_position_embeddings, H))
         add("bert.embeddings.token_type_embeddings.weight", (cfg.type_vocab_size, H))
         add("bert.embeddings.LayerNorm.weight", (H,))
@@ -169,8 +182,15 @@ class _Layout:
         if head == "sequence":
             add("bert.pooler.dense.weight", (H, H))
             add("bert.pooler.dense.bias", (H,))
-        add("classifier.weight", (cfg.num_labels, H))
-        add("classifier.bias", (cfg.num_labels,))
+        if mlm:
+            add("cls.predictions.bias", (cfg.vocab_size,), self.vocab_pad)
+            add("cls.predictions.transform.dense.weight", (H, H))
+            add("cls.predictions.transform.dense.bias", (H,))
+            add("cls.predictions.transform.LayerNorm.weight", (H,))
+            add("cls.predictions.transform.LayerNorm.bias", (H,))
+        else:
+            add("classifier.weight", (cfg.num_labels, H))
+            add("classifier.bias", (cfg.num_labels,))
         if L_ > 0:
             lb, _le, lbl = self.buckets[-1]
             self.buckets[-1] = (lb, off, lbl + "+head")
@@ -183,8 +203,8 @@ class _Layout:
         return self.entries[name][0]
 
 
-# HF named_parameters() order (201 tensors for 12 layers, 199 without the pooler); differs from the flat order only
-# inside attention.self
+# HF named_parameters() order (201 tensors for 12 layers, 199 without the pooler, 202 for the MLM head); differs from
+# the flat order only inside attention.self
 def _hf_order(cfg, head="sequence"):
     names = ["bert.embeddings.word_embeddings.weight", "bert.embeddings.position_embeddings.weight",
              "bert.embeddings.token_type_embeddings.weight", "bert.embeddings.LayerNorm.weight",
@@ -196,6 +216,10 @@ def _hf_order(cfg, head="sequence"):
             names += [p + m + ".weight", p + m + ".bias"]
     if head == "sequence":
         names += ["bert.pooler.dense.weight", "bert.pooler.dense.bias"]
+    if head == "mlm":
+        return names + ["cls.predictions.bias", "cls.predictions.transform.dense.weight",
+                        "cls.predictions.transform.dense.bias", "cls.predictions.transform.LayerNorm.weight",
+                        "cls.predictions.transform.LayerNorm.bias"]
     names += ["classifier.weight", "classifier.bias"]
     return names
 
@@ -237,12 +261,13 @@ class _StepFn(torch.autograd.Function):
         eng.start_pass(accumulate)
         eng.backward(d_logits, d_loss if ctx.has_loss else None)
         eng.end_pass()
-        # Gradients live in the engine's bf16 bucket space, not in `.grad`.  The anchor (classifier.bias) gets its
-        # true gradient as a 6-float fp32 probe: it is the column sum of d_logits, so an inf/nan anywhere upstream
+        # Gradients live in the engine's bf16 bucket space, not in `.grad`.  The anchor (classifier.bias, or
+        # cls.predictions.bias) gets its true gradient as an fp32 probe: it is the column sum of d_logits, so an
+        # inf/nan anywhere upstream
         # of the model shows up in it -- which is what torch.cuda.amp.GradScaler's inf check needs to see.  Autograd
         # sums the probes of an accumulation window's backwards; the final one reads the folded window sum, so the
         # probe is non-finite exactly when some pass of the window was.
-        off, shape = ctx.model._layout.entries["classifier.bias"]
+        off, shape = ctx.model._layout.entries[model._anchor]
         n = 1
         for d in shape:
             n *= d
@@ -256,6 +281,7 @@ class _BertClassifier(nn.Module):
     """What the classification models share: the HF parameter skeleton over one flat fp32 space, construction,
     device movement, state dicts, the dropout stream and no_sync().  The subclass names its head kind (_Layout)."""
     _head = None
+    _anchor = "classifier.bias"   # the parameter _StepFn's autograd output hangs on (its gradient is the probe)
     _config_extra = {}       # written into save_pretrained's config.json over the config's attributes
 
     def __init__(self, config):
@@ -569,6 +595,86 @@ class BertForTokenClassification(_BertClassifier):
         return self._ce
 
 
+def _check_mlm_labels(labels, input_ids):
+    """masked-LM labels: int64 token ids of the input's shape (the compaction kernel reads them as int64)"""
+    if labels.dtype != torch.int64 or tuple(labels.shape) != tuple(input_ids.shape):
+        raise TypeError("masked-LM labels are int64 token ids of the input's shape %s (-100: ignored), got %s %s"
+                        % (list(input_ids.shape), labels.dtype, list(labels.shape)))
+
+
+class BertForMaskedLM(_BertClassifier):
+    """HF's BertForMaskedLM: BertModel without the pooler, then cls.predictions -- transform (dense, erf GELU,
+    LayerNorm) and a decoder tied to the word embeddings, ``logits = transform(x) @ word_embeddings.weight^T +
+    cls.predictions.bias`` -- and with labels HF's ``CrossEntropyLoss()`` over ``logits.view(-1, V)`` /
+    ``labels.view(-1)`` (-100 ignored; config.problem_type is not read).  Logits are fp32 [batch, seq, V] over every
+    row (or [bins, bin_len, V] packed).  The loss, and a backward from the loss alone, run the head on the labelled
+    rows only (csrc/mlm_head.cu); a backward that reaches the logits takes their dense gradient."""
+    _head = "mlm"
+    _anchor = "cls.predictions.bias"
+    _config_extra = {"architectures": ["BertForMaskedLM"]}
+
+    def forward(self, input_ids=None, token_type_ids=None, attention_mask=None, labels=None, position_ids=None,
+                segments=None, **unused):
+        """`position_ids` / `segments` (both or neither): the rows of `input_ids` are the bins of
+        `packing.pack_batch`, and `labels` its packed "labels" (unused bin rows hold -100)."""
+        if self._engine is None:
+            raise RuntimeError("BertForMaskedLM (b200) only runs on CUDA: call model.cuda() first; there is no CPU "
+                               "path.")
+        if input_ids is None:
+            raise ValueError("input_ids is required")
+        packed = None
+        if segments is not None or position_ids is not None:
+            if position_ids is None or segments is None:
+                raise ValueError("a packed batch needs position_ids and segments together")
+            packed = (position_ids, segments, None)
+        if labels is not None:
+            _check_mlm_labels(labels, input_ids)
+        if torch.is_grad_enabled() and self.training:
+            anchor = self._params_by_name[self._anchor]
+            logits, loss = _StepFn.apply(anchor, self, input_ids, token_type_ids, attention_mask, labels, packed)
+            return SequenceClassifierOutput(loss=loss if labels is not None else None, logits=logits)
+        logits, loss = self._engine.forward(input_ids, token_type_ids, attention_mask, labels,
+                                            training=self.training, need_backward=False, packed=packed)
+        return SequenceClassifierOutput(loss=None if loss is None else loss.clone(), logits=logits.clone())
+
+    def masked_lm_eval(self, input_ids, token_type_ids=None, attention_mask=None, labels=None, ignore_index=-100):
+        """The dropout-free forward on the labelled rows only: (mean loss, predicted ids, labels) as device tensors,
+        the last two over the labelled tokens in token order.  No [batch, seq, V] logits are built."""
+        if self._engine is None:
+            raise RuntimeError("BertForMaskedLM (b200) only runs on CUDA: call model.cuda() first")
+        if labels is None:
+            raise ValueError("masked_lm_eval needs labels: it evaluates the labelled tokens")
+        _check_mlm_labels(labels, input_ids)
+        with torch.no_grad():
+            _logits, loss = self._engine.forward(input_ids, token_type_ids, attention_mask, labels, training=False,
+                                                 need_backward=False, mlm_full=False, ignore_index=ignore_index)
+        gb = self._engine.mlm_last
+        n = int(gb["count"].item())
+        return loss.clone(), gb["pred"][:n].long(), gb["labels"][:n].long()
+
+    def state_dict(self, *args, **kwargs):
+        """HF's keys, with the tied decoder as HF lists it: cls.predictions.decoder.weight (the word-embedding tensor)
+        and cls.predictions.decoder.bias (cls.predictions.bias)"""
+        sd = super().state_dict(*args, **kwargs)
+        prefix = kwargs.get("prefix", args[1] if len(args) > 1 else "")
+        for tied, src in MLM_TIED.items():
+            if prefix + src in sd:
+                sd[prefix + tied] = sd[prefix + src]
+        return sd
+
+    def load_state_dict(self, state_dict, strict=True, assign=False):
+        """accepts an HF state dict with or without the tied decoder keys (their tensors are the word embeddings and
+        cls.predictions.bias, loaded under those names)"""
+        sd = OrderedDict((k, v) for k, v in state_dict.items() if k not in MLM_TIED)
+        return super().load_state_dict(sd, strict=strict, assign=assign)
+
+    @classmethod
+    def from_pretrained(cls, model_path, config=None, **kwargs):
+        """as the classifiers' (a BertForPreTraining checkpoint's bert.pooler.* and cls.seq_relationship.* are
+        ignored, as HF ignores them); a checkpoint without cls.predictions keeps HF's fresh init of the head"""
+        return super().from_pretrained(model_path, config=config, **kwargs)
+
+
 class _LocalTransport:
     """The facts the optimizer's step schedule (optim._FusedOptimizer: bucket_ready, step, the clip phases) needs about
     where gradients and weights live, on one GPU.  DistributedDataParallel answers the same questions for a peer group
@@ -635,6 +741,14 @@ class _Engine:
         cd = getattr(cfg, "classifier_dropout", None)
         self.p_cls = float(cd if cd is not None else cfg.hidden_dropout_prob)
         self.token_head = self.lay.head == "token"     # a classifier on every token row instead of pooler + classifier
+        self.mlm = self.lay.head == "mlm"               # cls.predictions on the labelled rows (csrc/mlm_head.cu)
+        self.per_token = self.token_head or self.mlm    # packed bins need no cls_index
+        self.V, self.Vp = cfg.vocab_size, self.lay.vocab_pad
+        self._mlm_ws = {}
+        self._mlm_shared = None
+        self._mlm_saved = None
+        self._mlm_pending = None     # (head buffers, transform input, labelled-row buffers or None) of the backward
+        self.mlm_last = None
         n = self.lay.total
         self.shadow = torch.empty(n, dtype=torch.bfloat16, device=self.dev)   # bf16 copy the GEMMs read
         self.grads = torch.zeros(n, dtype=torch.bfloat16, device=self.dev)    # bf16 gradient bucket space
@@ -758,7 +872,7 @@ class _Engine:
 
     def head_rows(self, B, S, packed):
         """rows of the head's logits: every token (token head), else one per sequence (packed: its cls rows)"""
-        if self.token_head:
+        if self.per_token:
             return B * S
         return B if packed is None else packed[1].numel()
 
@@ -797,7 +911,7 @@ class _Engine:
                  "x1f": e(M, H, dtype=f32) if self.fused_ln else None,
                  "x2f": e(M, H, dtype=f32) if (self.fused_ln and li < nl - 1) else None}
                 for li in range(nl)],
-            "pooled": None if self.token_head else e(Bo, H), "logits": e(Bo, self.C, dtype=f32),
+            "pooled": None if self.per_token else e(Bo, H), "logits": e(Bo, self.C, dtype=f32),
             "loss": e((), dtype=f32),
             "dlogits": e(Bo, self.C, dtype=f32), "dloss_logits": e(Bo, self.C, dtype=f32),
             # gradient of the residual stream: fp32 (12 layers of residual adds would otherwise each round it to bf16);
@@ -806,7 +920,7 @@ class _Engine:
             "emb_dx": e(M, H), "dctx": e(M, H),
             # the token head's fp32 parameter-gradient partials, the sequence head's two [batch, H] planes
             "head_scratch": e(int(L.load().b2_token_head_scratch_floats(M, H, self.C)), dtype=f32) if self.token_head
-            else e(2 * Bo, H, dtype=f32),
+            else None if self.mlm else e(2 * Bo, H, dtype=f32),
             # operands of the weight-gradient GEMMs, double-buffered by layer parity (see _backward_from_dlogits)
             "dzd": [e(M, H), e(M, H)], "dz1d": [e(M, H), e(M, H)], "dU": [e(M, I), e(M, I)],
             "dqkv": [e(M, 3 * H), e(M, 3 * H)],
@@ -885,11 +999,16 @@ class _Engine:
 
     # ---- forward --------------------------------------------------------------------------------------------------------
     def forward(self, input_ids, token_type_ids, attention_mask, labels, training, need_backward, packed=None,
-                loss_fn=None):
+                loss_fn=None, mlm_full=True, ignore_index=-100, mlm_capacity=None, mlm_dloss=None):
         """packed: None, or (position_ids int64 [bins, S], segments int32 [bins, S], cls_index int64 [batch]) -- the
         rows of `input_ids` are then S-token bins produced by packing.pack_batch (S a multiple of 128, at most 512),
         not sequences.
-        loss_fn: the losses.Loss of `labels` (None: the model's problem-type loss, HF's in-model loss)."""
+        loss_fn: the losses.Loss of `labels` (None: the model's problem-type loss, HF's in-model loss).
+        Masked-LM head: `labels` int64 [B, S] with `ignore_index`; the loss runs on the labelled rows only, in a
+        capacity of mlm_capacity rows (None: their count rounded up to 128, read from the device); mlm_full: also
+        the logits of every row (returned as [B, S, V]; else None); mlm_dloss: a device scalar d(objective)/d(loss)
+        -- the same cross-entropy launch then also writes the labelled rows' d_logits for the backward (the
+        captured steps' one pass)."""
         cfg, H, I = self.cfg, self.H, self.I
         if input_ids.dim() != 2:
             raise ValueError("input_ids must be [batch, seq]")
@@ -901,16 +1020,16 @@ class _Engine:
                 raise ValueError("packed bins carry their own (block-diagonal) mask: pass attention_mask=None")
             for t, nm, dt, shape in ((pos_ids, "position_ids", torch.int64, (B, S)), (segs, "segments", torch.int32, (B, S)),
                                      (cls_rows, "cls_index", torch.int64, None)):
-                if t is None and self.token_head and nm == "cls_index":
+                if t is None and self.per_token and nm == "cls_index":
                     continue      # the token head reads every bin row
                 if t.device != self.dev or t.dtype != dt or (shape is not None and tuple(t.shape) != shape):
                     raise TypeError("%s must be a %s tensor%s on %s" % (nm, dt, "" if shape is None else " of shape %s"
                                                                         % (shape,), self.dev))
             pos_ids, segs = pos_ids.contiguous(), segs.contiguous()
-            if not self.token_head:
+            if not self.per_token:
                 cls_rows = cls_rows.contiguous().view(-1)
                 Bo = cls_rows.numel()
-        if self.token_head:
+        if self.per_token:
             Bo = B * S
         if B == 0 or S == 0:
             raise ValueError("empty batch")
@@ -924,7 +1043,7 @@ class _Engine:
                     raise RuntimeError("%s is on %s, model on %s" % (nm, t.device, self.dev))
                 if t is not labels and t.dtype != torch.int64:
                     raise TypeError("%s must be int64 (as the reference Collate produces)" % nm)
-        if labels is not None:
+        if labels is not None and not self.mlm:
             if loss_fn is None:
                 loss_fn = self.model._problem_type_loss(labels)
             labels = loss_fn.device_labels(labels, Bo)
@@ -983,6 +1102,12 @@ class _Engine:
                 w(pre + "output.LayerNorm.bias"), a["z2"].data_ptr(), a["x2"].data_ptr(), L.ptr(a["x2f"]),
                 a["mean2"].data_ptr(), a["rstd2"].data_ptr())
             x, xf = a["x2"], a["x2f"]
+        if self.mlm:
+            logits, loss = self._mlm_forward(x, M, labels, need_backward, mlm_full, ignore_index, mlm_capacity,
+                                             mlm_dloss)
+            if need_backward:
+                self._saved = (B, S, mask, p_h, p_a, p_c, None if packed is None else (segs, None))
+            return (None if logits is None else logits.view(B, S, self.V)), loss
         if self.token_head:
             L.call("b2_token_head_fwd", x.data_ptr(), M, H, w("classifier.weight"), w("classifier.bias"), self.C, p_c,
                    rng, 1 + 3 * self.nl, ws["logits"].data_ptr(), s)
@@ -1007,6 +1132,191 @@ class _Engine:
             return ws["logits"].view(B, S, self.C), loss
         return ws["logits"], loss
 
+    # ---- masked-LM head (cls.predictions) ---------------------------------------------------------------------------------
+    def _mlm_buffers(self, M, rows, full=False):
+        """the head's activations over `rows` rows: the labelled rows' capacity, or (full) all M rows, the logits of
+        the eager output"""
+        key = (M, rows, full)
+        hb = self._mlm_ws.get(key)
+        if hb is not None:
+            return hb
+        H, Vp, dev = self.H, self.Vp, self.dev
+        e = lambda *shape, dtype=torch.bfloat16: torch.empty(*shape, dtype=dtype, device=dev)
+        f32, i32 = torch.float32, torch.int32
+        hb = {"rows": rows, "x": None if full else e(rows, H), "u": e(rows, H), "h": e(rows, H), "t": e(rows, H),
+              "mean": e(rows, dtype=f32), "rstd": e(rows, dtype=f32), "logits": e(rows, Vp, dtype=f32),
+              "row_loss": e(rows, dtype=f32), "pred": e(rows, dtype=i32), "loss": e((), dtype=f32),
+              "dlog": None, "dt": None,
+              # compaction: source row of each slot, slot of each token, label of each slot (-1: none), count
+              "src": e(rows, dtype=i32), "slot": e(M, dtype=i32), "labels": e(rows, dtype=i32),
+              "count": e(1, dtype=i32)}
+        self._mlm_ws[key] = hb
+        return hb
+
+    def _mlm_grad_buffers(self, hb):
+        """the backward's buffers over the head's rows, allocated by the first backward that needs them"""
+        if hb["dlog"] is None:
+            rows, H, dev = hb["rows"], self.H, self.dev
+            e = lambda *shape, dtype=torch.bfloat16: torch.empty(*shape, dtype=dtype, device=dev)
+            hb.update(dlog=e(rows, self.Vp), dt=e(rows, H, dtype=torch.float32), dh=e(rows, H, dtype=torch.float32),
+                      dh_bf=e(rows, H), du=e(rows, H), dx=e(rows, H, dtype=torch.float32))
+        if self._mlm_shared is None:
+            sms = torch.cuda.get_device_properties(self.dev).multi_processor_count
+            self._mlm_shared = {
+                # fp32 decoder part of the tied word-embedding gradient [vocab_pad, H]
+                "dec": torch.empty(self.Vp, self.H, dtype=torch.float32, device=self.dev),
+                # b2_colsum's at most 32 partial rows over vocab_pad columns
+                "colsum": torch.empty(32 * self.Vp, dtype=torch.float32, device=self.dev),
+                # the transform LayerNorm backward's per-block partials (one block per SM)
+                "ln_parts": torch.empty(sms * 3 * self.H, dtype=torch.float32, device=self.dev),
+                "n_lab_one": torch.ones(1, dtype=torch.int32, device=self.dev)}
+        return hb
+
+    def _mlm_head_fwd(self, x, hb):
+        """transform (dense + GELU, LayerNorm) and the fp32 logits over the rows of hb: bias fill, then the product
+        with the word-embedding table added by the GEMM (N = vocab_pad)"""
+        H, rows, s, w = self.H, hb["rows"], self.stream(), self.w
+        KM = L.MAJOR_K
+        self.gemm(rows, H, H, x.data_ptr(), H, KM, w("cls.predictions.transform.dense.weight"), H, KM,
+                  hb["h"].data_ptr(), H, L.EPI_BIAS_GELU, bias=w("cls.predictions.transform.dense.bias"),
+                  aux_out=hb["u"].data_ptr(), ld_aux_out=H)
+        L.call("b2_layernorm_fwd", hb["h"].data_ptr(), w("cls.predictions.transform.LayerNorm.weight"),
+               w("cls.predictions.transform.LayerNorm.bias"), rows, H, float(self.cfg.layer_norm_eps),
+               hb["t"].data_ptr(), hb["mean"].data_ptr(), hb["rstd"].data_ptr(), s)
+        L.call("b2_mlm_bias_fill", w("cls.predictions.bias"), rows, self.Vp, hb["logits"].data_ptr(), s)
+        self.gemm(rows, self.Vp, H, hb["t"].data_ptr(), H, KM, w("bert.embeddings.word_embeddings.weight"), H, KM,
+                  hb["logits"].data_ptr(), self.Vp, L.EPI_ACCUM_F32,
+                  splits=1 if torch.are_deterministic_algorithms_enabled() else 0)
+
+    def mlm_capacity(self, labels, ignore_index, M):
+        """the labelled rows' capacity for host labels: their count rounded up to 128 (at least 128, at most M).
+        Raises ValueError on a label outside [0, V) that is not ignore_index."""
+        lab = labels.reshape(-1)
+        bad = (lab != ignore_index) & ((lab < 0) | (lab >= self.V))
+        n_bad, n = (int(v) for v in torch.stack([bad.sum(), (lab != ignore_index).sum()]).tolist())
+        if n_bad:
+            raise ValueError("masked-LM label %d is outside [0, %d) and is not the ignore_index %d"
+                             % (int(lab[bad][0]), self.V, ignore_index))
+        return min(M, max(128, (n + 127) // 128 * 128)), n
+
+    def _mlm_forward(self, x, M, labels, need_backward, full, ignore_index, capacity, dloss=None):
+        s, V, Vp = self.stream(), self.V, self.Vp
+        loss, logits, gb = None, None, None
+        if labels is not None:
+            if labels.dtype != torch.int64 or labels.numel() != M:
+                raise TypeError("masked-LM labels must be int64 with one per token (%d), got %s %s"
+                                % (M, labels.dtype, list(labels.shape)))
+            if capacity is None:
+                capacity, _n = self.mlm_capacity(labels, ignore_index, M)
+            gb = self._mlm_buffers(M, capacity)
+            lab = labels.contiguous()
+            L.call("b2_mlm_compact", lab.data_ptr(), M, int(ignore_index), V, capacity, gb["src"].data_ptr(),
+                   gb["slot"].data_ptr(), gb["labels"].data_ptr(), gb["count"].data_ptr(), s)
+            L.call("b2_mlm_gather_rows", x.data_ptr(), gb["src"].data_ptr(), gb["count"].data_ptr(), capacity, self.H,
+                   gb["x"].data_ptr(), s)
+            self._mlm_head_fwd(gb["x"], gb)
+            cnt = gb["count"].data_ptr()
+            dlog = None
+            if dloss is not None:
+                dlog = self._mlm_grad_buffers(gb)["dlog"]
+            L.call("b2_mlm_ce", gb["logits"].data_ptr(), capacity, V, Vp, gb["labels"].data_ptr(), cnt, cnt,
+                   L.ptr(dloss), None, 0, gb["row_loss"].data_ptr(), gb["pred"].data_ptr(), L.ptr(dlog),
+                   gb["loss"].data_ptr(), s)
+            loss = gb["loss"]
+            if dlog is not None and need_backward:
+                # d_logits are final: the captured step's backward starts from them (_backward_from_dlogits)
+                self._mlm_pending = (gb, gb["x"], gb)
+            self.mlm_last = gb
+        fb = None
+        if full:
+            fb = self._mlm_buffers(M, M, full=True)
+            self._mlm_head_fwd(x, fb)
+            logits = fb["logits"][:, :V]
+        if need_backward:
+            # (labelled-row buffers, full-row buffers, the labels and their ignore index, the encoder output)
+            self._mlm_saved = (gb, fb, labels, ignore_index, x)
+        return logits, loss
+
+    def _mlm_dlogits(self, d_logits, d_loss):
+        """the bf16 d_logits of the head's rows: over the labelled rows from the loss alone, else dense over every
+        row (the incoming fp32 d_logits plus the loss's part)"""
+        gb, fb, labels, ignore_index, x = self._mlm_saved
+        s, V, Vp = self.stream(), self.V, self.Vp
+        dl_ptr = None if d_loss is None else d_loss.to(torch.float32).contiguous()
+        if d_logits is None:
+            if gb is None:
+                raise RuntimeError("masked-LM backward without labels and without a gradient of the logits")
+            hb = self._mlm_grad_buffers(gb)
+            cnt = gb["count"].data_ptr()
+            L.call("b2_mlm_ce", gb["logits"].data_ptr(), gb["rows"], V, Vp, gb["labels"].data_ptr(), cnt, cnt,
+                   L.ptr(dl_ptr), None, 0, gb["row_loss"].data_ptr(), None, hb["dlog"].data_ptr(), None, s)
+            self._mlm_pending = (hb, gb["x"], gb)
+        else:
+            hb = self._mlm_grad_buffers(fb)
+            M = fb["rows"]
+            extra = d_logits.to(torch.float32).reshape(M, V).contiguous()
+            lab32, n_lab = None, self._mlm_shared["n_lab_one"]
+            if dl_ptr is not None and gb is not None:
+                lab = labels.reshape(-1)
+                lab32 = torch.where(lab == ignore_index, torch.full_like(lab, -1), lab).to(torch.int32)
+                n_lab = gb["count"]
+            L.call("b2_mlm_ce", fb["logits"].data_ptr(), M, V, Vp, L.ptr(lab32), None, n_lab.data_ptr(),
+                   L.ptr(dl_ptr), extra.data_ptr(), V, fb["row_loss"].data_ptr(), None, hb["dlog"].data_ptr(), None,
+                   s)
+            self._mlm_pending = (hb, x, None)
+        self._mlm_saved = None
+
+    def _mlm_backward(self, x_last, dxA, det, main, side):
+        """the head's backward from the pending d_logits: d_hidden (fp32, every row of dxA) on the main stream, the
+        head's parameter gradients and the decoder's part of the tied word gradient on the weight-gradient stream.
+        Returns the event after which that decoder part (self._mlm_shared["dec"]) is final."""
+        hb, xin, gb = self._mlm_pending
+        self._mlm_pending = None
+        H, Vp, rows = self.H, self.Vp, hb["rows"]
+        w, g = self.w, self.g
+        KM, MN = L.MAJOR_K, L.MAJOR_MN
+        sh = self._mlm_shared
+        s = main.cuda_stream
+        side_s = side if self.nl > 0 else main
+        ss = side_s.cuda_stream
+        splits = 1 if det else 0
+        # d_t = d_logits E  (N = H, K = vocab_pad); then the transform's LayerNorm and GELU backward
+        L.call("b2_zero", hb["dt"].data_ptr(), hb["dt"].numel() * 4, s)
+        self.gemm(rows, H, Vp, hb["dlog"].data_ptr(), Vp, KM, w("bert.embeddings.word_embeddings.weight"), H, MN,
+                  hb["dt"].data_ptr(), H, L.EPI_ACCUM_F32, splits=splits)
+        nparts = ctypes.c_int32()
+        L.call("b2_layernorm_bwd", hb["dt"].data_ptr(), None, hb["h"].data_ptr(), hb["mean"].data_ptr(),
+               hb["rstd"].data_ptr(), w("cls.predictions.transform.LayerNorm.weight"), rows, H, 0.0, None, 0, 1,
+               hb["dh"].data_ptr(), hb["dh_bf"].data_ptr(), g("cls.predictions.transform.LayerNorm.weight"),
+               g("cls.predictions.transform.LayerNorm.bias"), None, sh["ln_parts"].data_ptr(),
+               sh["ln_parts"].numel() * 4, ctypes.addressof(nparts), s)
+        L.call("b2_mlm_gelu_bwd", hb["dh"].data_ptr(), hb["u"].data_ptr(), rows * H, hb["du"].data_ptr(), s)
+        # fork: the parameter gradients (fixed-order column sums in both modes) and the decoder's dense part
+        ev = torch.cuda.Event()
+        ev.record(main)
+        side_s.wait_event(ev)
+        L.call("b2_zero", sh["dec"].data_ptr(), sh["dec"].numel() * 4, ss)
+        self.gemm(Vp, H, rows, hb["dlog"].data_ptr(), Vp, MN, hb["t"].data_ptr(), H, MN, sh["dec"].data_ptr(), H,
+                  L.EPI_ACCUM_F32, splits=splits, stream=ss)
+        sc, scn = sh["colsum"].data_ptr(), sh["colsum"].numel() * 4
+        L.call("b2_colsum", hb["dlog"].data_ptr(), rows, Vp, Vp, g("cls.predictions.bias"), sc, scn, ss)
+        L.call("b2_colsum_finish", sh["ln_parts"].data_ptr(), nparts.value, 3, H,
+               g("cls.predictions.transform.LayerNorm.weight"), g("cls.predictions.transform.LayerNorm.bias"), None,
+               ss)
+        self.gemm(H, H, rows, hb["du"].data_ptr(), H, MN, xin.data_ptr(), H, MN,
+                  g("cls.predictions.transform.dense.weight"), H, split=True, stream=ss)
+        L.call("b2_colsum", hb["du"].data_ptr(), rows, H, H, g("cls.predictions.transform.dense.bias"), sc, scn, ss)
+        dec_done = torch.cuda.Event()
+        dec_done.record(side_s)
+        # d_hidden = du W_t: straight into dxA over every row, or over the labelled rows and scattered
+        out = dxA if gb is None else hb["dx"]
+        L.call("b2_zero", out.data_ptr(), out.numel() * 4, s)
+        self.gemm(rows, H, H, hb["du"].data_ptr(), H, KM, w("cls.predictions.transform.dense.weight"), H, MN,
+                  out.data_ptr(), H, L.EPI_ACCUM_F32, splits=splits)
+        if gb is not None:
+            L.call("b2_mlm_scatter_rows", out.data_ptr(), gb["slot"].data_ptr(), dxA.shape[0], H, dxA.data_ptr(), s)
+        return dec_done
+
     # ---- backward ---------------------------------------------------------------------------------------------------------
     def backward(self, d_logits, d_loss=None, stream=None):
         """d_logits: fp32 [B, C] gradient wrt the returned logits; d_loss: optional scalar gradient wrt HF's loss."""
@@ -1014,6 +1324,9 @@ class _Engine:
             raise RuntimeError("backward called without a training forward")
         B, S, mask, p_h, p_a, p_c, packed = self._saved
         self._saved = None
+        if self.mlm:
+            self._mlm_dlogits(d_logits, d_loss)
+            return self._backward_from_dlogits(None, B, S, mask, p_h, p_a, p_c, packed)
         Bo = self.head_rows(B, S, packed)
         ws = self.workspace(B, S, Bo)
         dl = ws["dlogits"]
@@ -1058,7 +1371,9 @@ class _Engine:
         if self.nl > 0:
             # the side stream may still be busy with the previous step's tail; it must also not overtake this step
             side.wait_stream(main)
-        if self.token_head:
+        if self.mlm:
+            dec_done = self._mlm_backward(x_last, ws["dxA"], det, main, side)
+        elif self.token_head:
             # every row of d_hidden is written: no memset
             L.call("b2_token_head_bwd_split", dl.data_ptr(), x_last.data_ptr(), M, H, w("classifier.weight"), self.C,
                    p_c, rng, 1 + 3 * self.nl, g("classifier.weight"), g("classifier.bias"), ws["dxA"].data_ptr(),
@@ -1219,6 +1534,12 @@ class _Engine:
             L.call(emb_fn, *emb_in, *emb_tail)
         else:
             L.call(emb_fn, *emb_in, ws["pos32"].data_ptr(), *emb_tail)
+        if self.mlm:
+            # the tied decoder's dense part of the word-embedding gradient, on top of the scatter the embedding
+            # backward stored (the pad row included: padding_idx only zeroes the scatter part)
+            main.wait_event(dec_done)
+            L.call("b2_mlm_tied_add", self._mlm_shared["dec"].data_ptr(), g("bert.embeddings.word_embeddings.weight"),
+                   self.V * H, s)
         # Whoever consumes the gradients next on the main stream (optimizer.step, grad_dict) must see the weight-gradient
         # stream's work.  Where the per-bucket side stream has taken those dependencies, optimizer.step() (or
         # end_pass) joins it; in every other case join here.

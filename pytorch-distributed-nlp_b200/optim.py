@@ -215,7 +215,7 @@ class _FusedOptimizer(torch.optim.Optimizer):
         """Gradients live in the bf16 bucket space and are overwritten by every backward: nothing to clear
         (the reference's zero_grad [:172] exists only because torch accumulates into .grad).  The one real `.grad`
         is the small fp32 probe the eager backward leaves on classifier.bias for GradScaler's inf check."""
-        self._model._params_by_name["classifier.bias"].grad = None
+        self._model._params_by_name[self._model._anchor].grad = None
         return None
 
     def update_range(self, begin, end, world, rank, peer_grads, peer_shadow, stream, background=False, grad_f32=None):
@@ -409,7 +409,7 @@ class _FusedOptimizer(torch.optim.Optimizer):
         model._grads_live = False
         # the inf-check probe has served its purpose (GradScaler reads it before calling step); the -amp scripts never
         # call zero_grad, so drop it here or it would accumulate
-        model._params_by_name["classifier.bias"].grad = None
+        model._params_by_name[model._anchor].grad = None
         return loss
 
     def _views(self, flat):

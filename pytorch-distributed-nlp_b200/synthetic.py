@@ -24,6 +24,20 @@ def synthetic_batch(cfg, batch, seq, seed, padded=False, device="cpu"):
             "label": lab.to(device)}
 
 
+def synthetic_mlm_batch(cfg, batch, seq, seed, padded=False, mlm_probability=0.15):
+    """synthetic_batch's dict for BertForMaskedLM: ids with [SEP] (102) closing each row, masked by masking.mask_tokens
+    (its generator seeded from `seed`), and `label` the int64 [batch, seq] masked-LM labels (-100: not predicted)"""
+    from .masking import mask_tokens
+    b = synthetic_batch(cfg, batch, seq, seed, padded=padded)
+    ids, mask = b["input_ids"], b["attention_mask"]
+    last = mask.sum(1) - 1
+    ids[torch.arange(batch), last] = min(102, cfg.vocab_size - 1)
+    g = torch.Generator().manual_seed(seed + 1)
+    inputs, labels = mask_tokens(ids, mask, mlm_probability=mlm_probability, mask_token_id=min(103, cfg.vocab_size - 1),
+                                 vocab_size=cfg.vocab_size, generator=g)
+    return {"input_ids": inputs, "token_type_ids": b["token_type_ids"], "attention_mask": mask, "label": labels}
+
+
 # Token-length histogram of the reference's own data (data/train.json, 40 133 rows): characters of the text without the
 # segmentation blanks (BertTokenizer splits Chinese text into single characters) + [CLS] + [SEP], capped at
 # max_seq_len = 128 (multi-gpu-distributed-cls.py:66-98).  (length, rows); mean 19.8 tokens -- the reference pads all of

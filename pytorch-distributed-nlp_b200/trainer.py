@@ -83,7 +83,27 @@ def _is_token(model):
     return _unwrap(model)._layout.head == "token"
 
 
+def _is_mlm(model):
+    """a BertForMaskedLM (or a wrapper of one)"""
+    return _unwrap(model)._layout.head == "mlm"
+
+
 TOKEN_PROBLEM_TYPE = "token_classification"     # what Trainer.problem_type reports for a token model (not stored)
+MLM_PROBLEM_TYPE = "masked_lm"                  # ... and for a masked-LM model (not stored)
+
+
+def check_mlm_criterion(criterion, device_loss=False):
+    """the criteria of a masked-LM model: CrossEntropyLoss (HF's loss) or none.  device_loss: the loss is the device
+    head's over the labelled rows (captured steps, dev()), which computes the mean cross-entropy with an ignore_index
+    and nothing else: class weights, label smoothing or another reduction raise ValueError."""
+    if criterion is not None and not isinstance(criterion, torch.nn.CrossEntropyLoss):
+        raise ValueError("a BertForMaskedLM trains with CrossEntropyLoss (or no criterion: HF's in-model loss), got %s"
+                         % type(criterion).__name__)
+    if device_loss and criterion is not None and (criterion.weight is not None or criterion.label_smoothing != 0.0
+                                                  or criterion.reduction != "mean"):
+        raise ValueError("the masked-LM head on the device computes CrossEntropyLoss(reduction='mean') with an "
+                         "ignore_index only, not class weights, label smoothing or reduction=%r: set args.fused = "
+                         "False to apply this criterion to the full logits" % criterion.reduction)
 
 
 CHECKPOINT_PREFIX = "checkpoint"     # HF Trainer's PREFIX_CHECKPOINT_DIR: output_dir/checkpoint-{optimizer step}
@@ -122,6 +142,9 @@ def step_loss(model, criterion=None):
     ValueError), and with no criterion the model's problem-type loss -- single-label cross-entropy when the config has
     no problem_type and more than one label (the step then stages int64 labels, as the reference's Collate yields)."""
     m = _unwrap(model)
+    if _is_mlm(m):
+        check_mlm_criterion(criterion, device_loss=True)
+        return Loss(L.LOSS_CE, m.config.vocab_size, ignore_index=getattr(criterion, "ignore_index", -100))
     if _is_token(m):
         check_token_criterion(criterion)
         if criterion is None:
@@ -149,6 +172,11 @@ class _StagedGraphStep:
         self.loss_fn = step_loss(self.model, criterion)
         self.criterion_key = criterion_key(criterion)
         self.token = _is_token(self.model)     # labels per token row: B * S int64 slots
+        # masked-LM: the head runs on the labelled rows; the host counts them while staging, and the graphs are kept
+        # per capacity (the count rounded up to 128)
+        self.mlm = _is_mlm(self.model)
+        self.token = self.token or self.mlm
+        self._cap, self._n_lab = None, 0
         z = lambda *s: torch.zeros(*s, dtype=torch.int64, device=dev)
         self.d_ids, self.d_tt, self.d_mask = z(batch_size, seq_len), z(batch_size, seq_len), z(batch_size, seq_len)
         self.d_lab, lab_slots = self._label_buffer(batch_size * seq_len if self.token else batch_size)
@@ -184,6 +212,10 @@ class _StagedGraphStep:
         fn = self.loss_fn
         if self.token:
             self._check_token_labels(lab)
+        if self.mlm:
+            n = int((lab != fn.ignore_index).sum())
+            self._n_lab = n
+            self._cap = min(lab.numel(), max(128, (n + 127) // 128 * 128))
         if not fn.float_labels:
             if lab.is_floating_point():
                 raise TypeError("%s was built for int64 class labels, got %s: pass a criterion (or config.problem_type)"
@@ -235,6 +267,16 @@ class _StagedGraphStep:
         self._d_stage_all = torch.zeros_like(self._h_stage_all, device=self.eng.dev)
         self.h_stage, self.d_stage = self._h_stage_all[:n], self._d_stage_all[:n]
 
+    def _mlm_kw(self, train):
+        """the masked-LM forward's arguments: labelled rows only, this batch's capacity, and in training the d_loss
+        scale that makes the loss launch also write d_logits"""
+        if not self.mlm:
+            return {}
+        kw = dict(mlm_full=False, ignore_index=self.loss_fn.ignore_index, mlm_capacity=self._cap)
+        if train:
+            kw["mlm_dloss"] = self._mlm_dloss
+        return kw
+
     def _stage_lr(self):
         opt = getattr(self, "opt", None)
         if opt is not None:
@@ -285,6 +327,8 @@ class _StagedGraphStep:
         # the body's accumulation mode (STORE / ADD / FOLD / none) follows from these two, and a graph replay runs no
         # Python: one graph per combination, and the host-side flags are kept current here
         self._role = (final, opt is not None and self.eng.accum_live)
+        if self.mlm:
+            self._role += (self._cap,)
         self._run_device()
         if opt is not None:
             self.eng.accum_live = not final
@@ -333,6 +377,8 @@ class _StagedGraphStep:
         self.deterministic = torch.are_deterministic_algorithms_enabled()
         self.accum_steps = accum_steps
         self.max_grad_norm = float(max_grad_norm) if max_grad_norm else None
+        # the masked-LM loss's gradient scale (1/k under accumulation), read by the cross-entropy launch
+        self._mlm_dloss = torch.full((), 1.0 / accum_steps, dtype=torch.float32, device=self.eng.dev)
         if accum_steps > 1:
             self.eng.ensure_accum()       # outside any capture
         # a valid lr in the device slot before any stage(): run_device() on inputs written straight into d_stage
@@ -362,13 +408,14 @@ class _StagedGraphStep:
         eng._saved = None
         Bo = eng.head_rows(B, S, packed)
         ws = eng.workspace(B, S, Bo)
-        if self.accum_steps > 1:
+        if self.accum_steps > 1 and not self.mlm:
             ws["dloss_logits"].mul_(1.0 / self.accum_steps)     # what an eager loop does with loss / k
         # d(loss)/d(logits) was produced by the loss kernel: the reference's criterion(logits, label) [:169]
         if final and self.max_grad_norm is not None:
             opt._clip_arm(self.max_grad_norm)     # the backward's per-bucket launches become the reduce phase
         eng.start_pass(not final)
-        eng._backward_from_dlogits(ws["dloss_logits"], B, S, mask, p_h, p_a, p_c, packed)
+        # (masked-LM: the forward's cross-entropy launch left the labelled rows' d_logits for the backward)
+        eng._backward_from_dlogits(None if self.mlm else ws["dloss_logits"], B, S, mask, p_h, p_a, p_c, packed)
         eng.end_pass()
         if final:
             opt.step()
@@ -396,7 +443,7 @@ class FusedTrainStep(_StagedGraphStep):
     def _body(self):
         self._unstage()
         self._train_body(lambda: self.eng.forward(self.d_ids, self.d_tt, self.d_mask, self.d_lab, training=True,
-                                                  need_backward=True, loss_fn=self.loss_fn))
+                                                  need_backward=True, loss_fn=self.loss_fn, **self._mlm_kw(True)))
 
     def __call__(self, batch_data, final=True):
         """batch_data: the dict the reference Collate yields (host int64 tensors; fp32 labels for regression and
@@ -458,7 +505,8 @@ class PackedTrainStep(_StagedGraphStep):
         self._unstage()
         packed = (self.d_pos, self.d_seg, None if self.token else self.d_cls)
         self._train_body(lambda: self.eng.forward(self.d_ids, self.d_tt, None, self.d_lab, training=True,
-                                                  need_backward=True, packed=packed, loss_fn=self.loss_fn))
+                                                  need_backward=True, packed=packed, loss_fn=self.loss_fn,
+                                                  **self._mlm_kw(True)))
 
     def __call__(self, packed, label, final=True):
         """label: per sequence [batch], or for a token model pack_batch's "labels" [bins, bin_len]"""
@@ -476,18 +524,33 @@ class FusedEvalStep(_StagedGraphStep):
     def __init__(self, model, batch_size, seq_len, use_graph=True, criterion=None):
         super().__init__(model, batch_size, seq_len, use_graph, criterion)
         shape = (batch_size, seq_len) if self.token else (batch_size,)
-        self.logits_out = torch.zeros(*shape, self.model.num_labels, dtype=torch.float32, device=self.eng.dev)
+        if self.mlm:
+            self.logits_out = None    # no [B, S, V] logits: the labelled rows' (pred, label) pairs instead
+            self.pred_out = torch.zeros(batch_size * seq_len, dtype=torch.int32, device=self.eng.dev)
+            self.lab_out = torch.zeros_like(self.pred_out)
+        else:
+            self.logits_out = torch.zeros(*shape, self.model.num_labels, dtype=torch.float32, device=self.eng.dev)
 
     def _body(self):
         self._unstage()
         logits, loss = self.eng.forward(self.d_ids, self.d_tt, self.d_mask, self.d_lab, training=False,
-                                        need_backward=False, loss_fn=self.loss_fn)
-        self.logits_out.copy_(logits)
+                                        need_backward=False, loss_fn=self.loss_fn, **self._mlm_kw(False))
+        if self.mlm:
+            gb, cap = self.eng.mlm_last, self._cap
+            self.pred_out[:cap].copy_(gb["pred"])
+            self.lab_out[:cap].copy_(gb["labels"])
+        else:
+            self.logits_out.copy_(logits)
         self.loss_out.copy_(loss)
 
     def __call__(self, batch_data):
+        """(logits, labels, mean loss); a masked-LM model: (predicted ids, labels, mean loss) of the labelled tokens,
+        in token order"""
         self.stage(batch_data)
         self.run_device()
+        if self.mlm:
+            n = self._n_lab
+            return self.pred_out[:n].long(), self.lab_out[:n].long(), self.loss_out
         return self.logits_out, self.d_lab.view(self.B, self.S) if self.token else self.d_lab, self.loss_out
 
 
@@ -564,7 +627,8 @@ class Trainer:
         label = d["label"]
         # a token model with a criterion leaves the loss to it: its in-model CrossEntropyLoss() would not know the
         # criterion's ignore_index
-        model_labels = None if self.criterion is not None and _is_token(self.model) else label
+        model_labels = None if self.criterion is not None and (_is_token(self.model) or _is_mlm(self.model)) \
+            else label
         output = self.model(input_ids=d["input_ids"], token_type_ids=d["token_type_ids"],
                             attention_mask=d["attention_mask"], labels=model_labels)
         return output, label
@@ -577,6 +641,8 @@ class Trainer:
     def problem_type(self, label):
         """the model's config.problem_type; when None, HF's rule applied to `label` (stored on the config, as the
         model's first labelled forward does)"""
+        if _is_mlm(self.model):
+            return MLM_PROBLEM_TYPE
         if _is_token(self.model):
             return TOKEN_PROBLEM_TYPE      # HF's token model never reads or sets config.problem_type
         cfg = _unwrap(self.model).config
@@ -591,6 +657,9 @@ class Trainer:
             if model_loss is None:
                 raise ValueError("Trainer has no criterion and the model returned no loss")
             return model_loss
+        if _is_mlm(self.model):
+            check_mlm_criterion(self.criterion)
+            return self.criterion(logits.reshape(-1, logits.shape[-1]), label.reshape(-1))
         if _is_token(self.model):
             check_token_criterion(self.criterion)
             C = _unwrap(self.model).num_labels
@@ -662,7 +731,7 @@ class Trainer:
         if getattr(self.args, "fused", True) and getattr(self.args, "pack", False) and \
                 batch_data["input_ids"].shape[1] <= MAX_BIN and not batch_data["input_ids"].is_cuda:
             bin_len = bin_length(batch_data["attention_mask"], batch_data["input_ids"].shape[1])
-            token = _is_token(self.model)
+            token = _is_token(self.model) or _is_mlm(self.model)
             packed = pack_batch(batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"],
                                 bin_len, labels=batch_data["label"] if token else None,
                                 ignore_index=self._ignore_index())
@@ -937,6 +1006,8 @@ class Trainer:
         (single-label; a token model's over the tokens whose label is not the ignore index), subset accuracy -- every column of (logits > 0) equal to (labels >= 0.5) -- (multi-label), or
         the Pearson correlation of predictions and labels (regression)."""
         self.model.eval()
+        if _is_mlm(self.model):
+            return self._dev_mlm(dev_loader)
         correct_total = 0
         num_total = 0
         loss_total = 0.
@@ -976,10 +1047,39 @@ class Trainer:
             return loss_total, float(np.corrcoef(np.concatenate(reg_preds), np.concatenate(reg_trues))[0, 1])
         return loss_total, correct_total / num_total
 
+    def _dev_mlm(self, dev_loader):
+        """dev() of a masked-LM model: (summed rank-mean loss, masked-token accuracy), both from the labelled rows on
+        the device (BertForMaskedLM.masked_lm_eval: no [batch, seq, V] logits are built or copied)"""
+        check_mlm_criterion(self.criterion, device_loss=True)
+        m = _unwrap(self.model)
+        ignore = self._ignore_index()
+        loss_total, correct, total = 0., None, None
+        for batch_data in dev_loader:
+            if getattr(self.args, "fused", True) and not batch_data["input_ids"].is_cuda:
+                B, S = batch_data["input_ids"].shape
+                key = (id(m), B, S, MLM_PROBLEM_TYPE, criterion_key(self.criterion))
+                if key not in self._fused_eval:
+                    self._fused_eval[key] = FusedEvalStep(self.model, B, S, criterion=self.criterion)
+                pred, lab, loss = self._fused_eval[key](batch_data)
+            else:
+                d = self._to_device(batch_data)
+                loss, pred, lab = m.masked_lm_eval(d["input_ids"], d["token_type_ids"], d["attention_mask"],
+                                                   d["label"], ignore_index=ignore)
+            loss_total += self.loss_reduce(loss)
+            c = torch.stack([(pred == lab).sum(), torch.tensor(lab.numel(), device=lab.device)]).double()
+            if isinstance(self.model, DistributedDataParallel):
+                c = self.model.all_gather_rows(c.view(1, 2)).sum(0)
+            correct = c[0] if correct is None else correct + c[0]
+            total = c[1] if total is None else total + c[1]
+        return loss_total, float(correct / total)
+
     def test(self, model, test_loader, labels):
         """sklearn's classification_report over the gathered rows: of the argmax class (single-label; a token model's
         over the tokens whose label is not the ignore index) or of the
         indicator arrays (logits > 0) against (labels >= 0.5) (multi-label).  Regression raises ValueError."""
+        if _is_mlm(model):
+            raise ValueError("test() prints a classification report, which is not useful over a vocabulary: use dev() "
+                             "for the masked-token accuracy")
         self.model = model
         self.model.eval()
         preds = []
