@@ -5,7 +5,13 @@ word-embedding gradient, the vocabulary padding under every optimizer, determini
 Kernel bounds.  fp32 unit roundoff u = 2^-24, bf16 2^-8 relative.  The cross-entropy kernel's log-sum-exp over V
 columns adds V terms of at most 1 (each exp within a few u of exact), so lse is off by at most (V + 8) u relative to
 the sum, i.e. (V + 8) u absolute in the log; a row loss lse - x_y is then off by that plus u |lse|.  d_logits is one
-bf16 rounding (2^-8 |ref|) of a value whose fp32 error is a few u times the scale.
+bf16 rounding (2^-8 |ref|) of a value whose fp32 error is a few u times the scale, plus u |ref| for the one fp32 add of
+the dense form's incoming gradient (d_extra).  check_mlm_ce holds these bounds; the training step's stage test
+(test_step_stages.py) applies them to the recorded launches.  The kernels are also run at their edges: argmax ties
+(torch's first occurrence), logits spanning +-1e4 and all-equal rows, means over rows past the 1024-thread stride,
+the 1024-thread compaction chunks, the gather / scatter thread-count limits, the GELU' and bias-fill grid strides,
+and every host-side argument rule.  The in-kernel traps (a label out of range, more labelled rows than the capacity)
+are not run: the host's mlm_capacity rejects both first.
 """
 import numpy as np
 import pytest
@@ -16,6 +22,7 @@ import mlm_oracle as mlm
 from parity import TOL_GRAD_REL_QK, TOL_LOSS, assert_grads_within_tolerance, b2, tiny_config
 from pytorch_distributed_nlp_b200 import _lib as L
 from pytorch_distributed_nlp_b200.modeling import vocab_pad
+from test_gemm_reference import U, bf_bound, gelu_grad64, gelu_grad_err
 
 gpu = pytest.mark.gpu
 U32 = 2.0 ** -24
@@ -44,56 +51,144 @@ def _to_dev(batch):
     return {k: v.to(DEV) for k, v in batch.items()}
 
 
-def _ce(logits, labels, rows, V, n_rows, d_loss=None, with_dl=True):
+def _ce(logits, labels, rows, V, n_rows, d_loss=None, with_dl=True, extra=None, n_lab=None):
+    """b2_mlm_ce on poisoned outputs; labels None: the extra-only form; n_rows None: every row live; n_lab None: the
+    labelled live rows' count"""
     Vp = logits.shape[1]
     dev = logits.device
-    lab = torch.tensor(labels, dtype=torch.int32, device=dev)
-    n_rows_t = torch.tensor([n_rows], dtype=torch.int32, device=dev)
-    n_lab = torch.tensor([int(((lab >= 0) & (torch.arange(rows, device=dev) < n_rows)).sum())], dtype=torch.int32,
-                         device=dev)
+    lab = None if labels is None else torch.tensor(labels, dtype=torch.int32, device=dev)
+    n_rows_t = None if n_rows is None else torch.tensor([n_rows], dtype=torch.int32, device=dev)
+    if n_lab is None:
+        live = torch.arange(rows, device=dev) < (rows if n_rows is None else n_rows)
+        n_lab = int(((lab >= 0) & live).sum())
+    n_lab_t = torch.tensor([n_lab], dtype=torch.int32, device=dev)
     row_loss = torch.full((rows,), float("nan"), device=dev)
     pred = torch.full((rows,), -7, dtype=torch.int32, device=dev)
     dl = torch.full((rows, Vp), float("nan"), dtype=torch.bfloat16, device=dev) if with_dl else None
     loss = torch.full((), float("nan"), device=dev)
-    L.call("b2_mlm_ce", logits.data_ptr(), rows, V, Vp, lab.data_ptr(), n_rows_t.data_ptr(), n_lab.data_ptr(),
-           L.ptr(d_loss), None, 0, row_loss.data_ptr(), pred.data_ptr(), L.ptr(dl), loss.data_ptr(), _stream())
+    L.call("b2_mlm_ce", logits.data_ptr(), rows, V, Vp, L.ptr(lab), L.ptr(n_rows_t), n_lab_t.data_ptr(),
+           L.ptr(d_loss), L.ptr(extra), 0 if extra is None else extra.shape[1], row_loss.data_ptr(), pred.data_ptr(),
+           L.ptr(dl), loss.data_ptr(), _stream())
     torch.cuda.synchronize()
-    return row_loss, pred, dl, loss, int(n_lab)
+    return row_loss, pred, dl, loss, n_lab
+
+
+def _within(got, ref, bound, what):
+    err = (got.double() - ref).abs()
+    bad = ~(err <= bound)
+    if bool(bad.any()):
+        raise AssertionError("%s: %d elements over the bound, worst error / bound %.3g" % (
+            what, int(bad.sum()), float((err / bound.clamp_min(1e-300)).max())))
+
+
+def check_mlm_ce(logits, labels, V, n_lab, d_loss=1.0, extra=None, n_rows=None, row_loss=None, pred=None, dl=None,
+                 loss=None, what="mlm ce", check=_within):
+    """b2_mlm_ce's outputs against float64 from the fp32 logits [rows, vocab_pad] it read and its int labels [rows]
+    (-1: no loss term; None: the extra-only form).  n_rows: rows at or past it are capacity padding (None: every row
+    is live); n_lab: the mean's divisor; d_loss: the loss part's scale; extra: the fp32 [rows, V] added onto d_logits.
+    Bounds as in the module docstring: row loss (V + 8) u + u |lse|, twice; the mean that plus rows u max |row|;
+    d_logits one bf16 rounding of a value within 16 u d_loss / n of the exact one, plus one fp32 add of extra.  pred
+    exactly torch's argmax over the first V columns (its first occurrence), d_logits columns V..vocab_pad and the
+    padding rows exactly 0.  check: the within(got, ref, bound, what) that asserts and reports."""
+    rows, dev = logits.shape[0], logits.device
+    x = logits.double()[:, :V]
+    live_row = torch.arange(rows, device=dev) < (rows if n_rows is None else n_rows)
+    lab = torch.full((rows,), -1, dtype=torch.long, device=dev) if labels is None else labels.long()
+    live = live_row & (lab >= 0)
+    lse = torch.logsumexp(x, 1)
+    zero = torch.zeros_like(lse)
+    ref_row = torch.where(live, lse - x.gather(1, lab.clamp(min=0)[:, None])[:, 0], zero)
+    bound = torch.where(live, ((V + 8) * U32 + U32 * lse.abs()) * 2, zero)
+    if row_loss is not None:
+        check(row_loss, ref_row, bound, what + " row_loss")
+    if loss is not None:
+        ref_loss = (ref_row.sum() / n_lab).reshape(1)
+        check(loss.reshape(1), ref_loss, (bound.max() + rows * U32 * ref_row.abs().max()).reshape(1), what + " loss")
+    if pred is not None:
+        ref_pred = torch.where(live, x.argmax(1), torch.full_like(lab, -1))
+        bad = pred.long() != ref_pred
+        assert not bool(bad.any()), "%s pred: %d rows differ, first %s" % (what, int(bad.sum()),
+                                                                          bad.nonzero()[0].tolist())
+    if dl is not None:
+        got = dl.double()
+        assert bool((got[:, V:] == 0).all()), what + " d_logits: a padding column is not 0"
+        assert bool((got[~live_row] == 0).all()), what + " d_logits: a capacity padding row is not 0"
+        onehot = torch.zeros_like(x)
+        onehot[torch.arange(rows, device=dev), lab.clamp(min=0)] = 1
+        ref = torch.where(live[:, None], (torch.softmax(x, 1) - onehot) * (d_loss / n_lab), torch.zeros_like(x))
+        E = torch.where(live, zero + 16 * U32 * abs(d_loss) / n_lab, zero)[:, None]
+        if extra is not None:
+            ref = ref + torch.where(live_row[:, None], extra.double(), torch.zeros_like(x))
+            E = E + U32 * ref.abs()            # the one fp32 add of extra
+        check(got[:, :V], ref, 2.0 ** -8 * ref.abs() + E, what + " d_logits")
+
+
+def _tie_logits(rows, V, Vp, gen):
+    """integer-valued logits whose maximum 30 repeats: within one thread's float4, at one thread's next 1024-column
+    stride, across lanes of a warp, across warps, at columns 0 and V-1; then V-1 alone and 0 alone"""
+    x = torch.randint(-20, 21, (rows, Vp), generator=gen).double()
+    ties = [(4000, 4001), (4000, 5024), (8, 20), (100, 900), (100, 900, 20000), (0, V - 1), (V - 1,), (0,),
+            (1023, 1024), (V - 5, V - 2)]
+    for r in range(rows):
+        for c in ties[r % len(ties)]:
+            x[r, c] = 30
+    return x
 
 
 @gpu
-@pytest.mark.parametrize("V", [64, 21128, 30522])
-def test_ce_kernel_against_float64(V):
+@pytest.mark.parametrize("V, form", [pytest.param(64, "loss", id="64"), pytest.param(21128, "loss", id="21128"),
+                                     pytest.param(30522, "loss", id="30522"),
+                                     pytest.param(1050, "extra", id="extra-1050"),
+                                     pytest.param(1050, "extra_only", id="extra_only-1050"),
+                                     pytest.param(21128, "ties", id="ties-21128"),
+                                     pytest.param(21128, "wide", id="wide-21128"),
+                                     pytest.param(1050, "mean1025", id="mean1025-1050"),
+                                     pytest.param(1050, "mean4096", id="mean4096-1050")])
+def test_ce_kernel_against_float64(V, form):
+    """loss: the labelled-rows form (loss, row losses, argmax, d_logits, capacity padding rows).  extra: the dense
+    backward's form, labels + d_loss + extra with some rows ignored, at ld_extra = V with V % 4 = 2 (the column
+    break inside a float4); extra_only: the extra alone (labels null).  ties: integer logits whose maximum repeats
+    within a thread, across the thread stride, lanes and warps, and at columns 0 and V-1.  wide: rows spanning
+    +-1e4, and rows of all-equal logits.  mean1025 / mean4096: the mean over rows past the 1024-thread stride, and
+    its bitwise repeatability."""
     torch.manual_seed(V)
-    rows, n_rows = 300, 261            # 300 is no multiple of any block size; rows past 261 are capacity padding
+    gen = torch.Generator().manual_seed(V + len(form))
     Vp = vocab_pad(V)
-    x = torch.randn(rows, Vp, dtype=torch.float64) * 3
+    rows, n_rows = 300, 261            # 300 is no multiple of any block size; rows past 261 are capacity padding
+    if form.startswith("mean"):
+        rows = n_rows = int(form[4:])
+    if form == "ties":
+        x = _tie_logits(rows, V, Vp, gen)
+    elif form == "wide":
+        x = (torch.rand(rows, Vp, generator=gen, dtype=torch.float64) * 2 - 1) * 1e4
+        x[::3] = 5.0                   # all-equal rows
+        x[1::6] = -7.25
+    else:
+        x = torch.randn(rows, Vp, dtype=torch.float64, generator=gen) * 3
     x[:, V:] = 1e4                     # the padded columns must not be read into the softmax
-    labels = torch.randint(0, V, (rows,))
+    labels = torch.randint(0, V, (rows,), generator=gen)
     labels[::7] = -1                   # ignored rows
     lx = x.float().to(DEV)
     d_loss = torch.tensor(1.7, device=DEV)
-    row_loss, pred, dl, loss, n = _ce(lx, labels.tolist(), rows, V, n_rows, d_loss)
-    xr = lx.double().cpu()[:, :V]
-    lse = torch.logsumexp(xr, 1)
-    live = (labels >= 0) & (torch.arange(rows) < n_rows)
-    ref_row = torch.where(live, lse - xr.gather(1, labels.clamp(min=0)[:, None])[:, 0], torch.zeros(rows,
-                                                                                                   dtype=torch.float64))
-    bound = ((V + 8) * U32 + U32 * lse.abs()) * 2
-    assert torch.all((row_loss.double().cpu() - ref_row).abs() <= torch.where(live, bound, torch.zeros_like(bound)))
-    ref_loss = ref_row.sum() / n
-    assert abs(float(loss) - float(ref_loss)) <= float(bound.max()) + rows * U32 * float(ref_row.abs().max())
-    ref_pred = torch.where(live, xr.argmax(1), torch.full((rows,), -1))
-    assert torch.equal(pred.long().cpu(), ref_pred)
-    sm = torch.softmax(xr, 1)
-    onehot = torch.zeros_like(sm)
-    onehot[torch.arange(rows), labels.clamp(min=0)] = 1
-    ref_dl = torch.where(live[:, None], (sm - onehot) * 1.7 / n, torch.zeros_like(sm))
-    got = dl.double().cpu()
-    assert torch.all(got[:, V:] == 0)
-    err = (got[:, :V] - ref_dl).abs()
-    assert torch.all(err <= 2.0 ** -8 * ref_dl.abs() + 16 * U32 * 1.7 / n), float(err.max())
-    assert torch.all(got[~live] == 0)
+    extra = None
+    if form.startswith("extra"):
+        n_rows = None
+        extra = (torch.randn(rows, V, generator=gen) * 1e-3).to(DEV)
+    if form == "extra_only":
+        row_loss, pred, dl, loss, n = _ce(lx, None, rows, V, None, None, extra=extra, n_lab=1)
+        check_mlm_ce(lx, None, V, 1, extra=extra, row_loss=row_loss, pred=pred, dl=dl, what="extra only")
+        return
+    row_loss, pred, dl, loss, n = _ce(lx, labels.tolist(), rows, V, n_rows, d_loss, extra=extra)
+    check_mlm_ce(lx, labels.to(DEV), V, n, d_loss=1.7, extra=extra, n_rows=n_rows, row_loss=row_loss, pred=pred,
+                 dl=dl, loss=loss, what=form)
+    if form == "ties":
+        # every tie pattern reached a labelled row (check_mlm_ce asserted each against torch's first occurrence)
+        assert set(pred[labels.to(DEV) >= 0].tolist()) >= {4000, 8, 100, 0, V - 1, 1023, V - 5}
+    if form.startswith("mean"):
+        again = _ce(lx, labels.tolist(), rows, V, n_rows, d_loss, extra=extra)
+        for a, b in zip((row_loss, pred, dl, loss), again[:4]):
+            assert torch.equal(a.view(torch.int16) if a.dtype == torch.bfloat16 else a,
+                               b.view(torch.int16) if b.dtype == torch.bfloat16 else b)
 
 
 @gpu
@@ -107,19 +202,45 @@ def test_ce_kernel_all_ignored_is_nan_with_zero_gradient():
 
 @gpu
 def test_compaction_exact():
-    torch.manual_seed(1)
-    M, V, cap = 4096, 21128, 768
-    lab = torch.full((M,), -100, dtype=torch.int64)
-    pick = torch.rand(M) < 0.15
-    lab[pick] = torch.randint(0, V, (int(pick.sum()),))
+    """15% of 4096 tokens labelled into a capacity of 768 rows; gather and scatter at H = 256"""
+    _compaction_case((4096, 768, -100, "sparse", 256, 256), seed=1)
+
+
+# (tokens, capacity, ignore_index, labels, gather hidden, scatter hidden): the 1024-thread chunk edges with every token
+# labelled (capacity == tokens), labels 0 and V-1, ignore_index -1 and 0, and the gather / scatter thread-count limits
+COMPACT_EDGES = [(1, 1, -1, "all", 8, 4096), (1000, 1000, -1, "all", 1024, 1024), (1024, 1024, -1, "all", 8, 4096),
+                 (1025, 1025, -1, "all", 1024, 1024), (3073, 3073, -1, "all", 256, 4096),
+                 (3073, 3072, 0, "zero_ignored", 8, 1024)]
+
+
+@gpu
+@pytest.mark.parametrize("case", COMPACT_EDGES, ids=lambda c: "%d-%d-%s-%d-%d" % (c[0], c[1], c[3], c[4], c[5]))
+def test_compaction_edges(case):
+    _compaction_case(case, seed=case[0] + case[1])
+
+
+def _compaction_case(case, seed):
+    """b2_mlm_compact exactly (rows, slots, slot labels, count), then gather and scatter around it"""
+    M, cap, ignore, kind, Hg, Hs = case
+    torch.manual_seed(seed)
+    V = 21128
+    if kind == "sparse":
+        lab = torch.full((M,), -100, dtype=torch.int64)
+        pick = torch.rand(M) < 0.15
+        lab[pick] = torch.randint(0, V, (int(pick.sum()),))
+    else:
+        lab = torch.randint(0, V, (M,))
+        lab[::5] = 0
+        lab[1::5] = V - 1
+        pick = lab != ignore
     n = int(pick.sum())
-    assert n <= cap
+    assert n <= cap and (kind != "all" or n == cap)
     d = lab.to(DEV)
     rows = torch.full((cap,), -7, dtype=torch.int32, device=DEV)
     slot = torch.full((M,), -7, dtype=torch.int32, device=DEV)
     slab = torch.full((cap,), -7, dtype=torch.int32, device=DEV)
-    cnt = torch.zeros(1, dtype=torch.int32, device=DEV)
-    L.call("b2_mlm_compact", d.data_ptr(), M, -100, V, cap, rows.data_ptr(), slot.data_ptr(), slab.data_ptr(),
+    cnt = torch.full((1,), -7, dtype=torch.int32, device=DEV)
+    L.call("b2_mlm_compact", d.data_ptr(), M, ignore, V, cap, rows.data_ptr(), slot.data_ptr(), slab.data_ptr(),
            cnt.data_ptr(), _stream())
     torch.cuda.synchronize()
     idx = torch.nonzero(pick)[:, 0]
@@ -130,18 +251,83 @@ def test_compaction_exact():
     ref_slot[idx] = torch.arange(n)
     assert torch.equal(slot.long().cpu(), ref_slot)
     # gather and scatter around the compaction
-    H = 256
-    x = torch.randn(M, H, device=DEV).to(torch.bfloat16)
-    g = torch.full((cap, H), float("nan"), dtype=torch.bfloat16, device=DEV)
-    L.call("b2_mlm_gather_rows", x.data_ptr(), rows.data_ptr(), cnt.data_ptr(), cap, H, g.data_ptr(), _stream())
-    src = torch.randn(cap, H, device=DEV)
-    dx = torch.full((M, H), float("nan"), device=DEV)
-    L.call("b2_mlm_scatter_rows", src.data_ptr(), slot.data_ptr(), M, H, dx.data_ptr(), _stream())
+    x = torch.randn(M, Hg, device=DEV).to(torch.bfloat16)
+    g = torch.full((cap, Hg), float("nan"), dtype=torch.bfloat16, device=DEV)
+    L.call("b2_mlm_gather_rows", x.data_ptr(), rows.data_ptr(), cnt.data_ptr(), cap, Hg, g.data_ptr(), _stream())
+    src = torch.randn(cap, Hs, device=DEV)
+    dx = torch.full((M, Hs), float("nan"), device=DEV)
+    L.call("b2_mlm_scatter_rows", src.data_ptr(), slot.data_ptr(), M, Hs, dx.data_ptr(), _stream())
     torch.cuda.synchronize()
     assert torch.equal(g[:n], x[idx.to(DEV)]) and torch.all(g[n:] == 0)
-    ref = torch.zeros(M, H, device=DEV)
+    ref = torch.zeros(M, Hs, device=DEV)
     ref[idx.to(DEV)] = src[:n]
     assert torch.equal(dx, ref)
+
+
+GELU_BWD_STRIDE = 132 * 16 * 256 * 8      # elements per pass of b2_mlm_gelu_bwd's grid-stride loop
+
+
+@gpu
+@pytest.mark.parametrize("n", [8, 2 * GELU_BWD_STRIDE + 8 * 37])
+def test_gelu_bwd_kernel_against_float64(n):
+    """du = bf16(dg gelu'(u)) against float64: one fp32 product and one bf16 rounding of the erf GELU' the GEMM's
+    EPI_GELU_BWD uses, u over [-10, 10] with 0 and the bf16 extremes, n = 8 and past two grid strides"""
+    gen = torch.Generator().manual_seed(n)
+    u = (torch.rand(n, generator=gen) * 20 - 10).to(torch.bfloat16)
+    edges = torch.tensor([0.0, -0.0, 10.0, -10.0, 3.3895313892515355e38, -3.3895313892515355e38, 1.1754943508222875e-38,
+                          -1.1754943508222875e-38], dtype=torch.bfloat16)
+    u[:edges.numel()] = edges
+    u[-edges.numel():] = edges.flip(0)
+    dg = torch.randn(n, generator=gen) * 4
+    du = torch.full((n,), float("nan"), dtype=torch.bfloat16, device=DEV)
+    ud, dgd = u.to(DEV), dg.to(DEV)
+    L.call("b2_mlm_gelu_bwd", dgd.data_ptr(), ud.data_ptr(), n, du.data_ptr(), _stream())
+    torch.cuda.synchronize()
+    x = ud.double()
+    r = dgd.double() * gelu_grad64(x)
+    _within(du, r, bf_bound(r, dgd.double().abs() * gelu_grad_err(x) + U * r.abs()), "gelu_bwd n=%d" % n)
+
+
+@gpu
+@pytest.mark.parametrize("rows", [1, 3, 2100])
+def test_bias_fill_kernel_exact(rows):
+    """logits[r, c] = float(bias[c]) over vocab_pad = 1088 (17 x 64, 8.5 x 128) columns; 2100 rows wrap the
+    grid-stride loop"""
+    Vp = 1088
+    bias = torch.randn(Vp, device=DEV).to(torch.bfloat16)
+    logits = torch.full((rows + 1, Vp), float("nan"), device=DEV)
+    L.call("b2_mlm_bias_fill", bias.data_ptr(), rows, Vp, logits.data_ptr(), _stream())
+    torch.cuda.synchronize()
+    assert torch.equal(logits[:rows], bias.float()[None].expand(rows, Vp))
+    assert bool(torch.isnan(logits[rows]).all())      # nothing past the rows
+
+
+@gpu
+def test_entry_points_reject_bad_arguments():
+    """each argument rule of the b2_mlm_* entry points raises RuntimeError on the host, before any launch"""
+    i32, dev = torch.int32, DEV
+    lab = torch.zeros(64, dtype=torch.int64, device=dev)
+    ib = torch.zeros(256, dtype=i32, device=dev)
+    fb = torch.zeros(256 * 1088, device=dev)
+    bb = torch.zeros(256 * 64, dtype=torch.bfloat16, device=dev)
+    p, s = lambda t: t.data_ptr(), _stream()
+    bad = [("b2_mlm_compact", (p(lab), 64, -100, 1000, 65, p(ib), p(ib), p(ib), p(ib), s), "capacity"),
+           ("b2_mlm_gather_rows", (p(bb), p(ib), p(ib), 4, 12, p(bb), s), "hidden"),
+           ("b2_mlm_scatter_rows", (p(fb), p(ib), 4, 6, p(fb), s), "hidden"),
+           ("b2_mlm_bias_fill", (p(bb), 4, 1000, p(fb), s), "vocab_pad"),
+           ("b2_mlm_ce", (p(fb), 4, 1000, 1000, p(ib), None, p(ib), None, None, 0, p(fb), None, p(bb), None, s),
+            "vocab"),
+           ("b2_mlm_ce", (p(fb), 4, 1000, 1088, p(ib), None, p(ib), None, None, 0, p(fb), None, p(bb), None, s),
+            "vocab"),
+           ("b2_mlm_ce", (p(fb), 4, 1000, 1024, p(ib), None, p(ib), None, p(fb), 1000, p(fb), None, None, None, s),
+            "d_extra")]
+    torch.cuda.synchronize()
+    before = L.launch_count()
+    for name, args, msg in bad:
+        with pytest.raises(RuntimeError, match=msg):
+            L.call(name, *args)
+    torch.cuda.synchronize()
+    assert L.launch_count() == before
 
 
 def _grads_vs_oracle(cfg, B, S, seed):

@@ -6,12 +6,17 @@ Recorder.  _lib.call is replaced for one step.  Every pointer argument is mapped
 workspace tensor, a parameter span of `shadow` / `grads` (query | key | value as one span), `bias_acc`, the det
 buffers or an input tensor; a pointer it cannot map fails the test, so a launch added later cannot go unchecked.
 The recorder synchronises the device around every launch and clones what the launch may read and write before and
-after it, so the side stream's operands are the values present at the fork and its outputs are read once it is done.
+after it (the clones are done before the launch, which may run on the other stream), so the side stream's operands are
+the values present at the fork and its outputs are read once it is done.  The masked-LM backward hands its kernels
+the gradients autograd passes the model: tensor hooks on the output's loss and logits register them as step inputs.
+One pointer is mapped by exception: the int32 labels the dense masked-LM cross-entropy builds on the fly, whose
+values the recorder copies (b2_copy_async) at the launch; any other unmappable pointer still fails.
 That serialisation can hide a race between the weight-gradient stream and the main stream; the comparisons against
 unrecorded and captured steps (below) are what catch one.
 
 Poison.  Before the recorded step, every workspace tensor of the step's shape, dq_accum, dq_parts, the LayerNorm
-partials and the whole bf16 gradient space are filled with NaN (rng, owner and bias_acc keep their state).  An
+partials, the masked-LM head's buffers and decoder part (int32 buffers: -7) and the whole bf16 gradient space are
+filled with NaN (rng, owner, bias_acc and the head's column-sum scratch keep their state).  An
 element a launch should have rewritten and did not fails its check.  After the step bias_acc must be all zero again.
 
 Wiring.  Each check first asserts which buffers the launch reads and writes (layer l's QKV GEMM reads layer l-1's x2,
@@ -45,32 +50,57 @@ uses (0, 1+3l, 2+3l, 3+3l, 1+3L; seed and step read from eng.rng).  Then its out
   head and loss   test_step_kernels.check_head_fwd / check_head_bwd / check_ce, and for the token head
                   test_token_classification.check_token_head_fwd / _bwd, at site 1 + 3L; the logits gradient the head
                   backward reads equals dloss_logits (in-model loss, d_loss = 1).
+  masked-LM head  compaction (rows, slots, labels, count), gather (rows, zeros past the count), scatter (rows, zero
+                  rows) and the bias fill (every row = the fp32 bias over vocab_pad columns) exactly; the transform
+                  GEMM as BIAS_GELU, its LayerNorm by ln_fwd_check on the bf16 h; the projection, d_t, decoder and
+                  d_x GEMMs as ACCUM_F32 onto the bias-filled logits or the zero b2_zero left (asserted); b2_mlm_ce
+                  by test_masked_lm.check_mlm_ce (pred exact, d_logits columns V..vocab_pad and the capacity padding
+                  rows exactly 0; the backward's row losses bitwise the forward's; the dense form's labels exactly
+                  the step's with ignore_index -> -1, its incoming d_logits bitwise R); the head's LayerNorm backward
+                  by ln_bwd_ref, dh_bf == bf16(dh), its partials through b2_colsum_finish (third target null);
+                  b2_mlm_gelu_bwd at bf_bound(r, |dg| gelu_grad_err(u) + U |r|); the two bias column sums at
+                  gamma(rows), the decoder bias's padding exactly 0; the split dW_t as a weight gradient; the tied
+                  add bitwise bf16(pre + dec) over V H, pre the embedding backward's output, rows V..vocab_pad 0 and
+                  the pad row bf16(dec[0]).  Streams: the decoder part, dW_t and the column sums on the
+                  weight-gradient stream, the rest on the main one.
 Every bound above is computed by the helper named, which takes this file's check as its check= callback.
 
-Coverage ledger.  Every element of the flat gradient space is claimed by exactly one check (round-8 padding: zero in
-the embedding bucket, untouched NaN elsewhere), and every (launch, workspace tensor) the launch changed by exactly
-one check; both are asserted after the step.  expected_grad_claims() builds the ledger from _Layout alone.
+Coverage ledger.  Every element of the flat gradient space is claimed by exactly one check (padding: zero in the
+embedding bucket and in cls.predictions.bias's vocab_pad - V entries, untouched NaN elsewhere; the masked-LM word
+table by the tied add, its embedding-backward value by check_embed_grads), and every (launch, workspace tensor) the
+launch changed by exactly one check; both are asserted after the step.  expected_grad_claims() builds the ledger
+from _Layout alone.
 
 Race sensitivity.  The same step on a model loaded from the same state, with the same warm-up, poison and
 seed_dropout(seed, step), runs again without the recorder.  In det mode its activations, gradient space and
 embedding-backward input must be bitwise the recorded step's, and so must the gradient space after one replay of the
 captured step (FusedTrainStep, or PackedTrainStep for packed bins), built on another such model with AdamW at lr 0
 and replayed at the same dropout key (its backward starts from dloss_logits directly, the eager one from
-0 + dloss_logits * 1: equal up to the sign of a zero, so gradients are compared by value).  With atomics on, the
-backward's sums have no fixed order, so only the forward's activations are compared bitwise (the loss, a mean over
-blocks, is left out).
+0 + dloss_logits * 1: equal up to the sign of a zero, so gradients are compared by value; the captured masked-LM step
+computes d_logits in the forward's cross-entropy launch, the eager one in the backward's).  mlm_dense skips the
+captured comparison: the captured step's objective is the loss alone.  With atomics on, the backward's sums have no
+fixed order, so only the forward's activations are compared bitwise (the loss, a mean over blocks, is left out).
+A split-K vocabulary projection would make the logits and what is read from them non-bitwise; at these shapes the
+automatic configuration did not split it, and the masked-LM forward buffers, logits included, compared bitwise.
 
 Planted defects.  On a recorded step the reference side is altered on the host and the named check must fail: layer
 l's weight gradients from layer l+2's operands, dropout at the neighbouring sublayer's site and at the previous step,
 the bf16 residual in place of x1f on the fused path, one gradient element and one workspace row restored to the
-previous step's values, the QKV bias gradient summed over one bin fewer.
+previous step's values, the QKV bias gradient summed over one bin fewer; the tied add against the warm-up step's
+decoder part, one gathered row restored to the warm-up step's, the cross-entropy reference on the neighbouring
+slot's label.
 
 Configurations, each with torch.use_deterministic_algorithms off and on: tiny (H 256, 3 layers, B 8 x 128, one
 sequence of padding only; unfused LayerNorm), hidden768 (4 layers, B 32 x 128, dropout on and off; the cluster
 LayerNorm, two parity reuses), large (H 1024, 3 layers, 16 heads, B 8), seq512 (padded B 4 x 512: dq_accum, b2_colsum,
 segment seg0 + 1, the ordered dQ), packed128 and packed512 (pack_batch bins; packed attention, embedding, cls rows),
 token128 and token512packed (BertForTokenClassification, 9 labels, padded B 16 x 128 and 512-token bins:
-b2_token_head_fwd / _bwd_split, the per-token loss with ignored rows).
+b2_token_head_fwd / _bwd_split, the per-token loss with ignored rows); BertForMaskedLM: mlm128 (V 21128, vocab_pad
+21184 = 165.5 x 128, 2 layers, padded B 16 x 128 with dropout; the labelled count is no multiple of 128, so the
+capacity has padding rows), mlm512packed (the same model, 8 sequences of up to 512 tokens in 512-token bins) and
+mlm_dense (H 256, V 1050: vocab_pad 1088 = 17 x 64, V % 4 = 2; B 8 x 128 with one sequence of padding only, every real
+token labelled, 768 = capacity; objective loss + (logits R).sum(), so the dense cross-entropy runs with labels,
+d_loss and d_logits, and the head's backward writes dxA over every row).
 
 Measured on an H100 80GB HBM3 (700 W power limit): worst error / bound per stage family and configuration, the larger
 of the two modes ("-": the configuration has no such stage).  Columns: tiny, hidden768, hidden768 without dropout,
@@ -115,13 +145,37 @@ large, seq512, packed128, packed512, token128, token512packed.
   token dW / db    -      -      -      -      -      -      -      0.97   0.98
   loss             0.028  0.026  0.027  0.0096 0.019  0.0043 0.028  0.017  0.0078
   dloss_logits     0.15   0.18   0.19   0.20   0.13   0.32   0.24   0.37   0.30
+The masked-LM head, same card and runs (columns mlm128, mlm512packed, mlm_dense; lab / full: the larger of the
+labelled-row and every-row launches):
+                   m128   m512p  mdense
+  transform u      0.80   0.81   0.94
+  transform h      0.97   0.97   0.97
+  LN fwd y         0.996  0.996  0.996
+  LN fwd mean      0.040  0.044  0.022
+  LN fwd rstd      0.073  0.076  0.12
+  logits           0.0021 0.0019 0.0027
+  ce row_loss      4e-4   5e-4   0.0057
+  ce loss          2e-5   4e-4   2e-4
+  ce d_logits      0.58   0.52   0.996
+  d_t              0.0092 0.0091 0.0012
+  LN bwd dh        0.13   0.14   0.22
+  LN bwd sums      0.98   0.95   0.91
+  gelu bwd         0.99   0.99   0.99
+  decoder dE       0.032  0.050  0.0012
+  bias colsum      0.99   0.99   0.77   (decoder bias; the transform bias 0.91 / 0.88 / 0.74)
+  dW_t             0.96   0.92   0.66
+  d_x              0.0020 0.0020 0.0037
+Compaction, gather, scatter, bias fill, pred and the tied add matched exactly everywhere.
 Keep bits and accum_finish matched bitwise everywhere; every row with no visible key kept lse < -1e38.  The bf16
 stores reach 0.99 because the half-ulp rounding itself dominates their bound.  Every det step was bitwise the
 unrecorded one, and its gradient space bitwise (by value) the captured step's after one replay.  Every atomic-mode
 forward was bitwise the unrecorded one.  Every planted defect failed its named check.  No check needed a new slack,
 and no library defect showed.
 Runtime, from one `pytest -m gpu tests/test_step_stages.py --durations=0` on that card: 25 tests in 76 s as pytest
-counts it.  The first test takes 28 s, mostly CUDA start-up; token512packed takes 7 s; the others take 0.1-4 s.
+counts it.  The first test takes 28 s, mostly CUDA start-up; token512packed takes 7 s; the others take 0.1-4 s.  The
+masked-LM cases and defects add 9 tests and about 10 s of calls (mlm512packed 2.8 / 1.5 s, mlm128 1.7 / 1.3 s,
+mlm_dense 0.3 / 0.3 s atomic / det, the three defects 1 s together, measured with tests/test_masked_lm.py in the same
+run).
 Every check reports to parity.report under tag "step_stages".
 """
 import ctypes
@@ -139,8 +193,10 @@ from pytorch_distributed_nlp_b200.packing import pack_batch
 from test_attention_reference import check_outputs
 from test_determinism import _bits
 from test_gemm_ln_reference import stats_bound
+from mlm_oracle import mlm_state_from_hf_init
 from test_gemm_reference import (C_ACC, U, bf_bound, drop_scale, gamma, gelu64, gelu_err, gelu_grad64,
                                  gelu_grad_err)
+from test_masked_lm import check_mlm_ce
 from test_packing import short_batch
 from test_packing_long import long_batch
 from test_step_kernels import check_ce, check_embed_grads, check_head_bwd, check_head_fwd, ln_bwd_ref, ln_fwd_check
@@ -154,6 +210,8 @@ SPLITS = 8                  # most split-K slices the GEMM's automatic configura
 SEED = 20261017
 POISON64 = 0x5A5A5A5A5A5A5A5A   # int64 poison: neither all-keep nor all-drop bits
 SCRATCH = ("head_scratch", "dq_accum", "dq_parts", "det_side", "split_ws", "partials")
+WORD = "bert.embeddings.word_embeddings.weight"
+MLM_BACKWARD = ("dlog", "dt", "dh", "dh_bf", "du", "dx")     # the masked-LM head buffers its backward writes
 
 
 def f32eq(a, b):
@@ -181,7 +239,7 @@ def param_spans(lay):
 def family(name):
     if name.startswith("bert.embeddings."):
         return "embedding backward"
-    if name.startswith(("bert.pooler.", "classifier.")):
+    if name.startswith(("bert.pooler.", "classifier.", "cls.")):
         return "head backward"
     if name.endswith(".weight") and "LayerNorm" not in name:
         return "weight gradient"
@@ -202,6 +260,30 @@ def expected_grad_claims(lay):
     if pos < lay.total:
         claims.append((pos, lay.total, "padding"))
     return claims
+
+
+def zero_padding(lay, b, e):
+    """whether the padding [b, e) of the gradient space reads exactly 0 after a step: the embedding bucket's (its
+    b2_zero clears the whole bucket, the word table's vocab_pad - V masked-LM rows included) and the masked-LM
+    cls.predictions.bias's entries V..vocab_pad (b2_colsum writes them; the optimizers rely on a zero gradient there).
+    Any other padding is never written."""
+    if e <= lay.buckets[0][1]:
+        return True
+    if lay.head == "mlm":
+        ob, (V,) = lay.entries["cls.predictions.bias"]
+        return (b, e) == (ob + V, ob + lay.vocab_pad)
+    return False
+
+
+def reserved_spans(lay):
+    """param_spans with the masked-LM word table and cls.predictions.bias at their vocab_pad reserve: the span the
+    vocabulary GEMMs and b2_colsum address"""
+    spans = param_spans(lay)
+    if lay.head == "mlm":
+        H = lay.entries[WORD][1][1]
+        for name, n in ((WORD, lay.vocab_pad * H), ("cls.predictions.bias", lay.vocab_pad)):
+            spans[name] = (spans[name][0], n)
+    return spans
 
 
 def assert_tiles(claims, total):
@@ -226,6 +308,9 @@ class Regions:
             b = t.data_ptr()
             self.items.append((b, b + t.numel() * t.element_size(), name, t, kind))
 
+    def covers(self, addr):
+        return any(it[0] <= addr < it[1] for it in self.items)
+
     def find(self, addr):
         hits = [it for it in self.items if it[0] <= addr < it[1]]
         if not hits:
@@ -235,10 +320,11 @@ class Regions:
         return name, (addr - b) // t.element_size()
 
 
-@pytest.mark.parametrize("head", ["sequence", "token"])
+@pytest.mark.parametrize("head", ["sequence", "token", "mlm"])
 @pytest.mark.parametrize("layers", [0, 1, 3])
 def test_ledger_tiles_the_gradient_space(head, layers):
-    lay = _Layout(tiny_config(num_hidden_layers=layers, type_vocab_size=3), head=head)
+    V = 1050 if head == "mlm" else 512                  # vocab_pad 1088: padding in the word table and the bias
+    lay = _Layout(tiny_config(num_hidden_layers=layers, type_vocab_size=3, vocab_size=V), head=head)
     claims = expected_grad_claims(lay)
     assert_tiles(claims, lay.total)
     spans = param_spans(lay)
@@ -248,6 +334,17 @@ def test_ledger_tiles_the_gradient_space(head, layers):
     if layers:
         want |= {"weight gradient", "LayerNorm column sums", "bias column sums"}
     assert fams == want
+    zero = [(b, e) for b, e, f in claims if f == "padding" and zero_padding(lay, b, e)]
+    eb, ee, _ = lay.buckets[0]
+    if head == "mlm":
+        ow, ob, H = lay.off(WORD), lay.off("cls.predictions.bias"), 256
+        assert lay.vocab_pad == 1088
+        assert (ow + V * H, ow + 1088 * H) in zero and (ob + V, ob + 1088) in zero
+        assert [z for z in zero if z[1] > ee] == [(ob + V, ob + 1088)]
+        spans = reserved_spans(lay)
+        assert spans[WORD] == (ow, 1088 * H) and spans["cls.predictions.bias"] == (ob, 1088)
+    else:
+        assert all(e <= ee for _b, e in zero)
     with pytest.raises(AssertionError, match="twice"):
         assert_tiles(claims + [claims[1]], lay.total)
     with pytest.raises(AssertionError, match="by no check"):
@@ -280,6 +377,7 @@ class Launch:
         self.pre, self.post = {}, {}
         self.g = None           # GemmArgs fields
         self.n_out = None
+        self.labels = None      # the dense masked-LM cross-entropy's on-the-fly int32 labels, copied at the launch
 
 
 _GEMM_PTRS = ("A", "B", "D", "bias", "aux_in", "aux_out", "colsum_out", "rng_state", "workspace")
@@ -337,6 +435,13 @@ class Recorder:
                 if name == "b2_layernorm_bwd" and i == 19:
                     ln.n_out = a            # host address of the partial-row count
                     continue
+                if name == "b2_mlm_ce" and i == 4 and args[8] is not None and a and not self.reg.covers(a):
+                    # the one pointer no tensor of the step owns: the int32 labels the dense form builds on the fly
+                    ln.labels = torch.empty(args[1], dtype=torch.int32, device=self.eng.dev)
+                    self.orig("b2_copy_async", ln.labels.data_ptr(), a, 4 * args[1],
+                              torch.cuda.current_stream().cuda_stream)
+                    torch.cuda.synchronize()
+                    continue
                 self.map(ln, i, a)
             elif t is not ctypes.c_void_p and not isinstance(a, (int, float)):
                 raise AssertionError("%s argument %d: %r is not recorded" % (name, i, a))
@@ -354,6 +459,8 @@ class Recorder:
         lns = self.describe(name, args)
         for ln in lns:
             ln.pre = self.snap(ln)
+        # the clones run on the current stream: they must be done before a launch on the weight-gradient stream
+        torch.cuda.synchronize()
         self.orig(name, *args)
         torch.cuda.synchronize()
         for ln in lns:
@@ -363,9 +470,31 @@ class Recorder:
         self.launches.extend(lns)
 
 
+def mlm_bufs(eng):
+    """name -> tensor: the masked-LM head's buffers ('mlm.lab.*' over the labelled rows' capacity, 'mlm.full.*' over
+    every row, 'mlm.dec' the decoder part of the tied word gradient); none for the other heads"""
+    out = {}
+    if not eng.mlm:
+        return out
+    kinds = [full for (_M, _rows, full) in eng._mlm_ws]
+    assert len(kinds) == len(set(kinds)), "one masked-LM buffer set of each kind"
+    for (_M, _rows, full), hb in eng._mlm_ws.items():
+        for k, t in hb.items():
+            if isinstance(t, torch.Tensor):
+                out["mlm.%s.%s" % ("full" if full else "lab", k)] = t
+    if eng._mlm_shared is not None:
+        out["mlm.dec"] = eng._mlm_shared["dec"]
+    return out
+
+
+def step_bufs(eng, ws):
+    """the step's activations: the workspace and the masked-LM head's buffers"""
+    return {**flat_ws(ws), **mlm_bufs(eng)}
+
+
 def register_step(rec, eng, ws, inputs):
     lay = eng.lay
-    for name, (b, n) in param_spans(lay).items():
+    for name, (b, n) in reserved_spans(lay).items():
         rec.register("g:" + name, eng.grads[b:b + n], "grad")
         rec.register("w:" + name, eng.shadow[b:b + n], "w")
     for k, v in ws.items():
@@ -384,6 +513,13 @@ def register_step(rec, eng, ws, inputs):
         for i in range(2):
             for j in range(2):
                 rec.register("ln_parts.%d.%d" % (i, j), parts[i][j], "ws")
+    for k, t in mlm_bufs(eng).items():
+        rec.register(k, t, "ws")
+    if eng.mlm:
+        sh = eng._mlm_shared
+        rec.register("mlm.colsum", sh["colsum"], "scratch")
+        rec.register("mlm.ln_parts", sh["ln_parts"], "scratch")
+        rec.register("mlm.n_lab_one", sh["n_lab_one"], "state")
     rec.register("bias_acc", eng.bias_acc, "acc")
     for k in ("rng", "owner", "bias_segs"):
         rec.register(k, getattr(eng, k), "state")
@@ -406,6 +542,8 @@ def poison(eng, ws):
         side, parts = eng._det_bufs
         for t in [side] + [p for pp in parts for p in pp]:
             t.view(f32).fill_(float("nan"))
+    for t in mlm_bufs(eng).values():
+        t.fill_(float("nan") if t.is_floating_point() else -7)
     eng.grads.fill_(float("nan"))
 
 
@@ -439,6 +577,7 @@ class Checker:
         self.worst = {}
         self.att_fwd = {}
         self.ln_parts = {}
+        self.V, self.Vp = self.cfg.vocab_size, self.lay.vocab_pad
 
     # ---- reporting -----------------------------------------------------------------------------------------------
     def within(self, got, ref, bound, what):
@@ -626,6 +765,8 @@ class Checker:
         self.c_b2_embed_fwd(ln, packed=True)
 
     def c_b2_gemm_bf16(self, ln):
+        if self.is_mlm(ln):
+            return self.mlm_gemm(ln)
         g = ln.g
         l = self.layer_of(ln)
         H, I = self.H, self.I
@@ -745,6 +886,8 @@ class Checker:
         self.claim_ws(ln, *[self.region(ln, k) for k in ("D", 4, 6, 8, 9)])
 
     def c_b2_layernorm_fwd(self, ln):
+        if self.is_mlm(ln):
+            return self.mlm_ln_fwd(ln)
         l = self.layer_of(ln)
         first = self.region(ln, 0) == "layers.%d.z1" % l
         tag = "1" if first else "2"
@@ -870,9 +1013,13 @@ class Checker:
         return l, tag, sub, (dy, xh, ex, dxd)
 
     def sums_check(self, got, terms, depth, what, bf_out, offset=None):
+        """the column sums got[k] of d_gamma, d_beta and (when dxd is given) d_bias"""
         dy, xh, ex, dxd = terms
         dy = dy.double()
-        parts = [(dy * xh, (dy.abs() * ex).sum(0) + 3 * U * (dy * xh).abs().sum(0)), (dy, 0.0), (dxd.double(), 0.0)]
+        parts = [(dy * xh, (dy.abs() * ex).sum(0) + 3 * U * (dy * xh).abs().sum(0)), (dy, 0.0)]
+        if dxd is not None:
+            parts.append((dxd.double(), 0.0))
+        assert len(got) == len(parts)
         for k, (t, extra) in enumerate(parts):
             off = offset[k] if offset is not None else 0.0
             ref = t.sum(0) + off
@@ -894,6 +1041,8 @@ class Checker:
                         offset=pre.double())
 
     def c_b2_layernorm_bwd(self, ln):
+        if self.is_mlm(ln):
+            return self.mlm_ln_bwd(ln)
         assert self.det, "the partial-row LayerNorm backward belongs to the det branch"
         l, tag, sub, terms = self.ln_bwd(ln, 0, 2, 3, 4, 5, 10, 12, 13)
         st = l & 1
@@ -901,6 +1050,8 @@ class Checker:
         self.ln_parts[(l, tag)] = (terms, ln.n_out)
 
     def c_b2_colsum_finish(self, ln):
+        if self.is_mlm(ln):
+            return self.mlm_colsum_finish(ln)
         a = ln.args
         reg = self.region(ln, 0)
         st, which = int(reg.split(".")[1]), int(reg.split(".")[2])
@@ -918,6 +1069,8 @@ class Checker:
             self.claim_grad(self.pname(l, nm))
 
     def c_b2_colsum(self, ln):
+        if self.is_mlm(ln):
+            return self.mlm_colsum(ln)
         a = ln.args
         l = self.layer_of(ln)
         st = l & 1
@@ -1005,8 +1158,20 @@ class Checker:
         self.claim_ws(ln, "loss", "dloss_logits")
 
     def c_b2_zero(self, ln):
+        reg = self.region(ln, 0)
+        if reg != "g:" + WORD:
+            # the masked-LM head's fp32 GEMM targets: d_t, the decoder part, d_hidden (labelled rows, or dxA dense)
+            assert self.eng.mlm and reg in ("mlm.lab.dt", "mlm.full.dt", "mlm.dec", "mlm.lab.dx", "dxA"), \
+                "%s: b2_zero of %s" % (self.case, reg)
+            t = self.rec.kind[reg][0]
+            assert ln.ptrs[0][1] == 0 and ln.args[1] == t.numel() * t.element_size(), "%s: b2_zero covers part of %s" % (
+                self.case, reg)
+            self.on(ln, 2, reg == "mlm.dec", "b2_zero " + reg)
+            self.same(ln.post[reg], torch.zeros_like(ln.post[reg]), "b2_zero " + reg)
+            self.claim_ws(ln, reg)
+            return
         eb, ee, _ = self.lay.buckets[0]
-        self.expect(ln, 0, "g:bert.embeddings.word_embeddings.weight", "embedding bucket clear")
+        self.expect(ln, 0, "g:" + WORD, "embedding bucket clear")
         assert ln.args[1] == 2 * (ee - eb)
 
     def dlogits(self, ln):
@@ -1066,6 +1231,287 @@ class Checker:
         self.claim_grad("classifier.bias")
         self.claim_ws(ln, "dxA")
 
+    # ---- masked-LM head ----------------------------------------------------------------------------------------------
+    def is_mlm(self, ln):
+        return any(reg.startswith(("mlm.", "w:cls.", "g:cls.")) for reg, _o in ln.ptrs.values())
+
+    def mlm_kind(self, *regs):
+        """'lab' (the labelled rows' capacity) or 'full' (every row): the head buffer set a launch addresses"""
+        kinds = {r.split(".")[1] for r in regs if r is not None and r.startswith(("mlm.lab.", "mlm.full."))}
+        assert len(kinds) == 1, "%s: head buffers %s" % (self.case, regs)
+        return kinds.pop()
+
+    def mlm_rows(self, kind):
+        return self.info["cap"] if kind == "lab" else self.M
+
+    def mlm_labels(self):
+        """the step's labels [M] and the labelled token indices in token order"""
+        lab = self.info["inputs"]["labels"].reshape(-1)
+        return lab, torch.nonzero(lab != -100)[:, 0]
+
+    def on(self, ln, i, side, what):
+        """the launch's stream argument: the weight-gradient stream (side) or the main stream"""
+        want = self.eng.wgrad_stream if side and self.nl > 0 else torch.cuda.current_stream(self.dev)
+        assert ln.args[i] == want.cuda_stream, "%s %s: not on the %s stream" % (
+            self.case, what, "weight-gradient" if side else "main")
+
+    def c_b2_mlm_compact(self, ln):
+        a = ln.args
+        names = ("src", "slot", "labels", "count")
+        self.expect(ln, 0, "in:labels", "mlm compact")
+        for i, k in enumerate(names):
+            self.expect(ln, 5 + i, "mlm.lab." + k, "mlm compact")
+        cap, M = a[4], self.M
+        assert (a[1], a[2], a[3], cap) == (M, -100, self.V, self.info["cap"])
+        self.on(ln, 9, False, "mlm compact")
+        lab, idx = self.mlm_labels()
+        n = idx.numel()
+        post = lambda k: ln.post["mlm.lab." + k]
+        i32 = dict(dtype=torch.int32, device=self.dev)
+        self.same(post("count"), torch.tensor([n], **i32), "mlm compact count")
+        rows = torch.zeros(cap, **i32)
+        rows[:n] = idx.int()
+        self.same(post("src"), rows, "mlm compact rows")
+        slab = torch.full((cap,), -1, **i32)
+        slab[:n] = lab[idx].int()
+        self.same(post("labels"), slab, "mlm compact labels")
+        slot = torch.full((M,), -1, **i32)
+        slot[idx] = torch.arange(n, **i32)
+        self.same(post("slot"), slot, "mlm compact slots")
+        self.claim_ws(ln, *["mlm.lab." + k for k in names])
+
+    def c_b2_mlm_gather_rows(self, ln):
+        a = ln.args
+        for k, v in {0: self.x_in(self.nl), 1: "mlm.lab.src", 2: "mlm.lab.count", 5: "mlm.lab.x"}.items():
+            self.expect(ln, k, v, "mlm gather")
+        H, cap = self.H, self.info["cap"]
+        assert a[3] == cap and a[4] == H
+        self.on(ln, 6, False, "mlm gather")
+        _lab, idx = self.mlm_labels()
+        ref = torch.zeros(cap, H, dtype=bf, device=self.dev)
+        ref[:idx.numel()] = self.mat(ln, 0, self.M, H, H)[idx]
+        self.same(ln.post["mlm.lab.x"], ref, "mlm gather")
+        self.claim_ws(ln, "mlm.lab.x")
+
+    def mlm_gemm(self, ln):
+        g = ln.g
+        A, Bw, D = self.region(ln, "A"), self.region(ln, "B"), self.region(ln, "D")
+        kind = self.mlm_kind(A, Bw, D)
+        hb, rows, H, Vp = "mlm.%s." % kind, self.mlm_rows(kind), self.H, self.Vp
+        x_in = self.x_in(self.nl) if kind == "full" else hb + "x"
+        tw = "w:cls.predictions.transform.dense.weight"
+        epi, side = g["epilogue"], False
+        if epi == L.EPI_BIAS_GELU:                                              # transform dense + GELU
+            want = (x_in, tw, hb + "h", rows, H, H)
+            self.expect(ln, "aux_out", hb + "u", "mlm transform")
+            self.expect(ln, "bias", "w:cls.predictions.transform.dense.bias", "mlm transform")
+            what = "mlm %s u, h" % kind
+        elif D == hb + "logits":                                                # onto the bias-filled logits
+            want = (hb + "t", "w:" + WORD, D, rows, Vp, H)
+            what = "mlm %s logits" % kind
+        elif D == hb + "dt":                                                    # d_t = d_logits E, K = vocab_pad
+            want = (hb + "dlog", "w:" + WORD, D, rows, H, Vp)
+            what = "mlm d_t"
+        elif D == "mlm.dec":                                                    # dE = d_logits^T t, M = vocab_pad
+            want, side = (hb + "dlog", hb + "t", D, Vp, H, rows), True
+            what = "mlm decoder dE"
+        elif D == "g:cls.predictions.transform.dense.weight":                   # split weight gradient
+            want, side = (hb + "du", x_in, D, H, H, rows), True
+            assert epi == L.EPI_NONE and g["workspace"], "mlm dW_t: the split weight-gradient form"
+            what = "mlm weight grads"
+        else:                                                                   # d_hidden = du W_t
+            want = (hb + "du", tw, "dxA" if kind == "full" else hb + "dx", rows, H, H)
+            what = "mlm d_x"
+        got = (A, Bw, D, g["M"], g["N"], g["K"])
+        assert got == want, "%s %s: operands %s, expected %s" % (self.case, what, got, want)
+        self.on(ln, 1, side, what)
+        if epi == L.EPI_ACCUM_F32:
+            if self.det:
+                assert g["force_splits"] == 1, "det: the head's GEMMs run unsplit"
+            if what != "mlm %s logits" % kind:
+                prior = self.mat(ln, "D", g["M"], g["N"], g["ldd"])
+                self.same(prior, torch.zeros_like(prior), what + " adds onto zero")
+        self.check_gemm(ln, what)
+        if D.startswith("g:"):
+            self.claim_grad(D[2:])
+        else:
+            self.claim_ws(ln, D, self.region(ln, "aux_out"))
+
+    def mlm_ln_fwd(self, ln):
+        a = ln.args
+        kind = self.mlm_kind(self.region(ln, 0))
+        hb, rows, H = "mlm.%s." % kind, self.mlm_rows(kind), self.H
+        w = "w:cls.predictions.transform.LayerNorm."
+        for k, v in {0: hb + "h", 1: w + "weight", 2: w + "bias", 6: hb + "t", 7: hb + "mean", 8: hb + "rstd"}.items():
+            self.expect(ln, k, v, "mlm LN fwd")
+        assert a[3] == rows and a[4] == H
+        self.on(ln, 9, False, "mlm LN fwd")
+        ln_fwd_check(self.mat(ln, 0, rows, H, H).double(), self.vec(ln, 7, rows, "post"), self.vec(ln, 8, rows, "post"),
+                     self.mat(ln, 6, rows, H, H, "post"), self.vec(ln, 1, H), self.vec(ln, 2, H), "mlm %s LN" % kind,
+                     check=self.within)
+        self.claim_ws(ln, hb + "t", hb + "mean", hb + "rstd")
+
+    def c_b2_mlm_bias_fill(self, ln):
+        a = ln.args
+        kind = self.mlm_kind(self.region(ln, 3))
+        hb, rows, Vp = "mlm.%s." % kind, self.mlm_rows(kind), self.Vp
+        self.expect(ln, 0, "w:cls.predictions.bias", "mlm bias fill")
+        self.expect(ln, 3, hb + "logits", "mlm bias fill")
+        assert a[1] == rows and a[2] == Vp and ln.post[hb + "logits"].shape == (rows, Vp)
+        self.on(ln, 4, False, "mlm bias fill")
+        bias = self.vec(ln, 0, Vp).float()
+        self.same(ln.post[hb + "logits"], bias[None].expand(rows, Vp), "mlm %s bias fill" % kind)
+        self.claim_ws(ln, hb + "logits")
+
+    def c_b2_mlm_ce(self, ln):
+        a = ln.args
+        kind = self.mlm_kind(self.region(ln, 0))
+        hb, rows, V, Vp = "mlm.%s." % kind, self.mlm_rows(kind), self.V, self.Vp
+        assert (a[1], a[2], a[3]) == (rows, V, Vp)
+        self.on(ln, 14, False, "mlm ce")
+        lab, idx = self.mlm_labels()
+        n = idx.numel()
+        fwd = a[13] is not None
+        want = {0: hb + "logits", 10: hb + "row_loss"}
+        extra, n_rows = None, None
+        if kind == "lab":
+            want.update({4: hb + "labels", 5: hb + "count", 6: hb + "count"})
+            if fwd:             # the eager forward: loss, row losses and argmax, no d_logits
+                want.update({11: hb + "pred", 13: hb + "loss"})
+                assert a[7] is None and a[12] is None
+            else:               # the backward from the loss: d_logits, the row losses again
+                want.update({7: "in:d_loss", 12: hb + "dlog"})
+                assert a[11] is None
+            assert a[8] is None
+            labels, n_rows = self.vec(ln, 4, rows), n
+        else:                   # the dense form: every row, the incoming d_logits, the loss's part
+            assert not fwd and a[5] is None and a[11] is None and a[9] == V and ln.labels is not None
+            want.update({6: "mlm.lab.count", 7: "in:d_loss", 8: "in:d_logits", 12: hb + "dlog"})
+            self.same(ln.labels, torch.where(lab == -100, torch.full_like(lab, -1), lab).int(), "mlm dense labels")
+            extra = self.mat(ln, 8, rows, V, V)
+            self.same(extra, self.info["R"].view(rows, V), "mlm incoming d_logits == R")
+            labels = ln.labels
+        for k, v in want.items():
+            self.expect(ln, k, v, "mlm %s ce" % kind)
+        if self.defect == "neighbour_label":
+            labels = labels.roll(1)
+        d_loss = float(self.vec(ln, 7, 1)) if 7 in want else 1.0
+        post = lambda k: ln.post[hb + k] if hb + k in ln.post else None
+        back_lab = kind == "lab" and not fwd
+        check_mlm_ce(self.mat(ln, 0, rows, Vp, Vp), labels, V, n, d_loss=d_loss, extra=extra, n_rows=n_rows,
+                     row_loss=None if back_lab else post("row_loss"), pred=post("pred") if fwd else None,
+                     dl=None if fwd else post("dlog"), loss=post("loss") if fwd else None,
+                     what="mlm %s ce" % kind, check=self.within)
+        if back_lab:
+            fw = [o for o in self.rec.launches if o.name == "b2_mlm_ce" and o.idx < ln.idx and o.args[13] is not None]
+            self.same(ln.post[hb + "row_loss"], fw[-1].post[hb + "row_loss"], "mlm backward row_loss == forward's")
+            self.claim_ws(ln, hb + "dlog")
+        elif fwd:
+            self.claim_ws(ln, hb + "row_loss", hb + "pred", hb + "loss")
+        else:
+            self.claim_ws(ln, hb + "row_loss", hb + "dlog")
+
+    def mlm_ln_bwd(self, ln):
+        a = ln.args
+        kind = self.mlm_kind(self.region(ln, 0))
+        hb, rows, H = "mlm.%s." % kind, self.mlm_rows(kind), self.H
+        w, gn = "cls.predictions.transform.LayerNorm.weight", "cls.predictions.transform.LayerNorm.bias"
+        for k, v in {0: hb + "dt", 2: hb + "h", 3: hb + "mean", 4: hb + "rstd", 5: "w:" + w, 12: hb + "dh",
+                     13: hb + "dh_bf", 14: "g:" + w, 15: "g:" + gn, 17: "mlm.ln_parts"}.items():
+            self.expect(ln, k, v, "mlm LN bwd")
+        # no dropout, the fp32 gradient and its bf16 copy, partial rows in both modes, no third sum
+        assert (a[1], a[6], a[7], a[8], a[11], a[16]) == (None, rows, H, 0.0, 1, None)
+        self.on(ln, 20, False, "mlm LN bwd")
+        dy = self.mat(ln, 0, rows, H, H)
+        ref, E, xh, ex = ln_bwd_ref(dy, self.mat(ln, 2, rows, H, H), self.vec(ln, 3, rows), self.vec(ln, 4, rows),
+                                    self.vec(ln, 5, H))
+        dh = self.mat(ln, 12, rows, H, H, "post")
+        self.within(dh, ref, E, "mlm LN bwd dh")
+        self.same(self.mat(ln, 13, rows, H, H, "post"), dh.to(bf), "mlm LN bwd dh_bf == bf16(dh)")
+        self.ln_parts["mlm"] = ((dy, xh, ex, None), ln.n_out, rows)
+        self.claim_ws(ln, hb + "dh", hb + "dh_bf")
+
+    def mlm_colsum_finish(self, ln):
+        a = ln.args
+        terms, n, rows = self.ln_parts.pop("mlm")
+        self.expect(ln, 0, "mlm.ln_parts", "mlm LN finish")
+        assert (a[1], a[2], a[3], a[6]) == (n, 3, self.H, None), "mlm LN finish: %s" % (a[:7],)
+        names = ["cls.predictions.transform.LayerNorm.weight", "cls.predictions.transform.LayerNorm.bias"]
+        for i, nm in enumerate(names):
+            self.expect(ln, 4 + i, "g:" + nm, "mlm LN finish")
+        self.on(ln, 7, True, "mlm LN finish")
+        got = [self.vec(ln, 4 + i, self.H, "post") for i in range(2)]
+        self.sums_check(got, terms, -(-rows // (8 * n)) + 8 + n + 9 + 1, "mlm LN bwd", True)
+        for nm in names:
+            self.claim_grad(nm)
+
+    def mlm_colsum(self, ln):
+        a = ln.args
+        src = self.region(ln, 0)
+        kind = self.mlm_kind(src)
+        hb, rows = "mlm.%s." % kind, self.mlm_rows(kind)
+        if src == hb + "dlog":
+            want, N = "cls.predictions.bias", self.Vp          # every vocab_pad column: the padding sums to 0
+        else:
+            assert src == hb + "du", "%s: b2_colsum of %s" % (self.case, src)
+            want, N = "cls.predictions.transform.dense.bias", self.H
+        self.expect(ln, 4, "g:" + want, "mlm colsum")
+        self.expect(ln, 5, "mlm.colsum", "mlm colsum")
+        assert (a[1], a[2], a[3]) == (rows, N, N)
+        self.on(ln, 7, True, "mlm colsum")
+        x = self.mat(ln, 0, rows, N, N).double()
+        ref = x.sum(0)
+        got = self.vec(ln, 4, N, "post")
+        self.within(got, ref, bf_bound(ref, gamma(rows) * x.abs().sum(0)), "mlm %s colsum" % want)
+        if N == self.Vp:
+            self.same(got[self.V:], torch.zeros_like(got[self.V:]), "mlm decoder bias padding")
+        self.claim_grad(want)
+
+    def c_b2_mlm_gelu_bwd(self, ln):
+        a = ln.args
+        kind = self.mlm_kind(self.region(ln, 0))
+        hb, rows, H = "mlm.%s." % kind, self.mlm_rows(kind), self.H
+        for k, v in {0: hb + "dh", 1: hb + "u", 3: hb + "du"}.items():
+            self.expect(ln, k, v, "mlm gelu bwd")
+        assert a[2] == rows * H
+        self.on(ln, 4, False, "mlm gelu bwd")
+        dg, u = self.mat(ln, 0, rows, H, H).double(), self.mat(ln, 1, rows, H, H).double()
+        r = dg * gelu_grad64(u)
+        self.within(self.mat(ln, 3, rows, H, H, "post"), r, bf_bound(r, dg.abs() * gelu_grad_err(u) + U * r.abs()),
+                    "mlm gelu bwd")
+        self.claim_ws(ln, hb + "du")
+
+    def c_b2_mlm_scatter_rows(self, ln):
+        a = ln.args
+        for k, v in {0: "mlm.lab.dx", 1: "mlm.lab.slot", 4: "dxA"}.items():
+            self.expect(ln, k, v, "mlm scatter")
+        M, H = self.M, self.H
+        assert a[2] == M and a[3] == H
+        self.on(ln, 5, False, "mlm scatter")
+        _lab, idx = self.mlm_labels()
+        ref = torch.zeros(M, H, dtype=f32, device=self.dev)
+        ref[idx] = self.mat(ln, 0, self.info["cap"], H, H)[:idx.numel()]
+        self.same(self.mat(ln, 4, M, H, H, "post"), ref, "mlm scatter")
+        self.claim_ws(ln, "dxA")
+
+    def c_b2_mlm_tied_add(self, ln):
+        a = ln.args
+        V, Vp, H = self.V, self.Vp, self.H
+        wreg = "g:" + WORD
+        self.expect(ln, 0, "mlm.dec", "mlm tied add")
+        self.expect(ln, 1, wreg, "mlm tied add")
+        assert a[2] == V * H
+        self.on(ln, 3, False, "mlm tied add")
+        emb = [o for o in self.rec.launches if o.name.startswith("b2_embed_bwd") and o.idx < ln.idx]
+        self.same(ln.pre[wreg], emb[-1].post[wreg], "mlm tied add reads the embedding backward's word gradient")
+        pre, post = ln.pre[wreg].view(Vp, H), ln.post[wreg].view(Vp, H)
+        dec = ln.pre["mlm.dec"].view(Vp, H)
+        self.same(post[:V], (pre[:V].float() + dec[:V]).to(bf), "mlm tied add")
+        self.same(post[V:], torch.zeros_like(post[V:]), "mlm tied add: word rows past the vocabulary")
+        pad = self.cfg.pad_token_id
+        self.same(post[pad], dec[pad].to(bf), "mlm tied add: the pad row")
+        self.claim_grad(WORD)
+
     # ---- embedding backward ------------------------------------------------------------------------------------------
     def c_b2_embed_bwd(self, ln, packed=False):
         a = ln.args
@@ -1099,7 +1545,8 @@ class Checker:
                           "embed", vocab=V, max_pos=P, unused=0.0, check=self.within)
         for n in ("word_embeddings.weight", "position_embeddings.weight", "token_type_embeddings.weight",
                   "LayerNorm.weight", "LayerNorm.bias"):
-            self.claim_grad("bert.embeddings." + n)
+            if not (self.eng.mlm and n == "word_embeddings.weight"):    # the masked-LM tied add owns its final value
+                self.claim_grad("bert.embeddings." + n)
         self.claim_ws(ln, "emb_dx")
 
     def c_b2_embed_bwd_packed(self, ln):
@@ -1118,8 +1565,8 @@ class Checker:
         pad = [(b, e) for b, e, f in expected_grad_claims(self.lay) if f == "padding"]
         for b, e in pad:
             t = grads[b:e]
-            if e <= ee:
-                self.same(t, torch.zeros_like(t), "embedding-bucket padding")
+            if zero_padding(self.lay, b, e):
+                self.same(t, torch.zeros_like(t), "padding [%d, %d)" % (b, e))
             else:
                 assert bool(torch.isnan(t).all()), "%s: padding [%d, %d) was written" % (self.case, b, e)
             self.grad_claims.append((b, e, "padding"))
@@ -1156,19 +1603,36 @@ def case_config(case):
         return full_config(hidden_size=1024, num_hidden_layers=3, num_attention_heads=16, intermediate_size=4096)
     if case.startswith("token"):
         return b2.chinese_bert_wwm_ext_config(num_labels=9, num_hidden_layers=3)
+    if case == "mlm_dense":
+        return tiny_config(vocab_size=1050, num_hidden_layers=2)        # vocab_pad 1088 = 17 x 64, V % 4 = 2
+    if case.startswith("mlm"):
+        return b2.chinese_bert_wwm_ext_config(num_hidden_layers=2)      # vocab_pad 21184 = 165.5 x 128
     return full_config(num_hidden_layers=3)
 
 
 def case_model(case, cfg, state, dev):
-    if case.startswith("token"):
-        m = b2.BertForTokenClassification(cfg)
+    if case.startswith(("token", "mlm")):
+        m = (b2.BertForTokenClassification if case.startswith("token") else b2.BertForMaskedLM)(cfg)
         m.load_state_dict(state, strict=True)
         return m.to(dev).train()
     return make_model(cfg, state, dev).train()
 
 
 def case_state(case, cfg):
+    if case.startswith("mlm"):
+        return mlm_state_from_hf_init(cfg, 9)
     return token_state_from_hf_init(cfg) if case.startswith("token") else state_from_hf_init(cfg)
+
+
+def dense_mlm_batch(cfg):
+    """B 8 x 128 with one sequence of padding only and every real token labelled: 768 = 6 x 128 labels, so the
+    labelled rows fill their capacity with no padding row"""
+    b = b2.synthetic_mlm_batch(cfg, 8, 128, 23, padded=True)
+    lens = torch.tensor([128, 100, 90, 120, 110, 0, 92, 128])
+    mask = (torch.arange(128)[None] < lens[:, None]).to(torch.int64)
+    ids = b["input_ids"] * mask
+    return {"input_ids": ids, "token_type_ids": torch.zeros_like(ids), "attention_mask": mask,
+            "label": torch.where(mask == 1, ids, torch.full_like(ids, -100))}
 
 
 def case_batch(case, cfg, dev):
@@ -1192,11 +1656,17 @@ def case_batch(case, cfg, dev):
         b = token_batch(cfg, 16, 128, 9)
     elif case == "token512packed":
         b = token_batch(cfg, 12, 512, 10, min_len=16)
+    elif case == "mlm128":
+        b = b2.synthetic_mlm_batch(cfg, 16, 128, 21, padded=True)
+    elif case == "mlm512packed":
+        b = b2.synthetic_mlm_batch(cfg, 8, 512, 22, padded=True)
+    elif case == "mlm_dense":
+        b = dense_mlm_batch(cfg)
     else:
         raise ValueError(case)
     host = {"batch": b}
-    token = case.startswith("token")
-    if case.startswith("packed") or case == "token512packed":
+    token = case.startswith(("token", "mlm"))          # a label per token
+    if case.startswith("packed") or case in ("token512packed", "mlm512packed"):
         S = 128 if case == "packed128" else 512
         pk = pack_batch(b["input_ids"], b["token_type_ids"], b["attention_mask"], S,
                         labels=b["label"] if token else None)
@@ -1220,14 +1690,27 @@ def case_batch(case, cfg, dev):
     cd = getattr(cfg, "classifier_dropout", None)
     info = dict(B=B, S=S, Bo=kw["labels"].numel(), packed="segments" in kw, inputs=inputs,
                 p_h=float(cfg.hidden_dropout_prob), p_a=float(cfg.attention_probs_dropout_prob),
-                p_c=float(cd if cd is not None else cfg.hidden_dropout_prob))
+                p_c=float(cd if cd is not None else cfg.hidden_dropout_prob), R=None)
+    if case.startswith("mlm"):
+        n = int((kw["labels"] != -100).sum())
+        info["cap"] = min(B * S, max(128, -(-n // 128) * 128))     # the labelled rows' capacity (mlm_capacity)
+        assert (n == info["cap"]) == (case == "mlm_dense"), "%s: %d labelled tokens" % (case, n)
+    if case == "mlm_dense":
+        # the objective's incoming gradient of the logits: loss + (logits R).sum()
+        gen = torch.Generator(device=dev).manual_seed(SEED)
+        info["R"] = torch.randn(B, S, cfg.vocab_size, generator=gen, device=dev)
     return kw, host, info
 
 
-def one_step(model, kw, step):
-    """seed the dropout stream at (SEED, step), then forward and the in-model loss's backward"""
+def objective(out, R):
+    """the in-model loss; for the dense masked-LM case loss + (logits R).sum(), so d_logits = R and d_loss = 1"""
+    return out.loss if R is None else out.loss + (out.logits * R).sum()
+
+
+def one_step(model, kw, step, R=None):
+    """seed the dropout stream at (SEED, step), then forward and the objective's backward"""
     model._engine.seed_dropout(SEED, step)
-    model(**kw).loss.backward()
+    objective(model(**kw), R).backward()
     torch.cuda.synchronize()
 
 
@@ -1242,9 +1725,9 @@ def run_case(case, det, dev):
     try:
         model = case_model(case, cfg, state, dev)
         eng = model._engine
-        one_step(model, kw, 0)
+        one_step(model, kw, 0, info["R"])
         ws = eng.workspace(info["B"], info["S"], info["Bo"])
-        prev = {"grads": eng.grads.clone(), "ws": {k: v.clone() for k, v in flat_ws(ws).items()}}
+        prev = {"grads": eng.grads.clone(), "ws": {k: v.clone() for k, v in step_bufs(eng, ws).items()}}
         poison(eng, ws)
         rec = Recorder(eng)
         register_step(rec, eng, ws, info["inputs"])
@@ -1254,12 +1737,19 @@ def run_case(case, det, dev):
         orig = L.call
         L.call = rec.call
         try:
-            model(**kw).loss.backward()
+            out = model(**kw)
+            if eng.mlm:
+                # the masked-LM backward passes d(objective)/d(loss) (and, dense, d_logits) to its kernels: the
+                # gradients autograd hands the model become step inputs
+                out.loss.register_hook(lambda g: rec.register("in:d_loss", g, "in"))
+                if info["R"] is not None:
+                    out.logits.register_hook(lambda g: rec.register("in:d_logits", g, "in"))
+            objective(out, info["R"]).backward()
         finally:
             L.call = orig
         torch.cuda.synchronize()
         return dict(case=case, cfg=cfg, state=state, kw=kw, host=host, info=info, model=model, rec=rec, ws=ws,
-                    prev=prev, grads=eng.grads.clone(), acts={k: v.clone() for k, v in flat_ws(ws).items()},
+                    prev=prev, grads=eng.grads.clone(), acts={k: v.clone() for k, v in step_bufs(eng, ws).items()},
                     acc_zero=bool((eng.bias_acc == 0).all()))
     finally:
         torch.use_deterministic_algorithms(was)
@@ -1299,11 +1789,11 @@ def unrecorded_step(r, dev):
     try:
         model = case_model(r["case"], r["cfg"], r["state"], dev)
         eng = model._engine
-        one_step(model, r["kw"], 0)
+        one_step(model, r["kw"], 0, info["R"])
         ws = eng.workspace(info["B"], info["S"], info["Bo"])
         poison(eng, ws)
-        one_step(model, r["kw"], 1)
-        return eng.grads.clone(), {k: v.clone() for k, v in flat_ws(ws).items()}
+        one_step(model, r["kw"], 1, info["R"])
+        return eng.grads.clone(), {k: v.clone() for k, v in step_bufs(eng, ws).items()}
     finally:
         torch.use_deterministic_algorithms(was)
 
@@ -1349,7 +1839,14 @@ def assert_same_ws(got, want, names, what):
 
 
 CASES = ["tiny", "hidden768", "hidden768_nodrop", "large", "seq512", "packed128", "packed512", "token128",
-         "token512packed"]
+         "token512packed", "mlm128", "mlm512packed", "mlm_dense"]
+
+
+def is_backward_buf(name):
+    """a buffer the backward writes (the rest are the forward's activations)"""
+    if name.startswith("mlm."):
+        return name == "mlm.dec" or name.split(".")[2] in MLM_BACKWARD
+    return name.startswith(BACKWARD_WS)
 
 
 @pytest.mark.gpu
@@ -1366,10 +1863,11 @@ def test_step_stages(cuda_dev, case, det):
         # every sum in a fixed order: bitwise the activations, the gradient space and the embedding backward's input
         assert_same_ws(acts, r["acts"], acts, case + " unrecorded det step")
         assert_same_grads(lay, grads, r["grads"], case + " unrecorded det step")
-        assert_same_grads(lay, captured_step(r, cuda_dev), r["grads"], case + " captured det step")
+        if case != "mlm_dense":         # the captured step's objective is the loss alone
+            assert_same_grads(lay, captured_step(r, cuda_dev), r["grads"], case + " captured det step")
     else:
         # atomics order the backward's sums freely; the forward has none but the loss's mean over blocks
-        fwd = [k for k in acts if not k.startswith(BACKWARD_WS) and k != "loss"]
+        fwd = [k for k in acts if not is_backward_buf(k) and k != "loss"]
         assert_same_ws(acts, r["acts"], fwd, case + " unrecorded step")
 
 
@@ -1408,6 +1906,10 @@ DEFECTS = {
     "stale_row": ("hidden768", False, is_layer(2, "b2_gemm_bf16"), r"L2 qkv: worst error"),
     "one_bin_fewer": ("packed128", True, lambda ln: ln.name == "b2_colsum" and Checker.region(None, ln, 0) == "dqkv.1",
                       r"L1 attention.self.qkv.bias colsum: worst error"),
+    "stale_dec": ("mlm128", False, lambda ln: ln.name == "b2_mlm_tied_add", r"mlm tied add: \d+ elements differ"),
+    "stale_gathered_row": ("mlm128", False, lambda ln: ln.name == "b2_mlm_gather_rows", r"mlm gather: \d+ elements differ"),
+    "neighbour_label": ("mlm128", False, lambda ln: ln.name == "b2_mlm_ce" and ln.args[13] is not None,
+                        r"mlm lab ce row_loss: worst error"),
 }
 
 
@@ -1430,6 +1932,14 @@ def test_planted_defect_fails(recorded, defect):
         ln = [x for x in rec.launches if only(x) and x.g["epilogue"] == L.EPI_BIAS][0]
         saved.append((ln.post["layers.2.qkv"], ln.post["layers.2.qkv"].clone()))
         ln.post["layers.2.qkv"][77] = r["prev"]["ws"]["layers.2.qkv"][77]
+    elif defect == "stale_dec":                     # the tied add's reference reads the warm-up step's decoder part
+        ln = [x for x in rec.launches if only(x)][0]
+        saved.append((ln.pre["mlm.dec"], ln.pre["mlm.dec"].clone()))
+        ln.pre["mlm.dec"].copy_(r["prev"]["ws"]["mlm.dec"])
+    elif defect == "stale_gathered_row":            # one gathered row back to the warm-up step's
+        ln = [x for x in rec.launches if only(x)][0]
+        saved.append((ln.post["mlm.lab.x"], ln.post["mlm.lab.x"].clone()))
+        ln.post["mlm.lab.x"][3] = r["prev"]["ws"]["mlm.lab.x"][3]
     try:
         with pytest.raises(AssertionError, match=fails):
             ck.run(only)
