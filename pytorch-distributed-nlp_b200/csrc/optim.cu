@@ -1009,6 +1009,11 @@ extern "C" int32_t b2_grad_norm_finalize(const double* partials, int64_t nslots,
     count_launches(1);
     return 0;
   }
+  // the exchange's arguments are checked before the share kernel runs: a rejected call leaves *total_norm untouched
+  B2_REQUIRE(peer_scratch && peer_flags && epoch, "grad_norm_finalize: null pointer");
+  B2_REQUIRE(slot >= 0 && slot < B2_FLAG_SLOTS, "grad_norm_finalize: slot=%d", slot);
+  for (int r = 0; r < world; ++r)
+    B2_REQUIRE(peer_scratch[r] && peer_flags[r], "grad_norm_finalize: null peer pointer for rank %d", r);
   // this rank's share -> *total_norm; rank-order mean of the shares -> *clip_coef; then the norm from that mean
   B2_LAUNCH(grad_norm_finalize_kernel, 1, kFinThreads, 0, s, partials, (long long)nslots, 1, world, max_norm, grad_scale,
             found_inf, total_norm, clip_coef, skip);
