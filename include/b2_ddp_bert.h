@@ -386,6 +386,25 @@ int32_t b2_mlm_ce(const float* logits, int64_t rows, int64_t vocab, int64_t voca
 int32_t b2_mlm_tied_add(const float* dec, void* grad, int64_t n, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------ */
+/* question-answering span loss (csrc/qa_head.cu, HF BertForQuestionAnswering's loss)                       */
+/* ------------------------------------------------------------------------------------------------------ */
+/* The head is the token head with num_labels = 2 and no dropout: logits fp32 [rows, 2], column 0 the start logit and
+ * column 1 the end logit of every row.  Sequence b covers rows [seq_first[b], seq_first[b] + seq_len[b]) (both NULL:
+ * padded, rows [b * ignored_index, (b + 1) * ignored_index)), 1 to 512 rows each.  Its targets are HF's
+ * clamp(0, ignored_index) of the raw int64 start_positions[b] / end_positions[b]; a target equal to ignored_index
+ * (the padded length) is ignored.  Per sequence and column, a softmax over the sequence's own rows:
+ *   seq_loss[2b + c] = logsumexp_r x[r, c] - x[t_c, c]   (0 when ignored)
+ *   loss = (sum_b seq_loss[2b] / n_start + sum_b seq_loss[2b + 1] / n_end) / 2   (nan for an all-ignored column)
+ *   d_logits[r, c] = (softmax - onehot) * (*d_loss) / (2 n_c)   (0 on an ignored column and on rows of no sequence)
+ * with n_c the sequences whose column-c target is not ignored.  d_loss NULL: 1; d_logits / loss NULL: not written;
+ * seq_loss: fp32 scratch [2 * num_seqs].  Every sum is in a fixed order without atomics: bitwise repeatable.  A
+ * target inside [0, ignored_index) but past its sequence's rows traps.                                          */
+int32_t b2_qa_span_loss(const float* logits, int64_t rows, const int64_t* start_positions,
+                        const int64_t* end_positions, int64_t num_seqs, int64_t ignored_index, const int64_t* seq_first,
+                        const int64_t* seq_len, const float* d_loss, float* seq_loss, float* d_logits, float* loss,
+                        void* stream);
+
+/* ------------------------------------------------------------------------------------------------------ */
 /* optimizer + gradient exchange                                                                          */
 /*   replaces: HF AdamW.step (transformers 4.28.1 optimization.py, built at multi-gpu-distributed-cls.py    */
 /*   :100-111, stepped :174), optimizer.zero_grad (:172), and the DDP Reducer's bucket all-reduce            */

@@ -117,6 +117,8 @@ _SIGNATURES = {
     "b2_mlm_bias_fill": [vp, i64, i64, vp, vp],
     "b2_mlm_ce": [vp, i64, i64, i64, vp, vp, vp, vp, vp, i64, vp, vp, vp, vp, vp],
     "b2_mlm_tied_add": [vp, vp, i64, vp],
+    # question-answering span loss (csrc/qa_head.cu)
+    "b2_qa_span_loss": [vp, i64, vp, vp, i64, i64, vp, vp, vp, vp, vp, vp, vp],
     "b2_bucket_reduce_adamw": [C.POINTER(vp), C.POINTER(vp), i32, i32, vp, vp, vp, vp, i64, i64,
                                C.POINTER(AdamWHParams), vp, vp],
     "b2_adamw_prepare": [C.POINTER(AdamWHParams), vp, vp, vp],

@@ -101,6 +101,23 @@ class SequenceClassifierOutput:
         return len(self.to_tuple())
 
 
+class QuestionAnsweringModelOutput:
+    """HF's QuestionAnsweringModelOutput, tuple-like: ``(loss, start_logits, end_logits)``, the loss left out when it is
+    None."""
+
+    def __init__(self, loss=None, start_logits=None, end_logits=None):
+        self.loss = loss
+        self.start_logits = start_logits
+        self.end_logits = end_logits
+
+    def to_tuple(self):
+        return tuple(v for v in (self.loss, self.start_logits, self.end_logits) if v is not None)
+
+    __getitem__ = SequenceClassifierOutput.__getitem__
+    __iter__ = SequenceClassifierOutput.__iter__
+    __len__ = SequenceClassifierOutput.__len__
+
+
 def _round8(n):
     return (n + 7) // 8 * 8
 
@@ -110,8 +127,8 @@ def vocab_pad(vocab_size):
     return (vocab_size + 63) // 64 * 64
 
 
-HEAD_KINDS = ("sequence", "token", "mlm")   # BertForSequenceClassification's pooler + classifier, a classifier per
-                                            # token, or BertForMaskedLM's cls.predictions
+HEAD_KINDS = ("sequence", "token", "mlm", "question_answering")   # BertForSequenceClassification's pooler +
+    # classifier, a classifier per token, BertForMaskedLM's cls.predictions, or BertForQuestionAnswering's qa_outputs
 MLM_TIED = {"cls.predictions.decoder.weight": "bert.embeddings.word_embeddings.weight",
             "cls.predictions.decoder.bias": "cls.predictions.bias"}    # HF's tied state-dict keys of the MLM head
 TOKEN_HEAD_MAX_LABELS = 64             # b2_token_head_fwd's bound
@@ -129,7 +146,8 @@ class _Layout:
     a kernel launch of its own.  head "token" (BertForTokenClassification): the tail is the classifier alone.  head
     "mlm" (BertForMaskedLM): the tail is cls.predictions (its decoder is the word-embedding table), and the word table
     and cls.predictions.bias reserve vocab_pad(V) rows / entries, so the vocabulary projection is one GEMM with a
-    multiple of 64 columns; the extra rows stay zero and lie outside every parameter view."""
+    multiple of 64 columns; the extra rows stay zero and lie outside every parameter view.  head "question_answering"
+    (BertForQuestionAnswering): the tail is qa_outputs [2, H] / [2] alone, like the token head's classifier."""
 
     def __init__(self, cfg, head="sequence"):
         if head not in HEAD_KINDS:
@@ -188,6 +206,9 @@ class _Layout:
             add("cls.predictions.transform.dense.bias", (H,))
             add("cls.predictions.transform.LayerNorm.weight", (H,))
             add("cls.predictions.transform.LayerNorm.bias", (H,))
+        elif head == "question_answering":
+            add("qa_outputs.weight", (cfg.num_labels, H))
+            add("qa_outputs.bias", (cfg.num_labels,))
         else:
             add("classifier.weight", (cfg.num_labels, H))
             add("classifier.bias", (cfg.num_labels,))
@@ -203,7 +224,8 @@ class _Layout:
         return self.entries[name][0]
 
 
-# HF named_parameters() order (201 tensors for 12 layers, 199 without the pooler, 202 for the MLM head); differs from
+# HF named_parameters() order (201 tensors for 12 layers, 199 without the pooler, 202 for the MLM head, 199 for the QA
+# head); differs from
 # the flat order only inside attention.self
 def _hf_order(cfg, head="sequence"):
     names = ["bert.embeddings.word_embeddings.weight", "bert.embeddings.position_embeddings.weight",
@@ -220,6 +242,8 @@ def _hf_order(cfg, head="sequence"):
         return names + ["cls.predictions.bias", "cls.predictions.transform.dense.weight",
                         "cls.predictions.transform.dense.bias", "cls.predictions.transform.LayerNorm.weight",
                         "cls.predictions.transform.LayerNorm.bias"]
+    if head == "question_answering":
+        return names + ["qa_outputs.weight", "qa_outputs.bias"]
     names += ["classifier.weight", "classifier.bias"]
     return names
 
@@ -228,10 +252,10 @@ class _StepFn(torch.autograd.Function):
     """logits (and HF's in-model loss) with a backward that runs the CUDA backward pass."""
 
     @staticmethod
-    def forward(ctx, anchor, model, input_ids, token_type_ids, attention_mask, labels, packed=None):
+    def forward(ctx, anchor, model, input_ids, token_type_ids, attention_mask, labels, packed=None, fwd_kw=None):
         eng = model._engine
         logits, loss = eng.forward(input_ids, token_type_ids, attention_mask, labels, training=model.training,
-                                   need_backward=True, packed=packed)
+                                   need_backward=True, packed=packed, **(fwd_kw or {}))
         ctx.model = model
         ctx.has_loss = loss is not None
         ctx.set_materialize_grads(False)
@@ -274,7 +298,7 @@ class _StepFn(torch.autograd.Function):
         probe = eng.grads[off:off + n].float().view(shape)
         if model._ddp is not None:
             probe = model._ddp.consensus_probe(probe)
-        return probe, None, None, None, None, None, None
+        return probe, None, None, None, None, None, None, None
 
 
 class _BertClassifier(nn.Module):
@@ -675,6 +699,75 @@ class BertForMaskedLM(_BertClassifier):
         return super().from_pretrained(model_path, config=config, **kwargs)
 
 
+def _qa_positions(start_positions, end_positions, nseq, device):
+    """HF's start / end positions (int64 [nseq], or [nseq, 1], squeezed) as the one int64 [2, nseq] tensor the span
+    loss reads: row 0 the start positions, row 1 the end positions, raw (the kernel applies HF's clamp)"""
+    out = []
+    for t, nm in ((start_positions, "start_positions"), (end_positions, "end_positions")):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.int64:
+            raise TypeError("%s must be an int64 tensor (token positions), got %s"
+                            % (nm, getattr(t, "dtype", type(t).__name__)))
+        if t.device != device:
+            raise RuntimeError("%s is on %s, model on %s" % (nm, t.device, device))
+        if tuple(t.shape) not in ((nseq,), (nseq, 1)):
+            raise ValueError("%s must be [%d] or [%d, 1] (one per sequence), got %s" % (nm, nseq, nseq, list(t.shape)))
+        out.append(t.reshape(nseq))
+    return torch.stack(out)
+
+
+class BertForQuestionAnswering(_BertClassifier):
+    """HF's BertForQuestionAnswering: BertModel without the pooler and ``qa_outputs``, a Linear(H, 2) on every token
+    with no dropout (the token head's kernels with two labels), split into start and end logits.  With
+    ``start_positions`` and ``end_positions`` the loss is HF's: both clamped to [0, S] with S ignored, one
+    ``CrossEntropyLoss(ignore_index=S)`` over the sequence axis for each, averaged (csrc/qa_head.cu).  Logits are fp32
+    [batch, seq] each, or [bins, bin_len] for a packed batch, where each sequence's softmax runs over its own tokens
+    (HF's loss on the sequence unpadded)."""
+    _head = "question_answering"
+    _anchor = "qa_outputs.bias"
+    _config_extra = {"architectures": ["BertForQuestionAnswering"]}
+
+    def __init__(self, config):
+        if int(config.num_labels) != 2:
+            raise ValueError("BertForQuestionAnswering: num_labels=%d, the span head needs exactly 2 (start and end "
+                             "logits)" % int(config.num_labels))
+        super().__init__(config)
+
+    def forward(self, input_ids=None, token_type_ids=None, attention_mask=None, start_positions=None,
+                end_positions=None, position_ids=None, segments=None, cls_index=None, ignored_index=None, **unused):
+        """`position_ids` / `segments` / `cls_index` (all three or none): the rows of `input_ids` are the bins of
+        `packing.pack_batch`, and the positions count from each sequence's first token.  `ignored_index` (packed
+        only): the padded length the positions were given for, HF's ignored index (None: the bin length); a position
+        inside [length, ignored_index) traps, and pack_batch rejects it first."""
+        if self._engine is None:
+            raise RuntimeError("BertForQuestionAnswering (b200) only runs on CUDA: call model.cuda() first; there is "
+                               "no CPU path.")
+        if input_ids is None:
+            raise ValueError("input_ids is required")
+        packed, kw = None, {}
+        if segments is not None or cls_index is not None or position_ids is not None:
+            if position_ids is None or segments is None or cls_index is None:
+                raise ValueError("a packed batch needs position_ids, segments and cls_index together")
+            packed = (position_ids, segments, cls_index)
+            if ignored_index is not None:
+                kw["qa_ignored_index"] = int(ignored_index)
+        elif ignored_index is not None:
+            raise ValueError("ignored_index applies to packed batches only (a padded batch ignores its length S)")
+        positions = None
+        if start_positions is not None and end_positions is not None:
+            nseq = input_ids.shape[0] if packed is None else cls_index.numel()
+            positions = _qa_positions(start_positions, end_positions, nseq, self._engine.dev)
+        if torch.is_grad_enabled() and self.training:
+            anchor = self._params_by_name[self._anchor]
+            logits, loss = _StepFn.apply(anchor, self, input_ids, token_type_ids, attention_mask, positions, packed, kw)
+            loss = loss if positions is not None else None
+        else:
+            logits, loss = self._engine.forward(input_ids, token_type_ids, attention_mask, positions,
+                                                training=self.training, need_backward=False, packed=packed, **kw)
+            loss = None if loss is None else loss.clone()
+        start, end = (t.contiguous() for t in logits.unbind(-1))
+        return QuestionAnsweringModelOutput(loss=loss, start_logits=start, end_logits=end)
+
+
 class _LocalTransport:
     """The facts the optimizer's step schedule (optim._FusedOptimizer: bucket_ready, step, the clip phases) needs about
     where gradients and weights live, on one GPU.  DistributedDataParallel answers the same questions for a peer group
@@ -740,7 +833,16 @@ class _Engine:
         self.p_attn = float(cfg.attention_probs_dropout_prob)
         cd = getattr(cfg, "classifier_dropout", None)
         self.p_cls = float(cd if cd is not None else cfg.hidden_dropout_prob)
-        self.token_head = self.lay.head == "token"     # a classifier on every token row instead of pooler + classifier
+        # a classifier on every token row instead of pooler + classifier; the QA head's qa_outputs is one with two labels
+        # and no dropout, followed by the span loss (csrc/qa_head.cu)
+        self.qa = self.lay.head == "question_answering"
+        self.token_head = self.lay.head == "token" or self.qa
+        self.cls_w, self.cls_b = ("qa_outputs.weight", "qa_outputs.bias") if self.qa else \
+            ("classifier.weight", "classifier.bias")
+        if self.qa:
+            self.p_cls = 0.0
+        self._qa_ws = {}
+        self.qa_last = None          # (per-sequence losses, positions [2, sequences], ignored index) of the last span loss
         self.mlm = self.lay.head == "mlm"               # cls.predictions on the labelled rows (csrc/mlm_head.cu)
         self.per_token = self.token_head or self.mlm    # packed bins need no cls_index
         self.V, self.Vp = cfg.vocab_size, self.lay.vocab_pad
@@ -999,7 +1101,8 @@ class _Engine:
 
     # ---- forward --------------------------------------------------------------------------------------------------------
     def forward(self, input_ids, token_type_ids, attention_mask, labels, training, need_backward, packed=None,
-                loss_fn=None, mlm_full=True, ignore_index=-100, mlm_capacity=None, mlm_dloss=None):
+                loss_fn=None, mlm_full=True, ignore_index=-100, mlm_capacity=None, mlm_dloss=None,
+                qa_ignored_index=None, qa_dloss=None):
         """packed: None, or (position_ids int64 [bins, S], segments int32 [bins, S], cls_index int64 [batch]) -- the
         rows of `input_ids` are then S-token bins produced by packing.pack_batch (S a multiple of 128, at most 512),
         not sequences.
@@ -1008,7 +1111,9 @@ class _Engine:
         capacity of mlm_capacity rows (None: their count rounded up to 128, read from the device); mlm_full: also
         the logits of every row (returned as [B, S, V]; else None); mlm_dloss: a device scalar d(objective)/d(loss)
         -- the same cross-entropy launch then also writes the labelled rows' d_logits for the backward (the
-        captured steps' one pass)."""
+        captured steps' one pass).
+        QA head: `labels` int64 [2, sequences], the raw start / end positions; qa_ignored_index: a packed batch's HF
+        ignored index (None: the bin length); qa_dloss: as mlm_dloss, for the span loss."""
         cfg, H, I = self.cfg, self.H, self.I
         if input_ids.dim() != 2:
             raise ValueError("input_ids must be [batch, seq]")
@@ -1020,8 +1125,8 @@ class _Engine:
                 raise ValueError("packed bins carry their own (block-diagonal) mask: pass attention_mask=None")
             for t, nm, dt, shape in ((pos_ids, "position_ids", torch.int64, (B, S)), (segs, "segments", torch.int32, (B, S)),
                                      (cls_rows, "cls_index", torch.int64, None)):
-                if t is None and self.per_token and nm == "cls_index":
-                    continue      # the token head reads every bin row
+                if t is None and self.per_token and not self.qa and nm == "cls_index":
+                    continue      # the token head reads every bin row (the QA loss needs each sequence's first row)
                 if t.device != self.dev or t.dtype != dt or (shape is not None and tuple(t.shape) != shape):
                     raise TypeError("%s must be a %s tensor%s on %s" % (nm, dt, "" if shape is None else " of shape %s"
                                                                         % (shape,), self.dev))
@@ -1029,6 +1134,8 @@ class _Engine:
             if not self.per_token:
                 cls_rows = cls_rows.contiguous().view(-1)
                 Bo = cls_rows.numel()
+            elif self.qa:
+                cls_rows = cls_rows.contiguous().view(-1)
         if self.per_token:
             Bo = B * S
         if B == 0 or S == 0:
@@ -1043,7 +1150,7 @@ class _Engine:
                     raise RuntimeError("%s is on %s, model on %s" % (nm, t.device, self.dev))
                 if t is not labels and t.dtype != torch.int64:
                     raise TypeError("%s must be int64 (as the reference Collate produces)" % nm)
-        if labels is not None and not self.mlm:
+        if labels is not None and not self.mlm and not self.qa:
             if loss_fn is None:
                 loss_fn = self.model._problem_type_loss(labels)
             labels = loss_fn.device_labels(labels, Bo)
@@ -1109,7 +1216,7 @@ class _Engine:
                 self._saved = (B, S, mask, p_h, p_a, p_c, None if packed is None else (segs, None))
             return (None if logits is None else logits.view(B, S, self.V)), loss
         if self.token_head:
-            L.call("b2_token_head_fwd", x.data_ptr(), M, H, w("classifier.weight"), w("classifier.bias"), self.C, p_c,
+            L.call("b2_token_head_fwd", x.data_ptr(), M, H, w(self.cls_w), w(self.cls_b), self.C, p_c,
                    rng, 1 + 3 * self.nl, ws["logits"].data_ptr(), s)
         elif packed is None:
             head_w = (w("bert.pooler.dense.weight"), w("bert.pooler.dense.bias"), w("classifier.weight"),
@@ -1122,7 +1229,10 @@ class _Engine:
             L.call("b2_head_fwd_packed", x.data_ptr(), cls_rows.data_ptr(), Bo, H, *head_w, self.C, p_c, rng,
                    1 + 3 * self.nl, ws["pooled"].data_ptr(), ws["logits"].data_ptr(), s)
         loss = None
-        if labels is not None:
+        if labels is not None and self.qa:
+            loss = self._qa_loss(ws, M, labels, S, None if packed is None else (segs, cls_rows), need_backward,
+                                 qa_ignored_index, qa_dloss)
+        elif labels is not None:
             loss_fn.launch(ws["logits"].data_ptr(), labels, Bo, ws["loss"].data_ptr(),
                            ws["dloss_logits"].data_ptr() if need_backward else None, s)
             loss = ws["loss"]
@@ -1131,6 +1241,38 @@ class _Engine:
         if self.token_head:
             return ws["logits"].view(B, S, self.C), loss
         return ws["logits"], loss
+
+    # ---- question-answering span loss -----------------------------------------------------------------------------------
+    def _qa_loss(self, ws, M, positions, S, packed, need_backward, ignored_index, dloss):
+        """b2_qa_span_loss over the head's [M, 2] logits: the loss into ws["loss"] and, for a backward, d(loss)/d(logits)
+        into ws["dloss_logits"] (scaled by the device scalar `dloss`, None: 1).  Padded: sequence b is rows
+        [b S, (b + 1) S) and S is HF's ignored index.  Packed (segs, cls_rows): sequence b starts at bin row
+        cls_rows[b] and its length is the extent of that row's segment."""
+        if positions.dtype != torch.int64 or positions.dim() != 2 or positions.shape[0] != 2:
+            raise TypeError("QA positions must be int64 [2, sequences] (start row, end row), got %s %s"
+                            % (positions.dtype, list(positions.shape)))
+        nseq = positions.shape[1]
+        pos = positions.contiguous()
+        first = lens = None
+        if packed is None:
+            if nseq * S != M:
+                raise ValueError("QA positions: %d sequences for %d rows of %d tokens" % (nseq, M // S, S))
+            ignored = S
+        else:
+            segs, first = packed
+            if first.numel() != nseq:
+                raise ValueError("QA positions: %d sequences, cls_index has %d" % (nseq, first.numel()))
+            seg = segs.view(-1)[first]
+            lens = ((seg >> 16) - (seg & 0xFFFF)).to(torch.int64)
+            ignored = S if ignored_index is None else int(ignored_index)
+        buf = self._qa_ws.get(nseq)
+        if buf is None:
+            buf = self._qa_ws[nseq] = torch.empty(2 * nseq, dtype=torch.float32, device=self.dev)
+        self.qa_last = (buf, pos, ignored)
+        L.call("b2_qa_span_loss", ws["logits"].data_ptr(), M, pos.data_ptr(), pos.data_ptr() + 8 * nseq, nseq,
+               ignored, L.ptr(first), L.ptr(lens), L.ptr(dloss), buf.data_ptr(),
+               ws["dloss_logits"].data_ptr() if need_backward else None, ws["loss"].data_ptr(), self.stream())
+        return ws["loss"]
 
     # ---- masked-LM head (cls.predictions) ---------------------------------------------------------------------------------
     def _mlm_buffers(self, M, rows, full=False):
@@ -1375,8 +1517,8 @@ class _Engine:
             dec_done = self._mlm_backward(x_last, ws["dxA"], det, main, side)
         elif self.token_head:
             # every row of d_hidden is written: no memset
-            L.call("b2_token_head_bwd_split", dl.data_ptr(), x_last.data_ptr(), M, H, w("classifier.weight"), self.C,
-                   p_c, rng, 1 + 3 * self.nl, g("classifier.weight"), g("classifier.bias"), ws["dxA"].data_ptr(),
+            L.call("b2_token_head_bwd_split", dl.data_ptr(), x_last.data_ptr(), M, H, w(self.cls_w), self.C,
+                   p_c, rng, 1 + 3 * self.nl, g(self.cls_w), g(self.cls_b), ws["dxA"].data_ptr(),
                    ws["head_scratch"].data_ptr(), ws["head_scratch"].numel(), s,
                    side.cuda_stream if self.nl > 0 else None)
         else:

@@ -26,7 +26,8 @@ def bin_length(attention_mask, seq_len):
     return BIN * max(1, -(-longest // BIN))
 
 
-def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN, labels=None, ignore_index=-100):
+def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN, labels=None, ignore_index=-100,
+               start_positions=None, end_positions=None):
     """input_ids / token_type_ids / attention_mask: int64 [B, S] host tensors as the reference's Collate yields them
     (valid tokens first: the tokenizer pads on the right).  Returns a dict of host tensors:
       input_ids, token_type_ids, position_ids   int64 [NB, bin_len]   (unused bin rows: pad id 0, position 0)
@@ -37,6 +38,12 @@ def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN, labels=No
       lengths                                    int64 [B]
       labels (when `labels`, int64 [B, S] token labels are given)
                                                  int64 [NB, bin_len]   unused bin rows: ignore_index
+      start_positions, end_positions, seq_len    (when question-answering positions, int64 [B] or [B, 1], are
+                                                 given) the positions as given, int64 [B] -- they count from each
+                                                 sequence's first token, which packing keeps -- and S, HF's ignored
+                                                 index.  A position in [length, S) targets a padding token, which
+                                                 packing drops: ValueError.  Negative positions and positions >= S
+                                                 pass through (the span loss clamps them as HF does).
     NB <= B; a sequence longer than bin_len is not supported (the reference truncates to max_seq_len = 128)."""
     if input_ids.dim() != 2:
         raise ValueError("input_ids must be [batch, seq]")
@@ -57,6 +64,23 @@ def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN, labels=No
         if bool((lab_np[~mask_np] != ignore_index).any()):
             raise ValueError("pack_batch: a masked position carries a label other than ignore_index=%d; packing drops "
                              "masked positions, so their labels must be ignored" % ignore_index)
+    if (start_positions is None) != (end_positions is None):
+        raise ValueError("pack_batch: start_positions and end_positions go together")
+    qa = None
+    if start_positions is not None:
+        qa = []
+        for t, nm in ((start_positions, "start_positions"), (end_positions, "end_positions")):
+            if t.is_floating_point() or tuple(t.shape) not in ((B,), (B, 1)):
+                raise ValueError("pack_batch: %s must be int64 [%d] or [%d, 1], got %s %s"
+                                 % (nm, B, B, t.dtype, list(t.shape)))
+            p = t.reshape(B).to(torch.int64)
+            bad = (p >= torch.from_numpy(lens)) & (p < S)
+            if bool(bad.any()):
+                i = int(bad.nonzero()[0, 0])
+                raise ValueError("pack_batch: %s[%d] = %d targets a padding token (the sequence has %d tokens, the batch "
+                                 "%d): packing drops padding, so the target would vanish" % (nm, i, int(p[i]),
+                                                                                             int(lens[i]), S))
+            qa.append(p.clone())
     if int(lens.max()) > bin_len:
         raise ValueError("pack_batch: a sequence has %d valid tokens, more than the %d-token bin"
                          % (int(lens.max()), bin_len))
@@ -102,4 +126,6 @@ def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN, labels=No
         lab = np.full(NB * bin_len, ignore_index, dtype=np.int64)
         lab[dst] = lab_np.reshape(-1)[src]
         out["labels"] = t(lab).view(NB, bin_len)
+    if qa is not None:
+        out["start_positions"], out["end_positions"], out["seq_len"] = qa[0], qa[1], S
     return out

@@ -38,6 +38,48 @@ def synthetic_mlm_batch(cfg, batch, seq, seed, padded=False, mlm_probability=0.1
     return {"input_ids": inputs, "token_type_ids": b["token_type_ids"], "attention_mask": mask, "label": labels}
 
 
+def synthetic_qa_batch(cfg, batch, seq, seed, padded=False, no_answer=0.2, ignored=0.1, min_len=16):
+    """A SQuAD-shaped batch for BertForQuestionAnswering, from generator seed `seed`: each row is [CLS] (101), 2 to 8
+    question tokens (token type 0), [SEP] (102), context tokens (token type 1), [SEP]; `padded` draws per-row valid
+    lengths ~ U{min_len..seq} (min_len >= 16) and zeroes ids / mask / token types beyond them.  start_positions <= end_positions lie inside
+    the context; a `no_answer` fraction of rows is (0, 0) ([CLS], SQuAD v2's no answer) and an `ignored` fraction has a
+    position >= seq (HF's loss clamps it to seq and ignores it).  Returns input_ids, token_type_ids, attention_mask,
+    start_positions and end_positions (int64; the positions [batch])."""
+    if not 16 <= min_len <= seq:
+        raise ValueError("synthetic_qa_batch: need 16 <= min_len=%d <= seq=%d" % (min_len, seq))
+    g = torch.Generator().manual_seed(seed)
+    V = cfg.vocab_size
+    ids = torch.randint(0, V, (batch, seq), generator=g, dtype=torch.int64)
+    lens = torch.randint(min_len, seq + 1, (batch,), generator=g) if padded else torch.full((batch,), seq)
+    qlen = torch.randint(2, 9, (batch,), generator=g)
+    kind = torch.rand(batch, generator=g)
+    u = torch.rand(batch, 3, generator=g)
+    tt = torch.zeros(batch, seq, dtype=torch.int64)
+    mask = (torch.arange(seq)[None] < lens[:, None]).to(torch.int64)
+    start = torch.zeros(batch, dtype=torch.int64)
+    end = torch.zeros(batch, dtype=torch.int64)
+    cls_id, sep_id = min(101, V - 1), min(102, V - 1)
+    for b in range(batch):
+        n, q = int(lens[b]), int(qlen[b])
+        ids[b, 0], ids[b, 1 + q], ids[b, n - 1] = cls_id, sep_id, sep_id
+        tt[b, 2 + q:n] = 1
+        lo, hi = 2 + q, n - 2                      # the context tokens, inclusive
+        s = lo + int(u[b, 0] * (hi - lo + 1))
+        e = s + int(u[b, 1] * min(hi - s + 1, 16))
+        if kind[b] < no_answer:
+            s = e = 0
+        elif kind[b] < no_answer + ignored:
+            over = seq + int(u[b, 2] * 8)
+            if u[b, 2] < 0.5:
+                s = over
+            else:
+                e = over
+        start[b], end[b] = s, e
+    ids = ids * mask
+    return {"input_ids": ids, "token_type_ids": tt * mask, "attention_mask": mask, "start_positions": start,
+            "end_positions": end}
+
+
 # Token-length histogram of the reference's own data (data/train.json, 40 133 rows): characters of the text without the
 # segmentation blanks (BertTokenizer splits Chinese text into single characters) + [CLS] + [SEP], capped at
 # max_seq_len = 128 (multi-gpu-distributed-cls.py:66-98).  (length, rows); mean 19.8 tokens -- the reference pads all of

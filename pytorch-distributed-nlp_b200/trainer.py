@@ -72,6 +72,8 @@ class Args:
     save_total_limit = None   # all); train(resume_from_checkpoint=...) continues from one
     full_determinism = False  # HF TrainingArguments' name: Trainer() calls torch.use_deterministic_algorithms(True), and
                               # every training path then runs its fixed-order backward (bitwise reproducible runs)
+    max_answer_length = 30    # run_qa.py's name: a question-answering model's dev() / test() predict spans of at most
+                              # this many tokens
 
 
 def _unwrap(model):
@@ -88,8 +90,52 @@ def _is_mlm(model):
     return _unwrap(model)._layout.head == "mlm"
 
 
+def _is_qa(model):
+    """a BertForQuestionAnswering (or a wrapper of one): start / end positions instead of labels"""
+    return _unwrap(model)._layout.head == "question_answering"
+
+
 TOKEN_PROBLEM_TYPE = "token_classification"     # what Trainer.problem_type reports for a token model (not stored)
 MLM_PROBLEM_TYPE = "masked_lm"                  # ... and for a masked-LM model (not stored)
+QA_PROBLEM_TYPE = "question_answering"          # ... and for a question-answering model (not stored)
+
+
+def check_qa_criterion(criterion):
+    """HF's question-answering head computes its own span loss and takes no external one: the criterion is None or a
+    plain CrossEntropyLoss() (both train that in-model loss); anything else raises ValueError."""
+    if criterion is None:
+        return
+    plain = (type(criterion) is torch.nn.CrossEntropyLoss and criterion.weight is None
+             and criterion.ignore_index == -100 and criterion.label_smoothing == 0.0 and criterion.reduction == "mean")
+    if not plain:
+        raise ValueError("a BertForQuestionAnswering trains HF's in-model span loss (a CrossEntropyLoss over each "
+                         "sequence's tokens, ignore_index = the padded length): pass no criterion or a plain "
+                         "CrossEntropyLoss(), got %r" % (criterion,))
+
+
+def qa_positions(batch_data):
+    """a question-answering batch's HF keys start_positions / end_positions (int64 [B] or [B, 1]) as one int64
+    [2, B] tensor: row 0 the starts, row 1 the ends"""
+    st, en = batch_data["start_positions"], batch_data["end_positions"]
+    if st.is_floating_point() or en.is_floating_point() or st.numel() != en.numel():
+        raise ValueError("start_positions / end_positions must be int64 with one per sequence, got %s %s / %s %s"
+                         % (st.dtype, list(st.shape), en.dtype, list(en.shape)))
+    return torch.stack([st.reshape(-1), en.reshape(-1)])
+
+
+def best_spans(start_logits, end_logits, attention_mask, max_answer_length=30):
+    """run_qa.py's span choice per sequence, as torch ops on the logits' device: the (s, e) with the largest
+    start_logits[s] + end_logits[e] among s <= e < s + max_answer_length, both valid tokens (attention_mask 1;
+    position 0 included, so (0, 0) is the no-answer prediction).  int64 [B, 2]."""
+    B, S = start_logits.shape
+    dev = start_logits.device
+    score = start_logits.float()[:, :, None] + end_logits.float()[:, None, :]
+    ar = torch.arange(S, device=dev)
+    ok = (ar[None, :] >= ar[:, None]) & (ar[None, :] < ar[:, None] + int(max_answer_length))
+    valid = torch.ones(B, S, dtype=torch.bool, device=dev) if attention_mask is None else attention_mask.to(dev) != 0
+    ok = ok[None] & valid[:, :, None] & valid[:, None, :]
+    best = score.masked_fill(~ok, float("-inf")).view(B, S * S).argmax(1)
+    return torch.stack([best // S, best % S], 1)
 
 
 def check_mlm_criterion(criterion, device_loss=False):
@@ -142,6 +188,9 @@ def step_loss(model, criterion=None):
     ValueError), and with no criterion the model's problem-type loss -- single-label cross-entropy when the config has
     no problem_type and more than one label (the step then stages int64 labels, as the reference's Collate yields)."""
     m = _unwrap(model)
+    if _is_qa(m):
+        check_qa_criterion(criterion)
+        return None       # the span loss (csrc/qa_head.cu) has no options
     if _is_mlm(m):
         check_mlm_criterion(criterion, device_loss=True)
         return Loss(L.LOSS_CE, m.config.vocab_size, ignore_index=getattr(criterion, "ignore_index", -100))
@@ -155,6 +204,21 @@ def step_loss(model, criterion=None):
     if pt is None:
         pt = "regression" if m.num_labels == 1 else "single_label_classification"
     return problem_type_loss(pt, m.num_labels)
+
+
+def qa_scores(spans):
+    """(exact match, position-level F1) of int64 [N, 4] rows (pred start, pred end, gold start, gold end): exact match
+    is pred == gold; F1 is that of the predicted and gold position ranges [start, end] (an empty predicted range, end <
+    start, cannot occur: best_spans keeps start <= end), averaged over the rows.  (nan, nan) for no rows."""
+    if spans.shape[0] == 0:
+        return float("nan"), float("nan")
+    p = spans.double()
+    em = float(((spans[:, 0] == spans[:, 2]) & (spans[:, 1] == spans[:, 3])).double().mean())
+    overlap = (torch.minimum(p[:, 1], p[:, 3]) - torch.maximum(p[:, 0], p[:, 2]) + 1).clamp(min=0)
+    prec = overlap / (p[:, 1] - p[:, 0] + 1)
+    rec = overlap / (p[:, 3] - p[:, 2] + 1)
+    f1 = torch.where(overlap > 0, 2 * prec * rec / (prec + rec), torch.zeros_like(overlap))
+    return em, float(f1.mean())
 
 
 class _StagedGraphStep:
@@ -176,6 +240,9 @@ class _StagedGraphStep:
         # per capacity (the count rounded up to 128)
         self.mlm = _is_mlm(self.model)
         self.token = self.token or self.mlm
+        # question answering: the start and end positions of each sequence, two int64 slots per sequence ([2, B])
+        self.qa = _is_qa(self.model)
+        self.ignored_index = seq_len      # HF's ignored index of the span loss (a packed step: the padded length)
         self._cap, self._n_lab = None, 0
         z = lambda *s: torch.zeros(*s, dtype=torch.int64, device=dev)
         self.d_ids, self.d_tt, self.d_mask = z(batch_size, seq_len), z(batch_size, seq_len), z(batch_size, seq_len)
@@ -201,6 +268,8 @@ class _StagedGraphStep:
         """device labels of `rows` sequences for self.loss_fn, and the int64 staging slots they take: int64 [rows]
         class indices, or fp32 [rows] / [rows, C] packed two to a slot"""
         dev = self.eng.dev
+        if self.qa:
+            return torch.zeros(2, rows, dtype=torch.int64, device=dev), 2 * rows
         shape = self.loss_fn.label_shape(rows)
         if not self.loss_fn.float_labels:
             return torch.zeros(shape, dtype=torch.int64, device=dev), rows
@@ -210,6 +279,12 @@ class _StagedGraphStep:
     def _stage_labels(self, hs, lab):
         """host labels -> the label slots `hs` of the pinned staging buffer (fp32 labels bit for bit)"""
         fn = self.loss_fn
+        if self.qa:
+            if lab.is_floating_point() or tuple(lab.shape) != tuple(self.d_lab.shape):
+                raise ValueError("%s was built for int64 start / end positions %s, got %s %s"
+                                 % (type(self).__name__, list(self.d_lab.shape), lab.dtype, list(lab.shape)))
+            hs.copy_(lab.reshape(-1))
+            return
         if self.token:
             self._check_token_labels(lab)
         if self.mlm:
@@ -244,7 +319,9 @@ class _StagedGraphStep:
                              "carry the ignore_index)" % (int(lab[bad].flatten()[0]), fn.C, fn.ignore_index))
 
     def _unstage_labels(self, st):
-        if self.loss_fn.float_labels:
+        if self.qa:
+            self.d_lab.view(-1).copy_(st)
+        elif self.loss_fn.float_labels:
             self.d_lab.view(-1).copy_(st.view(torch.float32)[:self.d_lab.numel()])
         else:
             self.d_lab.copy_(st)
@@ -267,9 +344,15 @@ class _StagedGraphStep:
         self._d_stage_all = torch.zeros_like(self._h_stage_all, device=self.eng.dev)
         self.h_stage, self.d_stage = self._h_stage_all[:n], self._d_stage_all[:n]
 
-    def _mlm_kw(self, train):
-        """the masked-LM forward's arguments: labelled rows only, this batch's capacity, and in training the d_loss
-        scale that makes the loss launch also write d_logits"""
+    def _head_kw(self, train):
+        """the head's forward arguments.  Masked-LM: labelled rows only, this batch's capacity, and in training the
+        d_loss scale that makes the loss launch also write d_logits.  Question answering: that d_loss scale, and a
+        packed step's ignored index."""
+        if self.qa:
+            kw = dict(qa_dloss=self._mlm_dloss) if train else {}
+            if isinstance(self, PackedTrainStep):
+                kw["qa_ignored_index"] = self.ignored_index
+            return kw
         if not self.mlm:
             return {}
         kw = dict(mlm_full=False, ignore_index=self.loss_fn.ignore_index, mlm_capacity=self._cap)
@@ -293,8 +376,8 @@ class _StagedGraphStep:
     def stage(self, batch_data):
         """Host batch (the dict the reference Collate yields, int64 tensors) -> pinned staging -> async H2D."""
         n = self.B * self.S
-        ids, tt, mask, lab = batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"], \
-            batch_data["label"]
+        ids, tt, mask = batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"]
+        lab = qa_positions(batch_data) if self.qa else batch_data["label"]
         if tuple(ids.shape) != (self.B, self.S):
             raise ValueError("%s was built for batch %dx%d, got %s"
                              % (type(self).__name__, self.B, self.S, tuple(ids.shape)))
@@ -377,7 +460,7 @@ class _StagedGraphStep:
         self.deterministic = torch.are_deterministic_algorithms_enabled()
         self.accum_steps = accum_steps
         self.max_grad_norm = float(max_grad_norm) if max_grad_norm else None
-        # the masked-LM loss's gradient scale (1/k under accumulation), read by the cross-entropy launch
+        # the masked-LM and span losses' gradient scale (1/k under accumulation), read by their loss launch
         self._mlm_dloss = torch.full((), 1.0 / accum_steps, dtype=torch.float32, device=self.eng.dev)
         if accum_steps > 1:
             self.eng.ensure_accum()       # outside any capture
@@ -408,13 +491,14 @@ class _StagedGraphStep:
         eng._saved = None
         Bo = eng.head_rows(B, S, packed)
         ws = eng.workspace(B, S, Bo)
-        if self.accum_steps > 1 and not self.mlm:
+        if self.accum_steps > 1 and not (self.mlm or self.qa):
             ws["dloss_logits"].mul_(1.0 / self.accum_steps)     # what an eager loop does with loss / k
         # d(loss)/d(logits) was produced by the loss kernel: the reference's criterion(logits, label) [:169]
         if final and self.max_grad_norm is not None:
             opt._clip_arm(self.max_grad_norm)     # the backward's per-bucket launches become the reduce phase
         eng.start_pass(not final)
-        # (masked-LM: the forward's cross-entropy launch left the labelled rows' d_logits for the backward)
+        # (masked-LM: the forward's cross-entropy launch left the labelled rows' d_logits for the backward; the span
+        # loss's launch left them scaled by 1/k)
         eng._backward_from_dlogits(None if self.mlm else ws["dloss_logits"], B, S, mask, p_h, p_a, p_c, packed)
         eng.end_pass()
         if final:
@@ -443,7 +527,7 @@ class FusedTrainStep(_StagedGraphStep):
     def _body(self):
         self._unstage()
         self._train_body(lambda: self.eng.forward(self.d_ids, self.d_tt, self.d_mask, self.d_lab, training=True,
-                                                  need_backward=True, loss_fn=self.loss_fn, **self._mlm_kw(True)))
+                                                  need_backward=True, loss_fn=self.loss_fn, **self._head_kw(True)))
 
     def __call__(self, batch_data, final=True):
         """batch_data: the dict the reference Collate yields (host int64 tensors; fp32 labels for regression and
@@ -460,8 +544,11 @@ class PackedTrainStep(_StagedGraphStep):
     them, since the bins a batch packs into vary with its lengths."""
 
     def __init__(self, model, optimizer, bins, batch, use_graph=True, accum_steps=1, max_grad_norm=None,
-                 criterion=None, bin_len=128):
+                 criterion=None, bin_len=128, seq_len=None):
+        """seq_len: a question-answering model's padded length before packing, HF's ignored index (None: bin_len)"""
         super().__init__(model, bins, bin_len, use_graph, criterion)
+        if seq_len is not None:
+            self.ignored_index = int(seq_len)
         dev = self.eng.dev
         self.bins, self.batch, self.bin_len = bins, batch, bin_len
         n = bins * bin_len
@@ -485,7 +572,7 @@ class PackedTrainStep(_StagedGraphStep):
 
     def stage(self, packed, label):
         n, hs = self.bins * self.bin_len, self.h_stage
-        want = (self.bins, self.bin_len) if self.token else (self.batch,)
+        want = (self.bins, self.bin_len) if self.token else (2, self.batch) if self.qa else (self.batch,)
         if packed["bins"] != self.bins or packed["input_ids"].shape[1] != self.bin_len or \
                 tuple(label.shape[:len(want)]) != want:
             raise ValueError("PackedTrainStep was built for %d bins of %d tokens / %d sequences"
@@ -506,10 +593,11 @@ class PackedTrainStep(_StagedGraphStep):
         packed = (self.d_pos, self.d_seg, None if self.token else self.d_cls)
         self._train_body(lambda: self.eng.forward(self.d_ids, self.d_tt, None, self.d_lab, training=True,
                                                   need_backward=True, packed=packed, loss_fn=self.loss_fn,
-                                                  **self._mlm_kw(True)))
+                                                  **self._head_kw(True)))
 
     def __call__(self, packed, label, final=True):
-        """label: per sequence [batch], or for a token model pack_batch's "labels" [bins, bin_len]"""
+        """label: per sequence [batch], for a token model pack_batch's "labels" [bins, bin_len], for a
+        question-answering model the int64 [2, batch] start / end positions (trainer.qa_positions of pack_batch's)"""
         self.stage(packed, label)
         self.run_device(final)
         return self.loss_out
@@ -529,12 +617,14 @@ class FusedEvalStep(_StagedGraphStep):
             self.pred_out = torch.zeros(batch_size * seq_len, dtype=torch.int32, device=self.eng.dev)
             self.lab_out = torch.zeros_like(self.pred_out)
         else:
+            if self.qa:
+                shape = (batch_size, seq_len)      # [B, S, 2]: start and end logits
             self.logits_out = torch.zeros(*shape, self.model.num_labels, dtype=torch.float32, device=self.eng.dev)
 
     def _body(self):
         self._unstage()
         logits, loss = self.eng.forward(self.d_ids, self.d_tt, self.d_mask, self.d_lab, training=False,
-                                        need_backward=False, loss_fn=self.loss_fn, **self._mlm_kw(False))
+                                        need_backward=False, loss_fn=self.loss_fn, **self._head_kw(False))
         if self.mlm:
             gb, cap = self.eng.mlm_last, self._cap
             self.pred_out[:cap].copy_(gb["pred"])
@@ -545,7 +635,7 @@ class FusedEvalStep(_StagedGraphStep):
 
     def __call__(self, batch_data):
         """(logits, labels, mean loss); a masked-LM model: (predicted ids, labels, mean loss) of the labelled tokens,
-        in token order"""
+        in token order; a question-answering model: ([B, S, 2] start / end logits, [2, B] positions, mean loss)"""
         self.stage(batch_data)
         self.run_device()
         if self.mlm:
@@ -560,6 +650,8 @@ class Trainer:
         step; it takes precedence over args.lr_scheduler_type"""
         if scheduler is not None and getattr(scheduler, "optimizer", None) is not optimizer:
             raise ValueError("the scheduler must belong to the Trainer's optimizer")
+        if model is not None and _is_qa(model):
+            check_qa_criterion(criterion)
         if getattr(args, "full_determinism", False):
             torch.use_deterministic_algorithms(True)      # as HF's enable_full_determinism does
         self.args = args
@@ -603,7 +695,8 @@ class Trainer:
     def _to_device(self, batch_data):
         dev = _unwrap(self.model)._engine.dev
         out = {}
-        for k in ("label", "input_ids", "token_type_ids", "attention_mask"):
+        keys = ("start_positions", "end_positions") if _is_qa(self.model) else ("label",)
+        for k in keys + ("input_ids", "token_type_ids", "attention_mask"):
             t = batch_data[k]
             if t.is_cuda:
                 out[k] = t
@@ -622,8 +715,14 @@ class Trainer:
         return out
 
     def _forward(self, batch_data):
-        """on_step's model call: (output, device label)"""
+        """on_step's model call: (output, device label); a question-answering model's label is the int64 [2, B]
+        start / end positions"""
         d = self._to_device(batch_data)
+        if _is_qa(self.model):
+            output = self.model(input_ids=d["input_ids"], token_type_ids=d["token_type_ids"],
+                                attention_mask=d["attention_mask"], start_positions=d["start_positions"],
+                                end_positions=d["end_positions"])
+            return output, qa_positions(d)
         label = d["label"]
         # a token model with a criterion leaves the loss to it: its in-model CrossEntropyLoss() would not know the
         # criterion's ignore_index
@@ -635,14 +734,21 @@ class Trainer:
 
     def on_step(self, batch_data):
         output, label = self._forward(batch_data)
-        logits = output.logits
-        return logits, label
+        return self._logits(output), label
+
+    def _logits(self, output):
+        """the output's logits; a question-answering model's start and end logits stacked as [B, S, 2]"""
+        if _is_qa(self.model):
+            return torch.stack([output.start_logits, output.end_logits], -1)
+        return output.logits
 
     def problem_type(self, label):
         """the model's config.problem_type; when None, HF's rule applied to `label` (stored on the config, as the
         model's first labelled forward does)"""
         if _is_mlm(self.model):
             return MLM_PROBLEM_TYPE
+        if _is_qa(self.model):
+            return QA_PROBLEM_TYPE         # HF's QA model never reads or sets config.problem_type
         if _is_token(self.model):
             return TOKEN_PROBLEM_TYPE      # HF's token model never reads or sets config.problem_type
         cfg = _unwrap(self.model).config
@@ -657,6 +763,11 @@ class Trainer:
             if model_loss is None:
                 raise ValueError("Trainer has no criterion and the model returned no loss")
             return model_loss
+        if _is_qa(self.model):
+            check_qa_criterion(self.criterion)      # a plain CrossEntropyLoss() stands for the in-model span loss
+            if model_loss is None:
+                raise ValueError("a BertForQuestionAnswering's loss is its own: the model returned none")
+            return model_loss
         if _is_mlm(self.model):
             check_mlm_criterion(self.criterion)
             return self.criterion(logits.reshape(-1, logits.shape[-1]), label.reshape(-1))
@@ -670,7 +781,7 @@ class Trainer:
 
     def _eager_loss(self, batch_data):
         """the eager loops' forward + loss: on_step and the criterion, or with no criterion the model's own loss"""
-        if self.criterion is None:
+        if self.criterion is None or _is_qa(self.model):
             output, _label = self._forward(batch_data)
             return output[0]
         logits, label = self.on_step(batch_data)
@@ -681,8 +792,8 @@ class Trainer:
         replay per batch instead of ~100 eager launches), else the eager call"""
         if not getattr(self.args, "fused", True) or batch_data["input_ids"].is_cuda:
             output, label = self._forward(batch_data)
-            return output.logits, label, output.loss
-        self.problem_type(batch_data["label"])
+            return self._logits(output), label, output.loss
+        self.problem_type(batch_data.get("label"))
         B, S = batch_data["input_ids"].shape
         m = _unwrap(self.model)
         # a token model's staged labels are checked against its loss's ignore_index: the criterion's
@@ -728,30 +839,37 @@ class Trainer:
         clip = self._max_grad_norm()
         first, final = self._micro == 0, self._micro >= k - 1
         self._micro = 0 if final else self._micro + 1
+        qa = _is_qa(self.model)
         if getattr(self.args, "fused", True) and getattr(self.args, "pack", False) and \
                 batch_data["input_ids"].shape[1] <= MAX_BIN and not batch_data["input_ids"].is_cuda:
             bin_len = bin_length(batch_data["attention_mask"], batch_data["input_ids"].shape[1])
             token = _is_token(self.model) or _is_mlm(self.model)
+            qa_kw = dict(start_positions=batch_data["start_positions"],
+                         end_positions=batch_data["end_positions"]) if qa else {}
             packed = pack_batch(batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"],
                                 bin_len, labels=batch_data["label"] if token else None,
-                                ignore_index=self._ignore_index())
+                                ignore_index=self._ignore_index(), **qa_kw)
             key = (packed["bins"], batch_data["input_ids"].shape[0], bin_len,
                    torch.are_deterministic_algorithms_enabled())
-            lkey = self._captured_loss_key(batch_data["label"])
+            if qa:
+                key += (packed["seq_len"],)        # the span loss's ignored index is part of the captured step
+            lkey = self._captured_loss_key(batch_data.get("label"))
             if key not in self._packed or (self._packed[key].accum_steps, self._packed[key].max_grad_norm,
                                            self._packed[key].loss_key) != (k, clip, lkey):
                 if len(self._packed) >= 16:           # bound the graph cache: drop the oldest entry
                     self._packed.pop(next(iter(self._packed)))
                 self._packed[key] = PackedTrainStep(self.model, self.optimizer, key[0], key[1], accum_steps=k,
-                                                    max_grad_norm=clip, criterion=self.criterion, bin_len=bin_len)
+                                                    max_grad_norm=clip, criterion=self.criterion, bin_len=bin_len,
+                                                    seq_len=packed["seq_len"] if qa else None)
                 self._packed[key].loss_key = lkey
             self.model.train()
-            loss = self._packed[key](packed, packed["labels"] if token else batch_data["label"], final)
+            label = packed["labels"] if token else qa_positions(packed) if qa else batch_data["label"]
+            loss = self._packed[key](packed, label, final)
             if final:
                 self._scheduler_step()      # after the replay: the next stage() reads the new lr
         elif getattr(self.args, "fused", True):
             B, S = batch_data["input_ids"].shape
-            lkey = self._captured_loss_key(batch_data["label"])
+            lkey = self._captured_loss_key(batch_data.get("label"))
             det = torch.are_deterministic_algorithms_enabled()
             if self._fused is None or (self._fused.B, self._fused.S, self._fused.accum_steps, self._fused.max_grad_norm,
                                        self._fused.loss_key, self._fused.deterministic) != (B, S, k, clip, lkey, det):
@@ -1008,6 +1126,9 @@ class Trainer:
         self.model.eval()
         if _is_mlm(self.model):
             return self._dev_mlm(dev_loader)
+        if _is_qa(self.model):
+            loss_total, spans = self._qa_spans(dev_loader)
+            return loss_total, qa_scores(spans)[0]
         correct_total = 0
         num_total = 0
         loss_total = 0.
@@ -1073,6 +1194,25 @@ class Trainer:
             total = c[1] if total is None else total + c[1]
         return loss_total, float(correct / total)
 
+    def _qa_spans(self, loader):
+        """(summed rank-mean loss, int64 [N, 4] rows (pred start, pred end, gold start, gold end)) of a
+        question-answering model over the gathered sequences whose gold span is not ignored.  Gold is HF's
+        clamp(0, S); the prediction is best_spans over the sequence's valid tokens."""
+        max_len = int(getattr(self.args, "max_answer_length", 30))
+        loss_total, rows = 0., []
+        with torch.no_grad():
+            for batch_data in loader:
+                logits, pos, loss = self._eval_forward(batch_data)
+                loss_total += self.loss_reduce(loss)
+                S = logits.shape[1]
+                mask = batch_data["attention_mask"].to(logits.device)
+                pred = best_spans(logits[..., 0], logits[..., 1], mask, max_len)
+                gold = pos.to(logits.device).t().clamp(0, S)
+                pred, gold = self.output_reduce(pred.contiguous(), gold.contiguous())
+                keep = (gold != S).all(1)
+                rows.append(torch.cat([pred, gold], 1)[keep].cpu())
+        return loss_total, torch.cat(rows) if rows else torch.zeros(0, 4, dtype=torch.int64)
+
     def test(self, model, test_loader, labels):
         """sklearn's classification_report over the gathered rows: of the argmax class (single-label; a token model's
         over the tokens whose label is not the ignore index) or of the
@@ -1080,6 +1220,14 @@ class Trainer:
         if _is_mlm(model):
             raise ValueError("test() prints a classification report, which is not useful over a vocabulary: use dev() "
                              "for the masked-token accuracy")
+        if _is_qa(model):
+            # a question-answering model: exact match and position-level F1 of the predicted spans (`labels` unused)
+            self.model = model
+            self.model.eval()
+            _loss, spans = self._qa_spans(test_loader)
+            em, f1 = qa_scores(spans)
+            print("【test】 exact match：{:.4f} f1：{:.4f}".format(em, f1))
+            return em, f1
         self.model = model
         self.model.eval()
         preds = []
