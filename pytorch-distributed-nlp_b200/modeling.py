@@ -118,6 +118,11 @@ class QuestionAnsweringModelOutput:
     __len__ = SequenceClassifierOutput.__len__
 
 
+class MultipleChoiceModelOutput(SequenceClassifierOutput):
+    """HF's MultipleChoiceModelOutput, tuple-like: ``(loss, logits)`` with logits [batch, num_choices], the loss left
+    out when it is None."""
+
+
 def _round8(n):
     return (n + 7) // 8 * 8
 
@@ -127,8 +132,9 @@ def vocab_pad(vocab_size):
     return (vocab_size + 63) // 64 * 64
 
 
-HEAD_KINDS = ("sequence", "token", "mlm", "question_answering")   # BertForSequenceClassification's pooler +
-    # classifier, a classifier per token, BertForMaskedLM's cls.predictions, or BertForQuestionAnswering's qa_outputs
+HEAD_KINDS = ("sequence", "token", "mlm", "question_answering", "multiple_choice")   # BertForSequenceClassification's
+    # pooler + classifier, a classifier per token, BertForMaskedLM's cls.predictions, BertForQuestionAnswering's
+    # qa_outputs, or BertForMultipleChoice's pooler + one-row classifier
 MLM_TIED = {"cls.predictions.decoder.weight": "bert.embeddings.word_embeddings.weight",
             "cls.predictions.decoder.bias": "cls.predictions.bias"}    # HF's tied state-dict keys of the MLM head
 TOKEN_HEAD_MAX_LABELS = 64             # b2_token_head_fwd's bound
@@ -147,7 +153,8 @@ class _Layout:
     "mlm" (BertForMaskedLM): the tail is cls.predictions (its decoder is the word-embedding table), and the word table
     and cls.predictions.bias reserve vocab_pad(V) rows / entries, so the vocabulary projection is one GEMM with a
     multiple of 64 columns; the extra rows stay zero and lie outside every parameter view.  head "question_answering"
-    (BertForQuestionAnswering): the tail is qa_outputs [2, H] / [2] alone, like the token head's classifier."""
+    (BertForQuestionAnswering): the tail is qa_outputs [2, H] / [2] alone, like the token head's classifier.  head
+    "multiple_choice" (BertForMultipleChoice): the sequence layout with a one-row classifier [1, H] / [1]."""
 
     def __init__(self, cfg, head="sequence"):
         if head not in HEAD_KINDS:
@@ -197,7 +204,7 @@ class _Layout:
             add(p + "output.LayerNorm.bias", (H,))
             self.buckets.append((b0, off, "layer%d" % l))
         b0 = off
-        if head == "sequence":
+        if head in ("sequence", "multiple_choice"):
             add("bert.pooler.dense.weight", (H, H))
             add("bert.pooler.dense.bias", (H,))
         if mlm:
@@ -210,8 +217,9 @@ class _Layout:
             add("qa_outputs.weight", (cfg.num_labels, H))
             add("qa_outputs.bias", (cfg.num_labels,))
         else:
-            add("classifier.weight", (cfg.num_labels, H))
-            add("classifier.bias", (cfg.num_labels,))
+            C = 1 if head == "multiple_choice" else cfg.num_labels     # HF's multiple-choice classifier ignores it
+            add("classifier.weight", (C, H))
+            add("classifier.bias", (C,))
         if L_ > 0:
             lb, _le, lbl = self.buckets[-1]
             self.buckets[-1] = (lb, off, lbl + "+head")
@@ -224,9 +232,8 @@ class _Layout:
         return self.entries[name][0]
 
 
-# HF named_parameters() order (201 tensors for 12 layers, 199 without the pooler, 202 for the MLM head, 199 for the QA
-# head); differs from
-# the flat order only inside attention.self
+# HF named_parameters() order (201 tensors for 12 layers, as for the multiple-choice head, 199 without the pooler, 202 for
+# the MLM head, 199 for the QA head); differs from the flat order only inside attention.self
 def _hf_order(cfg, head="sequence"):
     names = ["bert.embeddings.word_embeddings.weight", "bert.embeddings.position_embeddings.weight",
              "bert.embeddings.token_type_embeddings.weight", "bert.embeddings.LayerNorm.weight",
@@ -236,7 +243,7 @@ def _hf_order(cfg, head="sequence"):
         for m in ("attention.self.query", "attention.self.key", "attention.self.value", "attention.output.dense",
                   "attention.output.LayerNorm", "intermediate.dense", "output.dense", "output.LayerNorm"):
             names += [p + m + ".weight", p + m + ".bias"]
-    if head == "sequence":
+    if head in ("sequence", "multiple_choice"):
         names += ["bert.pooler.dense.weight", "bert.pooler.dense.bias"]
     if head == "mlm":
         return names + ["cls.predictions.bias", "cls.predictions.transform.dense.weight",
@@ -768,6 +775,79 @@ class BertForQuestionAnswering(_BertClassifier):
         return QuestionAnsweringModelOutput(loss=loss, start_logits=start, end_logits=end)
 
 
+def check_choice_labels(labels, batch):
+    """multiple-choice labels: int64 [batch], one choice index per example (-100: ignored)"""
+    if not isinstance(labels, torch.Tensor) or labels.dtype != torch.int64:
+        raise TypeError("multiple-choice labels are int64 choice indices, got %s"
+                        % getattr(labels, "dtype", type(labels).__name__))
+    if tuple(labels.shape) != (batch,):
+        raise ValueError("multiple-choice labels must be [%d] (one choice index per example), got %s"
+                         % (batch, list(labels.shape)))
+
+
+class BertForMultipleChoice(_BertClassifier):
+    """HF's BertForMultipleChoice: the B·N choice sequences of a [B, N, S] batch run flattened through the sequence
+    model's encoder, pooler, dropout (config.classifier_dropout, else hidden_dropout_prob) and a Linear(H, 1) -- the
+    sequence head's kernels with one label -- and the [B·N, 1] logits are read as [B, N].  With labels (int64 [B]) the
+    loss is HF's ``CrossEntropyLoss()`` over the choices (-100 ignored).  The classifier has one row whatever
+    config.num_labels says, and config.problem_type is neither read nor set, as in HF.  from_pretrained loads the
+    encoder and pooler and ignores a pre-training checkpoint's cls.*; a classifier of another shape (a sequence
+    classifier's [num_labels, H]) raises a size mismatch, as transformers does without ignore_mismatched_sizes."""
+    _head = "multiple_choice"
+    _config_extra = {"architectures": ["BertForMultipleChoice"]}
+
+    def __init__(self, config):
+        super().__init__(config)
+        self._ce = {}            # choices -> the in-model CrossEntropyLoss() over them
+
+    def forward(self, input_ids=None, token_type_ids=None, attention_mask=None, labels=None, position_ids=None,
+                segments=None, cls_index=None, **unused):
+        """Padded: input_ids / token_type_ids / attention_mask int64 [B, N, S].  `position_ids` / `segments` /
+        `cls_index` (all three or none): the rows of `input_ids` are the bins of `packing.pack_batch` over the B·N
+        choice sequences, and cls_index [B, N] gives the number of choices.  Returns fp32 logits [B, N]."""
+        if input_ids is None:
+            raise ValueError("input_ids is required")
+        packed = None
+        if segments is not None or cls_index is not None or position_ids is not None:
+            if position_ids is None or segments is None or cls_index is None:
+                raise ValueError("a packed batch needs position_ids, segments and cls_index together")
+            if cls_index.dim() != 2:
+                raise ValueError("cls_index of a packed multiple-choice batch must be [batch, num_choices], got %s"
+                                 % list(cls_index.shape))
+            B, N = cls_index.shape
+            packed = (position_ids, segments, cls_index)
+        else:
+            if input_ids.dim() != 3:
+                raise ValueError("input_ids must be [batch, num_choices, seq], got %s" % list(input_ids.shape))
+            B, N, S = input_ids.shape
+            for t, nm in ((token_type_ids, "token_type_ids"), (attention_mask, "attention_mask")):
+                if t is not None and tuple(t.shape) != (B, N, S):
+                    raise ValueError("%s must have input_ids' shape %s, got %s" % (nm, [B, N, S], list(t.shape)))
+            flat = lambda t: None if t is None else t.reshape(B * N, S)
+            input_ids, token_type_ids, attention_mask = flat(input_ids), flat(token_type_ids), flat(attention_mask)
+        if labels is not None:
+            check_choice_labels(labels, B)
+        if self._engine is None:
+            raise RuntimeError("BertForMultipleChoice (b200) only runs on CUDA: call model.cuda() first; there is no "
+                               "CPU path.")
+        kw = {"loss_fn": self.choice_loss(N)}
+        if torch.is_grad_enabled() and self.training:
+            anchor = self._params_by_name[self._anchor]
+            logits, loss = _StepFn.apply(anchor, self, input_ids, token_type_ids, attention_mask, labels, packed, kw)
+            loss = loss if labels is not None else None
+        else:
+            logits, loss = self._engine.forward(input_ids, token_type_ids, attention_mask, labels,
+                                                training=self.training, need_backward=False, packed=packed, **kw)
+            logits, loss = logits.clone(), None if loss is None else loss.clone()
+        return MultipleChoiceModelOutput(loss=loss, logits=logits.view(B, N))
+
+    def choice_loss(self, num_choices):
+        """HF's in-model loss: CrossEntropyLoss() over the num_choices logits of each example"""
+        if num_choices not in self._ce:
+            self._ce[num_choices] = Loss(L.LOSS_CE, num_choices)
+        return self._ce[num_choices]
+
+
 class _LocalTransport:
     """The facts the optimizer's step schedule (optim._FusedOptimizer: bucket_ready, step, the clip phases) needs about
     where gradients and weights live, on one GPU.  DistributedDataParallel answers the same questions for a peer group
@@ -829,6 +909,11 @@ class _Engine:
         self.dev = model._flat.device
         self.H, self.I = cfg.hidden_size, cfg.intermediate_size
         self.heads, self.nl, self.C = cfg.num_attention_heads, cfg.num_hidden_layers, cfg.num_labels
+        # the multiple-choice head is the sequence head with one label over the B·N choice sequences; its loss reads
+        # the [B·N, 1] logits as [B, N]
+        self.mc = self.lay.head == "multiple_choice"
+        if self.mc:
+            self.C = 1
         self.p_hidden = float(cfg.hidden_dropout_prob)
         self.p_attn = float(cfg.attention_probs_dropout_prob)
         cd = getattr(cfg, "classifier_dropout", None)
@@ -1107,6 +1192,8 @@ class _Engine:
         rows of `input_ids` are then S-token bins produced by packing.pack_batch (S a multiple of 128, at most 512),
         not sequences.
         loss_fn: the losses.Loss of `labels` (None: the model's problem-type loss, HF's in-model loss).
+        Multiple-choice head: the rows of `input_ids` are the B·N choice sequences, example-major; loss_fn is
+        required, its num_labels is N, and `labels` are int64 [B].
         Masked-LM head: `labels` int64 [B, S] with `ignore_index`; the loss runs on the labelled rows only, in a
         capacity of mlm_capacity rows (None: their count rounded up to 128, read from the device); mlm_full: also
         the logits of every row (returned as [B, S, V]; else None); mlm_dloss: a device scalar d(objective)/d(loss)
@@ -1150,10 +1237,17 @@ class _Engine:
                     raise RuntimeError("%s is on %s, model on %s" % (nm, t.device, self.dev))
                 if t is not labels and t.dtype != torch.int64:
                     raise TypeError("%s must be int64 (as the reference Collate produces)" % nm)
+        loss_rows = Bo
         if labels is not None and not self.mlm and not self.qa:
-            if loss_fn is None:
+            if self.mc:
+                # loss_fn's labels are the choices: B examples of N choice logits each
+                if loss_fn is None or Bo % loss_fn.C != 0:
+                    raise ValueError("multiple-choice loss: need the loss over N choices of %d choice sequences"
+                                     % Bo)
+                loss_rows = Bo // loss_fn.C
+            elif loss_fn is None:
                 loss_fn = self.model._problem_type_loss(labels)
-            labels = loss_fn.device_labels(labels, Bo)
+            labels = loss_fn.device_labels(labels, loss_rows)
         ws = self.workspace(B, S, Bo)
         M = B * S
         s = self.stream()
@@ -1233,7 +1327,7 @@ class _Engine:
             loss = self._qa_loss(ws, M, labels, S, None if packed is None else (segs, cls_rows), need_backward,
                                  qa_ignored_index, qa_dloss)
         elif labels is not None:
-            loss_fn.launch(ws["logits"].data_ptr(), labels, Bo, ws["loss"].data_ptr(),
+            loss_fn.launch(ws["logits"].data_ptr(), labels, loss_rows, ws["loss"].data_ptr(),
                            ws["dloss_logits"].data_ptr() if need_backward else None, s)
             loss = ws["loss"]
         if need_backward:

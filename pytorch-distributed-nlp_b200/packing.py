@@ -20,9 +20,9 @@ MAX_BIN = 512      # the attention kernels' longest sequence
 
 
 def bin_length(attention_mask, seq_len):
-    """the bin length pack_batch should use for a [B, seq_len] batch: the smallest multiple of BIN that holds its
-    longest valid sequence (attention_mask None: every token is valid)"""
-    longest = int(attention_mask.ne(0).sum(1).max()) if attention_mask is not None else seq_len
+    """the bin length pack_batch should use for a [B, seq_len] (or multiple-choice [B, N, seq_len]) batch: the
+    smallest multiple of BIN that holds its longest valid sequence (attention_mask None: every token is valid)"""
+    longest = int(attention_mask.ne(0).sum(-1).max()) if attention_mask is not None else seq_len
     return BIN * max(1, -(-longest // BIN))
 
 
@@ -44,9 +44,14 @@ def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN, labels=No
                                                  index.  A position in [length, S) targets a padding token, which
                                                  packing drops: ValueError.  Negative positions and positions >= S
                                                  pass through (the span loss clamps them as HF does).
-    NB <= B; a sequence longer than bin_len is not supported (the reference truncates to max_seq_len = 128)."""
+    NB <= B; a sequence longer than bin_len is not supported (the reference truncates to max_seq_len = 128).
+    A multiple-choice batch, int64 [B, N, S] tensors with `labels` int64 [B] (one choice index per example): the B·N
+    choice sequences are packed as above, example-major; cls_index and lengths come back as [B, N] and the labels
+    pass through as "labels"."""
+    if input_ids.dim() == 3:
+        return _pack_choices(input_ids, token_type_ids, attention_mask, bin_len, labels)
     if input_ids.dim() != 2:
-        raise ValueError("input_ids must be [batch, seq]")
+        raise ValueError("input_ids must be [batch, seq] (or [batch, num_choices, seq])")
     B, S = input_ids.shape
     ids_np = input_ids.numpy()
     mask_np = (attention_mask.numpy() != 0) if attention_mask is not None else np.ones((B, S), dtype=bool)
@@ -128,4 +133,22 @@ def pack_batch(input_ids, token_type_ids, attention_mask, bin_len=BIN, labels=No
         out["labels"] = t(lab).view(NB, bin_len)
     if qa is not None:
         out["start_positions"], out["end_positions"], out["seq_len"] = qa[0], qa[1], S
+    return out
+
+
+def _pack_choices(input_ids, token_type_ids, attention_mask, bin_len, labels):
+    """pack_batch of a [B, N, S] multiple-choice batch"""
+    B, N, S = input_ids.shape
+    for t, nm in ((token_type_ids, "token_type_ids"), (attention_mask, "attention_mask")):
+        if t is not None and tuple(t.shape) != (B, N, S):
+            raise ValueError("pack_batch: %s must have input_ids' shape %s, got %s" % (nm, [B, N, S], list(t.shape)))
+    if labels is not None and (labels.is_floating_point() or tuple(labels.shape) != (B,)):
+        raise ValueError("pack_batch: multiple-choice labels must be int64 [%d] (one choice index per example), got "
+                         "%s %s" % (B, labels.dtype, list(labels.shape)))
+    flat = lambda t: None if t is None else t.reshape(B * N, S)
+    out = pack_batch(flat(input_ids), flat(token_type_ids), flat(attention_mask), bin_len)
+    out["cls_index"] = out["cls_index"].view(B, N)
+    out["lengths"] = out["lengths"].view(B, N)
+    if labels is not None:
+        out["labels"] = labels
     return out

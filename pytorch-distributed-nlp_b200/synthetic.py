@@ -80,6 +80,39 @@ def synthetic_qa_batch(cfg, batch, seq, seed, padded=False, no_answer=0.2, ignor
             "end_positions": end}
 
 
+def synthetic_mc_batch(cfg, batch, choices, seq, seed, padded=False):
+    """A SWAG-shaped batch for BertForMultipleChoice, from generator seed `seed`: each of the `choices` rows of an
+    example is [CLS] (101), the example's context (token type 0), [SEP] (102), that choice's ending and [SEP] (token
+    type 1).  Every choice of an example shares its context.  `padded` draws the context length ~ U{2..seq/2 - 2} per
+    example and each ending's length ~ U{1..seq - context - 3} per choice, and zeroes ids / mask / token types beyond
+    them; otherwise the endings fill every row.  Returns input_ids, token_type_ids, attention_mask (int64 [batch,
+    choices, seq]) and label (int64 [batch], the right choice)."""
+    if seq < 8:
+        raise ValueError("synthetic_mc_batch: need seq >= 8, got %d" % seq)
+    g = torch.Generator().manual_seed(seed)
+    V = cfg.vocab_size
+    ids = torch.randint(0, V, (batch, choices, seq), generator=g, dtype=torch.int64)
+    ctx = torch.randint(2, seq // 2 - 1, (batch,), generator=g)
+    ctx_rows = ids[:, 0, :].clone()                  # one context per example, copied into each of its choices
+    u = torch.rand(batch, choices, generator=g)
+    lab = torch.randint(0, choices, (batch,), generator=g, dtype=torch.int64)
+    tt = torch.zeros(batch, choices, seq, dtype=torch.int64)
+    lens = torch.zeros(batch, choices, dtype=torch.int64)
+    cls_id, sep_id = min(101, V - 1), min(102, V - 1)
+    for b in range(batch):
+        c = int(ctx[b])
+        for k in range(choices):
+            room = seq - c - 3
+            end = 1 + int(u[b, k] * room) if padded else room
+            n = c + end + 3
+            ids[b, k, 1:1 + c] = ctx_rows[b, 1:1 + c]
+            ids[b, k, 0], ids[b, k, 1 + c], ids[b, k, n - 1] = cls_id, sep_id, sep_id
+            tt[b, k, 2 + c:n] = 1
+            lens[b, k] = n
+    mask = (torch.arange(seq)[None, None] < lens[..., None]).to(torch.int64)
+    return {"input_ids": ids * mask, "token_type_ids": tt * mask, "attention_mask": mask, "label": lab}
+
+
 # Token-length histogram of the reference's own data (data/train.json, 40 133 rows): characters of the text without the
 # segmentation blanks (BertTokenizer splits Chinese text into single characters) + [CLS] + [SEP], capped at
 # max_seq_len = 128 (multi-gpu-distributed-cls.py:66-98).  (length, rows); mean 19.8 tokens -- the reference pads all of

@@ -23,6 +23,7 @@ import time
 
 import numpy as np
 import torch
+import torch.nn as nn
 
 from .ddp import DistributedDataParallel
 from . import _lib as L
@@ -95,9 +96,33 @@ def _is_qa(model):
     return _unwrap(model)._layout.head == "question_answering"
 
 
+def _is_mc(model):
+    """a BertForMultipleChoice (or a wrapper of one): [B, N, S] inputs, one logit per choice"""
+    return _unwrap(model)._layout.head == "multiple_choice"
+
+
+def _choices(batch_data):
+    """the number of choices of a multiple-choice batch: the middle axis of its [B, N, S] input_ids"""
+    ids = batch_data["input_ids"]
+    if ids.dim() != 3:
+        raise ValueError("a multiple-choice batch's input_ids are [batch, num_choices, seq], got %s" % list(ids.shape))
+    return int(ids.shape[1])
+
+
 TOKEN_PROBLEM_TYPE = "token_classification"     # what Trainer.problem_type reports for a token model (not stored)
 MLM_PROBLEM_TYPE = "masked_lm"                  # ... and for a masked-LM model (not stored)
 QA_PROBLEM_TYPE = "question_answering"          # ... and for a question-answering model (not stored)
+MC_PROBLEM_TYPE = "multiple_choice"             # ... and for a multiple-choice model (not stored)
+
+
+def check_mc_criterion(criterion):
+    """A multiple-choice model's loss is a cross-entropy over each example's N choice logits (HF's CrossEntropyLoss
+    over logits.view(-1, N)); MSELoss / BCEWithLogitsLoss would need float targets per choice, which the multiple-choice
+    batch does not carry.  Raises ValueError for those two."""
+    if isinstance(criterion, (nn.MSELoss, nn.BCEWithLogitsLoss)):
+        raise ValueError("%s does not apply to a multiple-choice model: its labels are one int64 choice index per "
+                         "example (-100 on ignored ones) and its loss is CrossEntropyLoss over the [batch, num_choices] "
+                         "logits, as HF's BertForMultipleChoice computes it" % type(criterion).__name__)
 
 
 def check_qa_criterion(criterion):
@@ -183,11 +208,17 @@ def rotate_checkpoints(output_dir, save_total_limit):
         shutil.rmtree(path)
 
 
-def step_loss(model, criterion=None):
+def step_loss(model, criterion=None, choices=None):
     """The losses.Loss a captured step computes: `criterion`'s when it is one the device kernel reproduces (else
     ValueError), and with no criterion the model's problem-type loss -- single-label cross-entropy when the config has
-    no problem_type and more than one label (the step then stages int64 labels, as the reference's Collate yields)."""
+    no problem_type and more than one label (the step then stages int64 labels, as the reference's Collate yields).
+    A multiple-choice model's loss runs over `choices` logits per example."""
     m = _unwrap(model)
+    if _is_mc(m):
+        check_mc_criterion(criterion)
+        if criterion is None:
+            return m.choice_loss(choices)
+        return loss_from_criterion(criterion, choices, m._engine.dev if m._engine is not None else None)
     if _is_qa(m):
         check_qa_criterion(criterion)
         return None       # the span loss (csrc/qa_head.cu) has no options
@@ -225,15 +256,26 @@ class _StagedGraphStep:
     """Shared plumbing of the graph-captured steps: one pinned staging buffer for the four host tensors of a batch, one
     async H2D copy, two eager warm-up passes (first launches set kernel attributes), then capture + replay."""
 
-    def __init__(self, model, batch_size, seq_len, use_graph=True, criterion=None):
+    def __init__(self, model, batch_size, seq_len, use_graph=True, criterion=None, choices=None):
+        """choices: a multiple-choice model's N; its steps take [batch_size, N, seq_len] batches and run their
+        batch_size x N choice sequences as rows"""
         self.wrapper = model if isinstance(model, DistributedDataParallel) else None
         self.model = _unwrap(model)
         self.eng = self.model._engine
         if self.eng is None:
             raise RuntimeError("%s: model must be on CUDA" % type(self).__name__)
         dev = self.eng.dev
+        self.mc = _is_mc(self.model)
+        if self.mc != (choices is not None):
+            raise ValueError("%s: choices=N is %s" % (type(self).__name__, "required for a multiple-choice model"
+                                                       if self.mc else "for multiple-choice models only"))
+        self.N = choices
+        self.examples = batch_size            # labelled examples (sequences, or multiple-choice examples)
+        self.batch_shape = (batch_size, seq_len) if not self.mc else (batch_size, choices, seq_len)
+        if self.mc and not isinstance(self, PackedTrainStep):
+            batch_size *= choices             # one row per choice sequence
         self.B, self.S = batch_size, seq_len
-        self.loss_fn = step_loss(self.model, criterion)
+        self.loss_fn = step_loss(self.model, criterion, choices)
         self.criterion_key = criterion_key(criterion)
         self.token = _is_token(self.model)     # labels per token row: B * S int64 slots
         # masked-LM: the head runs on the labelled rows; the host counts them while staging, and the graphs are kept
@@ -246,7 +288,7 @@ class _StagedGraphStep:
         self._cap, self._n_lab = None, 0
         z = lambda *s: torch.zeros(*s, dtype=torch.int64, device=dev)
         self.d_ids, self.d_tt, self.d_mask = z(batch_size, seq_len), z(batch_size, seq_len), z(batch_size, seq_len)
-        self.d_lab, lab_slots = self._label_buffer(batch_size * seq_len if self.token else batch_size)
+        self.d_lab, lab_slots = self._label_buffer(batch_size * seq_len if self.token else self.examples)
         self._alloc_stage(3 * batch_size * seq_len + lab_slots)
         self.loss_out = torch.zeros((), dtype=torch.float32, device=dev)
         self.h_loss = torch.zeros((), dtype=torch.float32).pin_memory()
@@ -285,7 +327,7 @@ class _StagedGraphStep:
                                  % (type(self).__name__, list(self.d_lab.shape), lab.dtype, list(lab.shape)))
             hs.copy_(lab.reshape(-1))
             return
-        if self.token:
+        if self.token or self.mc:
             self._check_token_labels(lab)
         if self.mlm:
             n = int((lab != fn.ignore_index).sum())
@@ -306,17 +348,20 @@ class _StagedGraphStep:
 
     def _check_token_labels(self, lab):
         """host token labels: int64, one per staged row, each a class index or the loss's ignore_index (the loss
-        kernel traps on anything else; padding must carry the ignore index, as HF's tagging collators put there)"""
+        kernel traps on anything else; padding must carry the ignore index, as HF's tagging collators put there).
+        A multiple-choice step's labels likewise: one choice index per example."""
+        what = "choice" if self.mc else "token"
         if lab.is_floating_point():
-            raise TypeError("token labels are int64 class indices (CrossEntropyLoss), got %s" % lab.dtype)
-        if lab.numel() != self.d_lab.numel():
-            raise ValueError("%s was built for %d token labels, got %s" % (type(self).__name__, self.d_lab.numel(),
-                                                                           list(lab.shape)))
+            raise TypeError("%s labels are int64 class indices (CrossEntropyLoss), got %s" % (what, lab.dtype))
+        if lab.numel() != self.d_lab.numel() or (self.mc and lab.dim() != 1):
+            raise ValueError("%s was built for %d %s labels, got %s" % (type(self).__name__, self.d_lab.numel(), what,
+                                                                        list(lab.shape)))
         fn = self.loss_fn
         bad = (lab != fn.ignore_index) & ((lab < 0) | (lab >= fn.C))
         if bool(bad.any()):
-            raise ValueError("token label %d is outside [0, %d) and is not the ignore_index %d (padding positions must "
-                             "carry the ignore_index)" % (int(lab[bad].flatten()[0]), fn.C, fn.ignore_index))
+            raise ValueError("%s label %d is outside [0, %d) and is not the ignore_index %d%s"
+                             % (what, int(lab[bad].flatten()[0]), fn.C, fn.ignore_index,
+                                "" if self.mc else " (padding positions must carry the ignore_index)"))
 
     def _unstage_labels(self, st):
         if self.qa:
@@ -378,9 +423,9 @@ class _StagedGraphStep:
         n = self.B * self.S
         ids, tt, mask = batch_data["input_ids"], batch_data["token_type_ids"], batch_data["attention_mask"]
         lab = qa_positions(batch_data) if self.qa else batch_data["label"]
-        if tuple(ids.shape) != (self.B, self.S):
-            raise ValueError("%s was built for batch %dx%d, got %s"
-                             % (type(self).__name__, self.B, self.S, tuple(ids.shape)))
+        if tuple(ids.shape) != self.batch_shape:
+            raise ValueError("%s was built for batch %s, got %s"
+                             % (type(self).__name__, "x".join(map(str, self.batch_shape)), tuple(ids.shape)))
         hs = self.h_stage
         if self._h2d_done is not None:
             self._h2d_done.synchronize()  # previous step's copy out of the pinned staging buffer has drained
@@ -519,8 +564,8 @@ class FusedTrainStep(_StagedGraphStep):
     clip the gradient's 2-norm before the update (see clip_grad_norm_); the norm is left in optimizer._clip_buf."""
 
     def __init__(self, model, optimizer, batch_size, seq_len, use_graph=True, accum_steps=1, max_grad_norm=None,
-                 criterion=None):
-        super().__init__(model, batch_size, seq_len, use_graph, criterion)
+                 criterion=None, choices=None):
+        super().__init__(model, batch_size, seq_len, use_graph, criterion, choices)
         self._arm(optimizer, accum_steps, max_grad_norm)
 
     # the step body, expressed only with stream-ordered work (capturable)
@@ -544,20 +589,22 @@ class PackedTrainStep(_StagedGraphStep):
     them, since the bins a batch packs into vary with its lengths."""
 
     def __init__(self, model, optimizer, bins, batch, use_graph=True, accum_steps=1, max_grad_norm=None,
-                 criterion=None, bin_len=128, seq_len=None):
-        """seq_len: a question-answering model's padded length before packing, HF's ignored index (None: bin_len)"""
-        super().__init__(model, bins, bin_len, use_graph, criterion)
+                 criterion=None, bin_len=128, seq_len=None, choices=None):
+        """seq_len: a question-answering model's padded length before packing, HF's ignored index (None: bin_len).
+        choices: a multiple-choice model's N; the bins then carry batch x N choice sequences"""
+        super().__init__(model, bins, bin_len, use_graph, criterion, choices)
         if seq_len is not None:
             self.ignored_index = int(seq_len)
         dev = self.eng.dev
         self.bins, self.batch, self.bin_len = bins, batch, bin_len
+        self.ncls = batch * choices if self.mc else batch      # sequences in the bins
         n = bins * bin_len
-        # pinned staging: ids | token types | positions | segments (as int64) | cls rows | labels (per sequence, or
-        # per bin row for a token model: pack_batch's "labels")
+        # pinned staging: ids | token types | positions | segments (as int64) | cls rows | labels (per sequence or
+        # multiple-choice example, or per bin row for a token model: pack_batch's "labels")
         self.d_lab, lab_slots = self._label_buffer(n if self.token else batch)
-        self._alloc_stage(4 * n + batch + lab_slots)
+        self._alloc_stage(4 * n + self.ncls + lab_slots)
         z = lambda *sh: torch.zeros(*sh, dtype=torch.int64, device=dev)
-        self.d_pos, self.d_cls = z(bins, bin_len), z(batch)
+        self.d_pos, self.d_cls = z(bins, bin_len), z(self.ncls)
         self.d_seg = torch.zeros(bins, bin_len, dtype=torch.int32, device=dev)
         self._arm(optimizer, accum_steps, max_grad_norm)
 
@@ -567,24 +614,24 @@ class PackedTrainStep(_StagedGraphStep):
         self.d_tt.copy_(st[n:2 * n].view(self.bins, S))
         self.d_pos.copy_(st[2 * n:3 * n].view(self.bins, S))
         self.d_seg.copy_(st[3 * n:4 * n].view(self.bins, S))            # int64 -> int32
-        self.d_cls.copy_(st[4 * n:4 * n + self.batch])
-        self._unstage_labels(st[4 * n + self.batch:])
+        self.d_cls.copy_(st[4 * n:4 * n + self.ncls])
+        self._unstage_labels(st[4 * n + self.ncls:])
 
     def stage(self, packed, label):
         n, hs = self.bins * self.bin_len, self.h_stage
         want = (self.bins, self.bin_len) if self.token else (2, self.batch) if self.qa else (self.batch,)
         if packed["bins"] != self.bins or packed["input_ids"].shape[1] != self.bin_len or \
-                tuple(label.shape[:len(want)]) != want:
+                tuple(label.shape[:len(want)]) != want or packed["cls_index"].numel() != self.ncls:
             raise ValueError("PackedTrainStep was built for %d bins of %d tokens / %d sequences"
-                             % (self.bins, self.bin_len, self.batch))
+                             % (self.bins, self.bin_len, self.ncls))
         if self._h2d_done is not None:
             self._h2d_done.synchronize()
         hs[0:n].copy_(packed["input_ids"].reshape(-1))
         hs[n:2 * n].copy_(packed["token_type_ids"].reshape(-1))
         hs[2 * n:3 * n].copy_(packed["position_ids"].reshape(-1))
         hs[3 * n:4 * n].copy_(packed["segments"].reshape(-1))
-        hs[4 * n:4 * n + self.batch].copy_(packed["cls_index"])
-        self._stage_labels(hs[4 * n + self.batch:], label)
+        hs[4 * n:4 * n + self.ncls].copy_(packed["cls_index"].reshape(-1))
+        self._stage_labels(hs[4 * n + self.ncls:], label)
         self._stage_lr()
         self._h2d()
 
@@ -596,8 +643,9 @@ class PackedTrainStep(_StagedGraphStep):
                                                   **self._head_kw(True)))
 
     def __call__(self, packed, label, final=True):
-        """label: per sequence [batch], for a token model pack_batch's "labels" [bins, bin_len], for a
-        question-answering model the int64 [2, batch] start / end positions (trainer.qa_positions of pack_batch's)"""
+        """label: per sequence [batch] (a multiple-choice model: per example), for a token model pack_batch's "labels"
+        [bins, bin_len], for a question-answering model the int64 [2, batch] start / end positions
+        (trainer.qa_positions of pack_batch's)"""
         self.stage(packed, label)
         self.run_device(final)
         return self.loss_out
@@ -609,8 +657,8 @@ class FusedEvalStep(_StagedGraphStep):
     loss).  Returns device tensors that are overwritten by the next call (the callers below consume them before
     staging the next batch)."""
 
-    def __init__(self, model, batch_size, seq_len, use_graph=True, criterion=None):
-        super().__init__(model, batch_size, seq_len, use_graph, criterion)
+    def __init__(self, model, batch_size, seq_len, use_graph=True, criterion=None, choices=None):
+        super().__init__(model, batch_size, seq_len, use_graph, criterion, choices)
         shape = (batch_size, seq_len) if self.token else (batch_size,)
         if self.mlm:
             self.logits_out = None    # no [B, S, V] logits: the labelled rows' (pred, label) pairs instead
@@ -619,7 +667,8 @@ class FusedEvalStep(_StagedGraphStep):
         else:
             if self.qa:
                 shape = (batch_size, seq_len)      # [B, S, 2]: start and end logits
-            self.logits_out = torch.zeros(*shape, self.model.num_labels, dtype=torch.float32, device=self.eng.dev)
+            C = choices if self.mc else self.model.num_labels
+            self.logits_out = torch.zeros(*shape, C, dtype=torch.float32, device=self.eng.dev)
 
     def _body(self):
         self._unstage()
@@ -630,7 +679,7 @@ class FusedEvalStep(_StagedGraphStep):
             self.pred_out[:cap].copy_(gb["pred"])
             self.lab_out[:cap].copy_(gb["labels"])
         else:
-            self.logits_out.copy_(logits)
+            self.logits_out.copy_(logits.view(self.logits_out.shape))
         self.loss_out.copy_(loss)
 
     def __call__(self, batch_data):
@@ -726,8 +775,8 @@ class Trainer:
         label = d["label"]
         # a token model with a criterion leaves the loss to it: its in-model CrossEntropyLoss() would not know the
         # criterion's ignore_index
-        model_labels = None if self.criterion is not None and (_is_token(self.model) or _is_mlm(self.model)) \
-            else label
+        model_labels = None if self.criterion is not None and (_is_token(self.model) or _is_mlm(self.model)
+                                                               or _is_mc(self.model)) else label
         output = self.model(input_ids=d["input_ids"], token_type_ids=d["token_type_ids"],
                             attention_mask=d["attention_mask"], labels=model_labels)
         return output, label
@@ -749,6 +798,8 @@ class Trainer:
             return MLM_PROBLEM_TYPE
         if _is_qa(self.model):
             return QA_PROBLEM_TYPE         # HF's QA model never reads or sets config.problem_type
+        if _is_mc(self.model):
+            return MC_PROBLEM_TYPE         # nor does HF's multiple-choice model
         if _is_token(self.model):
             return TOKEN_PROBLEM_TYPE      # HF's token model never reads or sets config.problem_type
         cfg = _unwrap(self.model).config
@@ -775,6 +826,9 @@ class Trainer:
             check_token_criterion(self.criterion)
             C = _unwrap(self.model).num_labels
             return self.criterion(logits.reshape(-1, C), label.reshape(-1))
+        if _is_mc(self.model):
+            check_mc_criterion(self.criterion)
+            return self.criterion(logits, label)
         if _unwrap(self.model).num_labels == 1 and label.is_floating_point():
             return self.criterion(logits.reshape(-1), label.reshape(-1))
         return self.criterion(logits, label)
@@ -794,13 +848,15 @@ class Trainer:
             output, label = self._forward(batch_data)
             return self._logits(output), label, output.loss
         self.problem_type(batch_data.get("label"))
-        B, S = batch_data["input_ids"].shape
+        shape = tuple(batch_data["input_ids"].shape)
         m = _unwrap(self.model)
-        # a token model's staged labels are checked against its loss's ignore_index: the criterion's
-        crit = self.criterion if _is_token(m) else None
-        key = (id(m), B, S, m.config.problem_type, criterion_key(crit))     # `test` may swap the model [:222-224]
+        # a token (or multiple-choice) model's staged labels are checked against its loss's ignore_index: the
+        # criterion's
+        crit = self.criterion if _is_token(m) or _is_mc(m) else None
+        key = (id(m), shape, m.config.problem_type, criterion_key(crit))     # `test` may swap the model [:222-224]
         if key not in self._fused_eval:
-            self._fused_eval[key] = FusedEvalStep(self.model, B, S, criterion=crit)
+            choices = _choices(batch_data) if _is_mc(m) else None
+            self._fused_eval[key] = FusedEvalStep(self.model, shape[0], shape[-1], criterion=crit, choices=choices)
         return self._fused_eval[key](batch_data)
 
     def eval_step(self, batch_data):
@@ -840,9 +896,10 @@ class Trainer:
         first, final = self._micro == 0, self._micro >= k - 1
         self._micro = 0 if final else self._micro + 1
         qa = _is_qa(self.model)
+        choices = _choices(batch_data) if _is_mc(self.model) else None
         if getattr(self.args, "fused", True) and getattr(self.args, "pack", False) and \
-                batch_data["input_ids"].shape[1] <= MAX_BIN and not batch_data["input_ids"].is_cuda:
-            bin_len = bin_length(batch_data["attention_mask"], batch_data["input_ids"].shape[1])
+                batch_data["input_ids"].shape[-1] <= MAX_BIN and not batch_data["input_ids"].is_cuda:
+            bin_len = bin_length(batch_data["attention_mask"], batch_data["input_ids"].shape[-1])
             token = _is_token(self.model) or _is_mlm(self.model)
             qa_kw = dict(start_positions=batch_data["start_positions"],
                          end_positions=batch_data["end_positions"]) if qa else {}
@@ -853,6 +910,8 @@ class Trainer:
                    torch.are_deterministic_algorithms_enabled())
             if qa:
                 key += (packed["seq_len"],)        # the span loss's ignored index is part of the captured step
+            if choices is not None:
+                key += (choices,)
             lkey = self._captured_loss_key(batch_data.get("label"))
             if key not in self._packed or (self._packed[key].accum_steps, self._packed[key].max_grad_norm,
                                            self._packed[key].loss_key) != (k, clip, lkey):
@@ -860,7 +919,7 @@ class Trainer:
                     self._packed.pop(next(iter(self._packed)))
                 self._packed[key] = PackedTrainStep(self.model, self.optimizer, key[0], key[1], accum_steps=k,
                                                     max_grad_norm=clip, criterion=self.criterion, bin_len=bin_len,
-                                                    seq_len=packed["seq_len"] if qa else None)
+                                                    seq_len=packed["seq_len"] if qa else None, choices=choices)
                 self._packed[key].loss_key = lkey
             self.model.train()
             label = packed["labels"] if token else qa_positions(packed) if qa else batch_data["label"]
@@ -868,13 +927,13 @@ class Trainer:
             if final:
                 self._scheduler_step()      # after the replay: the next stage() reads the new lr
         elif getattr(self.args, "fused", True):
-            B, S = batch_data["input_ids"].shape
+            shape = tuple(batch_data["input_ids"].shape)
             lkey = self._captured_loss_key(batch_data.get("label"))
             det = torch.are_deterministic_algorithms_enabled()
-            if self._fused is None or (self._fused.B, self._fused.S, self._fused.accum_steps, self._fused.max_grad_norm,
-                                       self._fused.loss_key, self._fused.deterministic) != (B, S, k, clip, lkey, det):
-                self._fused = FusedTrainStep(self.model, self.optimizer, B, S, accum_steps=k, max_grad_norm=clip,
-                                             criterion=self.criterion)
+            if self._fused is None or (self._fused.batch_shape, self._fused.accum_steps, self._fused.max_grad_norm,
+                                       self._fused.loss_key, self._fused.deterministic) != (shape, k, clip, lkey, det):
+                self._fused = FusedTrainStep(self.model, self.optimizer, shape[0], shape[-1], accum_steps=k,
+                                             max_grad_norm=clip, criterion=self.criterion, choices=choices)
                 self._fused.loss_key = lkey
             self.model.train()
             loss = self._fused(batch_data, final)
@@ -1121,7 +1180,8 @@ class Trainer:
 
     def dev(self, dev_loader):
         """(summed rank-mean loss, metric) over the gathered rows.  The metric, higher is better: accuracy
-        (single-label; a token model's over the tokens whose label is not the ignore index), subset accuracy -- every column of (logits > 0) equal to (labels >= 0.5) -- (multi-label), or
+        (single-label; a token model's over the tokens whose label is not the ignore index, a multiple-choice model's
+        over the examples whose label is not), subset accuracy -- every column of (logits > 0) equal to (labels >= 0.5) -- (multi-label), or
         the Pearson correlation of predictions and labels (regression)."""
         self.model.eval()
         if _is_mlm(self.model):
@@ -1143,7 +1203,7 @@ class Trainer:
                 loss_total += loss
                 logits, label = self.output_reduce(logits, label)
                 logits = logits.detach().cpu().numpy()
-                if problem_type == TOKEN_PROBLEM_TYPE:
+                if problem_type in (TOKEN_PROBLEM_TYPE, MC_PROBLEM_TYPE):
                     label = label.reshape(-1).detach().cpu().numpy()
                     keep = label != self._ignore_index()
                     preds = np.argmax(logits.reshape(label.shape[0], -1), axis=1)
@@ -1215,7 +1275,8 @@ class Trainer:
 
     def test(self, model, test_loader, labels):
         """sklearn's classification_report over the gathered rows: of the argmax class (single-label; a token model's
-        over the tokens whose label is not the ignore index) or of the
+        over the tokens whose label is not the ignore index, a multiple-choice model's argmax choice over the examples
+        whose label is not) or of the
         indicator arrays (logits > 0) against (labels >= 0.5) (multi-label).  Regression raises ValueError."""
         if _is_mlm(model):
             raise ValueError("test() prints a classification report, which is not useful over a vocabulary: use dev() "
@@ -1241,7 +1302,7 @@ class Trainer:
                                      "use dev() for the Pearson correlation")
                 logits, label = self.output_reduce(logits, label)
                 logits = logits.detach().cpu().numpy()
-                if problem_type == TOKEN_PROBLEM_TYPE:
+                if problem_type in (TOKEN_PROBLEM_TYPE, MC_PROBLEM_TYPE):
                     label = label.reshape(-1).detach().cpu().numpy()
                     keep = label != self._ignore_index()
                     trues.extend(label[keep].tolist())
